@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Headline benchmark: faces/sec of the SynergyNet inference hot path on B200.
+"""Headline benchmark: faces/sec of the SynergyNet inference hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W          # this framework (one process per GPU)
     python bench.py --impl reference --steps K --warmup W  # the reference algorithm on host cores
+    python bench.py --steps K --dump-outputs DIR           # + the landmarks of the last timed step as DIR/*.npy
 
 A step = one pass of the hot path (MobileNetV2 backbone -> 62 3DMM params -> 68 landmarks) over
 one batch of 1024 synthetic 120x120 crops per GPU (BASELINE.json configs[1]); with N > 1 the batch
@@ -57,17 +58,12 @@ KERNEL_BYTES = {
     'heads_kernel': 4 * (1280 + 62), 'dense_recon_tc_kernel': 4 * (62 + 3 * 68), 'dense_alpha_kernel': 4 * 62,
 }
 DENSE_BYTES_PER_FACE = 3 * 53215 * 4          # SURVEY.md section 8(d): 638,580 B written per face
-MIN_TIMED_SECONDS = 2.0                       # the K steps are repeated until the timed region is this long
 
 
 def load_peaks():
-    fp = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(fp):
-        with open(fp) as f:
-            p = json.load(f)
-        return dict(bf16_sustained=p['bf16_tflops_sustained'], bf16_burst=p['bf16_tflops'],
-                    hbm=p['hbm_gbs'], source='measured (MEASURED_PEAKS.json)')
-    return dict(bf16_sustained=1400.0, bf16_burst=1590.0, hbm=6650.0, source='fallback (B200_PROFILING.md)')
+    # NVIDIA's H100 SXM data sheet (dense bf16, HBM3, 700 W card): the denominators of the roofline fractions, not
+    # rates this machine was measured to reach; a card with a lower power limit gets less
+    return dict(bf16_sustained=989.0, bf16_burst=989.0, hbm=3350.0, source='H100 SXM data sheet (700 W)')
 
 
 class ClockSampler:
@@ -120,10 +116,8 @@ class ClockSampler:
 
 def dominant_roofline(kernel_ms: dict, batch: int, peaks: dict):
     """`roofline` of the launch that takes the largest share of the step, against BOTH ceilings: algorithmic FLOP
-    of that launch / its CUDA-event duration vs the sustained bf16 peak (it runs inside a long step), and its
-    algorithmic HBM bytes (block in + out) vs the measured HBM peak.  `bound` names the ceiling that is closer,
-    i.e. the one that bounds the kernel.  `traffic` = DRAM bytes of one launch from the committed ncu capture
-    (profiles/kernel_traffic.json)."""
+    of that launch / its CUDA-event duration vs the bf16 peak, and its algorithmic HBM bytes (block in + out) vs the
+    HBM peak.  `bound` names the ceiling that is closer, i.e. the one that bounds the kernel."""
     if not kernel_ms:
         return None
     name = max(kernel_ms, key=kernel_ms.get)
@@ -133,19 +127,14 @@ def dominant_roofline(kernel_ms: dict, batch: int, peaks: dict):
     tflops = flop / (ms * 1e-3) / 1e12
     gbs = nbytes / (ms * 1e-3) / 1e9
     f_tensor, f_hbm = tflops / peaks['bf16_sustained'], gbs / peaks['hbm']
-    traffic = None
-    fp = os.path.join(ROOT, 'profiles', 'kernel_traffic.json')
-    if os.path.exists(fp):
-        with open(fp) as f:
-            traffic = json.load(f).get(name)
     hbm_bound = f_hbm >= f_tensor
     return {'kernel': name, 'bound': 'hbm' if hbm_bound else 'tensor',
             'achieved': gbs if hbm_bound else tflops, 'peak': peaks['hbm'] if hbm_bound else peaks['bf16_sustained'],
             'unit': 'GB/s' if hbm_bound else 'TFLOP/s', 'frac': f_hbm if hbm_bound else f_tensor,
             'frac_tensor': f_tensor, 'achieved_tflops': tflops, 'frac_hbm': f_hbm, 'achieved_gbs': gbs,
-            'traffic': traffic, 'ms_per_launch': ms, 'share_of_step': ms / sum(kernel_ms.values()),
+            'ms_per_launch': ms, 'share_of_step': ms / sum(kernel_ms.values()),
             'what': f'algorithmic {KERNEL_MACS.get(name, 0):,} MAC/face x 2 and {KERNEL_BYTES.get(name, 0):,} HBM B/face '
-                    f'x {batch} faces / CUDA-event time of one launch; peaks = sustained bf16 and HBM copy of {peaks["source"]}'}
+                    f'x {batch} faces / CUDA-event time of one launch; peaks = bf16 and HBM of the {peaks["source"]}'}
 
 
 def build_model(device: str):
@@ -384,11 +373,6 @@ def render_detect_measurement(dev, peaks, cpu_too=True):
     e2e_ms = (time.perf_counter() - t0) / 20 * 1e3
     nver, ntri = verts.shape[2], tri.shape[0]
     alg_bytes = B * nver * 12 + ntri * 12 + 2 * H * W * 3
-    try:      # DRAM bytes of one call from the committed ncu capture (profiles/r2_ncu_full_render.txt)
-        with open(os.path.join(ROOT, 'profiles', 'kernel_traffic.json')) as f:
-            render_traffic = json.load(f).get('render_call')
-    except Exception:
-        render_traffic = None
     out['render'] = {
         'workload': f'{B} meshes x {nver} vertices / {ntri} triangles -> one {H}x{W}x3 uint8 canvas (normals + lighting + z-buffer), '
                     'vertices read in place from the (B,3,N) layout of the dense stage',
@@ -397,11 +381,9 @@ def render_detect_measurement(dev, peaks, cpu_too=True):
         'e2e': {'ms': e2e_ms, 'meshes_per_s': B / e2e_ms * 1e3, 'h2d_bytes': int(verts.nbytes + H * W * 3), 'd2h_bytes': H * W * 3,
                 'what': 'pinned host vertices + canvas in, image out, synchronised per call'},
         'roofline': {'bound': 'hbm', 'achieved': alg_bytes / (ms_all * 1e-3) / 1e9, 'peak': peaks['hbm'], 'unit': 'GB/s',
-                     'frac': alg_bytes / (ms_all * 1e-3) / 1e9 / peaks['hbm'], 'traffic': render_traffic,
+                     'frac': alg_bytes / (ms_all * 1e-3) / 1e9 / peaks['hbm'],
                      'what': f'algorithmic {alg_bytes} B per call (vertices + triangle list once + canvas in and out) / CUDA-event time of '
-                             'the six launches; the stage is instruction-issue / atomic work (raster_depth_kernel: issue slots 82 % busy, '
-                             'DRAM 3 %) far below the HBM ceiling; traffic is 13x the algorithmic bytes because the (B,H,W) 64-bit key '
-                             'image is cleared and read back whole (100 MB of the 141 MB)'}}
+                             'the six launches; the (B,H,W) 64-bit depth-key image is cleared and read back whole on top of these bytes'}}
     # ---- detect ---------------------------------------------------------------------------------------------------------------
     ih, iw = 720, 1080
     P = detect.num_priors(ih, iw)
@@ -503,7 +485,7 @@ def run_b200(args):
     peaks = load_peaks()
 
     from synergynet_b200 import synthetic
-    n_rot = 3                                   # rotate 3 x 177 MB inputs: every step misses the 126 MB L2
+    n_rot = 3                                   # rotate 3 x 177 MB inputs: every step misses the 50 MB L2
     xs = [synthetic.make_inputs(B, seed=10 * rank + i).to(dev) for i in range(n_rot)]
     # two gather targets: the all-gather of step i runs on a side stream under the backbone of step i+1
     lmk_alls = [torch.empty((world * B, 3, 68), device=dev, dtype=torch.float32) for _ in range(2)]
@@ -525,22 +507,7 @@ def run_b200(args):
     for i in range(max(args.warmup, 3)):
         step(i)
     barrier()
-    # The K steps the driver asks for are repeated `rounds` times inside ONE timed region so that it lasts
-    # >= MIN_TIMED_SECONDS (sustained clocks, >= 10 clock samples); ms_per_step = region / (rounds * K).
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for i in range(args.steps):
-        step(i)
-    if world > 1:
-        og.wait()
-    e1.record()
-    barrier()
-    probe_ms = max(e0.elapsed_time(e1), 1e-3)
-    rounds = 1 if args.profile else max(1, int(np.ceil(MIN_TIMED_SECONDS * 1e3 / probe_ms)))
-    r = torch.tensor([rounds], device=dev, dtype=torch.int64)
-    if world > 1:
-        dist.all_reduce(r, op=dist.ReduceOp.MAX)
-    rounds = int(r.item())
+    # exactly --steps steps inside ONE CUDA-event region; ms_per_step = region / steps
     sampler = ClockSampler(local_rank) if rank == 0 else None
     if sampler:
         sampler.start()
@@ -550,8 +517,8 @@ def run_b200(args):
     barrier()
     t_wall0 = time.time()
     ev0.record()
-    for i in range(rounds * args.steps):
-        step(i)
+    for i in range(args.steps):
+        last = step(i)
     if world > 1:
         og.wait()                                       # the last gather ends inside the CUDA-event region
     ev1.record()
@@ -564,8 +531,15 @@ def run_b200(args):
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t.item())
-    n_timed = rounds * args.steps
+    n_timed = args.steps
     eng.raise_if_error()
+    if args.dump_outputs:
+        # what the timed path returned in its last step: the (B,3,68) landmarks of this rank's batch (all ranks' when
+        # gathered).  The inputs are seeded, so two builds run with the same arguments can be compared output for output.
+        out = lmk_alls[(args.steps - 1) & 1] if world > 1 else last
+        if rank == 0:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, 'landmarks.npy'), out.detach().float().cpu().numpy())
 
     # ---- multi-GPU correctness: the gathered tensor holds every rank's shard in rank order -----------------
     verify = None
@@ -647,16 +621,11 @@ def run_b200(args):
         d_ms = _time_cuda(dense_step, iters=50, warmup=5)
         img_dense_ms = _time_cuda(lambda: eng.reconstruct(eng.forward(xs[1]), dense=True), iters=20, warmup=3)
         dbytes = float(B) * DENSE_BYTES_PER_FACE
-        traffic = None
-        fp = os.path.join(ROOT, 'profiles', 'kernel_traffic.json')
-        if os.path.exists(fp):
-            with open(fp) as f:
-                traffic = json.load(f).get('dense_recon_fm_kernel')
         extra['dense'] = {
             'workload': 'configs[2]: batch=1024 params -> dense (B,3,53215) vertices', 'ms': d_ms,
             'faces_per_s': B / d_ms * 1e3, 'image_to_dense_ms': img_dense_ms, 'image_to_dense_faces_per_s': B / img_dense_ms * 1e3,
             'roofline': {'bound': 'hbm', 'achieved': dbytes / d_ms / 1e6, 'peak': peaks['hbm'], 'unit': 'GB/s',
-                         'frac': dbytes / d_ms / 1e6 / peaks['hbm'], 'traffic': traffic,
+                         'frac': dbytes / d_ms / 1e6 / peaks['hbm'],
                          'what': '638,580 B written per face x 1024 / CUDA-event time of alpha pre-pass + reconstruction kernel'}}
         del dense_out, params
         # ---- configs[0] shape on the GPU: one face per call, device-resident (eager launches vs one CUDA graph) ----
@@ -736,16 +705,16 @@ def run_b200(args):
             'config': {'workload': 'configs[1]: batch=1024 synthetic 120x120 crops, MobileNetV2 + 3DMM params + '
                                    '68-landmark reconstruction' + (' + all-gather of landmarks' if world > 1 else ''),
                        'batch_per_gpu': B, 'global_batch': world * B,
-                       'engine': {0: 'simt_fp32', 1: 'tcgen05_f16x3_unfused', 2: 'tcgen05_f16x3_fused',
-                                  3: 'tcgen05_f16x1_fused (not parity grade)'}.get(eng.engine, eng.engine),
+                       'engine': {0: 'simt_fp32', 1: 'wgmma_f16x3_unfused', 2: 'wgmma_f16x3_fused',
+                                  3: 'wgmma_f16x1_fused (not parity grade)'}.get(eng.engine, eng.engine),
                        'parallelism': f'dp{world}',
                        'collective': ('one all_gather_into_tensor of the (B,3,68) landmarks per step (NCCL), issued on a side '
                                       'stream under the next step\'s backbone; the last one completes inside the timed region'
                                       if world > 1 else None),
-                       'timed_region': f'{rounds} x {args.steps} steps in one CUDA-event region ({ms / 1e3:.2f} s)',
-                       'rounds': rounds, 'timed_steps': n_timed,
+                       'timed_region': f'{args.steps} steps in one CUDA-event region ({ms / 1e3:.2f} s)',
+                       'timed_steps': n_timed,
                        'l2': f'{n_rot} rotating device-resident input batches of {B * X_BYTES_PER_FACE / 1e6:.0f} MB '
-                             '(> 126 MB L2) + >1 GB of activations written per step'},
+                             '(> 50 MB L2) + >1 GB of activations written per step'},
             'e2e': {'value': world * B * e2e_steps / e2e_s, 'unit': 'faces/s',
                     'h2d_bytes_per_step': B * X_BYTES_PER_FACE, 'd2h_bytes_per_step': B * LMK_BYTES_PER_FACE,
                     'steps': e2e_steps, 'blocking_value': world * B * e2e_steps / e2e_block_s,
@@ -802,7 +771,7 @@ def main():
     ap.add_argument('--warmup', type=int, default=5)
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
     ap.add_argument('--batch', type=int, default=1024, help='faces per GPU per step')
-    ap.add_argument('--engine', type=int, default=None, help='0 = fp32 CUDA cores, 1 = tcgen05 split-fp16 x3, 2 = 1 + fused blocks (default), 3 = 2 with one fp16 pass')
+    ap.add_argument('--engine', type=int, default=None, help='0 = fp32 CUDA cores, 1 = tensor-core split-fp16 x3, 2 = 1 + fused blocks (default), 3 = 2 with one fp16 pass')
     ap.add_argument('--cpu-seconds', type=float, default=12.0)
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--profile', action='store_true', help='device-resident steps only (for ncu runs)')
@@ -810,7 +779,13 @@ def main():
     ap.add_argument('--no-config5', action='store_true', help='skip the ResNet-50 / PointNet heads measurement')
     ap.add_argument('--no-render', action='store_true', help='skip the Sim3DR / FaceBoxes post-processing measurement')
     ap.add_argument('--no-single-pass', action='store_true', help='skip the single-pass fp16 engine measurement')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the landmarks of the last timed step to DIR/landmarks.npy (float32)')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
+    if args.dump_outputs and args.impl == 'reference':
+        ap.error('--dump-outputs writes what the timed GPU path returned; the host reference arm has nothing to dump')
     if args.impl == 'reference':
         run_reference(args)
     else:

@@ -1,5 +1,5 @@
 /*
- * synergy_b200.h -- C ABI of the B200 (sm_100a) SynergyNet inference hot path.
+ * synergy_b200.h -- C ABI of the H100 (sm_90a) SynergyNet inference hot path.
  *
  * The reference (choyingw/SynergyNet) has no native boundary for this path: it is a Python
  * nn.Module API (model_building.py:65-165, synergy3DMM.py:70-207) whose arithmetic runs inside
@@ -19,8 +19,8 @@
  *     main_train.py:176).
  *   - tensors are fp32 and contiguous in the layouts the reference uses.
  */
-#ifndef SYNERGY_B200_H_
-#define SYNERGY_B200_H_
+#ifndef SYNERGY_H100_H_
+#define SYNERGY_H100_H_
 
 #include <stdint.h>
 
@@ -37,15 +37,15 @@ enum {
   SYN_ERR_STATE = 3,     /* call order violated (e.g. forward before syn_commit)               */
   SYN_ERR_SHAPE = 4,     /* "length of params mismatch" (model_building.py:116-119) and alike  */
   SYN_ERR_NOMEM = 5,
-  SYN_ERR_UNSUPPORTED = 6 /* not an sm_100 device, or an engine the build does not contain      */
+  SYN_ERR_UNSUPPORTED = 6 /* not an sm_90 device, or an engine the build does not contain      */
 };
 
 /* Compute engines for the 1x1 convolutions / basis products (syn_set_engine). */
 enum {
   SYN_ENGINE_SIMT_FP32 = 0,   /* CUDA-core fp32 FMA everywhere (bring-up / cross-check path)     */
-  SYN_ENGINE_TC_SPLIT3 = 1,   /* tcgen05.mma, operands split in fp16 hi+lo with exact power-of-two  */
+  SYN_ENGINE_TC_SPLIT3 = 1,   /* wgmma, operands split in fp16 hi+lo with exact power-of-two        */
                               /* pre-scaling, 3 MMAs per product (hi*hi + hi*lo + lo*hi), fp32      */
-                              /* accumulation in TMEM: meets the 1e-4 parity bar (a bf16 split, the  */
+                              /* accumulation in registers: meets the 1e-4 parity bar (a bf16 split, */
                               /* first version, measured 1.7e-4 and was dropped); convs unfused      */
   SYN_ENGINE_TC_BF16X3 = 1,   /* old name of SYN_ENGINE_TC_SPLIT3                                    */
   SYN_ENGINE_TC_FUSED = 2,    /* default: the same arithmetic with the stem + all 17 inverted-       */
@@ -310,7 +310,7 @@ int syn_debug_forward_until(syn_handle_t* h, const float* x_dev, int batch, int 
 int syn_debug_heads_buffer(syn_handle_t* h, int which, float* out_host, int64_t n);
 
 /* Host-only: the face-group plan the fused engine uses for a launch over `batch` faces on a GPU with
- * `sms` SMs and `faces_per_tile` (1, 2 or 8) faces per full tile.  Groups [0, *split) hold
+ * `sms` SMs and `faces_per_tile` (1, 2 or 4) faces per full tile.  Groups [0, *split) hold
  * faces_per_tile faces each; for two-face tiles the groups [*split, *face_groups) hold ONE face each
  * (the partial last wave is split so that more SMs share it), otherwise the last group may be
  * partial.  Lets the host logic be tested without a GPU. */
@@ -319,4 +319,4 @@ int syn_debug_tile_plan(int batch, int sms, int faces_per_tile, int* split, int*
 #ifdef __cplusplus
 }
 #endif
-#endif  /* SYNERGY_B200_H_ */
+#endif  /* SYNERGY_H100_H_ */

@@ -2,7 +2,7 @@
 
 This is a CPU restatement of the reference algorithm, used as the checker by ``tests/``,
 ``__graft_entry__.smoke()`` and the ``cpu_baseline`` / ``--impl reference`` legs of
-``bench.py``.  Nothing in ``synergynet_b200/`` may import it: the product path is the sm_100a
+``bench.py``.  Nothing in ``synergynet_b200/`` may import it: the product path is the sm_90a
 library and fails loudly without it.
 
 Parity status: PINNED.  The reference has no tests or golden vectors of its own for this path
@@ -321,7 +321,7 @@ def max_rel_err(new, ref) -> float:
 @torch.no_grad()
 def resnet50_forward(sd: Dict[str, torch.Tensor], x: torch.Tensor, prefix: str = 'I2P.backbone.'):
     """ResNet._forward_impl with Bottleneck blocks [3,4,6,3], backbone_nets/resnet_backbone.py:120-146,227-249.
-    Returns (out102 = ori|shape|exp|tex, pooled 2048-d feature).  The adapter of the B200 shim (and of the golden
+    Returns (out102 = ori|shape|exp|tex, pooled 2048-d feature).  The adapter of the H100 shim (and of the golden
     vectors) for the (param62, avgpool) contract the reference's I2P expects is out102[:, :62], pooled."""
     sd = {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
 

@@ -1,7 +1,6 @@
 #!/usr/bin/env python
 """Design aid: shared-memory bank-conflict degree of the lane -> address mappings used by the fused MBConv
-kernel (synergynet_b200/csrc/kernels_fused.cuh).  The formulas below restate the kernel's indexing; the
-numbers they predict were checked against ncu (`L1 Wavefronts Shared Excessive`, profiles/r1_final_ncu_smem_*).
+kernel (synergynet_b200/csrc/kernels_fused.cuh).  The formulas below restate the kernel's indexing.
 
 Model: 32 banks x 4 B.  A 128-bit access is served per quarter-warp (8 lanes), a 64-bit access per half-warp
 (16 lanes), a 32-bit access per warp; lanes reading the SAME address are merged (broadcast).  Degree 1 =

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Stage-by-stage comparison of MLP_for on the GPU against the CPU oracle (debug aid, B200 only)."""
+"""Stage-by-stage comparison of MLP_for on the GPU against the CPU oracle (debug aid, needs an H100)."""
 import os
 import sys
 import types

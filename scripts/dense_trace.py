@@ -1,17 +1,16 @@
 #!/usr/bin/env python
 """Timeline of dense_recon_fm_kernel's CTA 0 (SYN_DENSE_TRACE=<file> makes the library dump clock64 stamps), cycles:
-issuer per item: [wait accumulator buffer | plane 0 / 1 / 2 landed | MMAs issued]; epilogue (thread 0) per item:
-[wait alpha + meta | wait MMAs | accumulators read (buffer released) | staged + stored]."""
+loader per item: [plane 0 / 1 / 2 requested (its ring slot was free)]; team 0 (thread 0) per item:
+[wait alpha + meta | MMAs of the three planes done | staged + stored]."""
 import sys
 
 rows = [l.split() for l in open(sys.argv[1])]
 ep = {(r[0], int(r[1])): [int(x) for x in r[2:]] for r in rows}
 t0 = min(v[0] for v in ep.values() if v[0] > 0)
-print(' item | issuer: start  w.tmem  plane0  plane1  plane2  issued | epilogue: start  w.meta  w.mma  ld+1st half  2nd half    end')
-d = lambda a, k: a[k] - a[k - 1] if a[k] and a[k - 1] else -1
+print(' item | loader: plane0  plane1  plane2 | team 0: start  w.meta   mma  stored')
 for i in range(0, 64):
-    iss = ep.get(('issuer', i)); e = ep.get(('epi0', i))
-    if not iss or iss[0] == 0:
+    ld = ep.get(('loader', i)); e = ep.get(('team0', i))
+    if not e or e[0] == 0:
         break
-    print(f' {i:4d} | {iss[0] - t0:13d} {d(iss, 1):7d} {d(iss, 2):7d} {d(iss, 3):7d} {d(iss, 4):7d} {d(iss, 5):7d} |'
-          f' {e[0] - t0:15d} {d(e, 1):7d} {d(e, 2):6d} {d(e, 3):12d} {d(e, 4):9d} {e[4] - t0:6d}')
+    pl = [f'{v - t0:7d}' if ld and v else '      -' for v in (ld[:3] if ld else [0, 0, 0])]
+    print(f' {i:4d} | {" ".join(pl)} | {e[0] - t0:13d} {e[1] - e[0]:7d} {e[2] - e[1]:5d} {e[4] - e[2]:7d}')

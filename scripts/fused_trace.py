@@ -4,9 +4,8 @@
     nvcc ... -DSYN_FUSED_TRACE -o synergynet_b200/libsynergy_b200_trace.so synergynet_b200/csrc/synergy_b200.cu
     SYN_LIB_PATH=$PWD/synergynet_b200/libsynergy_b200_trace.so python scripts/fused_trace.py 12 2 8
 
-Prints, for CTA 0's second tile of each requested block, clock64 deltas (cycles) per chunk:
-worker thread 0 (wait D1 | barrier | EPI1 | barrier + wait G2 | DW) and the issuer
-(wait EPI1 | issue GEMM1 | wait A2 | issue GEMM2 | wait G2 + refill)."""
+Prints, for CTA 0's second tile of each requested block, clock64 deltas (cycles) per chunk of worker thread 0:
+barrier | GEMM1 + EPI1 | barrier | depthwise | barrier + GEMM2."""
 import ctypes
 import os
 import sys
@@ -32,21 +31,18 @@ def main():
     lib.syn_debug_read_trace(buf, n)
     t = np.frombuffer(buf, dtype=np.int64).reshape(18, 2, 64, 8)
     for b in blocks:
-        w, i = t[b, 0], t[b, 1]
+        w = t[b, 0]
         t0 = w[63, 0]
-        print(f'== block {b}: tile start 0, chunks done {w[63, 1] - t0}, EPI2 wait..start {w[63, 2] - t0}..{w[63, 3] - t0}, '
-              f'EPI2 end {w[63, 4] - t0}; issuer: wait X {i[63, 0] - t0}..{i[63, 1] - t0}, GEMM1(0) issued {i[63, 2] - t0}')
+        print(f'== block {b}: tile start 0, chunks done {w[63, 1] - t0}, EPI2 start {w[63, 2] - t0}, EPI2 end {w[63, 4] - t0}')
         q = w[62]
         if q[0]:
             print(f'   prep(next tile): start {q[0] - t0}, staged {q[1] - t0}, all workers {q[2] - t0}, converted {q[3] - t0}, published {q[4] - t0}; first batch: loads issued {q[5] - t0}, first item stored {q[6] - t0}, batch done {q[7] - t0}')
-        print('  c | worker: start  waitD1   bar   EPI1  bar+G2     DW | issuer: start waitEPI1  G1iss  waitA2  G2iss  waitG2')
-        for c in range(63):
+        print('  c | worker: start    bar  G1+EPI1    bar     DW  bar+G2')
+        for c in range(62):
             if w[c, 0] == 0:
                 break
-            wd = [w[c, k + 1] - w[c, k] for k in range(5)]
-            idl = [i[c, k + 1] - i[c, k] if i[c, k + 1] and i[c, k] else -1 for k in range(5)]
-            print(f' {c:2d} | {w[c, 0] - t0:13d} {wd[0]:7d} {wd[1]:5d} {wd[2]:6d} {wd[3]:7d} {wd[4]:6d} | {i[c, 0] - t0:13d} '
-                  f'{idl[0]:8d} {idl[1]:6d} {idl[2]:7d} {idl[3]:6d} {idl[4]:7d}')
+            wd = [w[c, 1] - w[c, 0], w[c, 3] - w[c, 1], w[c, 4] - w[c, 3], w[c, 5] - w[c, 4], w[c, 6] - w[c, 5]]
+            print(f' {c:2d} | {w[c, 0] - t0:13d} {wd[0]:6d} {wd[1]:8d} {wd[2]:6d} {wd[3]:6d} {wd[4]:7d}')
 
 
 if __name__ == '__main__':

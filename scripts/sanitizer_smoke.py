@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Tiny pass over every kernel family for `compute-sanitizer --tool memcheck` (B200 only; batches of 1-3 faces)."""
+"""Tiny pass over every kernel family for `compute-sanitizer --tool memcheck` (needs an H100; batches of 1-3 faces)."""
 import os
 import sys
 import types

@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""The reference's single-image flow (singleImage.py:20-75, utils/render.py:31-53) on the B200 modules: detect faces,
+"""The reference's single-image flow (singleImage.py:20-75, utils/render.py:31-53) on the H100 modules: detect faces,
 regress 3DMM parameters, reconstruct landmarks / dense meshes / poses, draw the solid-mesh overlay.
 
     python scripts/single_image_demo.py [image.png] [--out overlay.png]
 
 Without an image a synthetic scene is used; without the reference's external assets (pretrained/best.pth.tar,
 3dmm_data/, FaceBoxes/weights/FaceBoxesProd.pth) the seeded synthetic stand-ins of synergynet_b200.synthetic are used, so
-the picture is meaningless but every stage runs exactly as it would with the real files.  Needs a B200."""
+the picture is meaningless but every stage runs exactly as it would with the real files.  Needs an H100."""
 import argparse
 import os
 import sys

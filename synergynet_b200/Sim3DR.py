@@ -1,4 +1,4 @@
-"""Sim3DR on the B200: vertex normals, lighting and z-buffer rasterisation (SURVEY.md section 8 row f2).
+"""Sim3DR on the H100: vertex normals, lighting and z-buffer rasterisation (SURVEY.md section 8 row f2).
 
 Reference-shaped surface (``Sim3DR/Sim3DR.py:8-29``, ``Sim3DR/lighting.py:23-79``): ``get_normal``, ``rasterize``,
 ``RenderPipeline`` take and return numpy arrays like the reference's Cython module does.  Underneath sits
@@ -42,7 +42,7 @@ class MeshRenderer:
     def __init__(self, triangles, nver: int, device=None):
         self._lib = _lib.load()
         if not torch.cuda.is_available():
-            raise RuntimeError('synergynet_b200.Sim3DR needs a CUDA device (B200, sm_100a); there is no CPU fallback')
+            raise RuntimeError('synergynet_b200.Sim3DR needs a CUDA device (H100, sm_90a); there is no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         tri = np.ascontiguousarray(np.asarray(triangles), dtype=np.int32)
         if tri.ndim != 2 or tri.shape[1] != 3:
@@ -138,7 +138,7 @@ _renderers = {}
 
 def _renderer_for(triangles: np.ndarray, nver: int) -> MeshRenderer:
     if not torch.cuda.is_available():
-        raise RuntimeError('synergynet_b200.Sim3DR needs a CUDA device (B200, sm_100a); there is no CPU fallback')
+        raise RuntimeError('synergynet_b200.Sim3DR needs a CUDA device (H100, sm_90a); there is no CPU fallback')
     tri = np.ascontiguousarray(triangles, dtype=np.int32)
     key = (hash(tri.tobytes()), tri.shape, int(nver), torch.cuda.current_device())
     r = _renderers.get(key)

@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) implementation of SynergyNet's batched inference hot path.
+"""H100-native (sm_90a) implementation of SynergyNet's batched inference hot path.
 
 Public surface mirrors the reference: ``synergynet_b200.model_building.SynergyNet(args)``,
 ``synergynet_b200.synergy3DMM.SynergyNet()``, ``parse_param_62``, ``ParamsPack``.

@@ -139,7 +139,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f'{LIB_PATH} not found: build it with `python -m synergynet_b200.build` '
-            '(nvcc, sm_100a). There is no CPU or eager fallback for this path.')
+            '(nvcc, sm_90a). There is no CPU or eager fallback for this path.')
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         try:

@@ -125,7 +125,7 @@ class MobileNetV2Params(nn.Module):
 
     def forward(self, *a, **k):  # pragma: no cover
         raise RuntimeError('MobileNetV2Params is a parameter container; the forward pass runs in '
-                           'the sm_100a library via synergynet_b200.engine.Engine')
+                           'the sm_90a library via synergynet_b200.engine.Engine')
 
 
 def mobilenet_v2(pretrained: bool = False, **_):
@@ -133,7 +133,7 @@ def mobilenet_v2(pretrained: bool = False, **_):
 
 
 class _PointMLPParams(nn.Module):
-    """Parameter container in the reference's key schema; ``forward`` runs in the sm_100a library through the engine
+    """Parameter container in the reference's key schema; ``forward`` runs in the sm_90a library through the engine
     of the model that owns the module (``_engine_provider`` is installed by ``model_building._SynergyBase``)."""
     _NET = -1
 
@@ -150,7 +150,7 @@ class _PointMLPParams(nn.Module):
         if self._engine_provider is None:
             raise RuntimeError(f'{type(self).__name__}: not attached to a SynergyNet model (its engine owns the GPU state)')
         if self.num_pts != 68:
-            raise RuntimeError('the sm_100a PointNet heads are built for 68 landmarks (MLP_for(68) / MLP_rev(68))')
+            raise RuntimeError('the sm_90a PointNet heads are built for 68 landmarks (MLP_for(68) / MLP_rev(68))')
         return self._engine_provider(t, self._NET)
 
 
@@ -212,7 +212,7 @@ class _Bottleneck(nn.Module):
 
 class ResNet50Params(nn.Module):
     """Key schema of ``resnet_backbone.resnet50()`` (conv1/bn1, layer1..4.{i}.conv{1,2,3}/bn{1,2,3}/downsample.{0,1},
-    fc_tex/fc_ori/fc_shape/fc_exp); parameter container, the forward pass runs in the sm_100a library."""
+    fc_tex/fc_ori/fc_shape/fc_exp); parameter container, the forward pass runs in the sm_90a library."""
     feature_dim = 2048
 
     def __init__(self):
@@ -241,7 +241,7 @@ class ResNet50Params(nn.Module):
                 nn.init.constant_(m.bias, 0)
 
     def forward(self, *a, **k):  # pragma: no cover
-        raise RuntimeError('ResNet50Params is a parameter container; the forward pass runs in the sm_100a library')
+        raise RuntimeError('ResNet50Params is a parameter container; the forward pass runs in the sm_90a library')
 
 
 def resnet50_conv_keys():

@@ -1,4 +1,4 @@
-"""Build the sm_100a C-ABI library in-tree with nvcc (no torch cpp_extension, no JIT cache).
+"""Build the sm_90a C-ABI library in-tree with nvcc (no torch cpp_extension, no JIT cache).
 
 ``python -m synergynet_b200.build`` or ``__graft_entry__.build()``.  The resulting
 ``synergynet_b200/libsynergy_b200.so`` is git-ignored but travels with the work tree.
@@ -15,7 +15,7 @@ CSRC = os.path.join(PKG_DIR, 'csrc')
 LIB_NAME = 'libsynergy_b200.so'
 LIB_PATH = os.path.join(PKG_DIR, LIB_NAME)
 
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '--use_fast_math=false', '-Xcompiler', '-fPIC', '-shared', '-Xptxas', '-v']
 
 
@@ -23,7 +23,7 @@ def _nvcc() -> str:
     for cand in (os.environ.get('NVCC'), shutil.which('nvcc'), '/usr/local/cuda/bin/nvcc'):
         if cand and os.path.exists(cand):
             return cand
-    raise RuntimeError('nvcc not found; cannot build the sm_100a library')
+    raise RuntimeError('nvcc not found; cannot build the sm_90a library')
 
 
 def _sources():

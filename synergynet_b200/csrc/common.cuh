@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a SynergyNet hot-path library.
+// Shared helpers for the sm_90a SynergyNet hot-path library.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,18 +1,18 @@
-// 3DMM reconstruction on tcgen05 (reference model_building.py:106-139, reconstruct_vertex_62):
+// 3DMM reconstruction on tensor cores (wgmma; reference model_building.py:106-139, reconstruct_vertex_62):
 //   S[b, 3v+c] = u[3v+c] + sum_k W[3v+c, k] * alpha[b, k]      (k = 40 shape + 10 expression)
 //   V[b, i, v] = sum_c P[b, i, c] * S[b, 3v+c] + t[b, i];   V[b, 1, v] = 121 - V[b, 1, v]
 // The basis product is a GEMM with M = vertices, N = faces, K = 50 (padded to 64); running it once per
-// coordinate plane (x, y, z) puts the three coordinates of vertex v in the SAME TMEM lane, so the
-// 3x3 pose transform is per-thread arithmetic and the (B,3,N) output rows are written with fully
-// coalesced 128-byte warp stores.  The kernel is HBM-write bound: 638,580 B per face (dense).
+// coordinate plane (x, y, z) puts the three coordinates of vertex v in the SAME accumulator position of the
+// same thread, so the 3x3 pose transform is per-thread arithmetic.  The kernel is HBM-write bound:
+// 638,580 B per face (dense).
 //
 //   dense_alpha_kernel     params (B,62) -> de-whitened pose (B,12) fp32 + alpha as fp16 hi/lo B tiles
 //   dense_recon_tc_kernel  persistent; item = (128-vertex tile, 64-face tile), vertex-tile major; the
 //                          96 KB basis tile (3 planes x hi/lo) stays in smem while the CTA walks over
 //                          the face tiles
-//     warp 16 lane 0: loader + MMA issuer (3 planes x 3 passes x 4 K-steps, N = 64), 2 TMEM buffers
-//     warps 0-15:     epilogue in two groups of 8 warps, one per TMEM buffer (lane = vertex; the two
-//                     warps of a lane quarter split the 64 faces)
+//     warp 16: loader (bulk copies of basis tiles and alpha / pose tiles)
+//     warps 0-15: four warpgroups; warpgroup w runs the MMAs (3 planes x 3 passes x 4 K-steps, N = 32) of
+//                 vertices 64 (w & 1) .. +63 x faces 32 (w >> 1) .. +31 of every item and their epilogue
 // Split-16x3 precision scheme of kernels_tc.cuh; basis rows are pre-scaled per vertex row and alpha
 // per coefficient (both powers of two, folded back exactly in the epilogue / the basis image).
 #pragma once
@@ -33,7 +33,7 @@ constexpr int kDnBSlot = kDnBTile + kDnPoseTile;
 constexpr int kDnMetaTile = 128 * 6 * 4;                  // per vertex tile: u[3][128], 1/rowscale[3][128]
 constexpr int kDnBSlots = 4;                              // alpha/pose ring: loads run 3 items ahead of the MMAs
 constexpr int kDnSmem = kDnATile + 2 * kDnMetaTile + kDnBSlots * kDnBSlot + 1024;
-constexpr int kDnEpiWarps = 16;                          // 4 per TMEM lane quarter: 16 faces each
+constexpr int kDnEpiWarps = 16;                          // four warpgroups: MMA + epilogue
 constexpr int kDnThreads = (kDnEpiWarps + 1) * 32;
 
 // ---- pre-pass -----------------------------------------------------------------------------------------
@@ -47,7 +47,7 @@ __global__ void __launch_bounds__(kDnAlphaThreads) dense_alpha_kernel(const floa
                                                                       const float* __restrict__ stdv, const float* __restrict__ ascale,
                                                                       uint8_t* __restrict__ aimg, float* __restrict__ pose, int batch,
                                                                       int whitening, const float* __restrict__ roi5) {
-  // the reconstruction kernel may start its prologue (barriers, TMEM, basis planes) now; it waits for this grid
+  // the reconstruction kernel may start its prologue (barriers, basis planes) now; it waits for this grid
   // (griddepcontrol.wait) before it touches the alpha image or the pose rows
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   const int f = threadIdx.x & (kDnFaces - 1), kg = threadIdx.x / kDnFaces, tile = blockIdx.x;
@@ -97,21 +97,19 @@ struct DenseArgs {
   int batch, nver, n_vtiles, n_ftiles, transform;
   int affine;                 // apply the per-face crop -> image affine stored behind the pose rows
   int stream_stores;          // 1: st.global.cs (evict-first), 0: plain write-back stores (L2 merges neighbouring 512-byte runs)
-  long long* trace;           // debug (SYN_DENSE_TRACE): clock64 stamps of CTA 0, 8 events x 64 items x {group 0, group 1, issuer}
+  long long* trace;           // debug (SYN_DENSE_TRACE): clock64 stamps of CTA 0, 8 events x 64 items x {team 0, unused, loader}
   int* err;
 };
 
-// Synchronisation (item i uses B slot / TMEM buffer i & 1; `use` = i >> 1 is its per-slot sequence number):
-//   bar_a       basis tile + meta landed (one phase per vertex tile)       loader -> issuer, epilogue
-//   bar_bfull   alpha + pose tile landed                                    loader -> issuer, epilogue
-//   bar_dfull   MMAs of the item complete                                   tcgen05.commit -> epilogue
-//   bar_dfree   epilogue done with the item (TMEM buffer, B slot, and -- at a vertex-tile change --
-//               the meta rows of its basis tile have been read)              256 arrivals -> issuer
+// Synchronisation (item i uses B slot i % kDnBSlots; items are processed in order by every warpgroup):
+//   bar_a        basis tile + meta landed (one phase per vertex tile)       loader -> compute warps
+//   bar_bfull[s] alpha + pose tile landed                                    loader -> compute warps
+//   bar_done[s]  all 512 compute threads are done with the item in slot s (its B slot, and -- at a vertex-tile
+//                change -- the basis tile and its meta rows may be overwritten)                  -> loader
 __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_tc_kernel(const DenseArgs p) {
   using namespace tc;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_a, bar_bfull[kDnBSlots], bar_dfull[2], bar_dfree[2];
-  __shared__ uint32_t tmem_base_s;
+  __shared__ __align__(8) uint64_t bar_a, bar_bfull[kDnBSlots], bar_done[kDnBSlots];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sA = smem;
   float* sMeta = reinterpret_cast<float*>(smem + kDnATile);          // 2 slots (vertex-tile load parity)
@@ -124,87 +122,84 @@ __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_tc_kernel(const Den
 
   if (tid == 0) {
     mbar_init(smem_u32(&bar_a), 1);
-    for (int i = 0; i < kDnBSlots; ++i) mbar_init(smem_u32(&bar_bfull[i]), 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&bar_dfull[i]), 1);
-      mbar_init(smem_u32(&bar_dfree[i]), kDnEpiWarps * 16);     // one group of 8 warps per TMEM buffer
+    for (int i = 0; i < kDnBSlots; ++i) {
+      mbar_init(smem_u32(&bar_bfull[i]), 1);
+      mbar_init(smem_u32(&bar_done[i]), kDnEpiWarps * 32);
     }
     fence_mbar_init();
   }
-  if (warp == kDnEpiWarps) tmem_alloc<512>(smem_u32(&tmem_base_s));
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = tmem_base_s;
 
   if (warp < kDnEpiWarps) {
-    // ------------------------------ epilogue ------------------------------------------------------
-    // Two groups of 8 warps: group g owns TMEM buffer g and every item with (i & 1) == g, so that the MMAs
-    // of item i+1 (other buffer, other group) and their completion latency overlap this group's work.
-    // Inside a group: warp & 3 = TMEM lane quarter, (warp >> 2) & 1 = which 32 of the 64 faces.
-    const int grp = warp >> 3, half = (warp >> 2) & 1;
-    const int lane_v = tid & 127;
+    // ------------------------------ MMA + epilogue ------------------------------------------------
+    const int t = tid & 127, wg = tid >> 7, slab = wg & 1, fh = wg >> 1;
     const int vt0 = it0 / p.n_ftiles;
     int cur_vt = -1;
-    float ux = 0.f, uy = 0.f, uz = 0.f, ox = 0.f, oy = 0.f, oz = 0.f;
-    for (int it = it0 + grp, i = grp; it < it1; it += 2, i += 2) {
+    float ux[2] = {}, uy[2] = {}, uz[2] = {}, ox[2] = {}, oy[2] = {}, oz[2] = {};
+    const uint32_t d_hi = smem_desc_hi(128);
+    const uint32_t a_lo = smem_desc_lo(smem_u32(sA) + slab * 1024, 2048);
+    for (int it = it0, i = 0; it < it1; ++it, ++i) {
       const int vt = it / p.n_ftiles, ft = it - vt * p.n_ftiles;
-      const uint32_t use_par = (uint32_t)(i >> 1) & 1;
       const int sb = i % kDnBSlots;
-      mbar_wait(smem_u32(&bar_bfull[sb]), (uint32_t)(i / kDnBSlots) & 1, p.err);   // pose tile visible to this thread
-      mbar_wait(smem_u32(&bar_dfull[grp]), use_par, p.err);
-      tc_fence_after_sync();
-      if (vt != cur_vt) {             // new basis tile: its meta rows (landed before the MMAs of this item ran)
+      mbar_wait(smem_u32(&bar_bfull[sb]), (uint32_t)(i / kDnBSlots) & 1, p.err);
+      if (vt != cur_vt) {             // new basis tile and its meta rows
         cur_vt = vt;
         mbar_wait(smem_u32(&bar_a), (uint32_t)(vt - vt0) & 1, p.err);
         const float* m = sMeta + ((vt - vt0) & 1) * (kDnMetaTile / 4);
-        ux = m[0 * 128 + lane_v]; uy = m[1 * 128 + lane_v]; uz = m[2 * 128 + lane_v];
-        ox = m[3 * 128 + lane_v]; oy = m[4 * 128 + lane_v]; oz = m[5 * 128 + lane_v];
-      }
-      const int v = vt * 128 + lane_v;
 #pragma unroll
-      for (int rnd = 0; rnd < 2; ++rnd) {                            // 2 x 16 faces per thread
-        const int fofs = half * 32 + rnd * 16;
-        const float* pose = reinterpret_cast<const float*>(sB + sb * kDnBSlot + kDnBTile) + fofs * kDnPoseStride;
-        const uint32_t trow = tmem + ((uint32_t)((warp & 3) * 32) << 16) + grp * 192 + fofs;
-        float sx[16], sy[16], sz[16];
-        tmem_ld16x3(trow, trow + 64, trow + 128, sx, sy, sz);   // three loads in flight, one wait
-        const int b0 = ft * kDnFaces + fofs;
-        if (v < p.nver) {
-#pragma unroll
-          for (int f = 0; f < 16; ++f) {
-            if (b0 + f < p.batch) {
-              const float4 r0 = *reinterpret_cast<const float4*>(pose + f * kDnPoseStride);
-              const float4 r1 = *reinterpret_cast<const float4*>(pose + f * kDnPoseStride + 4);
-              const float4 r2 = *reinterpret_cast<const float4*>(pose + f * kDnPoseStride + 8);
-              const float X = fmaf(sx[f], ox, ux), Y = fmaf(sy[f], oy, uy), Z = fmaf(sz[f], oz, uz);
-              float vx = fmaf(r0.x, X, fmaf(r0.y, Y, fmaf(r0.z, Z, r0.w)));
-              float vy = fmaf(r1.x, X, fmaf(r1.y, Y, fmaf(r1.z, Z, r1.w)));
-              float vz = fmaf(r2.x, X, fmaf(r2.y, Y, fmaf(r2.z, Z, r2.w)));
-              if (p.transform) vy = (float)(kImg + 1) - vy;          // model_building.py:129,137
-              if (p.affine) {                                        // utils/inference.py:131-136, numpy's fp32 mul then add
-                const float4 q = *reinterpret_cast<const float4*>(pose + f * kDnPoseStride + 12);
-                vx = __fadd_rn(__fmul_rn(vx, q.x), q.y);
-                vy = __fadd_rn(__fmul_rn(vy, q.z), q.w);
-                vz = __fmul_rn(vz, pose[f * kDnPoseStride + 16]);
-              }
-              float* o = p.out + (size_t)(b0 + f) * 3 * p.nver + v;
-              __stcs(o, vx); __stcs(o + p.nver, vy); __stcs(o + 2 * (size_t)p.nver, vz);   // write-once stream
-            }
-          }
+        for (int h = 0; h < 2; ++h) {
+          const int lv = 64 * slab + acc_row(t, 2 * h);
+          ux[h] = m[0 * 128 + lv]; uy[h] = m[1 * 128 + lv]; uz[h] = m[2 * 128 + lv];
+          ox[h] = m[3 * 128 + lv]; oy[h] = m[4 * 128 + lv]; oz[h] = m[5 * 128 + lv];
         }
       }
-      tc_fence_before_sync();
-      mbar_arrive(smem_u32(&bar_dfree[grp]));
+      const uint32_t b_lo = smem_desc_lo(smem_u32(sB + sb * kDnBSlot) + fh * 4 * 128, 1024);   // faces 32 fh ..
+      float acc[3][16];
+      wgmma_fence();
+#pragma unroll
+      for (int plane = 0; plane < 3; ++plane) {
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass) {
+          const uint32_t a_off = (plane * 2 + (pass == 2 ? 1 : 0)) * kDnAPlane;   // W: hi,hi,lo
+          const uint32_t b_off = (pass == 1 ? kDnBPlane : 0);                     // alpha: hi,lo,hi
+#pragma unroll
+          for (int ks = 0; ks < kDnK / 16; ++ks)
+            wgmma_f16<32>(acc[plane], desc64(d_hi, a_lo + ((a_off + ks * 4096) >> 4)),
+                          desc64(d_hi, b_lo + ((b_off + ks * 2048) >> 4)), (pass > 0 || ks > 0) ? 1u : 0u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      const float* pose_tile = reinterpret_cast<const float*>(sB + sb * kDnBSlot + kDnBTile);
+#pragma unroll
+      for (int q = 0; q < 16; ++q) {
+        const int h = (q >> 1) & 1;
+        const int v = vt * 128 + 64 * slab + acc_row(t, q);
+        const int fl = 32 * fh + acc_col(t, q), b = ft * kDnFaces + fl;
+        if (v < p.nver && b < p.batch) {
+          const float* pose = pose_tile + fl * kDnPoseStride;
+          const float4 r0 = *reinterpret_cast<const float4*>(pose);
+          const float4 r1 = *reinterpret_cast<const float4*>(pose + 4);
+          const float4 r2 = *reinterpret_cast<const float4*>(pose + 8);
+          const float X = fmaf(acc[0][q], ox[h], ux[h]), Y = fmaf(acc[1][q], oy[h], uy[h]), Z = fmaf(acc[2][q], oz[h], uz[h]);
+          float vx = fmaf(r0.x, X, fmaf(r0.y, Y, fmaf(r0.z, Z, r0.w)));
+          float vy = fmaf(r1.x, X, fmaf(r1.y, Y, fmaf(r1.z, Z, r1.w)));
+          float vz = fmaf(r2.x, X, fmaf(r2.y, Y, fmaf(r2.z, Z, r2.w)));
+          if (p.transform) vy = (float)(kImg + 1) - vy;          // model_building.py:129,137
+          if (p.affine) {                                        // utils/inference.py:131-136, numpy's fp32 mul then add
+            const float4 a4 = *reinterpret_cast<const float4*>(pose + 12);
+            vx = __fadd_rn(__fmul_rn(vx, a4.x), a4.y);
+            vy = __fadd_rn(__fmul_rn(vy, a4.z), a4.w);
+            vz = __fmul_rn(vz, pose[16]);
+          }
+          float* o = p.out + (size_t)b * 3 * p.nver + v;
+          __stcs(o, vx); __stcs(o + p.nver, vy); __stcs(o + 2 * (size_t)p.nver, vz);   // write-once stream
+        }
+      }
+      mbar_arrive(smem_u32(&bar_done[sb]));
     }
   } else if (warp == kDnEpiWarps) {
-    // ------------------------------ loader + MMA issuer -------------------------------------------
-    // The whole warp runs this control flow convergently; bulk copies and MMA batches sit under one
-    // elect.sync each, so the descriptors come straight from uniform registers (a `tid == X` branch costs
-    // ~170 cycles per MMA, tools/umma_timing: 36 MMAs per item made the issuer the bottleneck of round 1).
-    const uint32_t idesc = make_idesc_f16(128, kDnFaces);
-    const uint32_t d_hi = smem_desc_hi(128);
-    const uint32_t a_lo = smem_desc_lo(smem_u32(sA), 2048);
+    // ------------------------------ loader (converged warp, bulk copies under elect.sync) -----------------
     auto load_b = [&](int it, int s) {
       if (elect_one()) {
         const int ft = it % p.n_ftiles;
@@ -215,8 +210,8 @@ __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_tc_kernel(const Den
       }
       __syncwarp();
     };
-    auto dfree_wait = [&](int j) {                                   // epilogue finished item j (>= 0)
-      mbar_wait(smem_u32(&bar_dfree[j & 1]), (uint32_t)(j >> 1) & 1, p.err);
+    auto done_wait = [&](int j) {                                   // every compute thread finished item j (>= 0)
+      mbar_wait(smem_u32(&bar_done[j % kDnBSlots]), (uint32_t)(j / kDnBSlots) & 1, p.err);
     };
     int cur_vt = -1;
     const int vt0 = it0 / p.n_ftiles;
@@ -225,11 +220,9 @@ __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_tc_kernel(const Den
       if (it0 + k < it1) load_b(it0 + k, k);
     for (int it = it0, i = 0; it < it1; ++it, ++i) {
       const int vt = it / p.n_ftiles;
-      const int s = i & 1;
       if (vt != cur_vt) {
-        // the basis tile in smem is overwritten: every MMA of the previous tile must be complete and every
-        // epilogue thread past its bar_a wait, both implied by the epilogue having finished item i-1
-        if (i >= 1) dfree_wait(i - 1);
+        // the basis tile in smem is overwritten: every thread must be done with item i-1 (its MMAs read the old tile)
+        if (i >= 1) done_wait(i - 1);
         cur_vt = vt;
         if (elect_one()) {
           mbar_expect_tx(smem_u32(&bar_a), kDnATile + kDnMetaTile);
@@ -238,78 +231,48 @@ __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_tc_kernel(const Den
                    smem_u32(&bar_a));
         }
         __syncwarp();
-        mbar_wait(smem_u32(&bar_a), (uint32_t)(vt - vt0) & 1, p.err);
       }
-      const int sb = i % kDnBSlots;
-      mbar_wait(smem_u32(&bar_bfull[sb]), (uint32_t)(i / kDnBSlots) & 1, p.err);
-      if (i >= 2) dfree_wait(i - 2);                               // TMEM buffer s drained
-      tc_fence_after_sync();
-      const uint32_t b_lo = smem_desc_lo(smem_u32(sB + sb * kDnBSlot), 1024);
-      if (elect_one()) {
-#pragma unroll
-        for (int plane = 0; plane < 3; ++plane) {
-#pragma unroll
-          for (int pass = 0; pass < 3; ++pass) {
-            const uint32_t a_off = (plane * 2 + (pass == 2 ? 1 : 0)) * kDnAPlane;   // W: hi,hi,lo
-            const uint32_t b_off = (pass == 1 ? kDnBPlane : 0);                     // alpha: hi,lo,hi
-#pragma unroll
-            for (int ks = 0; ks < kDnK / 16; ++ks)
-              umma_f16(tmem + s * 192 + plane * 64, desc64(d_hi, a_lo + ((a_off + ks * 4096) >> 4)),
-                       desc64(d_hi, b_lo + ((b_off + ks * 2048) >> 4)), idesc, (pass > 0 || ks > 0) ? 1u : 0u);
-          }
-        }
-        umma_commit(smem_u32(&bar_dfull[s]));
-      }
-      __syncwarp();
-      // prefetch alpha/pose three items ahead into the slot last used by item i-1 (MMA + epilogue done)
+      // prefetch alpha/pose three items ahead into the slot last used by item i-1
       if (it + kDnBSlots - 1 < it1) {
-        if (i >= 1) dfree_wait(i - 1);
+        if (i >= 1) done_wait(i - 1);
         load_b(it + kDnBSlots - 1, (i + kDnBSlots - 1) % kDnBSlots);
       }
     }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == kDnEpiWarps) {
-    __syncwarp();
-    tmem_dealloc<512>(tmem);
   }
 }
 
 
 // -------------------------------------------------------------------------------------------------------------------
 // Face-major variant for the dense mesh (configs[2]).  The kernel above walks vertex-tile major: a CTA writes 512 B
-// to each of 64 faces x 3 rows and moves on to OTHER faces, so every DRAM page is touched once per visit (measured:
-// 2.1 TB/s of 6.5).  Here a CTA keeps one 64-face tile and walks over consecutive vertex tiles: each of its 192
-// output rows grows by 512 contiguous bytes per item.  The price is a new basis tile per item; it streams from L2
-// (40 MB image, resident) coordinate plane by coordinate plane (32 KB = hi + lo of one coordinate) through a 4-slot
-// ring, two planes ahead of the MMAs.
+// to each of 64 faces x 3 rows and moves on to OTHER faces, so every DRAM page is touched once per visit.  Here a CTA
+// keeps one 64-face tile and walks over consecutive vertex tiles: each of its 192 output rows grows by 512 contiguous
+// bytes per item.  The price is a new basis tile per item; it streams from L2 (40 MB image, resident in the 50 MB L2)
+// coordinate plane by coordinate plane (32 KB = hi + lo of one coordinate) through a 4-slot ring, ahead of the MMAs.
 //
 // WHOLE-SECTOR STORES.  The output rows of the reference layout (B,3,53215) fp32 start on every 4-byte phase, so a warp
-// that stores "lane = vertex" always writes two partial 32-byte sectors per 128 bytes.  Measured with the store stream
-// alone (tools/dense_store_probe.cu): that pattern tops out at 2.95 TB/s -- exactly what the previous version of this
-// kernel reached -- while the same bytes written as whole aligned sectors go at 5.1 TB/s.  So the epilogue does not
-// store from the TMEM lane mapping: a TEAM of four warps (the four lane quarters = 128 vertices, 16 faces) stages
-// 12 output rows at a time in shared memory and writes them back out with the lane -> address mapping shifted by each
-// row's own phase (address / 4 mod 8), so that every warp store covers whole aligned sectors.  The <= 7 floats that
-// fall off the end of a row piece are carried (sCarry) into the next item's piece of the same row; only the two ends of
-// a CTA's band are written with bounds-checked stores.
-//   bar_pfull[slot]   plane landed                                                    loader -> issuer
-//   bar_pempty[slot]  the 12 MMAs that read the plane are complete (tcgen05.commit)  -> loader
-//   bar_mfull[slot]   meta rows of item i (slot i % 4) landed                         loader -> epilogue
+// that stores "lane = vertex" always writes two partial 32-byte sectors per 128 bytes; the same bytes written as whole
+// aligned sectors are much cheaper for the memory system.  So the epilogue does not store from the accumulator layout:
+// a TEAM (one warpgroup: 128 vertices = two 64-row MMA slabs, 16 faces) stages 24 output rows (8 faces x 3 coordinates)
+// at a time in shared memory and writes them back out with the lane -> address mapping shifted by each row's own
+// phase (address / 4 mod 8), so that every warp store covers whole aligned sectors.  The <= 7 floats that fall off the
+// end of a row piece are carried (sCarry) into the next item's piece of the same row; only the two ends of a CTA's
+// band are written with bounds-checked stores.
+//   bar_pfull[slot]   plane landed                                                    loader -> teams
+//   bar_pempty[slot]  all 512 team threads' MMAs that read the plane are complete     teams -> loader
+//   bar_mfull[slot]   meta rows of item i (slot i % 4) landed                         loader -> teams
 //   bar_bfull         alpha + pose tile of the CTA's face tile landed (once)
-//   bar_dfull[s]      accumulator buffer s complete                                   issuer -> epilogue
-//   bar_dfree[s]      all 512 epilogue threads have read buffer s into registers (before they stage / store the second half)
 constexpr int kFmPlane = 2 * kDnAPlane;                   // 32 KB: [hi|lo] of one coordinate of one vertex tile
 #ifndef SYN_FM_SPLIT
-#define SYN_FM_SPLIT 1                                    // bulk copies per plane (1, 2, 4, 8: measured no difference)
+#define SYN_FM_SPLIT 1                                    // bulk copies per plane (1, 2, 4, 8)
 #endif
 constexpr int kFmPSlots = 4, kFmMetaSlots = 4;
-constexpr int kFmTeams = 4;                               // 4 warps each: faces 16t .. 16t+15 of the item
-constexpr int kFmSubFaces = 4;                            // faces staged per sub-round -> 12 rows
+constexpr int kFmTeams = 4;                               // one warpgroup each: faces 16t .. 16t+15 of the item
+constexpr int kFmSubFaces = 8;                            // faces staged per sub-round -> 24 rows
 constexpr int kFmRows = 3 * kFmSubFaces;
-constexpr int kFmPitch = 128;                             // floats per staged row (position = vertex within the tile)
-constexpr int kFmStage = 2 * kFmRows * kFmPitch * 4;      // per team, double buffered: 12 KB
+// floats per staged row (position = vertex within the tile).  128 + 4: the accumulator layout writes rows 6 apart from
+// the four lanes of a quad; the pad puts them on four different groups of 8 banks
+constexpr int kFmPitch = 132;
+constexpr int kFmStage = kFmRows * kFmPitch * 4;          // per team: 12.4 KB
 constexpr int kFmCarry = 16 * 3 * 8 * 4;                  // per team: 48 rows x 8 floats
 constexpr int kFmSmem = kFmPSlots * kFmPlane + kFmMetaSlots * kDnMetaTile + kDnBSlot + kFmTeams * (kFmStage + kFmCarry) + 1024;
 static_assert(kDnATile == 3 * kFmPlane, "basis tile = three coordinate planes");
@@ -346,21 +309,19 @@ template <bool kTrace, bool kAffine>
 __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_fm_kernel(const DenseArgs p) {
   using namespace tc;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_pfull[kFmPSlots], bar_pempty[kFmPSlots], bar_mfull[kFmMetaSlots], bar_bfull,
-      bar_dfull[2], bar_dfree[2];
-  __shared__ uint32_t tmem_base_s;
+  __shared__ __align__(8) uint64_t bar_pfull[kFmPSlots], bar_pempty[kFmPSlots], bar_mfull[kFmMetaSlots], bar_bfull;
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sP = smem;                                                                      // plane ring
   float* sMeta = reinterpret_cast<float*>(smem + kFmPSlots * kFmPlane);                   // kFmMetaSlots meta tiles
   uint8_t* sB = smem + kFmPSlots * kFmPlane + kFmMetaSlots * kDnMetaTile;                 // alpha + pose tile of this CTA's face tile
-  float* sStage = reinterpret_cast<float*>(sB + kDnBSlot);                                // [team][buf][row][kFmPitch]
+  float* sStage = reinterpret_cast<float*>(sB + kDnBSlot);                                // [team][row][kFmPitch]
   float* sCarry = sStage + kFmTeams * (kFmStage / 4);                                     // [team][48 rows][8]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   // Work split: CTA = (face tile ft, BAND of consecutive vertex tiles); the bands are the same for every face tile and
   // the CTAs of one band are neighbours in the grid, so the CTAs that need a given basis tile ask for it at about the
   // same time and all but the first hit in L2 (a plain contiguous split of the item list gives every face tile its own
-  // band boundaries: ncu showed the 40 MB basis image read 4.4x from DRAM).
+  // band boundaries, and the basis image is read several times from DRAM).
   const int n_bands = max(1, (int)gridDim.x / p.n_ftiles);
   const int band_len = (p.n_vtiles + n_bands - 1) / n_bands;
   const int ft = (int)blockIdx.x % p.n_ftiles, my_band = (int)blockIdx.x / p.n_ftiles;
@@ -368,135 +329,143 @@ __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_fm_kernel(const Den
   const int n_items = vt_hi - vt_lo;                                 // item i = vertex tile vt_lo + i
 
   if (tid == 0) {
-    for (int i = 0; i < kFmPSlots; ++i) { mbar_init(smem_u32(&bar_pfull[i]), 1); mbar_init(smem_u32(&bar_pempty[i]), 1); }
+    for (int i = 0; i < kFmPSlots; ++i) {
+      mbar_init(smem_u32(&bar_pfull[i]), 1);
+      mbar_init(smem_u32(&bar_pempty[i]), kDnEpiWarps * 32);
+    }
     for (int i = 0; i < kFmMetaSlots; ++i) mbar_init(smem_u32(&bar_mfull[i]), 1);
     mbar_init(smem_u32(&bar_bfull), 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&bar_dfull[i]), 1);
-      mbar_init(smem_u32(&bar_dfree[i]), kDnEpiWarps * 32);
-    }
     fence_mbar_init();
   }
-  if (warp == kDnEpiWarps) tmem_alloc<512>(smem_u32(&tmem_base_s));
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = tmem_base_s;
 
   if (warp < kDnEpiWarps) {
-    // ------------------------------ epilogue: 4 teams x 4 warps, every team works on every item ------------------------
-    const int team = warp >> 2, tt = tid & 127, wq = warp & 3;       // tt = TMEM lane = vertex within the tile
+    // ------------------------------ 4 teams (warpgroups), every team works on every item ------------------------------
+    const int team = warp >> 2, t = tid & 127, wq = warp & 3;
     const int f0 = team * 16;                                        // first face (within the tile) of this team
     float* stage = sStage + team * (kFmStage / 4);
     float* carry = sCarry + team * (kFmCarry / 4);
     const float* pose_tile = reinterpret_cast<const float*>(sB + kDnBTile);
+    const uint32_t d_hi = smem_desc_hi(128);
+    const uint32_t b_lo = smem_desc_lo(smem_u32(sB) + (f0 / 8) * 128, 1024);   // alpha rows of faces f0 .. f0 + 15
     for (int i = 0; i < n_items; ++i) {
-      const int vt = vt_lo + i, s = i & 1;
+      const int vt = vt_lo + i;
       const bool tr = kTrace && blockIdx.x == 0 && tid == 0 && i < 64;
       if (tr) p.trace[i * 8 + 0] = clock64();
-      mbar_wait_inl(smem_u32(&bar_bfull), 0, p.err);                                       // pose tile visible to this thread
+      mbar_wait_inl(smem_u32(&bar_bfull), 0, p.err);                                       // alpha / pose tile visible
       mbar_wait_inl(smem_u32(&bar_mfull[i % kFmMetaSlots]), (uint32_t)(i / kFmMetaSlots) & 1, p.err);   // meta rows visible
-      const float* m = sMeta + (i % kFmMetaSlots) * (kDnMetaTile / 4);
-      const float ux = m[0 * 128 + tt], uy = m[1 * 128 + tt], uz = m[2 * 128 + tt];
-      const float ox = m[3 * 128 + tt], oy = m[4 * 128 + tt], oz = m[5 * 128 + tt];
+      // this thread's four vertices: 64 s + acc_row(t, 2 h), s = MMA slab, h = row half
+      float ux[4], uy[4], uz[4], ox[4], oy[4], oz[4];
+      {
+        const float* m = sMeta + (i % kFmMetaSlots) * (kDnMetaTile / 4);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const int lv = 64 * (u >> 1) + acc_row(t, 2 * (u & 1));
+          ux[u] = m[0 * 128 + lv]; uy[u] = m[1 * 128 + lv]; uz[u] = m[2 * 128 + lv];
+          ox[u] = m[3 * 128 + lv]; oy[u] = m[4 * 128 + lv]; oz[u] = m[5 * 128 + lv];
+        }
+      }
       if (tr) p.trace[i * 8 + 1] = clock64();
-      mbar_wait_inl(smem_u32(&bar_dfull[s]), (uint32_t)(i >> 1) & 1, p.err);
-      tc_fence_after_sync();
+      float acc[3][2][8];                                            // [coordinate][slab][16 faces]
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const int q = 3 * i + c, slot = q % kFmPSlots;
+        mbar_wait_inl(smem_u32(&bar_pfull[slot]), (uint32_t)(q / kFmPSlots) & 1, p.err);
+        const uint32_t a_lo = smem_desc_lo(smem_u32(sP + slot * kFmPlane), 2048);
+        wgmma_fence();
+#pragma unroll
+        for (int sl = 0; sl < 2; ++sl)
+#pragma unroll
+          for (int pass = 0; pass < 3; ++pass) {
+            const uint32_t a_off = sl * 1024 + (pass == 2 ? kDnAPlane : 0);        // W: hi,hi,lo
+            const uint32_t b_off = (pass == 1 ? kDnBPlane : 0);                     // alpha: hi,lo,hi
+#pragma unroll
+            for (int ks = 0; ks < kDnK / 16; ++ks)
+              wgmma_f16<16>(acc[c][sl], desc64(d_hi, a_lo + ((a_off + ks * 4096) >> 4)),
+                            desc64(d_hi, b_lo + ((b_off + ks * 2048) >> 4)), (pass > 0 || ks > 0) ? 1u : 0u);
+          }
+        wgmma_commit();
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int c = 0; c < 3; ++c) mbar_arrive(smem_u32(&bar_pempty[(3 * i + c) % kFmPSlots]));   // planes may be refilled
       if (tr) p.trace[i * 8 + 2] = clock64();
-      const uint32_t trow = tmem + ((uint32_t)((warp & 3) * 32) << 16) + s * 192 + f0;
       const bool first = i == 0, last = i == n_items - 1;
       const bool edge = first || last || (ft + 1) * kDnFaces > p.batch;     // CTA-uniform
       const int nvalid = min(128, p.nver - vt * 128);
       float* item_row0 = p.out + ((size_t)(ft * kDnFaces + f0) * 3 + wq) * p.nver + (size_t)vt * 128;   // face f0, row wq
-      uint32_t sx[8], sy[8], sz[8];                                  // 8 faces x 3 coordinates at a time (96-register budget)
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        tmem_ld8_async(trow + h * 8, sx);
-        tmem_ld8_async(trow + 64 + h * 8, sy);
-        tmem_ld8_async(trow + 128 + h * 8, sz);
-        tmem_wait_ld();
-        if (h == 1) {                                                // accumulators are in registers: the buffer is free
-          tc_fence_before_sync();
-          mbar_arrive(smem_u32(&bar_dfree[s]));
-          if (tr) p.trace[i * 8 + 3] = clock64();
-        }
 #pragma unroll
-        for (int s2 = 0; s2 < 2; ++s2) {
-          const int sr = 2 * h + s2;
-          float* T = stage + s2 * (kFmRows * kFmPitch);
-          const int bq = ft * kDnFaces + f0 + sr * kFmSubFaces;      // first face (batch index) of the sub-round
-          // ---- stage: row (face, coordinate), position = this thread's vertex (no shift: the reader applies the phase)
-          const float* pose = pose_tile + (f0 + sr * kFmSubFaces) * kDnPoseStride;
-          float4 n0 = *reinterpret_cast<const float4*>(pose);       // [R|t] rows, loaded one face ahead of their use
-          float4 n1 = *reinterpret_cast<const float4*>(pose + 4);
-          float4 n2 = *reinterpret_cast<const float4*>(pose + 8);
+      for (int sr = 0; sr < 2; ++sr) {                               // faces 8 sr .. 8 sr + 7 of the team = accumulator values 4 sr ..
+        const int bq = ft * kDnFaces + f0 + sr * kFmSubFaces;        // first face (batch index) of the sub-round
+        // ---- stage: row (face, coordinate), position = vertex (no shift: the reader applies the phase)
 #pragma unroll
-          for (int fl = 0; fl < kFmSubFaces; ++fl, pose += kDnPoseStride) {
-            const int f8 = s2 * kFmSubFaces + fl;
-            const float4 r0 = n0, r1 = n1, r2 = n2;
-            if (fl + 1 < kFmSubFaces) {
-              n0 = *reinterpret_cast<const float4*>(pose + kDnPoseStride);
-              n1 = *reinterpret_cast<const float4*>(pose + kDnPoseStride + 4);
-              n2 = *reinterpret_cast<const float4*>(pose + kDnPoseStride + 8);
-            }
-            const float X = fmaf(__uint_as_float(sx[f8]), ox, ux), Y = fmaf(__uint_as_float(sy[f8]), oy, uy),
-                        Z = fmaf(__uint_as_float(sz[f8]), oz, uz);
+        for (int e = 0; e < 2; ++e) {
+          const int fl = 2 * (t & 3) + e;                            // face within the sub-round
+          const float* pose = pose_tile + (f0 + sr * kFmSubFaces + fl) * kDnPoseStride;
+          const float4 r0 = *reinterpret_cast<const float4*>(pose);
+          const float4 r1 = *reinterpret_cast<const float4*>(pose + 4);
+          const float4 r2 = *reinterpret_cast<const float4*>(pose + 8);
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            const int sl = u >> 1, h = u & 1, vi = 4 * sr + 2 * h + e;
+            const float X = fmaf(acc[0][sl][vi], ox[u], ux[u]), Y = fmaf(acc[1][sl][vi], oy[u], uy[u]),
+                        Z = fmaf(acc[2][sl][vi], oz[u], uz[u]);
             float vx = fmaf(r0.x, X, fmaf(r0.y, Y, fmaf(r0.z, Z, r0.w)));
             float vy = fmaf(r1.x, X, fmaf(r1.y, Y, fmaf(r1.z, Z, r1.w)));
             float vz = fmaf(r2.x, X, fmaf(r2.y, Y, fmaf(r2.z, Z, r2.w)));
             if (p.transform) vy = (float)(kImg + 1) - vy;            // model_building.py:129,137
             if (kAffine) {                                           // utils/inference.py:131-136, numpy's fp32 mul then add
-              const float4 q = *reinterpret_cast<const float4*>(pose + 12);
-              vx = __fadd_rn(__fmul_rn(vx, q.x), q.y);
-              vy = __fadd_rn(__fmul_rn(vy, q.z), q.w);
+              const float4 a4 = *reinterpret_cast<const float4*>(pose + 12);
+              vx = __fadd_rn(__fmul_rn(vx, a4.x), a4.y);
+              vy = __fadd_rn(__fmul_rn(vy, a4.z), a4.w);
               vz = __fmul_rn(vz, pose[16]);
             }
-            T[(fl * 3 + 0) * kFmPitch + tt] = vx;
-            T[(fl * 3 + 1) * kFmPitch + tt] = vy;
-            T[(fl * 3 + 2) * kFmPitch + tt] = vz;
+            const int lv = 64 * sl + acc_row(t, 2 * h);
+            stage[(fl * 3 + 0) * kFmPitch + lv] = vx;
+            stage[(fl * 3 + 1) * kFmPitch + lv] = vy;
+            stage[(fl * 3 + 2) * kFmPitch + lv] = vz;
           }
-          asm volatile("bar.sync %0, 128;" ::"r"(team + 1) : "memory");
-          // ---- write out: warp wq takes rows wq + 4k.  Window position pos (0 = the sector boundary at or below the row
-          // piece) holds vertex pos - phase of this item, or, below phase, the previous item's overhang.  Lane j stores
-          // positions j, 32 + j, 64 + j, 96 + j: every warp store is four whole aligned sectors.
-          const float* Tw = T + wq * kFmPitch + lane;
-          float* crw = carry + (sr * kFmRows + wq) * 8 + lane;
-          float* piece = item_row0 + (size_t)(sr * kFmRows) * p.nver;   // row wq of the sub-round, first float of the piece
-          if (!edge) {
-#pragma unroll
-            for (int k = 0; k < kFmRows / 4; ++k, piece += 4 * (size_t)p.nver) {
-              const int phase = (int)((reinterpret_cast<uintptr_t>(piece) >> 2) & 7u);
-              const float* src = Tw + 4 * k * kFmPitch - phase;
-              float* cr = crw + 4 * k * 8;
-              const bool low = lane < phase;
-              const float v0 = *(low ? cr : src);
-              const float v1 = src[32], v2 = src[64], v3 = src[96];
-              if (low) *cr = src[128];                               // this item's overhang (vertices 128 - phase .. 127)
-              float* win = piece - phase + lane;                     // plain stores: .cs needs a policy descriptor per store
-              win[0] = v0; win[32] = v1; win[64] = v2; win[96] = v3;
-            }
-          } else {                                                   // first / last item of the band, ragged face tile
-            fm_write_edge(p, Tw, crw, piece, bq, wq, lane, first, last, nvalid);
-          }
-          // the other staging buffer is written next; this one again two sub-rounds later, after the next team barrier
         }
+        asm volatile("bar.sync %0, 128;" ::"r"(team + 1) : "memory");
+        // ---- write out: warp wq takes rows wq + 4k.  Window position pos (0 = the sector boundary at or below the row
+        // piece) holds vertex pos - phase of this item, or, below phase, the previous item's overhang.  Lane j stores
+        // positions j, 32 + j, 64 + j, 96 + j: every warp store is four whole aligned sectors.
+        const float* Tw = stage + wq * kFmPitch + lane;
+        float* crw = carry + (sr * kFmRows + wq) * 8 + lane;
+        float* piece = item_row0 + (size_t)(sr * kFmRows) * p.nver;   // row wq of the sub-round, first float of the piece
+        if (!edge) {
+#pragma unroll
+          for (int k = 0; k < kFmRows / 4; ++k, piece += 4 * (size_t)p.nver) {
+            const int phase = (int)((reinterpret_cast<uintptr_t>(piece) >> 2) & 7u);
+            const float* src = Tw + 4 * k * kFmPitch - phase;
+            float* cr = crw + 4 * k * 8;
+            const bool low = lane < phase;
+            const float v0 = *(low ? cr : src);
+            const float v1 = src[32], v2 = src[64], v3 = src[96];
+            if (low) *cr = src[128];                               // this item's overhang (vertices 128 - phase .. 127)
+            float* win = piece - phase + lane;
+            win[0] = v0; win[32] = v1; win[64] = v2; win[96] = v3;
+          }
+        } else {                                                   // first / last item of the band, ragged face tile
+          fm_write_edge(p, Tw, crw, piece, bq, wq, lane, first, last, nvalid);
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(team + 1) : "memory");   // the staging rows are rewritten next
       }
       if (tr) p.trace[i * 8 + 4] = clock64();
     }
   } else if (warp == kDnEpiWarps) {
-    // ------------------------------ loader + MMA issuer (converged warp, elect.sync) ------------------------------
-    const uint32_t idesc = make_idesc_f16(128, kDnFaces);
-    const uint32_t d_hi = smem_desc_hi(128);
+    // ------------------------------ loader (converged warp, elect.sync) ------------------------------
     int next_plane = 0;                                               // next plane to request (plane q = 3 * item + coordinate)
     const uint64_t keep = l2_policy_evict_last();                     // the basis image is re-read once per face tile
     // Request planes up to (and including) `upto`.  Plane q reuses the slot of plane q - kFmPSlots, whose MMAs must be
     // complete (bar_pempty, consumed strictly in order).  The meta rows of item v go to slot v % 4, last read by the
-    // epilogue of item v - 4 BEFORE it released its accumulator buffer, which the issuer has waited for by then.
+    // teams at the start of item v - 4, before they released any plane of item v - 2, which is waited for here.
     auto request_planes = [&](int upto) {
       upto = min(upto, 3 * n_items - 1);
       for (; next_plane <= upto; ++next_plane) {
         const int q = next_plane, slot = q % kFmPSlots, v = q / 3, c = q - 3 * v;
         if (q >= kFmPSlots) mbar_wait_inl(smem_u32(&bar_pempty[slot]), (uint32_t)(q / kFmPSlots - 1) & 1, p.err);
+        if (kTrace && blockIdx.x == 0 && lane == 0 && v < 64) p.trace[(128 + v) * 8 + c] = clock64();
         if (elect_one()) {
           mbar_expect_tx(smem_u32(&bar_pfull[slot]), kFmPlane);
 #pragma unroll
@@ -525,44 +494,7 @@ __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_fm_kernel(const Den
       }
       __syncwarp();
     }
-    const uint32_t b_lo = smem_desc_lo(smem_u32(sB), 1024);
-    for (int i = 0; i < n_items; ++i) {
-      const int s = i & 1;
-      const bool tr = kTrace && blockIdx.x == 0 && lane == 0 && i < 64;
-      if (tr) p.trace[(128 + i) * 8 + 0] = clock64();
-      if (i == 0) mbar_wait_inl(smem_u32(&bar_bfull), 0, p.err);
-      if (i >= 2) mbar_wait_inl(smem_u32(&bar_dfree[s]), (uint32_t)((i - 2) >> 1) & 1, p.err);   // buffer s read out
-      if (tr) p.trace[(128 + i) * 8 + 1] = clock64();
-      for (int c = 0; c < 3; ++c) {
-        const int q = 3 * i + c, slot = q % kFmPSlots;
-        request_planes(q + kFmPSlots - 2);                           // the slot freed by the previous plane's MMAs
-        mbar_wait_inl(smem_u32(&bar_pfull[slot]), (uint32_t)(q / kFmPSlots) & 1, p.err);
-        if (tr) p.trace[(128 + i) * 8 + 2 + c] = clock64();            // plane c landed
-        tc_fence_after_sync();
-        const uint32_t a_lo = smem_desc_lo(smem_u32(sP + slot * kFmPlane), 2048);
-        if (elect_one()) {
-#pragma unroll
-          for (int pass = 0; pass < 3; ++pass) {
-            const uint32_t a_off = (pass == 2 ? kDnAPlane : 0);                     // W: hi,hi,lo
-            const uint32_t b_off = (pass == 1 ? kDnBPlane : 0);                     // alpha: hi,lo,hi
-#pragma unroll
-            for (int ks = 0; ks < kDnK / 16; ++ks)
-              umma_f16(tmem + s * 192 + c * 64, desc64(d_hi, a_lo + ((a_off + ks * 4096) >> 4)),
-                       desc64(d_hi, b_lo + ((b_off + ks * 2048) >> 4)), idesc, (pass > 0 || ks > 0) ? 1u : 0u);
-          }
-          umma_commit(smem_u32(&bar_pempty[slot]));                  // the plane may be overwritten once these MMAs are done
-          if (c == 2) umma_commit(smem_u32(&bar_dfull[s]));
-        }
-        __syncwarp();
-      }
-      if (tr) p.trace[(128 + i) * 8 + 5] = clock64();                  // MMAs of the item issued
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == kDnEpiWarps) {
-    __syncwarp();
-    tmem_dealloc<512>(tmem);
+    request_planes(3 * n_items - 1);
   }
 }
 

@@ -98,7 +98,7 @@ __global__ void faceboxes_rank_decode_kernel(const float* __restrict__ loc, cons
 }  // namespace syn
 
 // ---- the detector network (FaceBoxes/models/faceboxes.py:8-150) -------------------------------------------------------
-// 33 small convolutions on one image of arbitrary size (0.7 GMAC at 720 x 1080).  A first, plain B200 path: fp32 FMA on
+// 33 small convolutions on one image of arbitrary size (0.7 GMAC at 720 x 1080).  A first, plain H100 path: fp32 FMA on
 // CUDA cores as a shared-memory-tiled implicit GEMM (M = output pixels, N = output channels, K = kh*kw*cin), BatchNorm
 // folded into weights and bias on the host in float64, activation and the channel concatenations fused into the store
 // (every layer writes its slice of the NHWC tensor the next layer reads).  NHWC is also how the image arrives (H,W,3

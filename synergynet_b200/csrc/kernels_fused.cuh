@@ -1,35 +1,36 @@
-// Fused inverted-residual block on tcgen05:  1x1 expand (+BN+ReLU6) -> 3x3 depthwise (+BN+ReLU6)
+// Fused inverted-residual block on tensor cores (wgmma):  1x1 expand (+BN+ReLU6) -> 3x3 depthwise (+BN+ReLU6)
 // -> 1x1 project (+BN)(+skip), reference backbone_nets/mobilenetv2_backbone.py:45-74, in ONE
 // kernel, so the 6x-expanded hidden tensor (up to 1.38 MB per face) never touches HBM.
 // The same kernel, with an im2col loader, fuses the 3x3/s2 stem conv with block 1
 // (mobilenetv2_backbone.py:127 + features[1]).
 //
 // Work item (tile) = RO output rows of one face (large maps) or FACES whole faces (8x8 / 4x4 maps).
-// Per tile the block input is converted once to fp16 hi/lo and stored in TMEM (XA, tcgen05.st); then, for
+// Per tile the block input is converted once to fp16 hi/lo and stored in shared memory (XA); then, for
 // each chunk of NC hidden channels:
-//   GEMM1  D1[t] (128 x NC, TMEM)  = XA[t] (TMEM, TS mode) * W1c^T (smem)                      (tensor)
+//   GEMM1  D1 (64-row slabs x NC, registers) = XA * W1c^T (smem x smem)                        (tensor)
 //   EPI1   Hs[pixel][NC] (fp32, smem, zero halo) = relu6(s1 * D1 + b1) / 6  (one FFMA.SAT)   (CUDA)
 //   DW     A2[out pixel][NC] (fp16 hi/lo, smem)  = split(relu6(dw3x3(6 Hs) + bdw))          (CUDA)
-//   GEMM2  D2[t] (128 x COUT_P, TMEM) += A2[t] * W3c^T                                      (tensor)
-// and finally EPI2: out = s3 * D2 + b3 (+ x).  GEMM1 of chunk c+1 and GEMM2 of chunk c run on the
-// tensor pipe while the worker warps do EPI1/DW; the depthwise phase (shared-memory loads) is the
-// critical path.  CTAs are persistent (grid = #SMs).  Weights (fp16 hi/lo, split-16x3 scheme of
-// kernels_tc.cuh) are either resident in shared memory for the whole kernel (early blocks, <= 83 KB) or
-// streamed chunk by chunk through a 2-3-slot bulk-copy (TMA) ring (late blocks).
+//   GEMM2  D2 (64-row slabs x column pieces, registers) += A2 * W3c^T                       (tensor)
+// and finally EPI2: out = s3 * D2 + b3 (+ x).  The worker warpgroups issue the MMAs themselves: a warpgroup
+// owns a fixed set of (64-row slab, column piece) items of D2 for the whole tile, so the D2 accumulator stays
+// in its registers across the chunks (a 128 x 320 fp32 accumulator would not: blocks 15 / 17 use 4-face tiles).
+// CTAs are persistent (grid = #SMs).  Weights (fp16 hi/lo, split-16x3 scheme of kernels_tc.cuh) are either
+// resident in shared memory for the whole kernel (early blocks) or streamed chunk by chunk through a 2-3-slot
+// bulk-copy (TMA) ring (late blocks).
 //
-// Roles: warps 0..NWW-1 = workers (thread = GEMM row / pixel / TMEM lane; channel groups own the column
-// octets of a chunk), warp NWW = MMA issuer + weight loader (converged warp, issue under elect.sync).
-// smem operand tiles use the canonical K-major no-swizzle layout of tc_common.cuh (SBO 128 B,
-// LBO = rows/8 * 128 B).  DESIGN.md section 5 lists the measurements behind each of these choices.
+// Roles: warps 0..NWW-1 = workers (thread = GEMM row / pixel in the conversion, channel octets in EPI1 / DW, MMA
+// operand slabs per warpgroup), warp NWW = weight loader and stem-row stager (converged warp, bulk copies under
+// elect.sync).  smem operand tiles use the canonical K-major no-swizzle layout of tc_common.cuh (SBO 128 B,
+// LBO = rows/8 * 128 B).
 #pragma once
 #include "common.cuh"
 #include "tc_common.cuh"
 
 namespace syn {
 
-constexpr int ceil_div_c(int a, int b) { return (a + b - 1) / b; }
+__host__ __device__ constexpr int ceil_div_c(int a, int b) { return (a + b - 1) / b; }
 // tile shapes / chunk widths / batching depths worth re-measuring when the kernel changes: build variants
-// with -D... and compare them on one box with scripts/ab_variants.sh
+// with -D... (scripts/build_variant.sh) and compare them with scripts/quick_variant_check.py
 #ifndef SYN_RO_STEM
 #define SYN_RO_STEM 6
 #endif
@@ -45,18 +46,21 @@ constexpr int ceil_div_c(int a, int b) { return (a + b - 1) / b; }
 #ifndef SYN_NC_B2
 #define SYN_NC_B2 32
 #endif
-// block 3: 48-channel chunks on 10-row strips (3 chunks per tile instead of 9 with 16 channels on 15 rows: fewer
-// per-chunk barrier / wait round trips) measured 0.307 vs 0.325 ms; 48 channels on 6-row strips 0.381 ms
+// block 3: 48-channel chunks (3 chunks per tile: fewer per-chunk barrier round trips).  Strip heights of blocks 3-6
+// are bounded by shared memory: the block input (XA) is staged there next to the hidden window.
 #ifndef SYN_NC_B3
 #define SYN_NC_B3 48
 #endif
 #ifndef SYN_RO_B3
-#define SYN_RO_B3 10
+#define SYN_RO_B3 6
 #endif
 #ifndef SYN_RO_B4
-#define SYN_RO_B4 15
+#define SYN_RO_B4 5
 #endif
-// programmatic dependent launch over the fused launches (measured -1.1 % of the step, round 2)
+#ifndef SYN_RO_B56
+#define SYN_RO_B56 5
+#endif
+// programmatic dependent launch over the fused launches: a block's prologue overlaps the previous block's tail
 #ifndef SYN_PDL
 #define SYN_PDL 1
 #endif
@@ -66,7 +70,7 @@ constexpr int ceil_div_c(int a, int b) { return (a + b - 1) / b; }
 // SYN_DW3: depthwise items of one channel quad x 2 output rows x 5 output columns on the stride-1 60^2 / 30^2 / 15^2 maps
 // (15.2 shared-memory loads per 16 outputs instead of 26 + conflicted tap loads, DESIGN.md section 5)
 #ifndef SYN_DW3
-#define SYN_DW3 0      // measured SLOWER than the 2 x 2 items (2.46 vs 2.32 ms/step): one long item per thread serialises
+#define SYN_DW3 0      // off: one long item per thread serialises the depthwise phase
 #endif
 // output columns of a DW3 item: 3 (76 live registers; 17 warps leave 96 per thread: 5 warps share one sub-partition's
 // 16 K registers) or 5 (fewer loads per output, needs ~105 registers: spills unless the CTA has <= 16 warps)
@@ -83,28 +87,15 @@ constexpr int ceil_div_c(int a, int b) { return (a + b - 1) / b; }
 #define SYN_NC_B7 64
 #endif
 #ifndef SYN_NC_B12
-#define SYN_NC_B12 64
+#define SYN_NC_B12 32
 #endif
 #ifndef SYN_NC_B14
-#define SYN_NC_B14 64
+#define SYN_NC_B14 32
 #endif
 #ifndef SYN_NC_B17
 #define SYN_NC_B17 32
 #endif
-#ifndef SYN_EB_STEM
-#define SYN_EB_STEM 1
-#endif
-#ifndef SYN_EB_WIDE
-#define SYN_EB_WIDE 1
-#endif
-#ifndef SYN_EB_MID
-#define SYN_EB_MID 1
-#endif
-#ifndef SYN_EB_SMALL
-#define SYN_EB_SMALL 1
-#endif
-constexpr int round_up_c(int a, int b) { return ceil_div_c(a, b) * b; }
-constexpr int pow2_cols(int c) { return c <= 32 ? 32 : c <= 64 ? 64 : c <= 128 ? 128 : c <= 256 ? 256 : 512; }
+__host__ __device__ constexpr int round_up_c(int a, int b) { return ceil_div_c(a, b) * b; }
 
 template <int CIN_, int CHID_, int NC_, int COUT_, int W_, int STRIDE_, int RO_, int FACES_, bool RES_, bool STEM_,
           int WSTREAM_>
@@ -116,8 +107,6 @@ struct FusedCfg {
   static constexpr int CIN_P = round_up_c(CIN_, 16);
   static constexpr int CHID = CHID_, NC = NC_, NCHUNK = CHID_ / NC_;
   static constexpr int COUT = COUT_, COUT_P = round_up_c(COUT_, 16);
-  static constexpr int NSPLIT = ceil_div_c(COUT_P, 256);                 // MMA N <= 256
-  static constexpr int N2 = COUT_P / NSPLIT;
   static constexpr int W = W_, STRIDE = STRIDE_, WO = (W_ - 1) / STRIDE_ + 1;
   static constexpr int RO = RO_, STRIPS = WO / RO_, FACES = FACES_;
   static constexpr int RWIN = (RO_ - 1) * STRIDE_ + 3;                   // window rows incl. halo
@@ -138,13 +127,7 @@ struct FusedCfg {
   static constexpr int HS_FACE = RWIN * HS_COLS, HS_PIX = FACES_ * HS_FACE, HS_STRIDE = NC_ + 4;
   static constexpr int DWS = NC_ + 4;     // floats between the tap rows of a chunk: mirrored lanes of the 2x2 depthwise read
                                           // taps kx and 2-kx, which must not lie a multiple of 128 bytes apart
-  static constexpr int D2_COL = round_up_c(MT1 * NC_, 32);
-  // EPI1 TMEM loads kept in flight per wait (measured per map size, scripts/ab_variants.sh)
-  static constexpr int EPI1_BATCH = STEM_ ? SYN_EB_STEM : W_ >= 30 ? SYN_EB_WIDE : W_ >= 15 ? SYN_EB_MID : SYN_EB_SMALL;
-  // GEMM1's A operand (the block input as fp16 hi/lo) lives in TMEM, not in shared memory: per M tile
-  // CIN_P/2 columns of hi K-pairs, then CIN_P/2 columns of lo K-pairs
-  static constexpr int XA_COL = D2_COL + MT2 * COUT_P;
-  static constexpr int TM_COLS = pow2_cols(XA_COL + MT1 * CIN_P);
+  static constexpr int SLABS1 = ceil_div_c(M1_MAX, 64), SLABS2 = ceil_div_c(M2_MAX, 64);   // 64-row MMA slabs
   // ---- weight image: [b3 | s3] then NCHUNK x { W1c hi, W1c lo, W3c hi, W3c lo, DW rows } -----------
   static constexpr int B3_BYTES = round_up_c(2 * COUT_P * 4, 128);       // [2][COUT_P] fp32: b3, s3
   static constexpr int W1_PLANE = NC_ * CIN_P * 2;                       // bytes, one plane of one chunk
@@ -156,10 +139,13 @@ struct FusedCfg {
   static constexpr int WSTAGES = WSTREAM_ > 0 ? WSTREAM_ : NCHUNK;       // chunk slots held in smem
   // ---- shared memory carve-up --------------------------------------------------------------------
   static constexpr int A2_PLANE = MT2 * 128 * NC_ * 2;
+  // GEMM1's A operand: the block input as fp16 hi/lo, [hi plane | lo plane], each SLABS1 slabs of 64 rows x CIN_P
+  // (canonical, SBO = 128, LBO = 1 KB)
+  static constexpr int XA_TILE = 64 * CIN_P * 2, XA_PLANE = SLABS1 * XA_TILE;
   static constexpr int S_B3 = 0;
   static constexpr int S_WCH = S_B3 + B3_BYTES;
-  static constexpr int S_X = S_WCH + WSTAGES * CHUNK_BYTES;
-  static constexpr int S_A2 = S_X;
+  static constexpr int S_XA = S_WCH + WSTAGES * CHUNK_BYTES;
+  static constexpr int S_A2 = S_XA + 2 * XA_PLANE;
   static constexpr int S_H = S_A2 + 2 * A2_PLANE;
   // stem only: staged input rows [3][IN_ROWS][120] fp32, exactly as they lie in the NCHW crop (one bulk
   // copy per channel); the left zero-pad column is a predicate in the im2col gather
@@ -170,9 +156,8 @@ struct FusedCfg {
   static_assert(CHID_ % NC_ == 0 && NC_ % 16 == 0, "hidden chunking");
   static_assert(WO % RO_ == 0, "strips must tile the output");
   static_assert(FACES_ == 1 || RO_ == WO, "multi-face tiles hold whole faces");
-  static_assert(XA_COL + MT1 * CIN_P <= 512, "TMEM columns");
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
-  static_assert(N2 % 16 == 0 && N2 <= 256, "MMA N");
+  static_assert(NC_ <= 256, "MMA N");
   static_assert(WSTREAM_ == 0 || (WSTREAM_ >= 2 && WSTREAM_ <= 4 && NCHUNK >= WSTREAM_), "weight ring");
   // DW3 bank-conflict conditions.  Window loads: lane (s, r) of a quarter-warp reads 16 bytes at group offset
   // S*G*s + 2*HS_COLS*G*r (S = DW3_S, G = HS_STRIDE/4, both odd) and the eight offsets must differ mod 8; operand stores: 8-byte halves
@@ -201,7 +186,7 @@ struct FusedArgs {
 };
 
 // Phase trace (debug builds only, -DSYN_FUSED_TRACE): clock64 stamps of CTA 0's second tile, one row of 8
-// events per (block, role, chunk); read back with syn_debug_read_trace.  role 0 = worker thread 0, 1 = issuer.
+// events per (block, role, chunk); read back with syn_debug_read_trace.  role 0 = worker thread 0 (role 1 is unused).
 #ifdef SYN_FUSED_TRACE
 __device__ long long g_fused_trace[18 * 2 * 64 * 8];
 #define SYN_TRACE(role, chunk, ev)                                                                        \
@@ -223,36 +208,44 @@ __device__ __forceinline__ void group_bar_sync(int grp) {
   }
 }
 
-// NWW = worker warps (multiple of 4: TMEM lane quarter = warp % 4); the issuer is warp NWW.
+// D2 column pieces: the fewest (halving the width) that give every worker warpgroup at least one (slab, piece) item
+__host__ __device__ constexpr int fused_d2_pieces(int cout_p, int slabs, int nwg) {
+  int s = 1;
+  while (slabs * s < nwg && (cout_p / (2 * s)) % 8 == 0) s *= 2;
+  return s;
+}
+
+// NWW = worker warps (multiple of 4: whole warpgroups); the loader is warp NWW.
 template <class C, int NWW>
 __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const FusedArgs p) {
   constexpr int NWT = NWW * 32;          // worker threads
-  constexpr int NWG = NWW / 4;           // worker groups: group g owns every NWG-th (tile, column-chunk) pair
+  constexpr int NWG = NWW / 4;           // worker warpgroups
   static_assert(NWW % 4 == 0 && NWW >= 4 && NWW <= 24, "worker warps");
-  // Channel groups: the hidden channels of a chunk are split between NG groups of worker warps.  A group
-  // drains ITS channels from TMEM (EPI1) and runs the depthwise conv on ITS channels, so the only
-  // synchronisation between EPI1 and DW is a named barrier among the group's warps, and the groups drift
-  // freely against each other (one can be in EPI1 while another is in DW).
+  // EPI1 and the depthwise conv are separated by a barrier of all workers (every warpgroup's GEMM1 slabs hold all
+  // NC channels of their rows), so the depthwise items are spread over all workers as one channel group
   constexpr int NKG_ = C::NC / 8;
-  constexpr int NG = (NWG % 4 == 0 && NKG_ % 4 == 0) ? 4 : (NWG % 2 == 0 && NKG_ % 2 == 0) ? 2 : 1;
-  constexpr int WPG = NWW / NG, TPG = WPG * 32;      // warps / threads per group (WPG is a multiple of 4)
-  constexpr int KPG = NKG_ / NG;                       // 8-channel groups owned by a worker group
-  constexpr int SUBS = WPG / 4;                        // sub-groups of 128 threads (one TMEM lane each)
+  constexpr int NG = 1;
+  constexpr int WPG = NWW / NG, TPG = WPG * 32;
+  constexpr int KPG = NKG_ / NG;
+  // GEMM2 / EPI2 items: (64-row slab, column piece of N2 channels); item i belongs to warpgroup i % NWG
+  constexpr int NSPL = fused_d2_pieces(C::COUT_P, C::SLABS2, NWG);
+  constexpr int N2 = C::COUT_P / NSPL;
+  constexpr int IPW = ceil_div_c(C::SLABS2 * NSPL, NWG);               // items per warpgroup (at most)
+  static_assert(N2 % 8 == 0 && N2 <= 256, "MMA N");
   using namespace tc;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_w, bar_wfull[4], bar_x, bar_d1, bar_epi1, bar_a2, bar_g2, bar_d2free, bar_in;
-  __shared__ uint32_t tmem_base_s;
+  __shared__ __align__(8) uint64_t bar_w, bar_wfull[4], bar_wempty[4], bar_x, bar_in;
 
   // keep the pointer in the shared address space (no integer round trip): a generic pointer here
   // turns every tile access into LD.E/ST.E instead of LDS/STS
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int tid = threadIdx.x, warp = tid >> 5;
-  const int row = tid & 127, wg = tid >> 7;   // GEMM row / TMEM lane of this worker, and its 128-thread slice
+  const int row = tid & 127, wg = tid >> 7;   // GEMM row of this worker in the conversion, and its warpgroup
   const int grp = warp / WPG;                  // channel group (workers only)
-  const int gtid = tid - grp * TPG, gsub = gtid >> 7;
+  const int gtid = tid - grp * TPG;
   const int ntiles = p.face_groups * C::STRIPS;
-  // faces of a face group.  Two-face tiles (8x8 maps): 512 groups over 148 SMs would leave the last wave
-  // 46 % full, so the host turns the groups of that wave into single-face groups (twice as many CTAs busy,
+  // faces of a face group.  Two-face tiles (8x8 maps): 512 groups over 132 SMs would leave the last wave
+  // 88 % full, so the host turns the groups of that wave into single-face groups (twice as many CTAs busy,
   // each done sooner); small batches become single-face groups altogether.
   auto group_faces = [&](int fg, int& f0, int& nfaces) {
     if constexpr (C::FACES == 2) {
@@ -269,29 +262,24 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
 #endif
   if (tid == 0) {
     mbar_init(smem_u32(&bar_w), 1);
-    for (int i = 0; i < 4; ++i) mbar_init(smem_u32(&bar_wfull[i]), 1);
+    for (int i = 0; i < 4; ++i) {
+      mbar_init(smem_u32(&bar_wfull[i]), 1);
+      mbar_init(smem_u32(&bar_wempty[i]), NWT);
+    }
     mbar_init(smem_u32(&bar_x), NWT);
-    mbar_init(smem_u32(&bar_d1), 1);
-    mbar_init(smem_u32(&bar_epi1), NWT);
-    mbar_init(smem_u32(&bar_a2), NWT);
-    mbar_init(smem_u32(&bar_g2), 1);
-    mbar_init(smem_u32(&bar_d2free), NWT);
     mbar_init(smem_u32(&bar_in), 1);
     fence_mbar_init();
   }
-  if (warp == NWW) tmem_alloc<C::TM_COLS>(smem_u32(&tmem_base_s));
   if constexpr (C::STEM) {     // staged-row buffer: the left pad column (and everything else) starts as zero;
     float* z = reinterpret_cast<float*>(smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u) + C::S_IN);
     for (int i = threadIdx.x; i < 3 * C::IN_ROWS * C::IN_STRIDE / 4; i += blockDim.x)   // before any bulk copy
       reinterpret_cast<float4*>(z)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     tc::fence_proxy_async_smem();
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = tmem_base_s;
 
   uint8_t* sWch = smem + C::S_WCH;
+  uint8_t* sXA = smem + C::S_XA;
   uint8_t* sA2 = smem + C::S_A2;
   float* sH = reinterpret_cast<float*>(smem + C::S_H);
   const float* sB3 = reinterpret_cast<const float*>(smem + C::S_B3);
@@ -303,12 +291,14 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
     for (int i = tid; i < C::HS_PIX * C::HS_STRIDE / 4; i += NWT)
       reinterpret_cast<float4*>(sH)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     mbar_wait(smem_u32(&bar_w), 0, p.err);                // b3/s3 (and, if resident, all chunks) landed
-    uint32_t n_d1 = 0, n_g2 = 0, g = 0, n_in = 0;                   // completed-phase counters; g = chunk counter
+    uint32_t g = 0, n_in = 0;                             // g = chunk counter, n_in = staged-row phases consumed
     asm volatile("bar.sync 5, %0;" ::"n"(NWT) : "memory");
+    const uint32_t d_hi = smem_desc_hi(128);
+    constexpr uint32_t LBO_W1 = (C::NC / 8) * 128, LBO_W3 = (C::COUT_P / 8) * 128;
 
-    // Geometry of a tile + "prep": stage / convert its input into the GEMM1 A operand and publish it.
-    // prep(next tile) is issued BEFORE the current tile's EPI2, so the issuer can run GEMM1(next, 0) --
-    // and the global-load latency of the conversion is hidden -- while the workers drain D2.
+    // Geometry of a tile + "prep": stage / convert its input into the GEMM1 A operand.  prep(next tile) runs
+    // BEFORE the current tile's EPI2 (XA is free once the last GEMM1 of the tile is done), so the global-load
+    // latency of the conversion overlaps the output stores.
     auto prep = [&](int tile) {
       const int fg = tile / C::STRIPS, sp = tile - fg * C::STRIPS;
       int f0, nfaces;
@@ -345,7 +335,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
             }
             *reinterpret_cast<float4*>(sIn + (ci * C::IN_ROWS + r) * C::IN_STRIDE + c4 * 4) = v;
           }
-        } else {                              // fp32 crops: rows were bulk-copied by the issuer one tile ahead
+        } else {                              // fp32 crops: rows were bulk-copied by the loader one tile ahead
           mbar_wait(smem_u32(&bar_in), n_in & 1, p.err);
           ++n_in;
           for (int r = 0; r < nin; ++r) {     // rows outside the image are not copied: zero them (edge strips)
@@ -360,30 +350,32 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
         asm volatile("bar.sync 5, %0;" ::"n"(NWT) : "memory");
       }
       SYN_TRACE(0, 62, 2);
-      // ---- X tile -> fp16 hi/lo K pairs in TMEM ---------------------------------------------------
+      // ---- X tile -> fp16 hi/lo operand in smem ---------------------------------------------------
       // The conversion sits between the last depthwise and EPI2 of the current tile, so its global-load
       // latency is exposed once per batch of loads: all loads of a batch are issued unconditionally (from a
       // clamped, always valid address) before the first use, and masked afterwards -- a predicated load per
       // item would put a branch between the loads and serialise one DRAM latency per item.
       {
         constexpr int KG = C::CIN_P / 8;
-        constexpr int ITERS = (C::MT1 * KG + NWG - 1) / NWG;             // items per thread
+        constexpr int NXG = NWT / 64;                                    // thread groups of 64 = one slab's rows
+        constexpr int ITERS = (C::SLABS1 * KG + NXG - 1) / NXG;          // items per thread
         constexpr int PB = ITERS < SYN_PREP_BATCH ? ITERS : SYN_PREP_BATCH;
-        const int n_items = mt1 * KG;
-        for (int e0 = wg; e0 < n_items; e0 += PB * NWG) {
+        const int r64 = tid & 63, xg = tid >> 6;
+        const int n_items = ((M1 + 63) >> 6) * KG;
+        for (int e0 = xg; e0 < n_items; e0 += PB * NXG) {
           float v[PB][8];
           if constexpr (C::STEM) {
             // im2col of the 3x3 stride-2 pad-1 stem conv from the staged rows: k = (ci*3+ky)*3+kx.  All PB items of a
             // thread are gathered before the first conversion (independent shared loads in flight instead of one
-            // load -> convert -> TMEM-store chain per item); the kg switch makes every tap offset a compile-time constant.
+            // load -> convert -> store chain per item); the kg switch makes every tap offset a compile-time constant.
 #pragma unroll
             for (int u = 0; u < PB; ++u) {
 #pragma unroll
               for (int j = 0; j < 8; ++j) v[u][j] = 0.f;
-              const int e = e0 + u * NWG;
+              const int e = e0 + u * NXG;
               if (e >= n_items) continue;
               const int t = e / KG, kg = e - t * KG;
-              const int mr = t * 128 + row;                     // FACES == 1
+              const int mr = t * 64 + r64;                      // FACES == 1
               if (mr < M1) {
                 const int yl = mr / C::W, xx = mr - yl * C::W;
                 const float* base = sIn + (2 * yl) * C::IN_STRIDE + 2 * xx - 1;   // column 2xx-1+kx; -1 is the zero pad
@@ -406,10 +398,10 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
             bool ok[PB];
 #pragma unroll
             for (int u = 0; u < PB; ++u) {
-              const int e = min(e0 + u * NWG, n_items - 1);
+              const int e = min(e0 + u * NXG, n_items - 1);
               const int t = e / KG, kg = e - t * KG;
-              const int m = t * 128 + row;
-              ok[u] = (e0 + u * NWG < n_items) && (m < M1) && (kg * 8 < C::CIN);
+              const int m = t * 64 + r64;
+              ok[u] = (e0 + u * NXG < n_items) && (m < M1) && (kg * 8 < C::CIN);
               const int mc = min(m, M1 - 1), kgc = min(kg, (C::CIN - 1) / 8);
               const int f = (C::FACES > 1) ? mc / ppf : 0;
               const int mr = mc - f * ppf;                    // pixel inside the face's valid rows
@@ -417,7 +409,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
               qa[u] = __ldg(reinterpret_cast<const float4*>(src));
               qb[u] = __ldg(reinterpret_cast<const float4*>(src + 4));
             }
-            if (e0 == wg) SYN_TRACE(0, 62, 5);
+            if (e0 == xg) SYN_TRACE(0, 62, 5);
 #pragma unroll
             for (int u = 0; u < PB; ++u) {
               v[u][0] = ok[u] ? qa[u].x : 0.f; v[u][1] = ok[u] ? qa[u].y : 0.f; v[u][2] = ok[u] ? qa[u].z : 0.f; v[u][3] = ok[u] ? qa[u].w : 0.f;
@@ -426,8 +418,8 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
           }
 #pragma unroll
           for (int u = 0; u < PB; ++u) {
-            const int e = e0 + u * NWG;
-            if (e < n_items) {                                // warp-uniform: tcgen05.st is .sync.aligned
+            const int e = e0 + u * NXG;
+            if (e < n_items) {
               const int t = e / KG, kg = e - t * KG;
               uint32_t h[4], l[4];
               float vmax = 0.f;
@@ -436,20 +428,19 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
               if (vmax * kActScale > 60000.f) *p.sat = 1;          // the clamp below changes a value: tell the host (sticky)
 #pragma unroll
               for (int j = 0; j < 4; ++j) split2_f16(v[u][2 * j] * kActScale, v[u][2 * j + 1] * kActScale, h[j], l[j]);
-              // TMEM lane = GEMM row of this thread; 8 K values = 4 columns of fp16 pairs
-              const uint32_t xa = tmem + ((uint32_t)((warp & 3) * 32) << 16) + C::XA_COL + t * C::CIN_P + kg * 4;
-              tmem_st4(xa, h[0], h[1], h[2], h[3]);
-              tmem_st4(xa + C::CIN_P / 2, l[0], l[1], l[2], l[3]);
-              if (e == wg) SYN_TRACE(0, 62, 6);
+              // canonical K-major operand: row of this thread in slab t, 8 K values = one 16-byte core-matrix row
+              uint8_t* xa = sXA + t * C::XA_TILE + (r64 >> 3) * 128 + kg * 1024 + (r64 & 7) * 16;
+              *reinterpret_cast<uint4*>(xa) = make_uint4(h[0], h[1], h[2], h[3]);
+              *reinterpret_cast<uint4*>(xa + C::XA_PLANE) = make_uint4(l[0], l[1], l[2], l[3]);
+              if (e == xg) SYN_TRACE(0, 62, 6);
             }
           }
-          if (e0 == wg) SYN_TRACE(0, 62, 7);
+          if (e0 == xg) SYN_TRACE(0, 62, 7);
         }
       }
       SYN_TRACE(0, 62, 3);
-      tmem_wait_st();
-      tc_fence_before_sync();
-      mbar_arrive(smem_u32(&bar_x));
+      fence_proxy_async_smem();                             // XA is read by wgmma after the next worker barrier
+      mbar_arrive(smem_u32(&bar_x));                        // (stem) the staged rows are consumed
       SYN_TRACE(0, 62, 4);
 
     };
@@ -470,7 +461,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
       }
     };
 #if SYN_PDL
-    // Programmatic dependent launch: everything above (barriers, TMEM, the zeroed window, the weight image) does not
+    // Programmatic dependent launch: everything above (barriers, the zeroed window, the weight image) does not
     // depend on the previous kernel; its output -- this kernel's input -- is first touched below, and this kernel's
     // first global store comes later still.
     asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -495,23 +486,20 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
       const int M2 = nfaces * C::M2F;
       const int mt2 = (M2 + 127) >> 7;
 
+      float acc2[IPW][N2 / 2];                             // this warpgroup's D2 items, accumulated over the chunks
       for (int c = 0; c < C::NCHUNK; ++c, ++g) {
         const int slot = C::WSTREAM ? (int)(g % C::WSTAGES) : c;
         if constexpr (C::WSTREAM) mbar_wait(smem_u32(&bar_wfull[slot]), (g / C::WSTAGES) & 1, p.err);
         const float* dwc = reinterpret_cast<const float*>(sWch + slot * C::CHUNK_BYTES + C::CH_DW);
         SYN_TRACE(0, c, 0);
-        // ---- EPI1: D1 -> relu6(s1*D1 + b1) -> hidden window --------------------------------------
-        mbar_wait(smem_u32(&bar_d1), n_d1 & 1, p.err);
-        ++n_d1;
-        tc_fence_after_sync();
+        // every worker is done with the previous chunk: its depthwise reads of Hs and its GEMM2 reads of A2
+        // (c == 0: XA of this tile is complete)
+        group_bar_sync<TPG>(grp);
         SYN_TRACE(0, c, 1);
-        group_bar_sync<TPG>(grp);   // the group is done reading ITS Hs columns (DW c-1)
-        SYN_TRACE(0, c, 2);
         if (c == 0) {
-          // ---- strip mode: window rows outside the image must read as zero (may hold a previous tile);
-          //      every group clears its own channel columns
+          // ---- strip mode: window rows outside the image must read as zero (may hold a previous tile)
           if constexpr (C::STRIPS > 1) {
-            constexpr int CQ = KPG * 2;                               // float4 per pixel owned by the group
+            constexpr int CQ = KPG * 2;                               // float4 per pixel
             if (iy0 < 0)
               for (int i = gtid; i < C::HS_COLS * CQ; i += TPG)
                 *reinterpret_cast<float4*>(sH + (size_t)(i / CQ) * C::HS_STRIDE + grp * KPG * 8 + (i % CQ) * 4) =
@@ -523,62 +511,49 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
           }
         }
         {
-          // EPI1: 8 columns (one channel octet) per TMEM load; the expand scale is one power of two per
-          // layer (row 11 is constant) and the octet's biases stay in registers, so an element costs one
-          // FFMA.SAT plus a quarter of a 16-byte shared store
+          // ---- GEMM1 + EPI1, one 64-row slab of D1 at a time per warpgroup: relu6(s1*D1 + b1) / 6 -> hidden window.
+          // The expand scale is one power of two per layer (row 11 is constant), so an element costs one FFMA.SAT.
           const float sc1 = dwc[11 * C::DWS];
-          int cur_k = -1;
-          float bq[8];
-          const int n_e = mt1 * KPG;
-          constexpr int EB = C::EPI1_BATCH;
-          for (int e0 = gsub; e0 < n_e; e0 += EB * SUBS) {
-            uint32_t vr[EB][8];
+          const float* b1 = dwc + 10 * C::DWS;
+          const uint32_t w_lo = smem_desc_lo(smem_u32(sWch + slot * C::CHUNK_BYTES + C::CH_W1), LBO_W1);
+          const int slabs1 = (M1 + 63) >> 6;
+          for (int s1 = wg; s1 < slabs1; s1 += NWG) {          // warpgroup-uniform
+            float acc1[C::NC / 2];
+            const uint32_t a_lo = smem_desc_lo(smem_u32(sXA + s1 * C::XA_TILE), 1024);
+            wgmma_fence();
 #pragma unroll
-            for (int u = 0; u < EB; ++u) {                  // up to EB TMEM loads in flight, one wait
-              const int e = e0 + u * SUBS;
-              if (e < n_e) {                                // warp-uniform
-                const int t = e / KPG, kq = grp * KPG + (e - t * KPG);
-                tmem_ld8_async(tmem + ((uint32_t)((warp & 3) * 32) << 16) + t * C::NC + kq * 8, vr[u]);
-              }
+            for (int pass = 0; pass < 3; ++pass) {
+              if (pass >= p.npass) break;                           // single-pass engine: hi * hi only
+#pragma unroll
+              for (int ks = 0; ks < C::CIN_P / 16; ++ks)
+                wgmma_f16<C::NC>(acc1, desc64(d_hi, a_lo + (((pass == 2 ? C::XA_PLANE : 0) + ks * 2048) >> 4)),
+                                 desc64(d_hi, w_lo + (((pass == 1 ? C::W1_PLANE : 0) + ks * 2 * LBO_W1) >> 4)),
+                                 (pass > 0 || ks > 0) ? 1u : 0u);
             }
-            tmem_wait_ld();
+            wgmma_commit();
+            wgmma_wait<0>();
 #pragma unroll
-            for (int u = 0; u < EB; ++u) {
-              const int e = e0 + u * SUBS;
-              if (e < n_e) {
-                const int t = e / KPG, kq = grp * KPG + (e - t * KPG), j0 = kq * 8;
-                if (kq != cur_k) {
-                  cur_k = kq;
-                  const float4 b0 = *reinterpret_cast<const float4*>(dwc + 10 * C::DWS + j0);
-                  const float4 b1 = *reinterpret_cast<const float4*>(dwc + 10 * C::DWS + j0 + 4);
-                  bq[0] = b0.x; bq[1] = b0.y; bq[2] = b0.z; bq[3] = b0.w; bq[4] = b1.x; bq[5] = b1.y; bq[6] = b1.z; bq[7] = b1.w;
-                }
-                const int m = t * 128 + row;
-                if (m < M1) {
-                  const int f = (C::FACES > 1) ? m / ppf : 0;
-                  const int mr = m - f * ppf;
-                  const int yl = mr / C::W, xx = mr - yl * C::W;
-                  float* hrow = sH + (size_t)(f * C::HS_FACE + (rf - iy0 + yl) * C::HS_COLS + xx + 1) * C::HS_STRIDE + j0;
-                  *reinterpret_cast<float4*>(hrow) =
-                      make_float4(__saturatef(fmaf(__uint_as_float(vr[u][0]), sc1, bq[0])), __saturatef(fmaf(__uint_as_float(vr[u][1]), sc1, bq[1])),
-                                  __saturatef(fmaf(__uint_as_float(vr[u][2]), sc1, bq[2])), __saturatef(fmaf(__uint_as_float(vr[u][3]), sc1, bq[3])));
-                  *reinterpret_cast<float4*>(hrow + 4) =
-                      make_float4(__saturatef(fmaf(__uint_as_float(vr[u][4]), sc1, bq[4])), __saturatef(fmaf(__uint_as_float(vr[u][5]), sc1, bq[5])),
-                                  __saturatef(fmaf(__uint_as_float(vr[u][6]), sc1, bq[6])), __saturatef(fmaf(__uint_as_float(vr[u][7]), sc1, bq[7])));
+            for (int h = 0; h < 2; ++h) {
+              const int m = 64 * s1 + acc_row(row, 2 * h);
+              if (m < M1) {
+                const int f = (C::FACES > 1) ? m / ppf : 0;
+                const int mr = m - f * ppf;
+                const int yl = mr / C::W, xx = mr - yl * C::W;
+                float* hrow = sH + (size_t)(f * C::HS_FACE + (rf - iy0 + yl) * C::HS_COLS + xx + 1) * C::HS_STRIDE;
+#pragma unroll
+                for (int q = 0; q < C::NC / 8; ++q) {
+                  const int i = 4 * q + 2 * h, j0 = acc_col(row, i);
+                  const float2 bq = *reinterpret_cast<const float2*>(b1 + j0);
+                  *reinterpret_cast<float2*>(hrow + j0) =
+                      make_float2(__saturatef(fmaf(acc1[i], sc1, bq.x)), __saturatef(fmaf(acc1[i + 1], sc1, bq.y)));
                 }
               }
             }
           }
         }
         SYN_TRACE(0, c, 3);
-        tc_fence_before_sync();
-        mbar_arrive(smem_u32(&bar_epi1));
-        group_bar_sync<TPG>(grp);   // the group's channel columns of the window are complete
+        group_bar_sync<TPG>(grp);   // the hidden window of this chunk is complete
         // ---- DW: 3x3 depthwise on the window -> A2 operand ----------------------------------------
-        if (c > 0) {                                        // A2 is free once GEMM2(c-1) has completed
-          mbar_wait(smem_u32(&bar_g2), n_g2 & 1, p.err);
-          ++n_g2;
-        }
         SYN_TRACE(0, c, 4);
         if constexpr (C::DW3) {
           // Stride-1 60^2 / 30^2 / 15^2 maps.  The depthwise phase is bound by shared-memory wavefronts (every LDS.128 of
@@ -673,7 +648,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
           // an even number of 16-byte bank groups apart, and the mirror image shifts lanes 4-7 onto the odd
           // groups: every window load (quarter-warp) and every 8-byte operand store (half-warp) is
           // bank-conflict free.
-          // 8x8 maps (SYN_DW2_SMALL; measured -2.2 % of the step with scripts/quick_variant_check.py): the 8 lanes
+          // 8x8 maps (SYN_DW2_SMALL): the 8 lanes
           // are 4 column pairs x 2 row pairs; the second row pair lies 2 window rows = 4 bank groups further
           // and is the mirrored half.
           constexpr int XL = (C::WO >= 15) ? 8 : 4, YL = 8 / XL;           // lanes of a unit along x / along row pairs
@@ -692,7 +667,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
             if (ox >= C::WO || oy >= C::RO) continue;
             const bool two = (oy + 1 < C::RO);
             const float* wq = dwc + j0;
-            float2 w[3][3][2];                                             // [ky][local kx][channel pair] (FFMA2 operands)
+            float2 w[3][3][2];                                             // [ky][local kx][channel pair]
 #pragma unroll
             for (int ky = 0; ky < 3; ++ky)
 #pragma unroll
@@ -765,8 +740,8 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
           constexpr int XG = (C::WO + GX - 1) / GX;                        // x groups per output row
           // small maps (8x8, 4x4) have fewer row-pair items than worker threads: one output row per item
           // there, so that every thread has work and the per-chunk dependency chain is half as long
-          // (measured: pays when at most a quarter of the threads would have a row-pair item, blocks 7/14/17;
-          // with half of them busy the extra window loads of single rows cost more than the idle warps)
+          // (chosen when at most a quarter of the threads would have a row-pair item: with half of them busy the
+          // extra window loads of single rows cost more than the idle warps)
           constexpr int RPI = (4 * C::FACES * ((C::RO + 1) / 2) * ((C::WO + GX - 1) / GX) * GX * NKG <= NWT) ? 1 : 2;
           constexpr int RP = (C::RO + RPI - 1) / RPI, RPG = (RP + GY - 1) / GY;   // row pairs (rows), groups of them
           constexpr int PER_FACE = XG * RPG;
@@ -793,7 +768,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
                 const float* wbase = dwc + kg * 8;
                 const float* h0 = sH + (size_t)(f * C::HS_FACE + (oy * C::STRIDE) * C::HS_COLS + ox * C::STRIDE) * C::HS_STRIDE + kg * 8;
                 const bool two = (RPI == 2) && (oy + 1 < C::RO);             // second output row exists
-                float2 acc0[4], acc1[4];                                     // channel pairs (FFMA2 operands)
+                float2 acc0[4], acc1[4];                                     // channel pairs
                 {
                   const float4 a = *reinterpret_cast<const float4*>(wbase + 9 * C::DWS + q0);
                   const float4 e = *reinterpret_cast<const float4*>(wbase + 9 * C::DWS + q1);
@@ -857,7 +832,35 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
         }
         SYN_TRACE(0, c, 5);
         fence_proxy_async_smem();
-        mbar_arrive(smem_u32(&bar_a2));
+        group_bar_sync<TPG>(grp);   // A2 of this chunk is complete
+        {
+          // ---- GEMM2: D2 += A2 * W3c^T on this warpgroup's items (accumulators stay in registers over the chunks)
+          const uint32_t w_lo = smem_desc_lo(smem_u32(sWch + slot * C::CHUNK_BYTES + C::CH_W3), LBO_W3);
+          const int items2 = ((M2 + 63) >> 6) * NSPL;
+          wgmma_fence();
+#pragma unroll
+          for (int u = 0; u < IPW; ++u) {
+            const int it = wg + u * NWG;
+            if (it < items2) {                                       // warpgroup-uniform
+              const int s2 = it / NSPL, pc = it - s2 * NSPL;
+              const uint32_t a_lo = smem_desc_lo(smem_u32(sA2 + (s2 >> 1) * (128 * C::NC * 2)) + (s2 & 1) * 1024, 2048);
+              const uint32_t b_lo = w_lo + ((pc * (N2 / 8) * 128) >> 4);
+#pragma unroll
+              for (int pass = 0; pass < 3; ++pass) {
+                if (pass >= p.npass) break;
+#pragma unroll
+                for (int ks = 0; ks < C::NC / 16; ++ks)
+                  wgmma_f16<N2>(acc2[u], desc64(d_hi, a_lo + (((pass == 2 ? C::A2_PLANE : 0) + ks * 4096) >> 4)),
+                                desc64(d_hi, b_lo + (((pass == 1 ? C::W3_PLANE : 0) + ks * 2 * LBO_W3) >> 4)),
+                                (c > 0 || pass > 0 || ks > 0) ? 1u : 0u);
+              }
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+        }
+        if constexpr (C::WSTREAM) mbar_arrive(smem_u32(&bar_wempty[slot]));   // the chunk's slot may be refilled
+        SYN_TRACE(0, c, 6);
       }
       SYN_TRACE(0, 63, 1);
 
@@ -865,9 +868,6 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
       prefetch_x(tile + 2 * (int)gridDim.x);
       // ---- EPI2: s3*D2 + b3 (+ skip) -> global NHWC --------------------------------------------------
       SYN_TRACE(0, 63, 2);
-      constexpr int JW = (C::COUT_P % 32 == 0 && C::MT2 * (C::COUT_P / 32) >= 2 * NWG) ? 32
-                         : (C::MT2 * (C::COUT_P / 16) >= 2 * NWG) ? 16 : 8;
-      constexpr int JC = C::COUT_P / JW;
       // GEMM2 row m2 -> output pixel of the tile (rows are padded to WOP pixels when DW3 needs it); -1 = no pixel
       auto out_pixel = [&](int m2) -> int {
         if (m2 >= M2) return -1;
@@ -875,67 +875,44 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
         const int oyl = m2 / C::WOP, oxl = m2 - oyl * C::WOP;
         return oxl < C::WO ? oyl * C::WO + oxl : -1;
       };
-      // The skip connection (stride 1, CIN == COUT: the same pixel of the block input) is a dependent global load per
-      // 16 bytes of output: fetch it BEFORE waiting for the last GEMM2, one item ahead of its use afterwards.
-      float4 res_cur[JW / 4];
-      auto load_res = [&](int e, float4 (&r)[JW / 4]) {
-        if constexpr (C::RES) {
-          const int t = e / JC, j0 = (e - t * JC) * JW;
-          const int pix = out_pixel(t * 128 + row);
+      const int items2 = ((M2 + 63) >> 6) * NSPL;
 #pragma unroll
-          for (int j = 0; j < JW; j += 4) {
-            r[j / 4] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (pix >= 0 && j0 + j < C::COUT)
-              r[j / 4] = __ldg(reinterpret_cast<const float4*>(p.x + ((size_t)(f0 * C::W + oy0) * C::W + pix) * C::CIN + j0 + j));
-          }
-        }
-      };
-      if constexpr (C::RES) {
-        if (wg < mt2 * JC) load_res(wg, res_cur);
-      }
-      mbar_wait(smem_u32(&bar_g2), n_g2 & 1, p.err);
-      ++n_g2;
-      tc_fence_after_sync();
-      SYN_TRACE(0, 63, 3);
-      {
-        for (int e = wg; e < mt2 * JC; e += NWG) {
-          const int t = e / JC, j0 = (e - t * JC) * JW;
-          const int pix = out_pixel(t * 128 + row);
-          float* orow = p.y + ((size_t)(f0 * C::WO + oy0) * C::WO + max(pix, 0)) * C::COUT;
-          float v[JW];
-          const uint32_t taddr = tmem + ((uint32_t)((warp & 3) * 32) << 16) + C::D2_COL + t * C::COUT_P + j0;
-          if constexpr (JW == 32) tmem_ld32(taddr, v); else if constexpr (JW == 16) tmem_ld16(taddr, v); else tmem_ld8(taddr, v);
-          if (pix >= 0) {
+      for (int u = 0; u < IPW; ++u) {
+        const int it = wg + u * NWG;
+        if (it >= items2) break;
+        const int s2 = it / NSPL, pc = it - s2 * NSPL;
 #pragma unroll
-            for (int j = 0; j < JW; j += 4) {
-              if (j0 + j < C::COUT) {
-                const float4 bb = *reinterpret_cast<const float4*>(sB3 + j0 + j);
-                const float4 sc = *reinterpret_cast<const float4*>(sB3 + C::COUT_P + j0 + j);
-                float4 o = make_float4(fmaf(v[j], sc.x, bb.x), fmaf(v[j + 1], sc.y, bb.y), fmaf(v[j + 2], sc.z, bb.z),
-                                       fmaf(v[j + 3], sc.w, bb.w));
-                if constexpr (C::RES) {
-                  const float4 r = res_cur[j / 4];
-                  o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
-                }
-                *reinterpret_cast<float4*>(orow + j0 + j) = o;
-              }
+        for (int h = 0; h < 2; ++h) {
+          const int pix = out_pixel(64 * s2 + acc_row(row, 2 * h));
+          if (pix < 0) continue;
+          float* orow = p.y + ((size_t)(f0 * C::WO + oy0) * C::WO + pix) * C::COUT;
+          const float* xrow = p.x + ((size_t)(f0 * C::W + oy0) * C::W + pix) * C::CIN;   // skip: same pixel, CIN == COUT
+          float2 res[N2 / 8];
+          if constexpr (C::RES) {                                   // all skip loads in flight before the first use
+#pragma unroll
+            for (int q = 0; q < N2 / 8; ++q) {
+              const int j = pc * N2 + acc_col(row, 4 * q);
+              res[q] = j < C::COUT ? __ldg(reinterpret_cast<const float2*>(xrow + j)) : make_float2(0.f, 0.f);
             }
           }
-          if constexpr (C::RES) {                                  // next item's skip values: in flight during its TMEM load
-            if (e + NWG < mt2 * JC) load_res(e + NWG, res_cur);
+#pragma unroll
+          for (int q = 0; q < N2 / 8; ++q) {
+            const int i = 4 * q + 2 * h, j = pc * N2 + acc_col(row, i);
+            if (j < C::COUT) {                                      // COUT is even: pairs never straddle it
+              const float2 bb = *reinterpret_cast<const float2*>(sB3 + j);
+              const float2 sc = *reinterpret_cast<const float2*>(sB3 + C::COUT_P + j);
+              float2 o = make_float2(fmaf(acc2[u][i], sc.x, bb.x), fmaf(acc2[u][i + 1], sc.y, bb.y));
+              if constexpr (C::RES) { o.x += res[q].x; o.y += res[q].y; }
+              *reinterpret_cast<float2*>(orow + j) = o;
+            }
           }
         }
       }
       SYN_TRACE(0, 63, 4);
-      tc_fence_before_sync();
-      mbar_arrive(smem_u32(&bar_d2free));
     }
   } else if (warp == NWW) {
-    // =============================== MMA issuer / weight loader ====================================
-    // The whole warp runs this control flow convergently and every batch of tcgen05.mma / bulk copies sits
-    // under one elect.sync: the compiler then knows a single thread issues them (no per-instruction
-    // uniformisation loop, descriptors straight from uniform registers).  Measured with tools/umma_timing:
-    // ~170 cycles per MMA from a `tid == X` branch against 32 + N/4 (the operand-read floor) this way.
+    // =============================== weight loader / stem-row stager ================================
+    // The whole warp runs this control flow convergently and every batch of bulk copies sits under one elect.sync.
     const int my_tiles = (ntiles > (int)blockIdx.x) ? (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
     const uint32_t total_chunks = (uint32_t)my_tiles * C::NCHUNK;
     auto load_chunk = [&](uint32_t gi) {                     // streaming: chunk gi -> slot gi % WSTAGES
@@ -956,67 +933,17 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
       }
     }
     __syncwarp();
-    mbar_wait(smem_u32(&bar_w), 0, p.err);
-    const uint32_t idesc1 = make_idesc_f16(128, C::NC);
-    const uint32_t idesc2 = make_idesc_f16(128, C::N2);
-    constexpr uint32_t LBO_W1 = (C::NC / 8) * 128, LBO_W3 = (C::COUT_P / 8) * 128;
-    uint32_t n_x = 0, n_epi1 = 0, n_a2 = 0, n_free = 0, n_g2i = 0;
-    uint32_t g = 0;                                          // chunk counter of the current GEMM2
-    int ntile_local = 0;
-
-    // descriptor halves that never change (SBO = 128 everywhere); per MMA only `lo` moves by (bytes >> 4)
-    const uint32_t d_hi = smem_desc_hi(128);
-    const uint32_t a2_lo = smem_desc_lo(smem_u32(sA2), 2048);
-    const uint32_t w_lo1 = smem_desc_lo(smem_u32(sWch) + C::CH_W1, LBO_W1), w_lo3 = smem_desc_lo(smem_u32(sWch) + C::CH_W3, LBO_W3);
-    auto gemm1 = [&](uint32_t gi, int c, int mt1) {
-      const int slot = C::WSTREAM ? (int)(gi % C::WSTAGES) : c;
-      if constexpr (C::WSTREAM) mbar_wait(smem_u32(&bar_wfull[slot]), (gi / C::WSTAGES) & 1, p.err);
-      const uint32_t wb = w_lo1 + ((slot * C::CHUNK_BYTES) >> 4);
-      if (elect_one()) {
-      for (int t = 0; t < mt1; ++t) {
-        const uint32_t xa = tmem + C::XA_COL + t * C::CIN_P;     // A from TMEM: N/2 cycles per MMA, no smem read of X
-#pragma unroll
-        for (int pass = 0; pass < 3; ++pass) {
-          if (pass >= p.npass) break;                              // single-pass engine: hi * hi only
-#pragma unroll
-          for (int ks = 0; ks < C::CIN_P / 16; ++ks)
-            umma_f16_ts(tmem + t * C::NC, xa + (pass == 2 ? C::CIN_P / 2 : 0) + ks * 8,
-                        desc64(d_hi, wb + (((pass == 1 ? C::W1_PLANE : 0) + ks * 2 * LBO_W1) >> 4)), idesc1,
-                        (pass > 0 || ks > 0) ? 1u : 0u);
-        }
+    if constexpr (C::WSTREAM) {
+      // chunk gi reuses the slot of chunk gi - WSTAGES once every worker's GEMM2 of that chunk is done
+      for (uint32_t gi = C::WSTAGES; gi < total_chunks; ++gi) {
+        mbar_wait(smem_u32(&bar_wempty[gi % C::WSTAGES]), (gi / C::WSTAGES - 1) & 1, p.err);
+        if (elect_one()) load_chunk(gi);
+        __syncwarp();
       }
-      umma_commit(smem_u32(&bar_d1));
-      }
-      __syncwarp();
-    };
-    auto gemm2 = [&](uint32_t gi, int c, int mt2) {
-      const int slot = C::WSTREAM ? (int)(gi % C::WSTAGES) : c;
-      const uint32_t wb = w_lo3 + ((slot * C::CHUNK_BYTES) >> 4);
-      const uint32_t acc0 = (c > 0) ? 1u : 0u;
-      if (elect_one()) {
-      for (int t = 0; t < mt2; ++t) {
-        const uint32_t ab = a2_lo + ((t * (128 * C::NC * 2)) >> 4);
-#pragma unroll
-        for (int pass = 0; pass < 3; ++pass) {
-          if (pass >= p.npass) break;
-#pragma unroll
-          for (int ks = 0; ks < C::NC / 16; ++ks)
-#pragma unroll
-            for (int hh = 0; hh < C::NSPLIT; ++hh)
-              umma_f16(tmem + C::D2_COL + t * C::COUT_P + hh * C::N2,
-                       desc64(d_hi, ab + (((pass == 2 ? C::A2_PLANE : 0) + ks * 4096) >> 4)),
-                       desc64(d_hi, wb + (((pass == 1 ? C::W3_PLANE : 0) + ks * 2 * LBO_W3 + hh * (C::N2 / 8) * 128) >> 4)),
-                       idesc2, (pass > 0 || ks > 0) ? 1u : acc0);
-        }
-      }
-      umma_commit(smem_u32(&bar_g2));
-      }
-      __syncwarp();
-    };
-
-    // stem, fp32 crops: bulk-copy (TMA) the crop rows of a tile into sIn, one tile ahead of the workers
-    auto stage_rows = [&](int tile) {
-      if constexpr (C::STEM) {
+    }
+    if constexpr (C::STEM) {
+      // fp32 crops: bulk-copy (TMA) the crop rows of a tile into sIn, one tile ahead of the workers
+      auto stage_rows = [&](int tile) {
         if (p.x_u8 != nullptr || tile >= ntiles) return;
         if (!elect_one()) return;
         const int fgq = tile / C::STRIPS, spq = tile - fgq * C::STRIPS;
@@ -1030,71 +957,21 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
         for (int ci = 0; ci < 3; ++ci)
           bulk_g2s(smem_u32(sIn + (ci * C::IN_ROWS + r_lo) * C::IN_STRIDE),
                    p.x + ((size_t)(fgq * 3 + ci) * kImg + iy_first + r_lo) * kImg, bytes, smem_u32(&bar_in));
-      }
-    };
+      };
 #if SYN_PDL
-    asm volatile("griddepcontrol.wait;" ::: "memory");     // the stem's crop rows are the previous step's business only in
-#endif                                                     // theory (inputs), but the rule is kept uniform
-    stage_rows(blockIdx.x);
-
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++ntile_local) {
-      const int fg = tile / C::STRIPS, sp = tile - fg * C::STRIPS;
-      int f0_unused, nfaces;
-      group_faces(fg, f0_unused, nfaces);
-      const int iy0 = sp * C::RO * C::STRIDE - 1;
-      const int rf = max(iy0, 0), rl = min(iy0 + C::RWIN - 1, C::W - 1);
-      const int mt1 = (nfaces * (rl - rf + 1) * C::W + 127) >> 7;
-      const int mt2 = (nfaces * C::M2F + 127) >> 7;
-#ifdef SYN_FUSED_TRACE
-      const bool trace_on = blockIdx.x == 0 && tile == (int)gridDim.x && tid == NWT;
+      asm volatile("griddepcontrol.wait;" ::: "memory");   // the crop rows are inputs; the rule is kept uniform
 #endif
-      SYN_TRACE(1, 63, 0);
-      mbar_wait(smem_u32(&bar_x), n_x & 1, p.err);
-      ++n_x;
-      tc_fence_after_sync();
-      SYN_TRACE(1, 63, 1);
-      gemm1(g, 0, mt1);
-      SYN_TRACE(1, 63, 2);
-      stage_rows(tile + gridDim.x);          // sIn is free again: the conversion of this tile has consumed it
-      for (int c = 0; c < C::NCHUNK; ++c, ++g) {
-        SYN_TRACE(1, c, 0);
-        if (c + 1 < C::NCHUNK) {
-          mbar_wait(smem_u32(&bar_epi1), n_epi1 & 1, p.err);    // D1 drained by the workers
-          ++n_epi1;
-          tc_fence_after_sync();
-          SYN_TRACE(1, c, 1);
-          gemm1(g + 1, c + 1, mt1);
-          SYN_TRACE(1, c, 2);
-        }
-        mbar_wait(smem_u32(&bar_a2), n_a2 & 1, p.err);
-        ++n_a2;
-        if (c == 0 && ntile_local > 0) {                         // D2 of the previous tile drained
-          mbar_wait(smem_u32(&bar_d2free), n_free & 1, p.err);
-          ++n_free;
-        }
-        tc_fence_after_sync();
-        SYN_TRACE(1, c, 3);
-        gemm2(g, c, mt2);
-        SYN_TRACE(1, c, 4);
-        if constexpr (C::WSTREAM) {
-          // the slot of chunk g may be refilled once GEMM2(g) has read W3c (the workers are already past it)
-          mbar_wait(smem_u32(&bar_g2), n_g2i & 1, p.err);
-          if (g + C::WSTAGES < total_chunks && elect_one()) load_chunk(g + C::WSTAGES);
-          __syncwarp();
-          SYN_TRACE(1, c, 5);
-        }
-        ++n_g2i;
+      stage_rows(blockIdx.x);
+      __syncwarp();
+      uint32_t n_x = 0;
+      // uint8 crops are staged by the workers themselves; then nothing here waits on their bar_x phases
+      for (int tile = blockIdx.x; p.x_u8 == nullptr && tile < ntiles; tile += gridDim.x) {
+        mbar_wait(smem_u32(&bar_x), n_x & 1, p.err);        // the conversion of this tile has consumed sIn
+        ++n_x;
+        stage_rows(tile + gridDim.x);
+        __syncwarp();
       }
-      // the last chunk's EPI1 arrival is not consumed above: keep the phase counter in step
-      mbar_wait(smem_u32(&bar_epi1), n_epi1 & 1, p.err);
-      ++n_epi1;
     }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == NWW) {
-    __syncwarp();
-    tmem_dealloc<C::TM_COLS>(tmem);
   }
 }
 
@@ -1118,14 +995,15 @@ using FusedStemB1 = FusedCfg<27, 32, 32, 16, 60, 1, SYN_RO_STEM, 1, false, true,
 using FusedB2 = FusedCfg<16, 96, SYN_NC_B2, 24, 60, 2, SYN_RO_B2, 1, false, false, 0>;       // features[2]
 using FusedB3 = FusedCfg<24, 144, SYN_NC_B3, 24, 30, 1, SYN_RO_B3, 1, true, false, 0>;      // features[3]
 using FusedB4 = FusedCfg<24, 144, SYN_NC_B4, 32, 30, 2, SYN_RO_B4, 1, false, false, 0>;      // features[4]
-using FusedB56 = FusedCfg<32, 192, SYN_NC_B56, 32, 15, 1, 15, 1, true, false, 0>;     // features[5], [6]
+using FusedB56 = FusedCfg<32, 192, SYN_NC_B56, 32, 15, 1, SYN_RO_B56, 1, true, false, 0>;     // features[5], [6]
 using FusedB7 = FusedCfg<32, 192, SYN_NC_B7, 64, 15, 2, 8, 1, false, false, 0>;      // features[7]
 using FusedB8 = FusedCfg<64, 384, 64, 64, 8, 1, 8, 2, true, false, 3>;         // features[8..10]
 using FusedB11 = FusedCfg<64, 384, 64, 96, 8, 1, 8, 2, false, false, 2>;       // features[11]
 using FusedB12 = FusedCfg<96, 576, SYN_NC_B12, 96, 8, 1, 8, 2, true, false, SYN_NC_B12 == 32 ? 3 : 2>;        // features[12], [13]
 using FusedB14 = FusedCfg<96, 576, SYN_NC_B14, 160, 8, 2, 4, 2, false, false, SYN_NC_B14 == 32 ? 3 : 2>;      // features[14]
-// three ring slots for blocks 15/16 (measured -6 %); narrower chunks in deeper rings were slower everywhere else
-using FusedB15 = FusedCfg<160, 960, 32, 160, 4, 1, 4, 8, true, false, 3>;      // features[15], [16]
-using FusedB17 = FusedCfg<160, 960, SYN_NC_B17, 320, 4, 1, 4, 8, false, false, SYN_NC_B17 == 16 ? 3 : 2>;     // features[17]
+// blocks 15-17: four faces per tile (64 GEMM rows = one MMA slab), so that the 64 x COUT fp32 D2 accumulator fits the
+// registers of the worker warpgroups
+using FusedB15 = FusedCfg<160, 960, 32, 160, 4, 1, 4, 4, true, false, 3>;      // features[15], [16]
+using FusedB17 = FusedCfg<160, 960, SYN_NC_B17, 320, 4, 1, 4, 4, false, false, SYN_NC_B17 == 16 ? 3 : 2>;     // features[17]
 
 }  // namespace syn

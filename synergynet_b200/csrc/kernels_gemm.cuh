@@ -1,4 +1,4 @@
-// General fp32-accurate GEMM / implicit-GEMM convolution on tcgen05 for the layers outside the fused MobileNetV2
+// General fp32-accurate GEMM / implicit-GEMM convolution on tensor cores (wgmma) for the layers outside the fused MobileNetV2
 // blocks: the PointNet refinement heads MLP_for / MLP_rev (reference backbone_nets/pointnet_backbone.py:31-64,
 // 90-106; Conv1d(k=1) + BatchNorm1d + ReLU over B x 68 points) and the ResNet-50 backbone variant
 // (backbone_nets/resnet_backbone.py:227-249; 1x1 / 3x3 convolutions + BatchNorm2d + ReLU, NHWC here).
@@ -11,11 +11,11 @@
 // the hi/lo split -- exact, undone by one multiply in the epilogue, and immune to the |x| < ~937 range limit of
 // the fixed scale (ReLU outputs of these layers are unbounded).
 //
-// Roles: warps 0-7 = producers (thread = GEMM row x half of a chunk's k groups: gathers the fp32 row -- or, in conv
-// mode, the k x k x C patch of an NHWC pixel -- splits it and stores the canonical K-major operand), then the epilogue
-// (lane quarter = warp & 3, column half = warp >> 2); warp 8 = bulk-copy of the
-// pre-packed weight chunks + MMA issue (converged warp, elect.sync).  K streams in chunks of 32 through a 4-stage
-// ring (193 KB smem): the fp32 rows come from global memory / L2 and three chunks of look-ahead cover their latency.
+// Roles: 8 warps = two warpgroups, one code path.  Every thread is a producer (GEMM row tid % 128 x half tid / 128 of
+// a chunk's k groups: gathers the fp32 row -- or, in conv mode, the k x k x C patch of an NHWC pixel -- splits it and
+// stores the canonical K-major operand); warpgroup g then issues the wgmma of rows 64g..64g+63 (accumulators in
+// registers) and runs their epilogue.  Thread 0 also launches the bulk copy of each pre-packed weight chunk once its
+// ring slot is free.  K streams in chunks of 32 through a 4-stage ring (193 KB smem).
 #pragma once
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -24,8 +24,7 @@ namespace syn {
 
 constexpr int kGmKC = 32;                                 // K chunk
 constexpr int kGmStages = 4;                              // chunk ring: global-load latency of three chunks hidden
-constexpr int kGmProducerWarps = 8;                       // thread = (GEMM row, half of the chunk's k groups)
-constexpr int kGmThreads = (kGmProducerWarps + 1) * 32;
+constexpr int kGmThreads = 256;                           // thread = (GEMM row, half of the chunk's k groups)
 constexpr int kGmMaxNr = 256;
 constexpr int kGmStageA = 128 * kGmKC * 2;                // 8 KB: one plane (hi or lo) of the A tile
 constexpr int kGmStageB = kGmMaxNr * kGmKC * 2;           // 16 KB
@@ -63,11 +62,10 @@ __device__ __forceinline__ float exp2i(int e) { return __uint_as_float((unsigned
 __global__ void __launch_bounds__(kGmThreads, 1) tc_gemm_kernel(const GemmArgs p) {
   using namespace tc;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_full[kGmStages], bar_empty[kGmStages], bar_acc;
-  __shared__ uint32_t tmem_base_s;
+  __shared__ __align__(8) uint64_t bar_full[kGmStages], bar_empty[kGmStages];
   __shared__ __align__(16) float s_bias[kGmMaxNr], s_osc[kGmMaxNr];       // epilogue constants of this n-range
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int m0 = blockIdx.x * 128;
   const int n0 = blockIdx.y * p.nr;
   for (int i = tid; i < p.nr; i += kGmThreads) {              // the packed arrays are padded to nranges * nr entries
@@ -79,23 +77,19 @@ __global__ void __launch_bounds__(kGmThreads, 1) tc_gemm_kernel(const GemmArgs p
 
   if (tid == 0) {
     for (int i = 0; i < kGmStages; ++i) {
-      mbar_init(smem_u32(&bar_full[i]), kGmProducerWarps * 32 + 1);   // producer arrivals + the weight copy's expect_tx arrival
-      mbar_init(smem_u32(&bar_empty[i]), 1);
+      mbar_init(smem_u32(&bar_full[i]), kGmThreads + 1);     // producer arrivals + the weight copy's expect_tx arrival
+      mbar_init(smem_u32(&bar_empty[i]), kGmThreads);        // every thread, once its warpgroup's MMAs of the slot are done
     }
-    mbar_init(smem_u32(&bar_acc), 1);
     fence_mbar_init();
   }
-  if (warp == kGmProducerWarps) tmem_alloc<256>(smem_u32(&tmem_base_s));
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = tmem_base_s;
   auto stage_a = [&](int s, int plane) { return smem + s * kGmStage + plane * kGmStageA; };
   auto stage_b = [&](int s, int plane) { return smem + s * kGmStage + 2 * kGmStageA + plane * kGmStageB; };
 
-  if (warp < kGmProducerWarps) {
-    // ------------------------------ producers ---------------------------------------------------
+  {
+    // ------------------------------ producers + MMA ---------------------------------------------
     const int row = tid & 127, kh = tid >> 7, m = m0 + row;        // kh: which two of the chunk's four 8-element k groups
+    const int wg = kh;                                              // warpgroup: MMA rows 64 wg .. 64 wg + 63
     const bool row_ok = m < p.M;
     int b = 0, oy = 0, ox = 0;
     unsigned mx = 0;
@@ -116,6 +110,11 @@ __global__ void __launch_bounds__(kGmThreads, 1) tc_gemm_kernel(const GemmArgs p
     const int e_row = gemm_row_exp(mx);
     const float a_scale = exp2i(e_row);
     const float* arow = p.A + (size_t)m * p.lda;
+    const uint32_t lbo_b = (uint32_t)(p.nr >> 3) * 128;
+    const uint32_t d_hi = smem_desc_hi(128);
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
     for (int c = 0; c < nchunks; ++c) {
       const int s = c % kGmStages, use = c / kGmStages;
       const int k0 = c * kGmKC;
@@ -143,6 +142,13 @@ __global__ void __launch_bounds__(kGmThreads, 1) tc_gemm_kernel(const GemmArgs p
         }
       }
       mbar_wait(smem_u32(&bar_empty[s]), (use & 1) ^ 1, p.err);
+      if (tid == 0) {                                         // the weight chunk of this slot
+        const uint32_t plane_bytes = (uint32_t)p.nr * kc * 2;
+        const uint8_t* src = wimg + (size_t)p.nr * k0 * 4;    // chunks of this range are consecutive
+        mbar_expect_tx(smem_u32(&bar_full[s]), 2 * plane_bytes);
+        bulk_g2s(smem_u32(stage_b(s, 0)), src, plane_bytes, smem_u32(&bar_full[s]));
+        bulk_g2s(smem_u32(stage_b(s, 1)), src + plane_bytes, plane_bytes, smem_u32(&bar_full[s]));
+      }
       uint8_t* ah = stage_a(s, 0) + (row >> 3) * 128 + (row & 7) * 16;
       uint8_t* al = stage_a(s, 1) + (row >> 3) * 128 + (row & 7) * 16;
 #pragma unroll
@@ -160,122 +166,115 @@ __global__ void __launch_bounds__(kGmThreads, 1) tc_gemm_kernel(const GemmArgs p
       }
       fence_proxy_async_smem();
       mbar_arrive(smem_u32(&bar_full[s]));
-    }
-    // ------------------------------ epilogue ----------------------------------------------------
-    mbar_wait(smem_u32(&bar_acc), 0, p.err);
-    tc_fence_after_sync();
-    const uint32_t trow = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-    const int ncols = min(p.nr, p.N - n0);
-    const float inv_a = exp2i(-e_row);
-    float* orow = p.out ? p.out + (size_t)m * p.N + n0 : nullptr;
-    const float* rrow = p.residual ? p.residual + (size_t)m * p.N + n0 : nullptr;
-    const float* arow2 = p.addend ? p.addend + (size_t)(m / p.addend_group) * p.N + n0 : nullptr;
-    unsigned* crow = p.colmax_out ? p.colmax_out + (size_t)(m / p.colmax_group) * p.N + n0 : nullptr;
-    float rmax = 0.f;
-    const bool vec = (p.N & 3) == 0;                           // rows of out / residual / addend are 16-byte aligned
-    // max-pool over the rows of a group (PointNet): the 32 rows of a warp almost always belong to one group (68 points
-    // per face), so the warp reduces first (redux.sync) and issues ONE atomic per column instead of 32 on one address
-    const int cgrp = crow ? m / p.colmax_group : 0;
-    const bool warp_one_group = crow != nullptr && __all_sync(0xffffffffu, cgrp == __shfl_sync(0xffffffffu, cgrp, 0) && row_ok);
-    auto pool_max = [&](int col, float o) {                    // warp-uniform call sites only
-      const unsigned bits = row_ok ? __float_as_uint(o) : 0u;  // o >= 0 (ReLU): the bit pattern orders like the value
-      if (warp_one_group) {
-        const unsigned mx = __reduce_max_sync(0xffffffffu, bits);
-        if ((tid & 31) == 0) atomicMax(crow + col, mx);
-      } else if (row_ok) {
-        atomicMax(crow + col, bits);
-      }
-    };
-    for (int c0 = kh * 16; c0 < ncols; c0 += 32) {          // the two warps of a lane quarter interleave 16-column blocks
-      float v[16];
-      tmem_ld16(trow + c0, v);                              // warp-collective: the control flow below stays warp-uniform
-      if (vec && c0 + 16 <= ncols) {
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          const float4 sc = *reinterpret_cast<const float4*>(s_osc + c0 + j), bb = *reinterpret_cast<const float4*>(s_bias + c0 + j);
-          float4 o = make_float4(fmaf(v[j] * inv_a, sc.x, bb.x), fmaf(v[j + 1] * inv_a, sc.y, bb.y),
-                                 fmaf(v[j + 2] * inv_a, sc.z, bb.z), fmaf(v[j + 3] * inv_a, sc.w, bb.w));
-          if (row_ok) {
-            if (arow2) { const float4 a = *reinterpret_cast<const float4*>(arow2 + c0 + j); o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w; }
-            if (rrow) { const float4 r = __ldg(reinterpret_cast<const float4*>(rrow + c0 + j)); o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w; }
-          }
-          if (p.act == kActRelu6) { o.x = relu6f(o.x); o.y = relu6f(o.y); o.z = relu6f(o.z); o.w = relu6f(o.w); }
-          else if (p.act == kActRelu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-          if (row_ok) {
-            rmax = fmaxf(rmax, fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w))));
-            if (orow) *reinterpret_cast<float4*>(orow + c0 + j) = o;
-          }
-          if (crow) { pool_max(c0 + j, o.x); pool_max(c0 + j + 1, o.y); pool_max(c0 + j + 2, o.z); pool_max(c0 + j + 3, o.w); }
-        }
-        continue;
-      }
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        if (c0 + j >= ncols) break;                          // warp-uniform
-        float o = fmaf(v[j] * inv_a, s_osc[c0 + j], s_bias[c0 + j]);
-        if (row_ok) {
-          if (arow2) o += arow2[c0 + j];
-          if (rrow) o += rrow[c0 + j];
-        }
-        if (p.act == kActRelu6) o = relu6f(o); else if (p.act == kActRelu) o = fmaxf(o, 0.f);
-        if (row_ok) {
-          rmax = fmaxf(rmax, fabsf(o));
-          if (orow) orow[c0 + j] = o;
-        }
-        if (crow) pool_max(c0 + j, o);
-      }
-    }
-    if (row_ok && p.rowmax_out != nullptr) atomicMax(p.rowmax_out + m, __float_as_uint(rmax));
-  } else {
-    // ------------------------------ weight loader + MMA issuer (converged warp) -------------------
-    const uint32_t idesc = make_idesc_f16(128, p.nr);
-    const uint32_t lbo_b = (uint32_t)(p.nr >> 3) * 128;
-    const uint32_t d_hi = smem_desc_hi(128);
-    auto load_w = [&](int c) {                                // weight chunk c -> its ring slot (slot known to be free)
-      const int s = c % kGmStages, k0 = c * kGmKC;
-      const int kc = min(kGmKC, p.Kp - k0);
-      if (elect_one()) {
-        const uint32_t plane_bytes = (uint32_t)p.nr * kc * 2;
-        const uint8_t* src = wimg + (size_t)p.nr * k0 * 4;    // chunks of this range are consecutive
-        mbar_expect_tx(smem_u32(&bar_full[s]), 2 * plane_bytes);
-        bulk_g2s(smem_u32(stage_b(s, 0)), src, plane_bytes, smem_u32(&bar_full[s]));
-        bulk_g2s(smem_u32(stage_b(s, 1)), src + plane_bytes, plane_bytes, smem_u32(&bar_full[s]));
-      }
-      __syncwarp();
-    };
-    for (int c = 0; c < min(nchunks, kGmStages); ++c) load_w(c);      // the first use of every slot needs no wait
-    for (int c = 0; c < nchunks; ++c) {
-      const int s = c % kGmStages, use = c / kGmStages;
-      const int kc = min(kGmKC, p.Kp - c * kGmKC);
-      mbar_wait(smem_u32(&bar_full[s]), use & 1, p.err);
-      tc_fence_after_sync();
-      const uint32_t a_lo = smem_desc_lo(smem_u32(stage_a(s, 0)), 2048);
+      mbar_wait(smem_u32(&bar_full[s]), use & 1, p.err);     // the whole A chunk and the weight chunk landed
+      const uint32_t a_lo = smem_desc_lo(smem_u32(stage_a(s, 0)) + wg * 1024, 2048);
       const uint32_t b_lo = smem_desc_lo(smem_u32(stage_b(s, 0)), lbo_b);
-      if (elect_one()) {
+      wgmma_fence();
 #pragma unroll
-        for (int pass = 0; pass < 3; ++pass) {                 // hi*hi, hi*lo, lo*hi
-          const uint32_t a_off = (pass == 2 ? kGmStageA : 0), b_off = (pass == 1 ? kGmStageB : 0);
-          for (int ks = 0; ks < kc / 16; ++ks)
-            umma_f16(tmem, desc64(d_hi, a_lo + ((a_off + ks * 4096) >> 4)), desc64(d_hi, b_lo + ((b_off + ks * 2 * lbo_b) >> 4)),
-                     idesc, (c > 0 || pass > 0 || ks > 0) ? 1u : 0u);
-        }
-        umma_commit(smem_u32(&bar_empty[s]));
-        if (c == nchunks - 1) umma_commit(smem_u32(&bar_acc));
+      for (int pass = 0; pass < 3; ++pass) {                 // hi*hi, hi*lo, lo*hi
+        const uint32_t a_off = (pass == 2 ? kGmStageA : 0), b_off = (pass == 1 ? kGmStageB : 0);
+        for (int ks = 0; ks < kc / 16; ++ks)
+          wgmma_f16_rt(acc, p.nr, desc64(d_hi, a_lo + ((a_off + ks * 4096) >> 4)),
+                       desc64(d_hi, b_lo + ((b_off + ks * 2 * lbo_b) >> 4)), (c > 0 || pass > 0 || ks > 0) ? 1u : 0u);
       }
-      __syncwarp();
-      // refill the slot of chunk c - 1 (its MMAs were committed one iteration ago) with chunk c - 1 + stages
-      if (c >= 1 && c - 1 + kGmStages < nchunks) {
-        const int cp = c - 1, sp = cp % kGmStages;
-        mbar_wait(smem_u32(&bar_empty[sp]), (uint32_t)(cp / kGmStages) & 1, p.err);
-        load_w(cp + kGmStages);
+      wgmma_commit();
+      // retire the chunk's MMAs before the next chunk's (divergent) gather: no accumulator stays in flight there
+      wgmma_wait<0>();
+      mbar_arrive(smem_u32(&bar_empty[s]));                  // slot s may be refilled
+    }
+    // ------------------------------ epilogue from the accumulators -------------------------------
+    // thread t of the warpgroup holds rows r0 = acc_row(t, 0) and r0 + 8 of its 64, columns 8 j + 2 (t % 4) + {0, 1}
+    const int t = tid & 127;
+    const int ncols = min(p.nr, p.N - n0);
+    const bool pair_vec = (p.N & 1) == 0;                      // rows of out / residual / addend are 8-byte aligned
+    int mr[2];
+    bool ok[2];
+    float inv_a[2], rmax[2] = {0.f, 0.f};   // rmax: |out| of the row over this thread's columns
+    const float *rrow[2], *arow2[2];
+    float* orow[2];
+    unsigned* crow[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mr[h] = m0 + 64 * wg + acc_row(t, 2 * h);
+      ok[h] = mr[h] < p.M;
+      orow[h] = p.out ? p.out + (size_t)mr[h] * p.N + n0 : nullptr;
+      rrow[h] = p.residual ? p.residual + (size_t)mr[h] * p.N + n0 : nullptr;
+      arow2[h] = p.addend ? p.addend + (size_t)(mr[h] / p.addend_group) * p.N + n0 : nullptr;
+      crow[h] = p.colmax_out ? p.colmax_out + (size_t)(mr[h] / p.colmax_group) * p.N + n0 : nullptr;
+    }
+    {
+      // a row's dynamic scale was computed by its producer thread, which may sit in the other warpgroup
+      __shared__ float s_inv[128];
+      if (kh == 0) s_inv[row] = exp2i(-e_row);
+      __syncthreads();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) inv_a[h] = s_inv[64 * wg + acc_row(t, 2 * h)];
+    }
+    // max-pool over the rows of a group (PointNet): the 16 rows of a warp almost always belong to one group (68 points
+    // per face), so the warp reduces over its 8 row lanes first and issues ONE atomic per column instead of 16
+    // (the shuffle sits outside the && chain: every lane of the warp must execute it)
+    const int cgrp = __shfl_sync(0xffffffffu, p.colmax_out ? mr[0] / p.colmax_group : 0, 0);
+    const bool warp_one_group = p.colmax_out != nullptr &&
+        __all_sync(0xffffffffu, ok[0] && ok[1] && mr[0] / p.colmax_group == cgrp && mr[1] / p.colmax_group == cgrp);
+#pragma unroll
+    for (int i = 0; i < 128; i += 4) {
+      const int col = acc_col(t, i);
+      if (8 * (i >> 2) >= ncols) break;                        // warp-uniform: no column of this 8-column block is valid
+      const bool cv = col < ncols;                             // lanes differ: everything below stays convergent
+      float2 o[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float v0 = acc[i + 2 * h], v1 = acc[i + 2 * h + 1];
+        const bool one = cv && ok[h], two = col + 1 < ncols;
+        float x0 = cv ? fmaf(v0 * inv_a[h], s_osc[col], s_bias[col]) : 0.f;
+        float x1 = two ? fmaf(v1 * inv_a[h], s_osc[col + 1], s_bias[col + 1]) : 0.f;
+        if (one) {
+          if (arow2[h]) { x0 += arow2[h][col]; if (two) x1 += arow2[h][col + 1]; }
+          if (rrow[h]) { x0 += rrow[h][col]; if (two) x1 += rrow[h][col + 1]; }
+        }
+        if (p.act == kActRelu6) { x0 = relu6f(x0); x1 = relu6f(x1); }
+        else if (p.act == kActRelu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+        if (!two) x1 = 0.f;
+        if (one) {
+          rmax[h] = fmaxf(rmax[h], fmaxf(fabsf(x0), two ? fabsf(x1) : 0.f));
+          if (orow[h]) {
+            if (two && pair_vec) *reinterpret_cast<float2*>(orow[h] + col) = make_float2(x0, x1);
+            else { orow[h][col] = x0; if (two) orow[h][col + 1] = x1; }
+          }
+        }
+        o[h] = make_float2(x0, x1);
+      }
+      if (p.colmax_out != nullptr) {                           // o >= 0 (ReLU): the bit pattern orders like the value
+        if (warp_one_group) {
+          unsigned b0 = max(__float_as_uint(o[0].x), __float_as_uint(o[1].x));
+          unsigned b1 = max(__float_as_uint(o[0].y), __float_as_uint(o[1].y));
+#pragma unroll
+          for (int sh = 4; sh < 32; sh <<= 1) {               // the 8 row lanes sharing this column pair
+            b0 = max(b0, __shfl_xor_sync(0xffffffffu, b0, sh));
+            b1 = max(b1, __shfl_xor_sync(0xffffffffu, b1, sh));
+          }
+          if ((t & 31) < 4 && cv) {
+            atomicMax(crow[0] + col, b0);
+            if (col + 1 < ncols) atomicMax(crow[0] + col + 1, b1);
+          }
+        } else {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            if (ok[h] && cv) {
+              atomicMax(crow[h] + col, __float_as_uint(o[h].x));
+              if (col + 1 < ncols) atomicMax(crow[h] + col + 1, __float_as_uint(o[h].y));
+            }
+        }
       }
     }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == kGmProducerWarps) {
-    __syncwarp();
-    tmem_dealloc<256>(tmem);
+    if (p.rowmax_out != nullptr) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {                            // the 4 lanes of a row hold its column pairs
+        rmax[h] = fmaxf(rmax[h], __shfl_xor_sync(0xffffffffu, rmax[h], 1));
+        rmax[h] = fmaxf(rmax[h], __shfl_xor_sync(0xffffffffu, rmax[h], 2));
+        if ((t & 3) == 0 && ok[h]) atomicMax(p.rowmax_out + mr[h], __float_as_uint(rmax[h]));
+      }
+    }
   }
 }
 

@@ -1,14 +1,14 @@
-// Tail of the backbone on tcgen05: features[18] (1x1 conv 320 -> 1280 + BN + ReLU6) fused with the
+// Tail of the backbone on tensor cores (wgmma): features[18] (1x1 conv 320 -> 1280 + BN + ReLU6) fused with the
 // global average pool (reference backbone_nets/mobilenetv2_backbone.py:136,179-180), then the three
 // Linear heads (:147-158,184-188).  The 1280-channel map (82 KB/face) is never written to HBM.
 //
-// tail_conv_pool_kernel: transposed GEMM  D[ch, px] = W[ch, :] . X[px, :]  so that TMEM lanes are
-// output channels and the 16 pixels of a face are 16 adjacent accumulator columns: pooling is a
-// per-thread sum, no shuffles.  Weight-stationary: a CTA owns one 128-channel slice (its fp16 hi/lo
+// tail_conv_pool_kernel: transposed GEMM  D[ch, px] = W[ch, :] . X[px, :]  so that accumulator rows are
+// output channels and the 16 pixels of a face are 16 adjacent accumulator columns: pooling is a sum over
+// four values per thread and two shuffles.  Weight-stationary: a CTA owns one 128-channel slice (its fp16 hi/lo
 // weights, 160 KB, stay in smem) and walks over pixel tiles of 8 faces (128 px):
 //   warps 0-7   producers: fp32 NHWC rows -> fp16 hi/lo canonical B tiles, 2-stage ring (K chunks of 64)
-//   warps 8-11  epilogue:  TMEM -> relu6(s*v + b) -> mean over 16 px -> pooled (B,1280), coalesced
-//   warp 12     MMA issuer (split-16x3: 3 passes x 4 K-steps per chunk), 2 accumulator buffers
+//   warps 8-15  two MMA warpgroups, 64 channels each (split-16x3: 3 passes x 4 K-steps per chunk, accumulators
+//               in registers), then relu6(s*v + b) -> mean over 16 px -> pooled (B,1280)
 #pragma once
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -21,7 +21,7 @@ constexpr int kTailPlane = 128 * kTailKC * 2;                     // 16 KB: one 
 constexpr int kTailWBytes = kTailChunks * 2 * kTailPlane;         // 160 KB per 128-channel slice
 constexpr int kTailXStage = 2 * kTailPlane;                       // 32 KB
 constexpr int kTailSmem = kTailWBytes + 2 * kTailXStage + 1024;
-constexpr int kTailThreads = 13 * 32;
+constexpr int kTailThreads = 16 * 32;
 
 struct TailArgs {
   const float* x;        // (B,4,4,320) NHWC
@@ -38,8 +38,7 @@ struct TailArgs {
 __global__ void __launch_bounds__(kTailThreads, 1) tail_conv_pool_kernel(const TailArgs p) {
   using namespace tc;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_w, bar_xfull[2], bar_xempty[2], bar_dfull[2], bar_dfree[2];
-  __shared__ uint32_t tmem_base_s;
+  __shared__ __align__(8) uint64_t bar_w, bar_xfull[2], bar_xempty[2];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sW = smem;
   uint8_t* sX = smem + kTailWBytes;
@@ -53,17 +52,11 @@ __global__ void __launch_bounds__(kTailThreads, 1) tail_conv_pool_kernel(const T
     mbar_init(smem_u32(&bar_w), 1);
     for (int i = 0; i < 2; ++i) {
       mbar_init(smem_u32(&bar_xfull[i]), 256);
-      mbar_init(smem_u32(&bar_xempty[i]), 1);
-      mbar_init(smem_u32(&bar_dfull[i]), 1);
-      mbar_init(smem_u32(&bar_dfree[i]), 128);
+      mbar_init(smem_u32(&bar_xempty[i]), 256);          // every MMA thread, once its warpgroup's MMAs of the stage are done
     }
     fence_mbar_init();
   }
-  if (warp == 12) tmem_alloc<256>(smem_u32(&tmem_base_s));
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = tmem_base_s;
 
   if (warp < 8) {
     // ------------------------------ producers -----------------------------------------------------
@@ -98,78 +91,68 @@ __global__ void __launch_bounds__(kTailThreads, 1) tail_conv_pool_kernel(const T
         mbar_arrive(smem_u32(&bar_xfull[s]));
       }
     }
-  } else if (warp < 12) {
-    // ------------------------------ epilogue: pooling ---------------------------------------------
-    const int ch = slice * 128 + (tid & 127);
-    const float b = p.bias[ch], sc = p.oscale[ch];
+  } else {
+    // ------------------------------ MMA + pooling: warpgroup wg owns channels 64 wg .. 64 wg + 63 of the slice ----
+    const int t = tid & 127, wg = (tid >> 7) - 2;
+    if (warp == 8) {
+      if (elect_one()) {
+        mbar_expect_tx(smem_u32(&bar_w), kTailWBytes);
+        bulk_g2s(smem_u32(sW), p.wimg + (size_t)slice * kTailWBytes, kTailWBytes, smem_u32(&bar_w));
+      }
+      __syncwarp();
+    }
+    mbar_wait(smem_u32(&bar_w), 0, p.err);
+    float b[2], sc[2];
+    int ch[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      ch[h] = slice * 128 + 64 * wg + acc_row(t, 2 * h);
+      b[h] = p.bias[ch[h]];
+      sc[h] = p.oscale[ch[h]];
+    }
+    const uint32_t d_hi = smem_desc_hi(128);
+    const uint32_t w_lo = smem_desc_lo(smem_u32(sW) + wg * 1024, 2048), x_lo = smem_desc_lo(smem_u32(sX), 2048);
+    float acc[64];
+    uint32_t g = 0;
     for (int i = 0; i < my_tiles; ++i) {
       const int tile = pi + i * p.ctas_per_slice;
       const int f0 = tile * kTailFaces;
       const int nf = min(kTailFaces, p.batch - f0);
-      const int buf = i & 1;
-      mbar_wait(smem_u32(&bar_dfull[buf]), (i >> 1) & 1, p.err);
-      tc_fence_after_sync();
-#pragma unroll
-      for (int fp = 0; fp < kTailFaces / 2; ++fp) {        // two faces (32 columns) per TMEM load
-        float v[32];
-        tmem_ld32(tmem + ((uint32_t)((warp & 3) * 32) << 16) + buf * 128 + fp * 32, v);
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-          float s = 0.f;
-#pragma unroll
-          for (int j = 0; j < 16; ++j) s += relu6f(fmaf(v[hf * 16 + j], sc, b));
-          const int f = fp * 2 + hf;
-          if (f < nf) p.pooled[(size_t)(f0 + f) * kTailN + ch] = s * (1.0f / 16.0f);
-        }
-      }
-      tc_fence_before_sync();
-      mbar_arrive(smem_u32(&bar_dfree[buf]));
-    }
-  } else if (warp == 12) {
-    // ------------------------------ MMA issuer ----------------------------------------------------
-    // converged warp, MMA batches under one elect.sync with hoisted descriptors (a `tid == X` branch costs
-    // ~170 cycles per MMA against the 64-cycle operand-read floor of these M = N = 128 SS MMAs)
-    if (elect_one()) {
-      mbar_expect_tx(smem_u32(&bar_w), kTailWBytes);
-      bulk_g2s(smem_u32(sW), p.wimg + (size_t)slice * kTailWBytes, kTailWBytes, smem_u32(&bar_w));
-    }
-    __syncwarp();
-    mbar_wait(smem_u32(&bar_w), 0, p.err);
-    const uint32_t idesc = make_idesc_f16(128, 128);
-    const uint32_t d_hi = smem_desc_hi(128);
-    const uint32_t w_lo = smem_desc_lo(smem_u32(sW), 2048), x_lo = smem_desc_lo(smem_u32(sX), 2048);
-    uint32_t g = 0;
-    for (int i = 0; i < my_tiles; ++i) {
-      const int buf = i & 1;
-      mbar_wait(smem_u32(&bar_dfree[buf]), ((i >> 1) & 1) ^ 1, p.err);
-      tc_fence_after_sync();
       for (int kc = 0; kc < kTailChunks; ++kc, ++g) {
         const int s = g & 1;
         mbar_wait(smem_u32(&bar_xfull[s]), (g >> 1) & 1, p.err);
-        tc_fence_after_sync();
-        if (elect_one()) {
+        wgmma_fence();
 #pragma unroll
-          for (int pass = 0; pass < 3; ++pass) {
-            if (pass >= p.npass) break;
-            const uint32_t a_off = kc * 2 * kTailPlane + (pass == 2 ? kTailPlane : 0);   // W: hi,hi,lo
-            const uint32_t b_off = s * kTailXStage + (pass == 1 ? kTailPlane : 0);       // X: hi,lo,hi
+        for (int pass = 0; pass < 3; ++pass) {
+          if (pass >= p.npass) break;
+          const uint32_t a_off = kc * 2 * kTailPlane + (pass == 2 ? kTailPlane : 0);   // W: hi,hi,lo
+          const uint32_t b_off = s * kTailXStage + (pass == 1 ? kTailPlane : 0);       // X: hi,lo,hi
 #pragma unroll
-            for (int ks = 0; ks < kTailKC / 16; ++ks)
-              umma_f16(tmem + buf * 128, desc64(d_hi, w_lo + ((a_off + ks * 4096) >> 4)),
-                       desc64(d_hi, x_lo + ((b_off + ks * 4096) >> 4)), idesc, (kc > 0 || pass > 0 || ks > 0) ? 1u : 0u);
-          }
-          umma_commit(smem_u32(&bar_xempty[s]));
-          if (kc == kTailChunks - 1) umma_commit(smem_u32(&bar_dfull[buf]));
+          for (int ks = 0; ks < kTailKC / 16; ++ks)
+            wgmma_f16<128>(acc, desc64(d_hi, w_lo + ((a_off + ks * 4096) >> 4)),
+                           desc64(d_hi, x_lo + ((b_off + ks * 4096) >> 4)), (kc > 0 || pass > 0 || ks > 0) ? 1u : 0u);
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<0>();
+        mbar_arrive(smem_u32(&bar_xempty[s]));
+      }
+      // face f = accumulator columns 16f..16f+15 = values 8f..8f+7 of this thread (4 per row) and of the 3 other lanes
+      // of its quad
+#pragma unroll
+      for (int f = 0; f < kTailFaces; ++f) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float s = 0.f;
+#pragma unroll
+          for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) s += relu6f(fmaf(acc[(2 * f + jj) * 4 + 2 * h + e], sc[h], b[h]));
+          s += __shfl_xor_sync(0xffffffffu, s, 1);
+          s += __shfl_xor_sync(0xffffffffu, s, 2);
+          if ((t & 3) == 0 && f < nf) p.pooled[(size_t)(f0 + f) * kTailN + ch[h]] = s * (1.0f / 16.0f);
+        }
       }
     }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 12) {
-    __syncwarp();
-    tmem_dealloc<256>(tmem);
   }
 }
 

@@ -107,7 +107,10 @@ SYN_HD float ordered_float(uint32_t o) {
   c.u = (o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o;
   return c.f;
 }
-SYN_HD uint64_t depth_key(float depth, uint32_t tri) { return ((uint64_t)float_ordered(depth) << 32) | (uint64_t)(0xFFFFFFFFu - tri); }
+// -0 and +0 are one depth: the serial `>` test sees them as a tie, which the lower triangle index wins
+SYN_HD uint64_t depth_key(float depth, uint32_t tri) {
+  return ((uint64_t)float_ordered(depth == 0.0f ? 0.0f : depth) << 32) | (uint64_t)(0xFFFFFFFFu - tri);
+}
 SYN_HD uint32_t key_tri(uint64_t key) { return 0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull); }
 SYN_HD float key_depth(uint64_t key) { return ordered_float((uint32_t)(key >> 32)); }
 

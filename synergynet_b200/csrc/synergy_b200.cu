@@ -1,4 +1,4 @@
-// C-ABI implementation of the SynergyNet inference hot path for B200 (sm_100a).
+// C-ABI implementation of the SynergyNet inference hot path for H100 (sm_90a).
 // See include/synergy_b200.h for the contract and the reference lines each entry replaces.
 #include <math.h>
 #include <stdlib.h>
@@ -45,7 +45,7 @@ struct syn_handle {
   syn_heads* heads = nullptr;
   syn_resnet* resnet = nullptr;
   int sm_count = 0;
-  int engine = SYN_ENGINE_TC_FUSED;            // default: fused tcgen05 engine; 0/1 remain for cross-checks
+  int engine = SYN_ENGINE_TC_FUSED;            // default: fused tensor-core engine; 0/1 remain for cross-checks
   int center_crop = 0;                         // CenterCrop margin applied by the uint8 entry points (syn_set_center_crop)
   int npass() const { return engine == SYN_ENGINE_TC_FUSED_1PASS ? 1 : 3; }
   bool fused() const { return engine == SYN_ENGINE_TC_FUSED || engine == SYN_ENGINE_TC_FUSED_1PASS; }
@@ -345,7 +345,7 @@ int run_backbone(syn_handle* h, const float* x, int batch, float* params, float*
 }
 
 // Reconstruction kernels are launched with programmatic stream serialization: they start while dense_alpha_kernel
-// (which signals griddepcontrol.launch_dependents at its top) is still running, set up barriers / TMEM, stream in
+// (which signals griddepcontrol.launch_dependents at its top) is still running, set up barriers, stream in
 // basis data, and execute griddepcontrol.wait before the first access to the pre-pass' output.
 static cudaError_t launch_after_prepass(void (*kernel)(DenseArgs), int grid, int smem, cudaStream_t st, const DenseArgs& a) {
   cudaLaunchConfig_t cfg = {};
@@ -412,7 +412,7 @@ int run_reconstruct_tc(syn_handle* h, const float* params, int batch, int dense,
       cudaMemcpy(t.data(), a.trace, t.size() * sizeof(long long), cudaMemcpyDeviceToHost);
       if (FILE* f = fopen(trace_fp, "w")) {
         for (int r = 0; r < 192; ++r) {
-          fprintf(f, "%s %d", r < 64 ? "epi0" : r < 128 ? "epi1" : "issuer", r & 63);
+          fprintf(f, "%s %d", r < 64 ? "team0" : r < 128 ? "unused" : "loader", r & 63);
           for (int e = 0; e < 8; ++e) fprintf(f, " %lld", t[r * 8 + e]);
           fprintf(f, "\n");
         }
@@ -543,15 +543,16 @@ void pack_fused(std::vector<uint8_t>& img, const float* w1, int K, const float* 
   }
 }
 
-// Worker warps of the fused kernel: 16 by default (4 per SM sub-partition, measured best); SYN_FUSED_WARPS=8|12|16
-// selects another instantiation for tuning runs.
+// Worker warps of the fused kernel: 8 by default (H100, 1024-face step: 5.13 ms against 5.76 ms with 16, whose
+// 17-warp CTAs leave 96 registers per thread and spill); SYN_FUSED_WARPS=8|12|16 selects another instantiation for
+// tuning runs.
 inline int fused_worker_warps(int block) {
   static const struct Table {
     int v[18];
     Table() {
       const char* e = getenv("SYN_FUSED_WARPS");
-      const int n = e ? atoi(e) : 16;
-      const int all = (n == 8 || n == 12 || n == 16 || n == 20 || n == 24) ? n : 16;
+      const int n = e ? atoi(e) : 8;
+      const int all = (n == 8 || n == 12 || n == 16 || n == 20 || n == 24) ? n : 8;
       for (int i = 0; i < 18; ++i) v[i] = all;
       // per block: SYN_FUSED_WARPS_MAP="1:24,2:20" (tuning runs)
       const char* m = getenv("SYN_FUSED_WARPS_MAP");
@@ -578,8 +579,8 @@ int launch_fused_nww(syn_handle* h, const FusedArgs& a, int grid, cudaStream_t s
     if (getenv("SYN_DEBUG_OCC") != nullptr) {
       int nb = -1;
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fused_mbconv_kernel<C, NWW>, (NWW + 1) * 32, C::SMEM_BYTES);
-      fprintf(stderr, "[syn] fused CIN=%d CHID=%d W=%d: %d worker warps, %d B smem, %d TMEM cols -> %d CTA(s)/SM\n",
-              C::CIN, C::CHID, C::W, NWW, C::SMEM_BYTES, C::TM_COLS, nb);
+      fprintf(stderr, "[syn] fused CIN=%d CHID=%d W=%d: %d worker warps, %d B smem -> %d CTA(s)/SM\n",
+              C::CIN, C::CHID, C::W, NWW, C::SMEM_BYTES, nb);
     }
   }
 #if SYN_PDL
@@ -718,8 +719,8 @@ int syn_create(int device, syn_handle_t** out) {
   if (device < 0 || device >= ndev) return fail(SYN_ERR_INVALID, "syn_create: device %d of %d", device, ndev);
   cudaDeviceProp prop;
   SYN_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return fail(SYN_ERR_UNSUPPORTED, "syn_create: device %d is sm_%d%d; this library is built for sm_100a only",
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(SYN_ERR_UNSUPPORTED, "syn_create: device %d is sm_%d%d; this library is built for sm_90a only",
                 device, prop.major, prop.minor);
   DeviceGuard g(device);
   if (!g.ok) return fail(SYN_ERR_CUDA, "syn_create: cannot select device %d", device);
@@ -1094,7 +1095,7 @@ int syn_forward_landmarks_u8(syn_handle_t* h, const uint8_t* x_u8, int batch, fl
   return run_reconstruct(h, p, batch, 0, 1, 1, lmk, (cudaStream_t)stream);
 }
 
-// Faces per pipeline chunk: large enough that the 8x8 / 4x4 blocks still fill the 148 SMs, small enough that the copies
+// Faces per pipeline chunk: large enough that the 8x8 / 4x4 blocks still fill the 132 SMs, small enough that the copies
 // hide behind compute.  The FIRST chunk is small: its host->device copy is the only one nothing can overlap.
 // SYN_HOST_CHUNK / SYN_HOST_CHUNK0 override both for measurements.
 static int host_chunk_faces() {
@@ -1117,7 +1118,7 @@ static int host_first_chunk_faces() {
   static const int v = [] {
     const char* e = getenv("SYN_HOST_CHUNK0");
     const int c = e ? atoi(e) : 0;
-    return c > 0 ? c : 512;   // measured: [512, 512] beats [128, 448, 448] and [256, 448, 320] (round 2)
+    return c > 0 ? c : 512;
   }();
   return v;
 }
@@ -1132,8 +1133,8 @@ static int host_submit_impl(syn_handle_t* h, const void* x_host, int is_u8, int 
   DeviceGuard g(h->device);
   const unsigned long long seq = h->host_calls;
   if (seq >= 2) SYN_CUDA(cudaEventSynchronize(h->ev_call[seq & 1]));   // ticket seq - 2 owns this event: it must be done
-  // A blocking call can only overlap its own chunks (512 + 512 measured best); a submitted call overlaps with its
-  // neighbours in the queue, so it runs whole 1024-face launches (uint8: 409 K faces/s against 350 K with 512 + 512).
+  // A blocking call can only overlap its own chunks (512 + 512); a submitted call overlaps with its neighbours in the
+  // queue, so it runs whole 1024-face launches.
   const int chunk = std::min(batch, blocking ? host_chunk_faces() : host_submit_chunk_faces());
   const size_t x_face = (size_t)3 * kImg * kImg;
   const size_t elt = is_u8 ? 1 : sizeof(float);
@@ -1319,8 +1320,8 @@ int syn_debug_tile_plan(int batch, int sms, int faces_per_tile, int* split, int*
   switch (faces_per_tile) {     // one representative configuration per tile size
     case 1: fused_tile_plan<FusedB3>(batch, sms, *split, *face_groups); break;
     case 2: fused_tile_plan<FusedB8>(batch, sms, *split, *face_groups); break;
-    case 8: fused_tile_plan<FusedB15>(batch, sms, *split, *face_groups); break;
-    default: return fail(SYN_ERR_INVALID, "syn_debug_tile_plan: faces_per_tile must be 1, 2 or 8");
+    case 4: fused_tile_plan<FusedB15>(batch, sms, *split, *face_groups); break;
+    default: return fail(SYN_ERR_INVALID, "syn_debug_tile_plan: faces_per_tile must be 1, 2 or 4");
   }
   return SYN_OK;
 }

@@ -1,4 +1,4 @@
-"""FaceBoxes post-processing on the B200 (SURVEY.md section 8 row f3): prior boxes, box decode, score filter, ordering
+"""FaceBoxes post-processing on the H100 (SURVEY.md section 8 row f3): prior boxes, box decode, score filter, ordering
 and greedy NMS in ``libsynergy_b200.so`` (``csrc/kernels_detect.cuh``, NMS kernels in ``csrc/kernels_render.cuh``).
 
 Reference-shaped surface: :func:`nms` has the signature and return value of ``FaceBoxes/utils/nms_wrapper.py:13-18``
@@ -24,7 +24,7 @@ vis_thres = 0.5
 
 def _device():
     if not torch.cuda.is_available():
-        raise RuntimeError('synergynet_b200.detect needs a CUDA device (B200, sm_100a); there is no CPU fallback')
+        raise RuntimeError('synergynet_b200.detect needs a CUDA device (H100, sm_90a); there is no CPU fallback')
     return torch.device('cuda', torch.cuda.current_device())
 
 

@@ -1,4 +1,4 @@
-"""Per-device handle of the sm_100a library: weight hand-over and the compute entry points.
+"""Per-device handle of the sm_90a library: weight hand-over and the compute entry points.
 
 PyTorch is used for device memory, streams and (in bench.py) ``torch.distributed`` only; all
 arithmetic of the path runs in ``libsynergy_b200.so``.
@@ -31,7 +31,7 @@ class Engine:
     def __init__(self, device: int = 0):
         self._lib = _lib.load()
         if not torch.cuda.is_available():
-            raise RuntimeError('synergynet_b200 needs a CUDA device (B200, sm_100a); there is no '
+            raise RuntimeError('synergynet_b200 needs a CUDA device (H100, sm_90a); there is no '
                                'CPU fallback for the inference hot path')
         self.device = torch.device('cuda', int(device))
         h = C.c_void_p()

@@ -1,4 +1,4 @@
-"""The FaceBoxes detector on the B200 (SURVEY.md section 8 row f3): network, box decode and NMS all on the device.
+"""The FaceBoxes detector on the H100 (SURVEY.md section 8 row f3): network, box decode and NMS all on the device.
 
 Reference-shaped surface: :class:`FaceBoxes` has the constructor and call signature of ``FaceBoxes/FaceBoxes.py:46-143``
 (``FaceBoxes(timer_flag=False)``, ``face_boxes(img_bgr_uint8) -> [[xmin, ymin, xmax, ymax, score], ...]``) and loads the
@@ -53,7 +53,7 @@ class FaceBoxesNet:
     def __init__(self, state_dict: Dict[str, torch.Tensor], device=None):
         self._lib = _lib.load()
         if not torch.cuda.is_available():
-            raise RuntimeError('synergynet_b200.faceboxes needs a CUDA device (B200, sm_100a); there is no CPU fallback')
+            raise RuntimeError('synergynet_b200.faceboxes needs a CUDA device (H100, sm_90a); there is no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         h = C.c_void_p()
         _lib.check(self._lib.syn_fb_create(self.device.index or 0, C.byref(h)))

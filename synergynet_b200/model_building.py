@@ -2,7 +2,7 @@
 
 Same class names, constructor arguments, attributes, ``state_dict`` keys and method signatures
 (reference model_building.py:25-32,35-62,65-165,169-306); the arithmetic of ``forward_test`` and
-``reconstruct_vertex_62`` runs in the sm_100a library through ``Engine`` -- no torch conv/matmul is
+``reconstruct_vertex_62`` runs in the sm_90a library through ``Engine`` -- no torch conv/matmul is
 executed on the product path and nothing falls back to the CPU.
 """
 from __future__ import annotations
@@ -41,7 +41,7 @@ class _Runtime:
         self._sig: Dict[int, tuple] = {}
         self._pn_sig: Dict[tuple, tuple] = {}
         self._lock = threading.RLock()
-        self.engine_kind = None      # None: the library default (fused tcgen05 engine)
+        self.engine_kind = None      # None: the library default (fused tensor-core engine)
 
     @staticmethod
     def _signature(tensors) -> tuple:
@@ -51,7 +51,7 @@ class _Runtime:
             basis: Optional[Callable[[], Dict[str, torch.Tensor]]]) -> Engine:
         if device.type != 'cuda':
             raise RuntimeError('synergynet_b200: the forward pass needs inputs on a CUDA device '
-                               '(B200); there is no CPU fallback')
+                               '(H100); there is no CPU fallback')
         idx = device.index if device.index is not None else torch.cuda.current_device()
         sd = backbone_sd()
         bs = basis() if basis is not None else {}
@@ -103,7 +103,7 @@ class I2P(nn.Module):
             # avgpool = the 2048-d pooled feature.
             self.backbone = mobilenetv2_backbone.resnet50(pretrained=False)
         elif any(k in self.args.arch for k in ('mobilenet', 'resnet', 'ghostnet', 'resnest')):
-            raise RuntimeError(f"arch '{args.arch}': mobilenet_v2 and resnet50 are built for sm_100a "
+            raise RuntimeError(f"arch '{args.arch}': mobilenet_v2 and resnet50 are built for sm_90a "
                                '(SURVEY.md section 8; the other backbones are not on the hot path)')
         else:
             raise RuntimeError("Please choose [mobilenet_v2, mobilenet_1, resnet50, or ghostnet]")
@@ -147,7 +147,7 @@ class I2P(nn.Module):
         if w.is_cuda:
             return w.device
         if not torch.cuda.is_available():
-            raise RuntimeError('synergynet_b200: no CUDA device (B200) visible; there is no CPU fallback')
+            raise RuntimeError('synergynet_b200: no CUDA device (H100) visible; there is no CPU fallback')
         return torch.device('cuda', torch.cuda.current_device())
 
     def forward_test(self, input):
@@ -212,7 +212,7 @@ class _SynergyBase(nn.Module):
         return self.I2P._engine(device)
 
     def set_engine(self, kind: int) -> None:
-        """0 = fp32 CUDA-core engine, 1 = tcgen05 split-fp16 engine (unfused), 2 = fused tcgen05 engine (default);
+        """0 = fp32 CUDA-core engine, 1 = wgmma split-fp16 engine (unfused), 2 = fused wgmma engine (default);
         see include/synergy_b200.h."""
         for eng in self.I2P._rt._engines.values():
             eng.set_engine(int(kind))
@@ -236,7 +236,7 @@ class _SynergyBase(nn.Module):
         if self.param_mean.is_cuda:
             return self.param_mean.device
         if not torch.cuda.is_available():
-            raise RuntimeError('synergynet_b200: no CUDA device (B200) visible; there is no CPU fallback')
+            raise RuntimeError('synergynet_b200: no CUDA device (H100) visible; there is no CPU fallback')
         return torch.device('cuda', torch.cuda.current_device())
 
     def forward_test(self, input):

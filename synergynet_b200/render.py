@@ -1,4 +1,4 @@
-"""``utils/render.py`` of the reference on the B200: ``render(img, ver_lst, alpha, wfp, tex, connectivity)`` with the
+"""``utils/render.py`` of the reference on the H100: ``render(img, ver_lst, alpha, wfp, tex, connectivity)`` with the
 reference's signature and return value (utils/render.py:31-53).  The triangle list comes from the same place as the
 reference's (``3dmm_data/tri.mat`` through the parameter pack, 1-based in the file) unless ``connectivity`` is given; the
 per-face loop :41-45 is one batched call of :func:`synergynet_b200.Sim3DR.render` (normals, lighting, z-buffer on the

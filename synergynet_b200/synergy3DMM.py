@@ -2,7 +2,7 @@
 (reference synergy3DMM.py:70-207): no-argument constructor, MobileNetV2 fixed, weights looked up
 in ``pretrained/best.pth.tar`` next to the package (load errors swallowed like the reference,
 :109-113), ``.eval()``; ``forward_test`` / ``reconstruct_vertex_62`` / ``get_all_outputs`` run on
-the sm_100a library."""
+the sm_90a library."""
 from __future__ import annotations
 
 import os

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Generate ``tests/golden/ref_vectors.npz`` by running the UNMODIFIED reference.
+"""Generate the golden vectors (``tests/golden/ref_vectors*.npz``, split by ``vectors.py``) by running the UNMODIFIED
+reference.
 
 Run in the build container only (needs /root/reference):
 
@@ -186,9 +187,9 @@ def main():
     out['meta'] = np.array([f'torch={torch.__version__}', f'numpy={np.__version__}',
                             'reference=choyingw/SynergyNet@9de11e2', 'seed=0',
                             f'dense_stride={DENSE_STRIDE}', f'feat_stride={FEAT_STRIDE}'])
-    dst = os.path.join(ROOT, 'tests', 'golden', 'ref_vectors.npz')
-    np.savez_compressed(dst, **out)
-    print('wrote', dst, os.path.getsize(dst) // 1024, 'KiB;', len(out), 'arrays')
+    from vectors import save_ref_vectors      # this script's directory is on sys.path
+    save_ref_vectors(out)
+    print('wrote', len(out), 'arrays to tests/golden/ref_vectors*.npz')
     print('params[0,:6]', params[0, :6].numpy(), 'lmk range', float(lmk.min()), float(lmk.max()))
 
 

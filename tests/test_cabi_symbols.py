@@ -56,7 +56,7 @@ def test_fused_tile_plan_covers_every_face_once():
                 assert singles <= sms                       # the split tail is one wave
             else:
                 assert singles == (batch & 1)
-            for fpt in (1, 8):
+            for fpt in (1, 4):
                 s1, g1 = _plan(lib, batch, sms, fpt)
                 assert s1 == 0 and g1 == (batch + fpt - 1) // fpt
     assert lib.syn_debug_tile_plan(0, 148, 2, None, None) == 1

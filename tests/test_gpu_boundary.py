@@ -2,7 +2,7 @@
 benchmark.py:111-132 (DataParallel wrap + `module.`-prefixed checkpoint + `model.module.forward_test`) followed by
 benchmark.py:76-97 (`reconstruct_vertex(param, model.module.data_param)`), singleImage.py:28-37 (state-dict
 merge), the no-argument CPU-constructed wrapper of synergy3DMM.py:71-114, plus the error / saturation flags and
-the single-pass engine.  B200 only."""
+the single-pass engine.  H100 only."""
 import threading
 import types
 import warnings
@@ -113,7 +113,8 @@ def test_cpu_constructed_wrapper_runs_like_the_reference(synth_pack, sd, basis):
     lmk = model.reconstruct_vertex_62(params)
     assert not lmk.is_cuda
     assert rp.max_rel_err(lmk.numpy(), rp.reconstruct_vertex_62(want.numpy(), basis)) < TOL
-    gold = dict(np.load(__import__('os').path.join(__import__('os').path.dirname(__file__), 'golden', 'ref_vectors.npz')))
+    from golden.vectors import load_ref_vectors
+    gold = load_ref_vectors()
     rects = [list(r) for r in gold['scene_rects']]
     pts, verts, poses = model.get_all_outputs(gold['scene'].copy(), rects=rects)
     assert rp.max_rel_err(np.stack(pts), gold['scene_lmk']) < TOL

@@ -1,4 +1,4 @@
-"""The FaceBoxes detector on the B200 (SURVEY.md section 8 row f3) against the vectors recorded from the reference's own
+"""The FaceBoxes detector on the H100 (SURVEY.md section 8 row f3) against the vectors recorded from the reference's own
 network class (seeded synthetic checkpoint, tests/golden/make_golden_render.py) and against the CPU oracle."""
 import os
 

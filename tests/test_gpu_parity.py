@@ -1,5 +1,5 @@
-"""Parity of the sm_100a library against the CPU oracle and the reference's golden vectors.
-All calls go through the C ABI (ctypes) via the reference-shaped Python API.  B200 only."""
+"""Parity of the sm_90a library against the CPU oracle and the reference's golden vectors.
+All calls go through the C ABI (ctypes) via the reference-shaped Python API.  H100 only."""
 import os
 import types
 
@@ -14,7 +14,6 @@ from synergynet_b200.backbone import conv_plan
 
 pytestmark = pytest.mark.gpu
 
-GOLD = os.path.join(os.path.dirname(__file__), 'golden', 'ref_vectors.npz')
 TOL = 1e-4            # north_star: 1e-4 relative fp32 on params / landmarks / vertices
 # Intermediate activations are a diagnostic, not a north_star output: the calibrated synthetic network amplifies fp32
 # ordering noise to ~3e-5 per layer already (engine 0 vs the oneDNN oracle); the split-fp16 tensor-core engines measure
@@ -35,7 +34,8 @@ def _engine_available(model, kind):
 
 @pytest.fixture(scope='module')
 def gold():
-    return dict(np.load(GOLD, allow_pickle=False))
+    from golden.vectors import load_ref_vectors
+    return load_ref_vectors()
 
 
 @pytest.fixture(scope='module')

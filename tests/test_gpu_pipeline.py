@@ -1,4 +1,4 @@
-"""The reference's single-image flow (singleImage.py / utils/render.py) through the B200 modules end to end: detector ->
+"""The reference's single-image flow (singleImage.py / utils/render.py) through the H100 modules end to end: detector ->
 crops -> backbone -> landmarks, dense meshes, poses -> solid-mesh overlay, every stage on the device and chained without
 host copies where the reference hands numpy arrays around."""
 import types

@@ -1,4 +1,4 @@
-"""Parity of the Sim3DR and FaceBoxes post-processing kernels (SURVEY.md section 8 rows f2, f3) on the B200, through the
+"""Parity of the Sim3DR and FaceBoxes post-processing kernels (SURVEY.md section 8 rows f2, f3) on the H100, through the
 C ABI: bit-exact against the C oracle and the golden vectors recorded from the reference for normals, rasterisation and
 NMS index lists; lighting and box decode to the tolerance their one non-reproducible library call (pow / exp) allows."""
 import os
@@ -83,6 +83,21 @@ def test_rasterize_ties_large_and_degenerate_triangles(dev):
     img = torch.from_numpy(bg.copy()).to(dev)
     _, depth = r.rasterize(img, torch.from_numpy(ver).to(dev)[None], torch.from_numpy(col).to(dev)[None], return_depth=True)
     assert np.array_equal(img.cpu().numpy(), want) and np.array_equal(depth[0].cpu().numpy(), dwant)
+
+
+def test_rasterize_signed_zero_depth_tie(dev):
+    """Coplanar copies of one triangle at depth -0 and then +0 tie in the reference's serial `>`: the first one stays."""
+    xy = [[2, 2], [30, 3], [6, 25]]
+    ver = np.array([p + [-0.0] for p in xy] + [p + [0.0] for p in xy], np.float32)
+    tri = np.array([[0, 1, 2], [3, 4, 5]], np.int32)
+    col = np.array([[0.9, 0.1, 0.1]] * 3 + [[0.1, 0.1, 0.9]] * 3, np.float32)
+    bg = np.zeros((32, 32, 3), np.uint8)
+    want, dwant = rp.rasterize(ver, tri, col, bg.copy(), return_depth=True)
+    r = Sim3DR.MeshRenderer(tri, 6, dev)
+    img = torch.from_numpy(bg.copy()).to(dev)
+    _, depth = r.rasterize(img, torch.from_numpy(ver).to(dev)[None], torch.from_numpy(col).to(dev)[None], return_depth=True)
+    assert (want[..., 0] == 229).any() and np.array_equal(img.cpu().numpy(), want)
+    assert np.array_equal(depth[0].cpu().numpy(), dwant)
 
 
 def test_pipeline_reference_shaped_api(gold):

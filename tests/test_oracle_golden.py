@@ -10,13 +10,13 @@ from oracle import reference_port as rp
 from oracle import synth_model
 from synergynet_b200 import synthetic
 
-GOLD = os.path.join(os.path.dirname(__file__), 'golden', 'ref_vectors.npz')
 TOL = 2e-5       # oracle and reference run the same ATen kernels; slack is for cross-host ISA paths
 
 
 @pytest.fixture(scope='module')
 def gold():
-    return dict(np.load(GOLD, allow_pickle=False))
+    from golden.vectors import load_ref_vectors
+    return load_ref_vectors()
 
 
 @pytest.fixture(scope='module')

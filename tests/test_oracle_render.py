@@ -1,6 +1,6 @@
 """Pin the render / detection oracle (oracle/render_port.py, oracle/sim3dr_port.c) to the vectors recorded from the live
-reference (tests/golden/make_golden_render.py) and, where it has been built, to the reference's own C++ compiled in place
-(oracle/_ref/libsim3dr_ref.so).  CPU only."""
+reference (tests/golden/make_golden_render.py) and from the reference's own Sim3DR C++ compiled by oracle/Makefile
+(tests/golden/make_golden_sim3dr_ref.py).  CPU only."""
 import os
 
 import numpy as np
@@ -10,6 +10,7 @@ from oracle import render_port as rp
 from synergynet_b200 import synthetic
 
 GOLD = os.path.join(os.path.dirname(__file__), 'golden', 'render_vectors.npz')
+REF_GOLD = os.path.join(os.path.dirname(__file__), 'golden', 'sim3dr_ref_vectors.npz')
 LIGHT_TOL = 2e-7      # absolute, on light in [0,1]: numpy's float32 pow differs by an ulp between hosts (SVML or libm)
 
 
@@ -54,24 +55,21 @@ def test_pipeline_sequence(gold):
         assert np.array_equal(img, gold['render_steps'][b])
 
 
-@pytest.mark.skipif(not rp.have_ref(), reason='oracle/_ref not built (no /root/reference on this host)')
 def test_port_equals_compiled_reference():
-    tri = synthetic.make_render_topology(60, 70)
-    verts = synthetic.make_render_meshes(2, 200, 240, seed=5, rows=60, cols=70, size=120)
-    rng = np.random.default_rng(3)
-    # a few huge and degenerate triangles on top of the mesh
-    extra = np.array([[0, 4199, 2100], [10, 10, 500], [69, 4130, 35]], np.int32)
-    tri = np.ascontiguousarray(np.concatenate([tri, extra]))
-    for b in range(2):
-        ver = np.ascontiguousarray(verts[b].T)
-        n_p, n_r = rp.get_normal(ver, tri, 'port'), rp.get_normal(ver, tri, 'ref')
-        assert np.array_equal(n_p, n_r, equal_nan=True)
-        col = rng.uniform(0, 1, ver.shape).astype(np.float32)
-        bg = rng.integers(0, 256, (200, 240, 3), dtype=np.uint8)
-        for rev in (False, True):
-            a, da = rp.rasterize(ver, tri, col, bg.copy(), reverse=rev, kind='port', return_depth=True)
-            r, dr = rp.rasterize(ver, tri, col, bg.copy(), reverse=rev, kind='ref', return_depth=True)
-            assert np.array_equal(a, r) and np.array_equal(da, dr)
+    """The C restatement against the reference's own rasterize_kernel.cpp, recorded on these inputs by
+    tests/golden/make_golden_sim3dr_ref.py (normals, depth buffer and image bit for bit; ties, huge and degenerate
+    triangles included)."""
+    from golden.make_golden_sim3dr_ref import drawn_pixels, inputs
+    ref = np.load(REF_GOLD, allow_pickle=False)
+    tri, per_mesh = inputs()
+    for b, (ver, col, bg) in enumerate(per_mesh):
+        assert np.array_equal(rp.get_normal(ver, tri, 'port'), ref[f'normals_{b}'], equal_nan=True)
+        for rev in (0, 1):
+            img, depth = rp.rasterize(ver, tri, col, bg.copy(), reverse=bool(rev), kind='port', return_depth=True)
+            assert np.array_equal(depth, ref[f'depth_{b}_{rev}'])
+            drawn = drawn_pixels(ref[f'depth_{b}_{rev}'], rev)
+            assert drawn.any() and np.array_equal(img[drawn], ref[f'pixels_{b}_{rev}'])
+            assert np.array_equal(img[~drawn], bg[~drawn])
 
 
 def test_prior_boxes_bit_exact(gold):

@@ -131,6 +131,23 @@ def test_rasterize_ties_and_large_triangles(emul):
     assert (want != 17).any()
 
 
+def test_rasterize_signed_zero_depth_tie(emul):
+    """Two coplanar copies of one triangle at depth -0 and then +0: the reference's serial `>` sees a tie, so the FIRST
+    triangle's colour stays, whatever order the order-free key processes them in."""
+    xy = [[2, 2], [30, 3], [6, 25]]
+    ver = np.array([p + [-0.0] for p in xy] + [p + [0.0] for p in xy], np.float32)
+    tri = np.array([[0, 1, 2], [3, 4, 5]], np.int32)
+    col = np.array([[0.9, 0.1, 0.1]] * 3 + [[0.1, 0.1, 0.9]] * 3, np.float32)
+    bg = np.zeros((32, 32, 3), np.uint8)
+    want, dwant = rp.rasterize(ver, tri, col, bg.copy(), return_depth=True)
+    assert (want[..., 0] == 229).any() and not (want[..., 2] == 229).any()    # the reference keeps the first triangle
+    for shuffle in (0, 1):
+        img = bg.copy()
+        depth = np.zeros((1, 32, 32), np.float32)
+        emul.emul_rasterize(P(img), 32, 32, 3, P(ver), C.c_longlong(0), 3, 1, 1, 6, P(tri), 2, P(col), C.c_float(1.0), 0, P(depth), shuffle)
+        assert np.array_equal(img, want) and np.array_equal(depth[0], dwant)
+
+
 def test_nms_bitmatrix_equals_greedy(emul, gold):
     d = gold['nms_dets']
     order = d[:, 4].argsort()[::-1]
