@@ -254,6 +254,30 @@ int syn_faceboxes_decode(const float* loc_dev, const float* conf_dev, int im_hei
                          float box_scale_h, float scale, float conf_thresh, int top_k, int32_t* cand_ws_dev, float* dets_dev,
                          int32_t* n_dets_dev, void* stream);
 
+/* ---- crop + resize of uint8 BGR images (crop_img + cv2.resize) ---------------------------------------------------------
+ * The face crops of get_all_outputs (utils/inference.py:95-125 crop_img, then cv2.resize to 120x120: INTER_LANCZOS4 in
+ * synergy3DMM.py:187-188 / model_building.py:286-287, INTER_LINEAR in singleImage.py:76-77 / artistic.py:95) and the
+ * detector's shrink of oversized images (FaceBoxes/FaceBoxes.py:62-79, cv2.resize's default INTER_LINEAR; ROI = the whole
+ * image).  The output is OpenCV's, byte for byte, including the fast 2x2 area path INTER_LINEAR takes for an exact
+ * halving (csrc/resize_math.h states the arithmetic).  Handle-free, in two steps like syn_mesh_incidence_host +
+ * syn_mesh_normals: the host planner turns rois_host (B,4) int32 x0, y0, x1, y1 (crop_img's int(round(v)), may reach
+ * outside the image: crop pixels there are 0) into one plan buffer of syn_crop_resize_plan_size bytes (-1 on bad
+ * arguments) with the per-axis tap tables; the caller uploads it and syn_crop_resize reads image_dev (height,width,3)
+ * uint8 and writes B outputs of out_h x out_w x 3 through element strides: channel c of pixel (y, x) of ROI b is
+ * out_dev[b*stride_roi + y*stride_y + x*stride_x + c*stride_c] -- (3*h*w, w, 1, h*w) for planar (B,3,h,w) crops, (0, 3*w,
+ * 3, 1) for one interleaved (h,w,3) image.  batch, out_h, out_w and mode must be the ones the plan was built with.
+ * Empty ROIs are SYN_ERR_SHAPE, sizes < 1 SYN_ERR_INVALID, channels != 3 and other modes SYN_ERR_UNSUPPORTED. */
+enum {
+  SYN_INTER_LINEAR = 1,    /* cv::INTER_LINEAR   */
+  SYN_INTER_LANCZOS4 = 4   /* cv::INTER_LANCZOS4 */
+};
+int64_t syn_crop_resize_plan_size(int batch, int out_h, int out_w, int mode);
+int syn_crop_resize_plan_host(const int32_t* rois_host, int batch, int out_h, int out_w, int mode, void* plan_out,
+                              int64_t plan_bytes);
+int syn_crop_resize(const uint8_t* image_dev, int height, int width, int channels, const void* plan_dev, int batch, int out_h,
+                    int out_w, int mode, uint8_t* out_dev, int64_t stride_roi, int64_t stride_y, int64_t stride_x, int64_t stride_c,
+                    void* stream);
+
 /* The detector network (FaceBoxes/models/faceboxes.py:68-150, FaceBoxesNet in 'test' phase) on ONE image of any size.
  * A separate handle: the detector has its own weights and workspace and does not touch syn_handle_t.  Like syn_handle_t
  * it is bound to one device and is not re-entrant (its activation workspace is shared by consecutive calls, which are

@@ -38,6 +38,12 @@ def main():
     eng.reconstruct_image(params, roi5, dense=True)
     eng.reconstruct_image(params, roi5, dense=False)
     eng.pose_decode(params, roi5)
+    img = torch.from_numpy(synthetic.make_scene_u8(64, 96, 0)).to(dev)         # crop + resize: boxes over every image edge
+    boxes = [[-10, -5, 50, 55], [40, 20, 100, 80], [90, 60, 130, 100], [-40, -40, -20, -20]]
+    for mode in (inference.INTER_LINEAR, inference.INTER_LANCZOS4):
+        inference.crop_resize_device(img, boxes, (120, 120), mode)
+        inference.crop_resize_device(img, boxes, (37, 29), mode, planar=False)
+    inference.crop_resize_device(img, [[0, 0, 96, 64]], (48, 32), inference.INTER_LINEAR, planar=False)   # 2x2 area path
     loss = m(x, params + 0.1)
     torch.cuda.synchronize()
     rn = model_building.SynergyNet(types.SimpleNamespace(arch='resnet50', img_size=120, devices_id=[0]))

@@ -90,6 +90,9 @@ SIGNATURES = {
     'syn_mesh_lighting': (_I, [_F, _L, _I, _I, _I, _I, _F, C.POINTER(LightCfg), _F, _F, _F, _P]),
     'syn_rasterize': (_I, [_F, _I, _I, _I, _F, _L, _I, _I, _I, _I, _F, _I, _F, C.c_float, _I, _F, _F, _P]),
     'syn_nms': (_I, [_F, _I, C.c_double, _I, _F, _F, _F, _P]),
+    'syn_crop_resize_plan_size': (_L, [_I, _I, _I, _I]),
+    'syn_crop_resize_plan_host': (_I, [_P, _I, _I, _I, _I, _P, _L]),
+    'syn_crop_resize': (_I, [_P, _I, _I, _I, _P, _I, _I, _I, _I, _P, _L, _L, _L, _L, _P]),
     'syn_faceboxes_num_priors': (_I, [_I, _I]),
     'syn_fb_num_layers': (_I, []),
     'syn_fb_layer_desc': (_I, [_I, C.POINTER(FbLayerDesc)]),
@@ -117,6 +120,7 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_param_loss', 'syn_reconstruct_image', 'syn_pose_decode', 'syn_set_center_crop', 'syn_resnet_num_convs', 'syn_resnet_conv_desc',
                                              'syn_resnet_set_conv', 'syn_resnet_set_heads', 'syn_resnet_commit', 'syn_resnet50_forward', 'syn_debug_heads_buffer',
                                              'syn_mesh_incidence_host', 'syn_mesh_normals', 'syn_mesh_lighting', 'syn_rasterize', 'syn_nms',
+                                             'syn_crop_resize_plan_size', 'syn_crop_resize_plan_host', 'syn_crop_resize',
                                              'syn_faceboxes_num_priors', 'syn_faceboxes_decode', 'syn_fb_num_layers', 'syn_fb_layer_desc', 'syn_fb_create',
                                              'syn_fb_destroy', 'syn_fb_set_layer', 'syn_fb_commit', 'syn_fb_forward', 'syn_fb_launch_count')}
 

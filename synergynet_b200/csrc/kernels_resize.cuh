@@ -1,0 +1,34 @@
+// ROI crop + resize of uint8 BGR images on the GPU: crop_img followed by cv2.resize (synergy3DMM.py:186-188,
+// model_building.py:285-287, singleImage.py:76-77; the detector's shrink, FaceBoxes/FaceBoxes.py:62-79), bit-exact with
+// OpenCV.  The arithmetic and the plan layout are resize_math.h's; this file only maps threads onto output pixels.
+//
+// One thread per output pixel (all three channels), one grid z-slice per ROI: 8 x 8 source taps for Lanczos4, 2 x 2 for
+// linear, read straight from the image (the taps of neighbouring threads overlap, so L1 serves most of them).  The work
+// is small (16 Lanczos4 faces at 120 x 120 are ~44 M integer multiply-adds); the tables sit in the plan buffer the host
+// built, so the device computes no transcendental function.
+#pragma once
+#include "common.cuh"
+#include "resize_math.h"
+
+namespace syn {
+
+constexpr int kResizeBX = 32, kResizeBY = 8;
+
+// out[b*sb + oy*sy + ox*sx + c*sc] (element strides): planar (B,3,h,w) crops or an interleaved (h,w,3) image
+template <int K>
+__global__ void __launch_bounds__(kResizeBX * kResizeBY) crop_resize_kernel(const uint8_t* __restrict__ img, int height, int width,
+                                                                            const void* __restrict__ plan, int batch, int out_h,
+                                                                            int out_w, uint8_t* __restrict__ out, long long sb,
+                                                                            long long sy, long long sx, long long sc) {
+  const int ox = blockIdx.x * kResizeBX + threadIdx.x, oy = blockIdx.y * kResizeBY + threadIdx.y, b = blockIdx.z;
+  if (ox >= out_w || oy >= out_h) return;
+  const rsz::PlanView v = rsz::plan_view(plan, batch, out_h, out_w, K);
+  uint8_t px[3];
+  rsz::resize_pixel<K>(img, height, width, v, b, out_h, out_w, oy, ox, px);
+  uint8_t* o = out + b * sb + oy * sy + ox * sx;
+  o[0] = px[0];
+  o[sc] = px[1];
+  o[2 * sc] = px[2];
+}
+
+}  // namespace syn

@@ -1,8 +1,10 @@
 // C ABI of the stages either side of the 3DMM path (SURVEY.md section 8 rows f2, f3): Sim3DR normals / lighting /
-// rasterisation of the dense meshes, and the FaceBoxes box decode + greedy NMS that produces the crops.
+// rasterisation of the dense meshes, the FaceBoxes box decode + greedy NMS that produces the crops, and the crop + resize
+// that turns boxes (or an oversized detector input) into network inputs.
 // Handle-free: device pointers and workspaces belong to the caller (include/synergy_b200.h states the sizes).
 #include "kernels_render.cuh"
 #include "kernels_detect.cuh"
+#include "kernels_resize.cuh"
 
 #include <cmath>
 #include <new>
@@ -120,6 +122,51 @@ int syn_nms(const float* dets_dev, int n, double thresh, int mode, uint64_t* mas
     SYN_CUDA(cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, words * 8));
   nms_scan_kernel<<<1, kNmsScanThreads, words * 8, st>>>(reinterpret_cast<const unsigned long long*>(mask_ws_dev), n, keep_dev, n_keep_dev);
   SYN_LAUNCH_CHECK("nms_scan_kernel");
+  return SYN_OK;
+}
+
+int64_t syn_crop_resize_plan_size(int batch, int out_h, int out_w, int mode) {
+  if (batch <= 0 || out_h <= 0 || out_w <= 0 || (mode != SYN_INTER_LINEAR && mode != SYN_INTER_LANCZOS4)) return -1;
+  return rsz::plan_bytes(batch, out_h, out_w, rsz::taps_of(mode));
+}
+
+int syn_crop_resize_plan_host(const int32_t* rois_host, int batch, int out_h, int out_w, int mode, void* plan_out,
+                              int64_t plan_bytes) {
+  if (!rois_host || !plan_out || batch <= 0) return fail(SYN_ERR_INVALID, "syn_crop_resize_plan_host: null pointer or empty batch");
+  if (out_h < 1 || out_w < 1) return fail(SYN_ERR_INVALID, "syn_crop_resize_plan_host: output size %dx%d", out_h, out_w);
+  if (mode != SYN_INTER_LINEAR && mode != SYN_INTER_LANCZOS4)
+    return fail(SYN_ERR_UNSUPPORTED, "syn_crop_resize_plan_host: interpolation %d (only INTER_LINEAR = 1 and INTER_LANCZOS4 = 4)", mode);
+  for (int b = 0; b < batch; ++b) {
+    const int32_t* r = rois_host + 4 * b;
+    if (r[2] <= r[0] || r[3] <= r[1])        // crop_img would return an empty array, which cv2.resize rejects
+      return fail(SYN_ERR_SHAPE, "syn_crop_resize_plan_host: ROI %d (%d,%d,%d,%d) is empty", b, r[0], r[1], r[2], r[3]);
+  }
+  if (plan_bytes < syn_crop_resize_plan_size(batch, out_h, out_w, mode))
+    return fail(SYN_ERR_SHAPE, "syn_crop_resize_plan_host: plan buffer of %lld bytes, %lld needed", (long long)plan_bytes,
+                (long long)syn_crop_resize_plan_size(batch, out_h, out_w, mode));
+  rsz::build_plan(rois_host, batch, out_h, out_w, mode, plan_out);
+  return SYN_OK;
+}
+
+int syn_crop_resize(const uint8_t* image_dev, int height, int width, int channels, const void* plan_dev, int batch, int out_h,
+                    int out_w, int mode, uint8_t* out_dev, int64_t stride_roi, int64_t stride_y, int64_t stride_x, int64_t stride_c,
+                    void* stream) {
+  if (!image_dev || !plan_dev || !out_dev || batch <= 0) return fail(SYN_ERR_INVALID, "syn_crop_resize: null pointer or empty batch");
+  if (height < 1 || width < 1 || out_h < 1 || out_w < 1)
+    return fail(SYN_ERR_INVALID, "syn_crop_resize: image %dx%d, output %dx%d", height, width, out_h, out_w);
+  if (channels != 3) return fail(SYN_ERR_UNSUPPORTED, "syn_crop_resize: %d channels (BGR images only)", channels);
+  if (mode != SYN_INTER_LINEAR && mode != SYN_INTER_LANCZOS4)
+    return fail(SYN_ERR_UNSUPPORTED, "syn_crop_resize: interpolation %d (only INTER_LINEAR = 1 and INTER_LANCZOS4 = 4)", mode);
+  if (batch > 65535) return fail(SYN_ERR_SHAPE, "syn_crop_resize: %d ROIs exceed one launch's grid", batch);
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid((out_w + kResizeBX - 1) / kResizeBX, (out_h + kResizeBY - 1) / kResizeBY, batch), block(kResizeBX, kResizeBY);
+  if (mode == SYN_INTER_LANCZOS4)
+    crop_resize_kernel<8><<<grid, block, 0, st>>>(image_dev, height, width, plan_dev, batch, out_h, out_w, out_dev, stride_roi,
+                                                  stride_y, stride_x, stride_c);
+  else
+    crop_resize_kernel<2><<<grid, block, 0, st>>>(image_dev, height, width, plan_dev, batch, out_h, out_w, out_dev, stride_roi,
+                                                  stride_y, stride_x, stride_c);
+  SYN_LAUNCH_CHECK("crop_resize_kernel");
   return SYN_OK;
 }
 

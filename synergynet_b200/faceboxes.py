@@ -4,8 +4,9 @@ Reference-shaped surface: :class:`FaceBoxes` has the constructor and call signat
 (``FaceBoxes(timer_flag=False)``, ``face_boxes(img_bgr_uint8) -> [[xmin, ymin, xmax, ymax, score], ...]``) and loads the
 reference's checkpoint schema (``FaceBoxes/models/faceboxes.py``: ``conv1.conv.weight``, ``inception2.branch3x3.bn.*``,
 ``loc.0.bias`` ..., optional ``module.`` prefix, ``utils/functions.py:19-43``).  The 33 convolutions, the pools and the
-softmax run in ``libsynergy_b200.so`` (``csrc/kernels_detect.cuh``); only ``cv2.resize`` of oversized images stays on
-the host, as in the reference.  No CPU fallback.
+softmax run in ``libsynergy_b200.so`` (``csrc/kernels_detect.cuh``).  An image above 720 x 1080 is uploaded as it is
+and shrunk on the device (``inference.crop_resize_device``, ``csrc/kernels_resize.cuh``) to the bytes the reference's
+``cv2.resize`` makes on the host.  No CPU fallback.
 """
 from __future__ import annotations
 
@@ -17,6 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib, detect
+from .inference import INTER_LINEAR, crop_resize_device
 
 # FaceBoxes/FaceBoxes.py:24-25
 scale_flag = True
@@ -117,19 +119,17 @@ class FaceBoxes:
         self.timer_flag = timer_flag
 
     def __call__(self, img_: np.ndarray):
-        import cv2
-        img_raw = img_
+        image = torch.from_numpy(np.ascontiguousarray(img_, dtype=np.uint8)).to(self.net.device)
         scale = 1
         if scale_flag:                                                                        # FaceBoxes.py:62-79
-            h, w = img_raw.shape[:2]
+            h, w = img_.shape[:2]
             if h > HEIGHT:
                 scale = HEIGHT / h
             if w * scale > WIDTH:
                 scale *= WIDTH / (w * scale)
-            if scale != 1:
-                img_raw = cv2.resize(img_raw, dsize=(int(scale * w), int(scale * h)))
-        im_h, im_w = img_raw.shape[:2]
-        image = torch.from_numpy(np.ascontiguousarray(img_raw, dtype=np.uint8)).to(self.net.device)
+            if scale != 1:                                                                    # cv2.resize, INTER_LINEAR
+                image = crop_resize_device(image, [[0, 0, w, h]], (int(scale * w), int(scale * h)), INTER_LINEAR, planar=False)[0]
+        im_h, im_w = int(image.shape[0]), int(image.shape[1])
         loc, conf = self.net.forward(image)
         dets, n = detect.decode_device(loc, conf, im_h, im_w, scale=float(scale))
         n_host = int(n.item())

@@ -1,7 +1,7 @@
 """Host-side API semantics around the hot path, batched (reference ``utils/inference.py``).
 
-Only tiny per-face affine / pose algebra and the integer ROI crop live here; vertex
-reconstruction itself runs on the GPU (``Engine.reconstruct``).
+Only tiny per-face affine / pose algebra, the integer ROI crop (the host restatement the tests compare against) and its
+device twin ``crop_resize_device`` live here; vertex reconstruction itself runs on the GPU (``Engine.reconstruct``).
 """
 from __future__ import annotations
 
@@ -10,6 +10,7 @@ from typing import Sequence, Tuple
 import numpy as np
 
 STD_SIZE = 120
+INTER_LINEAR, INTER_LANCZOS4 = 1, 4        # cv2's constants, for crop_resize_device
 
 
 def parse_param(param: np.ndarray):
@@ -18,11 +19,16 @@ def parse_param(param: np.ndarray):
     return cam[:, :3], cam[:, 3:4], param[12:52].reshape(40, 1), param[52:62].reshape(10, 1)
 
 
+def roi_ints(roi_box: Sequence[float]) -> list:
+    """``x0, y0, x1, y1`` of a crop: ``int(round(v))`` with Python's round-half-even (utils/inference.py:98)."""
+    return [int(round(v)) for v in roi_box[:4]]
+
+
 def crop_img(img: np.ndarray, roi_box: Sequence[float]) -> np.ndarray:
     """Integer-rounded ROI crop with zero fill outside the image (utils/inference.py:95-125).
     Index arithmetic is bit-exact with the reference: Python ``round`` then clamping."""
     img_h, img_w = img.shape[:2]
-    x0, y0, x1, y1 = (int(round(v)) for v in roi_box[:4])
+    x0, y0, x1, y1 = roi_ints(roi_box)
     out = np.zeros((y1 - y0, x1 - x0) + tuple(img.shape[2:]), dtype=np.uint8)
     src_x0, src_y0 = max(x0, 0), max(y0, 0)
     src_x1, src_y1 = min(x1, img_w), min(y1, img_h)
@@ -30,6 +36,45 @@ def crop_img(img: np.ndarray, roi_box: Sequence[float]) -> np.ndarray:
     dst_x1 = (x1 - x0) - (x1 - src_x1)
     dst_y1 = (y1 - y0) - (y1 - src_y1)
     out[dst_y0:dst_y1, dst_x0:dst_x1] = img[src_y0:src_y1, src_x0:src_x1]
+    return out
+
+
+def resize_plan(rois: np.ndarray, out_h: int, out_w: int, interpolation: int) -> np.ndarray:
+    """Host-built tap tables for ``crop_resize_device`` (``syn_crop_resize_plan_host``): ``rois`` (B,4) int32 x0, y0, x1, y1."""
+    from . import _lib
+    lib = _lib.load()
+    rois = np.ascontiguousarray(rois, dtype=np.int32).reshape(-1, 4)
+    n = int(lib.syn_crop_resize_plan_size(rois.shape[0], out_h, out_w, interpolation))
+    plan = np.zeros(max(n, 1), np.uint8)
+    _lib.check(lib.syn_crop_resize_plan_host(rois.ctypes.data, rois.shape[0], out_h, out_w, interpolation, plan.ctypes.data, n))
+    return plan
+
+
+def crop_resize_device(image, roi_boxes: Sequence[Sequence[float]], dsize: Tuple[int, int] = (STD_SIZE, STD_SIZE),
+                       interpolation: int = INTER_LINEAR, planar: bool = True):
+    """Device twin of ``cv2.resize(crop_img(img, box), dsize, interpolation=...)`` for every box, byte for byte.
+
+    ``image``: (H,W,3) uint8 BGR CUDA tensor; ``dsize`` = (width, height) as cv2 takes it; ``interpolation``:
+    ``INTER_LINEAR`` or ``INTER_LANCZOS4``.  Returns uint8 (B,3,h,w) crops when ``planar`` (the backbone's input layout,
+    ``permute(0,3,1,2)`` of the stacked crops), else (B,h,w,3).  Runs on the current stream of the image's device."""
+    import torch
+    from . import _lib
+    if image.dtype != torch.uint8 or image.dim() != 3 or not image.is_cuda or not image.is_contiguous():
+        raise ValueError('image must be a contiguous (H,W,C) uint8 CUDA tensor')
+    out_w, out_h = int(dsize[0]), int(dsize[1])
+    plan = torch.from_numpy(resize_plan(np.array([roi_ints(b) for b in roi_boxes], np.int32), out_h, out_w, interpolation))
+    plan = plan.to(image.device)
+    B = len(roi_boxes)
+    if planar:
+        out = torch.empty((B, 3, out_h, out_w), dtype=torch.uint8, device=image.device)
+        strides = (3 * out_h * out_w, out_w, 1, out_h * out_w)
+    else:
+        out = torch.empty((B, out_h, out_w, 3), dtype=torch.uint8, device=image.device)
+        strides = (3 * out_h * out_w, 3 * out_w, 3, 1)
+    with torch.cuda.device(image.device):
+        _lib.check(_lib.load().syn_crop_resize(image.data_ptr(), image.shape[0], image.shape[1], image.shape[2], plan.data_ptr(), B,
+                                               out_h, out_w, interpolation, out.data_ptr(), *strides,
+                                               torch.cuda.current_stream(image.device).cuda_stream))
     return out
 
 

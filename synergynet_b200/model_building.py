@@ -18,7 +18,7 @@ import torch.nn as nn
 from . import backbone as mobilenetv2_backbone
 from .backbone import MLP_for, MLP_rev
 from .engine import Engine
-from .inference import crop_img, roi_affine, square_roi
+from .inference import INTER_LANCZOS4, INTER_LINEAR, crop_resize_device, roi_affine, square_roi
 from .params import ParamsPack, get_param_pack, set_param_pack  # noqa: F401  (re-exported)
 
 _LOSS_KEYS = ('loss_LMK_f0', 'loss_LMK_pointNet', 'loss_Param_In', 'loss_Param_S2', 'loss_Param_S1S2')
@@ -307,7 +307,6 @@ class _SynergyBase(nn.Module):
         ``rects`` are detector boxes ``[x0,y0,x1,y1,score]``.  The FaceBoxes detector is outside
         the hot path (SURVEY.md section 8 f3): pass ``rects`` or set ``self.face_detector``.
         """
-        import cv2
         if rects is None:
             if self.face_detector is None:
                 raise RuntimeError('no face detector configured: pass rects=[[x0,y0,x1,y1,score],...] '
@@ -316,14 +315,14 @@ class _SynergyBase(nn.Module):
         boxes = [square_roi(list(r)) for r in rects]
         if not boxes:
             return [], [], []
-        interp = cv2.INTER_LANCZOS4 if self.resize_interpolation == 'lanczos4' else cv2.INTER_LINEAR
-        # integer ROI crop + cv2 resize stay on the host (bit-exact index work / OpenCV's fixed-point Lanczos); everything
-        # after it is batched on the GPU: uint8 -> (v-127.5)/128, backbone, both reconstructions already mapped to image
-        # coordinates, pose decode.  One H2D of the uint8 crops, one D2H per output, no per-face arithmetic in Python.
-        crops = np.stack([cv2.resize(crop_img(input, b), dsize=(120, 120), interpolation=interp) for b in boxes])
+        interp = INTER_LANCZOS4 if self.resize_interpolation == 'lanczos4' else INTER_LINEAR
+        # everything is batched on the GPU: one H2D of the image, crop + resize to the planar uint8 (B,3,120,120) batch
+        # (OpenCV's fixed-point arithmetic, byte for byte), uint8 -> (v-127.5)/128, backbone, both reconstructions already
+        # mapped to image coordinates, pose decode.  One D2H per output, no per-face arithmetic in Python.
         dev = self._compute_device()
         eng = self._engine(dev)
-        batch = torch.from_numpy(crops).permute(0, 3, 1, 2).contiguous().to(dev)                 # uint8 (B,3,120,120)
+        image = torch.from_numpy(np.ascontiguousarray(input, dtype=np.uint8)).to(dev)    # crop_img's uint8 crops
+        batch = crop_resize_device(image, boxes, (120, 120), interp)
         _, params = eng.forward_landmarks(batch, want_params=True)
         roi5 = torch.from_numpy(roi_affine(boxes)).to(dev)
         lmk = eng.reconstruct_image(params, roi5, dense=False).cpu().numpy()
