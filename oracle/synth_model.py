@@ -73,6 +73,34 @@ def build_state_dict(seed: int = 0) -> Dict[str, torch.Tensor]:
 
 
 @torch.no_grad()
+def reparametrize_streams(sd: Dict[str, torch.Tensor], seed: int, lo: int, hi: int) -> Dict[str, torch.Tensor]:
+    """The same network with a wide spread of channel magnitudes, as trained checkpoints have.
+
+    Only the block streams (the 16/24/32/64/96/160/320-channel tensors between blocks) can be rescaled without changing
+    the function: they are the only tensors not followed by a ReLU6, which does not commute with scaling.  Channel c of
+    each stream gets a factor f_c = 2^k with k an integer drawn from [lo, hi] (one channel at each end of the range):
+    gamma and beta of every project BatchNorm that writes the stream are multiplied by f_c, and input column c of every
+    conv that reads it (the expands of the following blocks and the last conv) is divided by f_c.  Powers of two make
+    this exact in fp32: every block output becomes exactly f * the original and everything after it is unchanged."""
+    out = {k: v.clone() for k, v in sd.items()}
+    pre = 'I2P.backbone.'
+    g = torch.Generator().manual_seed(seed)
+    f = None
+    for spec in conv_plan():
+        if spec.kind in ('expand', 'last') and f is not None:
+            out[pre + spec.conv_key + '.weight'] /= f.view(1, -1, 1, 1)
+        if spec.kind == 'project':
+            if not spec.residual:                              # first block of a stage: a new stream
+                k = torch.randint(lo, hi + 1, (spec.cout,), generator=g)
+                ends = torch.randperm(spec.cout, generator=g)[:2]
+                k[ends[0]], k[ends[1]] = lo, hi
+                f = torch.pow(2.0, k.double()).float()
+            out[pre + spec.bn_key + '.weight'] *= f
+            out[pre + spec.bn_key + '.bias'] *= f
+    return out
+
+
+@torch.no_grad()
 def _calibrate_pointnet(sd: Dict[str, torch.Tensor], pooled: torch.Tensor, seed: int) -> None:
     """Same treatment for the BatchNorm1d layers of forwardDirection / reverseDirection (reference
     backbone_nets/pointnet_backbone.py:7-106): with arbitrary statistics every ReLU of the heads is dead (the
