@@ -330,8 +330,32 @@ int syn_poll_saturation(syn_handle_t* h, int* flag_out);
 int syn_debug_forward_until(syn_handle_t* h, const float* x_dev, int batch, int layer,
                             float* out_dev, void* stream);
 
-/* Debug only: one workspace buffer of the PointNet heads after syn_mlp_for / syn_mlp_rev (synchronises). */
-int syn_debug_heads_buffer(syn_handle_t* h, int which, float* out_host, int64_t n);
+/* Per-stage tests of the GEMM layers.  Both run the production launch sequence unchanged up to `stage` and copy that
+ * stage's fp32 output to out_dev and, when the stage records them, its per-row maxima (fp32 bit patterns, what the next
+ * GEMM scales its rows by) to rowmax_dev (nullable; left untouched for a stage that records none).
+ * ResNet-50 (NHWC rows, one per pixel): 0 stem (B*3600 x 64), 1 max-pool (B*900 x 64), 1 + i conv i of
+ * syn_resnet_conv_desc (i = 1..52; a block's downsample runs before its conv3 and records no row maxima), 54 avgpool
+ * (B x 2048), 55 heads (B x 102, no row maxima). */
+int syn_debug_resnet_until(syn_handle_t* h, const float* x_dev, int batch, int stage, float* out_dev, unsigned* rowmax_dev,
+                           void* stream);
+/* PointNet heads (rows = B*68 point-major, or B): net 0 = MLP_for: 0..4 conv1..conv5 (64, 64, 64, 128, 1024 columns;
+ * conv5 is written only by this call, without row maxima), 5 the max-pooled global features (B x 1024), 6 the face vector
+ * (B x 2360), 7 conv6's face part (B x 512, no row maxima), 8 conv6's point part (512), 9 conv7 (256), 10 conv8 (128),
+ * 11 conv9 (3, no row maxima), 12 point_residual (B,3,68).  pool1280_dev / params62_dev as for syn_mlp_for.
+ * net 1 = MLP_rev (pool1280_dev / params62_dev unused): 0..4 as above, 5 the global features (B x 1024), 6 the heads (B x 62). */
+int syn_debug_pointnet_until(syn_handle_t* h, int net, const float* lmk_dev, const float* pool1280_dev,
+                             const float* params62_dev, int batch, int stage, float* out_dev, unsigned* rowmax_dev,
+                             void* stream);
+/* One tc_gemm_kernel launch on a temporary layer built from host weights w_host (N x K fp32, K in the GEMM's k order,
+ * bias_host N): out[m, n] = act(sum_k A[m, k] W[n, k] + bias[n] + addend[m / addend_group, n] + residual[m, n]),
+ * act 0 none / 2 ReLU.  ksize = 0: plain rows, a_dev [M][lda]; ksize > 0: implicit GEMM over the ksize x ksize x C patch
+ * of NHWC a_dev (M / (HO*WO) maps of H x W x C, K = ksize*ksize*C).  rowmax_in_dev: the caller's max|a| per row (per
+ * input pixel in conv mode), as fp32 bits.  residual_dev, addend_dev, colmax_dev (zeroed by the caller) and
+ * rowmax_out_dev are nullable.  K and C must be multiples of 8.  Synchronises the stream. */
+int syn_debug_gemm(syn_handle_t* h, const float* w_host, const float* bias_host, int N, int K, int act, int ksize,
+                   int stride, int pad, int H, int W, int C, const float* a_dev, int M, int lda, const unsigned* rowmax_in_dev,
+                   const float* residual_dev, const float* addend_dev, int addend_group, unsigned* colmax_dev,
+                   int colmax_group, float* out_dev, unsigned* rowmax_out_dev, void* stream);
 
 /* Host-only: the face-group plan the fused engine uses for a launch over `batch` faces on a GPU with
  * `sms` SMs and `faces_per_tile` (1, 2 or 4) faces per full tile.  Groups [0, *split) hold

@@ -100,6 +100,64 @@ def reparametrize_streams(sd: Dict[str, torch.Tensor], seed: int, lo: int, hi: i
     return out
 
 
+def _pow2_factors(n: int, g: torch.Generator, lo: int, hi: int) -> torch.Tensor:
+    """n factors 2^k, k an integer drawn from [lo, hi], with one channel at each end of the range."""
+    k = torch.randint(lo, hi + 1, (n,), generator=g)
+    ends = torch.randperm(n, generator=g)[:2]
+    k[ends[0]], k[ends[1]] = lo, hi
+    return torch.pow(2.0, k.double()).float()
+
+
+def _rescale_hidden(out, bn: str, consumers, f: torch.Tensor) -> None:
+    """Multiply the BatchNorm ``bn`` (gamma and beta) by f per channel and divide input columns [c0, c0 + len(f)) of
+    every consumer weight by f.  The BN is followed by a ReLU, and ReLU(f x) = f ReLU(x) for f > 0."""
+    out[bn + '.weight'] *= f
+    out[bn + '.bias'] *= f
+    for key, c0 in consumers:
+        shape = [1, -1] + [1] * (out[key].dim() - 2)
+        out[key][:, c0:c0 + len(f)] /= f.view(shape)
+
+
+@torch.no_grad()
+def reparametrize_resnet(sd: Dict[str, torch.Tensor], seed: int, lo: int, hi: int, prefix: str = '') -> Dict[str, torch.Tensor]:
+    """ResNet-50 with a wide spread of hidden-channel magnitudes: in every bottleneck, bn1's channels are scaled by
+    powers of two 2^k, k in [lo, hi], and conv2's input columns divided by the same factors; likewise bn2 -> conv3.
+    Powers of two make this exact in fp32: the hidden activations become exactly f * the original, and every block
+    output is unchanged."""
+    out = {k: v.clone() for k, v in sd.items()}
+    g = torch.Generator().manual_seed(seed)
+    for li, blocks in enumerate((3, 4, 6, 3), 1):
+        for j in range(blocks):
+            p = f'{prefix}layer{li}.{j}'
+            for a, b in ((1, 2), (2, 3)):
+                f = _pow2_factors(out[f'{p}.bn{a}.weight'].numel(), g, lo, hi)
+                _rescale_hidden(out, f'{p}.bn{a}', [(f'{p}.conv{b}.weight', 0)], f)
+    return out
+
+
+@torch.no_grad()
+def reparametrize_pointnet(sd: Dict[str, torch.Tensor], seed: int, lo: int, hi: int) -> Dict[str, torch.Tensor]:
+    """The PointNet heads with a wide spread of hidden-channel magnitudes: each bn_i's channels scaled by powers of two
+    2^k, k in [lo, hi], and the input columns of every conv that reads them divided by the same factors -- conv_{i+1};
+    for bn2 also conv6's point-feature columns [0, 64); for bn5 the pooled global features, i.e. conv6's columns
+    [64, 1088) (MLP_for) and all three conv6_x heads (MLP_rev).  Exact in fp32 like ``reparametrize_streams``."""
+    out = {k: v.clone() for k, v in sd.items()}
+    g = torch.Generator().manual_seed(seed)
+    for pre, last in (('forwardDirection.', 8), ('reverseDirection.', 5)):
+        for i in range(1, last + 1):
+            if pre == 'forwardDirection.' and i == 5:
+                consumers = [(f'{pre}conv6.weight', 64)]
+            elif i == 5:
+                consumers = [(f'{pre}conv6_{k}.weight', 0) for k in (1, 2, 3)]
+            else:
+                consumers = [(f'{pre}conv{i + 1}.weight', 0)]
+                if pre == 'forwardDirection.' and i == 2:
+                    consumers.append((f'{pre}conv6.weight', 0))
+            f = _pow2_factors(out[f'{pre}bn{i}.weight'].numel(), g, lo, hi)
+            _rescale_hidden(out, f'{pre}bn{i}', consumers, f)
+    return out
+
+
 @torch.no_grad()
 def _calibrate_pointnet(sd: Dict[str, torch.Tensor], pooled: torch.Tensor, seed: int) -> None:
     """Same treatment for the BatchNorm1d layers of forwardDirection / reverseDirection (reference

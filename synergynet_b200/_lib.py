@@ -84,7 +84,9 @@ SIGNATURES = {
     'syn_resnet_set_heads': (_I, [_P, _F, _F]),
     'syn_resnet_commit': (_I, [_P]),
     'syn_resnet50_forward': (_I, [_P, _F, _I, _F, _F, _P]),
-    'syn_debug_heads_buffer': (_I, [_P, _I, _F, _L]),
+    'syn_debug_resnet_until': (_I, [_P, _F, _I, _I, _F, _P, _P]),
+    'syn_debug_pointnet_until': (_I, [_P, _I, _F, _F, _F, _I, _I, _F, _P, _P]),
+    'syn_debug_gemm': (_I, [_P, _F, _F, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _I, _I, _P, _F, _F, _I, _P, _I, _F, _P, _P]),
     'syn_mesh_incidence_host': (_I, [_F, _I, _I, _F, _F]),
     'syn_mesh_normals': (_I, [_F, _L, _I, _I, _I, _I, _F, _I, _F, _F, _F, _F, _P]),
     'syn_mesh_lighting': (_I, [_F, _L, _I, _I, _I, _I, _F, C.POINTER(LightCfg), _F, _F, _F, _P]),
@@ -118,7 +120,8 @@ SIGNATURES = {
 _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturation', 'syn_pointnet_set_layer',
                                              'syn_pointnet_commit', 'syn_mlp_for', 'syn_mlp_rev', 'syn_wing_loss',
                                              'syn_param_loss', 'syn_reconstruct_image', 'syn_pose_decode', 'syn_set_center_crop', 'syn_resnet_num_convs', 'syn_resnet_conv_desc',
-                                             'syn_resnet_set_conv', 'syn_resnet_set_heads', 'syn_resnet_commit', 'syn_resnet50_forward', 'syn_debug_heads_buffer',
+                                             'syn_resnet_set_conv', 'syn_resnet_set_heads', 'syn_resnet_commit', 'syn_resnet50_forward', 'syn_debug_resnet_until',
+                                             'syn_debug_pointnet_until', 'syn_debug_gemm',
                                              'syn_mesh_incidence_host', 'syn_mesh_normals', 'syn_mesh_lighting', 'syn_rasterize', 'syn_nms',
                                              'syn_crop_resize_plan_size', 'syn_crop_resize_plan_host', 'syn_crop_resize',
                                              'syn_faceboxes_num_priors', 'syn_faceboxes_decode', 'syn_fb_num_layers', 'syn_fb_layer_desc', 'syn_fb_create',

@@ -8,15 +8,16 @@ from __future__ import annotations
 import ctypes as C
 import threading
 import warnings
-from typing import Dict, Optional
+from typing import Dict, Optional, Tuple
 
 import numpy as np
 import torch
 
 from . import _lib
-from .backbone import HEAD_DIMS, conv_plan
+from .backbone import HEAD_DIMS, conv_plan, resnet50_conv_keys
 
 N_PARAMS = 62
+_RESNET_DOWNSAMPLES = {i for i, (ck, _) in enumerate(resnet50_conv_keys()) if 'downsample' in ck}
 
 
 def _host_f32(t) -> torch.Tensor:
@@ -408,6 +409,89 @@ class Engine:
             _lib.check(self._lib.syn_resnet50_forward(self._h, x.data_ptr(), b, out.data_ptr(), pool.data_ptr(), self._stream()))
             self._done()
         return out, pool
+
+    # ---- per-stage debug runs of the GEMM layers (include/synergy_b200.h syn_debug_*_until / syn_debug_gemm) ----
+    RESNET_STAGES = 56
+    FOR_STAGES = ((64, True), (64, True), (64, True), (128, True), (1024, False), (1024, False), (2360, True),
+                  (512, False), (512, True), (256, True), (128, True), (3, False), (3 * 68, False))   # (columns, row maxima)
+    REV_STAGES = FOR_STAGES[:5] + ((1024, True), (N_PARAMS, False))
+
+    def _debug_out(self, rows: int, cols: int, rowmax: bool):
+        out = torch.empty((rows, cols), device=self.device, dtype=torch.float32)
+        rm = torch.zeros((rows,), device=self.device, dtype=torch.int32) if rowmax else None
+        return out, rm
+
+    def debug_resnet_until(self, x: torch.Tensor, stage: int):
+        """ResNet-50 run up to ``stage`` (0 stem, 1 max-pool, 1 + i conv i of the plan, 54 avgpool, 55 heads): (that
+        stage's output as (rows, channels) -- one row per NHWC pixel, or per face --, its row maxima as int32 fp32 bit
+        patterns, or None for a stage that records none)."""
+        x = self._check_x(x)
+        b = x.shape[0]
+        if stage == 0:
+            rows, cols, rm = b * 3600, 64, True
+        elif stage == 1:
+            rows, cols, rm = b * 900, 64, True
+        elif stage <= 53:
+            d = _lib.ConvDesc()
+            _lib.check(self._lib.syn_resnet_conv_desc(stage - 1, C.byref(d)))
+            rows, cols, rm = b * d.h_out * d.h_out, d.cout, stage - 1 not in _RESNET_DOWNSAMPLES
+        else:
+            rows, cols, rm = b, 2048 if stage == 54 else 102, stage == 54
+        out, rmax = self._debug_out(rows, cols, rm)
+        with self._lock:
+            _lib.check(self._lib.syn_debug_resnet_until(self._h, x.data_ptr(), b, stage, out.data_ptr(),
+                                                        rmax.data_ptr() if rm else None, self._stream()))
+            self._done()
+        return out, rmax
+
+    def debug_pointnet_until(self, net: int, lmk: torch.Tensor, stage: int, pool: Optional[torch.Tensor] = None,
+                             params: Optional[torch.Tensor] = None):
+        """MLP_for (net 0) or MLP_rev (net 1) run up to ``stage`` (include/synergy_b200.h): (output (rows, columns),
+        row maxima as int32 fp32 bit patterns or None).  Rows are the B*68 points, point-major, or the B faces."""
+        lmk = self._dev_f32(lmk)
+        b = lmk.shape[0]
+        cols, rm = (self.FOR_STAGES if net == 0 else self.REV_STAGES)[stage]
+        per_face = stage >= 5 and not (net == 0 and 8 <= stage <= 11)
+        out, rmax = self._debug_out(b if per_face else b * 68, cols, rm)
+        pool = self._dev_f32(pool) if pool is not None else None
+        params = self._dev_f32(params) if params is not None else None
+        with self._lock:
+            _lib.check(self._lib.syn_debug_pointnet_until(
+                self._h, net, lmk.data_ptr(), pool.data_ptr() if pool is not None else None,
+                params.data_ptr() if params is not None else None, b, stage, out.data_ptr(),
+                rmax.data_ptr() if rm else None, self._stream()))
+            self._done()
+        return out, rmax
+
+    def debug_gemm(self, w: torch.Tensor, bias: torch.Tensor, a: torch.Tensor, rowmax_in: torch.Tensor, act: int = 0,
+                   conv: Optional[Tuple[int, int, int, int, int]] = None, residual: Optional[torch.Tensor] = None,
+                   addend: Optional[torch.Tensor] = None, addend_group: int = 1, colmax_group: int = 0):
+        """One tc_gemm_kernel launch on a layer built from ``w`` (N, K) and ``bias`` (N,).  ``a``: (M, lda) rows, or NHWC
+        maps when ``conv`` = (ksize, stride, pad, HO, WO); ``rowmax_in``: int32 fp32 bit patterns per row / input pixel.
+        act 0 none, 2 ReLU.  colmax_group > 0 also max-pools the output over groups of that many rows.
+        Returns (out (M, N), rowmax_out (M,) int32 bits, colmax (ceil(M / group), N) int32 bits or None)."""
+        w, bias = _host_f32(w), _host_f32(bias)
+        n, k = w.shape
+        a = self._dev_f32(a)
+        if conv is None:
+            m, lda, ks, st, pad, hh, ww, cc = a.shape[0], a.shape[1], 0, 1, 0, 0, 0, 0
+        else:
+            ks, st, pad, ho, wo = conv
+            bb, hh, ww, cc = a.shape
+            m, lda = bb * ho * wo, cc
+        out = torch.empty((m, n), device=self.device, dtype=torch.float32)
+        rmo = torch.zeros((m,), device=self.device, dtype=torch.int32)
+        cm = torch.zeros((-(-m // colmax_group), n), device=self.device, dtype=torch.int32) if colmax_group > 0 else None
+        rmi = rowmax_in.to(device=self.device, dtype=torch.int32).contiguous()
+        res = self._dev_f32(residual) if residual is not None else None
+        add = self._dev_f32(addend) if addend is not None else None
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        with self._lock:
+            _lib.check(self._lib.syn_debug_gemm(self._h, w.data_ptr(), bias.data_ptr(), n, k, act, ks, st, pad, hh, ww, cc,
+                                                a.data_ptr(), m, lda, rmi.data_ptr(), ptr(res), ptr(add), addend_group,
+                                                ptr(cm), colmax_group, out.data_ptr(), rmo.data_ptr(), self._stream()))
+            self._done()
+        return out, rmo, cm
 
     def debug_forward_until(self, x: torch.Tensor, layer: int) -> torch.Tensor:
         x = self._check_x(x)
