@@ -215,6 +215,24 @@ __host__ __device__ constexpr int fused_d2_pieces(int cout_p, int slabs, int nwg
   return s;
 }
 
+// The MMAs of one accumulator for one chunk as one committed group, in straight-line code: pass 0 = hi*hi, 1 = hi*lo
+// (B's lo plane), 2 = lo*hi (A's lo plane); KSTEPS steps of K = 16 each.  The pass count is a template parameter and
+// fence, MMAs and commit share one basic block: a branch or a join inside the group makes ptxas insert a
+// warpgroup.arrive there and serialise every wgmma.mma_async of the kernel.
+template <int N, int KSTEPS, int NPASS>
+__device__ __forceinline__ void fused_mma_group(float* acc, uint32_t d_hi, uint32_t a_lo, uint32_t a_plane, uint32_t a_kstep,
+                                                uint32_t b_lo, uint32_t b_plane, uint32_t b_kstep, bool acc_in) {
+  tc::wgmma_fence();
+#pragma unroll
+  for (int pass = 0; pass < NPASS; ++pass)
+#pragma unroll
+    for (int ks = 0; ks < KSTEPS; ++ks)
+      tc::wgmma_f16<N>(acc, tc::desc64(d_hi, a_lo + (((pass == 2 ? a_plane : 0) + ks * a_kstep) >> 4)),
+                       tc::desc64(d_hi, b_lo + (((pass == 1 ? b_plane : 0) + ks * b_kstep) >> 4)),
+                       (acc_in || pass > 0 || ks > 0) ? 1u : 0u);
+  tc::wgmma_commit();
+}
+
 // NWW = worker warps (multiple of 4: whole warpgroups); the loader is warp NWW.
 template <class C, int NWW>
 __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const FusedArgs p) {
@@ -240,7 +258,10 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
   // turns every tile access into LD.E/ST.E instead of LDS/STS
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int tid = threadIdx.x, warp = tid >> 5;
-  const int row = tid & 127, wg = tid >> 7;   // GEMM row of this worker in the conversion, and its warpgroup
+  // GEMM row of this worker in the conversion, and its warpgroup.  The warpgroup index is broadcast from lane 0 so that
+  // ptxas knows it is warp-uniform: the MMAs sit under branches on it, and in a path ptxas must treat as divergent it
+  // serialises every wgmma.mma_async.
+  const int row = tid & 127, wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
   const int grp = warp / WPG;                  // channel group (workers only)
   const int gtid = tid - grp * TPG;
   const int ntiles = p.face_groups * C::STRIPS;
@@ -295,6 +316,30 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
     asm volatile("bar.sync 5, %0;" ::"n"(NWT) : "memory");
     const uint32_t d_hi = smem_desc_hi(128);
     constexpr uint32_t LBO_W1 = (C::NC / 8) * 128, LBO_W3 = (C::COUT_P / 8) * 128;
+
+    // ---- MMA schedule.  A warpgroup keeps its tensor-core work in flight under its CUDA-core phases, and
+    // wgmma.wait_group retires groups in issue order, so the issue order is the schedule:
+    //   GEMM1 slab j of a chunk -> D1 buffer j & 1, issued before EPI1 of slab j - 1 (the next slab is always in
+    //   flight during an epilogue); the first slab of chunk c + 1 -> buffer 0, issued before the depthwise pass of
+    //   chunk c (after it when the weights stream through two slots: chunk c + 1 lands in the slot that GEMM2(c - 1)
+    //   releases only at the end of chunk c - 1).  Every accumulator receives the same MMAs in the same order as
+    //   a synchronous schedule.
+    // Every warpgroup commits the same sequence of groups on every path -- a slab or D2 item it does not have is an
+    // empty group -- so each wait_group count is a compile-time constant.  ptxas proves from these counts that no
+    // register of a pending MMA is read; with a run-time count it cannot, and serialises every MMA.
+    constexpr int SPW = ceil_div_c(C::SLABS1, NWG);       // GEMM1 slabs per warpgroup and chunk (at most)
+    constexpr bool LATE_G1 = C::WSTREAM && C::WSTAGES == 2;
+    auto issue_g1 = [&](bool on, float* acc, int s1, const uint8_t* wch) {
+      if (on) {
+        const uint32_t a_lo = smem_desc_lo(smem_u32(sXA + s1 * C::XA_TILE), 1024);
+        const uint32_t w_lo = smem_desc_lo(smem_u32(wch + C::CH_W1), LBO_W1);
+        if (p.npass == 1) fused_mma_group<C::NC, C::CIN_P / 16, 1>(acc, d_hi, a_lo, C::XA_PLANE, 2048, w_lo, C::W1_PLANE, 2 * LBO_W1, false);
+        else fused_mma_group<C::NC, C::CIN_P / 16, 3>(acc, d_hi, a_lo, C::XA_PLANE, 2048, w_lo, C::W1_PLANE, 2 * LBO_W1, false);
+      } else {
+        wgmma_fence();
+        wgmma_commit();
+      }
+    };
 
     // Geometry of a tile + "prep": stage / convert its input into the GEMM1 A operand.  prep(next tile) runs
     // BEFORE the current tile's EPI2 (XA is free once the last GEMM1 of the tile is done), so the global-load
@@ -486,75 +531,91 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
       const int M2 = nfaces * C::M2F;
       const int mt2 = (M2 + 127) >> 7;
 
+      const int slabs1 = (M1 + 63) >> 6;
+      float acc1[2][C::NC / 2];                            // D1 double buffer (see the MMA schedule above)
       float acc2[IPW][N2 / 2];                             // this warpgroup's D2 items, accumulated over the chunks
-      for (int c = 0; c < C::NCHUNK; ++c, ++g) {
-        const int slot = C::WSTREAM ? (int)(g % C::WSTAGES) : c;
-        if constexpr (C::WSTREAM) mbar_wait(smem_u32(&bar_wfull[slot]), (g / C::WSTAGES) & 1, p.err);
-        const float* dwc = reinterpret_cast<const float*>(sWch + slot * C::CHUNK_BYTES + C::CH_DW);
-        SYN_TRACE(0, c, 0);
-        // every worker is done with the previous chunk: its depthwise reads of Hs and its GEMM2 reads of A2
-        // (c == 0: XA of this tile is complete)
-        group_bar_sync<TPG>(grp);
-        SYN_TRACE(0, c, 1);
-        if (c == 0) {
-          // ---- strip mode: window rows outside the image must read as zero (may hold a previous tile)
-          if constexpr (C::STRIPS > 1) {
-            constexpr int CQ = KPG * 2;                               // float4 per pixel
-            if (iy0 < 0)
-              for (int i = gtid; i < C::HS_COLS * CQ; i += TPG)
-                *reinterpret_cast<float4*>(sH + (size_t)(i / CQ) * C::HS_STRIDE + grp * KPG * 8 + (i % CQ) * 4) =
-                    make_float4(0.f, 0.f, 0.f, 0.f);
-            if (iy0 + C::RWIN - 1 > C::W - 1)
-              for (int i = gtid; i < C::HS_COLS * CQ; i += TPG)
-                *reinterpret_cast<float4*>(sH + (size_t)((C::RWIN - 1) * C::HS_COLS + i / CQ) * C::HS_STRIDE +
-                                           grp * KPG * 8 + (i % CQ) * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-        }
-        {
-          // ---- GEMM1 + EPI1, one 64-row slab of D1 at a time per warpgroup: relu6(s1*D1 + b1) / 6 -> hidden window.
-          // The expand scale is one power of two per layer (row 11 is constant), so an element costs one FFMA.SAT.
-          const float sc1 = dwc[11 * C::DWS];
-          const float* b1 = dwc + 10 * C::DWS;
-          const uint32_t w_lo = smem_desc_lo(smem_u32(sWch + slot * C::CHUNK_BYTES + C::CH_W1), LBO_W1);
-          const int slabs1 = (M1 + 63) >> 6;
-          for (int s1 = wg; s1 < slabs1; s1 += NWG) {          // warpgroup-uniform
-            float acc1[C::NC / 2];
-            const uint32_t a_lo = smem_desc_lo(smem_u32(sXA + s1 * C::XA_TILE), 1024);
-            wgmma_fence();
+      // weight slot of chunk c (chunk counter gc); streamed slots are waited for by every worker: all of them read
+      // the chunk's depthwise taps and EPI1 constants
+      auto chunk_slot = [&](uint32_t gc, int c) -> const uint8_t* {
+        const int slot = C::WSTREAM ? (int)(gc % C::WSTAGES) : c;
+        if constexpr (C::WSTREAM) mbar_wait(smem_u32(&bar_wfull[slot]), (gc / C::WSTAGES) & 1, p.err);
+        return sWch + slot * C::CHUNK_BYTES;
+      };
+      // ---- GEMM1 + EPI1 of chunk c, one 64-row slab of D1 at a time per warpgroup: relu6(s1*D1 + b1) / 6 -> hidden
+      // window.  The first slab is in flight on entry.  The expand scale is one power of two per layer (row 11 is
+      // constant), so an element costs one FFMA.SAT.
+      auto gemm1_epi1 = [&](int c, const uint8_t* wch) {
+        const float* dwc = reinterpret_cast<const float*>(wch + C::CH_DW);
+        const float sc1 = dwc[11 * C::DWS];
+        const float* b1 = dwc + 10 * C::DWS;
 #pragma unroll
-            for (int pass = 0; pass < 3; ++pass) {
-              if (pass >= p.npass) break;                           // single-pass engine: hi * hi only
+        for (int j = 0; j < SPW; ++j) {
+          const int s1 = wg + j * NWG;                                // warpgroup-uniform
+          if (j + 1 < SPW) issue_g1(s1 + NWG < slabs1, acc1[(j + 1) & 1], s1 + NWG, wch);
+          // retire slab j; slab j + 1 stays in flight
+          if (j + 1 < SPW) wgmma_wait<1>();
+          else wgmma_wait<0>();
+          if (s1 >= slabs1) continue;
+          const float* acc = acc1[j & 1];
 #pragma unroll
-              for (int ks = 0; ks < C::CIN_P / 16; ++ks)
-                wgmma_f16<C::NC>(acc1, desc64(d_hi, a_lo + (((pass == 2 ? C::XA_PLANE : 0) + ks * 2048) >> 4)),
-                                 desc64(d_hi, w_lo + (((pass == 1 ? C::W1_PLANE : 0) + ks * 2 * LBO_W1) >> 4)),
-                                 (pass > 0 || ks > 0) ? 1u : 0u);
-            }
-            wgmma_commit();
-            wgmma_wait<0>();
+          for (int h = 0; h < 2; ++h) {
+            const int m = 64 * s1 + acc_row(row, 2 * h);
+            if (m < M1) {
+              const int f = (C::FACES > 1) ? m / ppf : 0;
+              const int mr = m - f * ppf;
+              const int yl = mr / C::W, xx = mr - yl * C::W;
+              float* hrow = sH + (size_t)(f * C::HS_FACE + (rf - iy0 + yl) * C::HS_COLS + xx + 1) * C::HS_STRIDE;
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int m = 64 * s1 + acc_row(row, 2 * h);
-              if (m < M1) {
-                const int f = (C::FACES > 1) ? m / ppf : 0;
-                const int mr = m - f * ppf;
-                const int yl = mr / C::W, xx = mr - yl * C::W;
-                float* hrow = sH + (size_t)(f * C::HS_FACE + (rf - iy0 + yl) * C::HS_COLS + xx + 1) * C::HS_STRIDE;
-#pragma unroll
-                for (int q = 0; q < C::NC / 8; ++q) {
-                  const int i = 4 * q + 2 * h, j0 = acc_col(row, i);
-                  const float2 bq = *reinterpret_cast<const float2*>(b1 + j0);
-                  *reinterpret_cast<float2*>(hrow + j0) =
-                      make_float2(__saturatef(fmaf(acc1[i], sc1, bq.x)), __saturatef(fmaf(acc1[i + 1], sc1, bq.y)));
-                }
+              for (int q = 0; q < C::NC / 8; ++q) {
+                const int i = 4 * q + 2 * h, j0 = acc_col(row, i);
+                const float2 bq = *reinterpret_cast<const float2*>(b1 + j0);
+                *reinterpret_cast<float2*>(hrow + j0) =
+                    make_float2(__saturatef(fmaf(acc[i], sc1, bq.x)), __saturatef(fmaf(acc[i + 1], sc1, bq.y)));
               }
             }
           }
         }
+        wgmma_wait<0>();
         SYN_TRACE(0, c, 3);
-        group_bar_sync<TPG>(grp);   // the hidden window of this chunk is complete
-        // ---- DW: 3x3 depthwise on the window -> A2 operand ----------------------------------------
+      };
+      {
+        SYN_TRACE(0, 0, 0);
+        const uint8_t* w0 = chunk_slot(g, 0);
+        // XA of this tile is complete (and every depthwise read of the previous tile's window is done)
+        group_bar_sync<TPG>(grp);
+        SYN_TRACE(0, 0, 1);
+        // ---- strip mode: window rows outside the image must read as zero (may hold a previous tile)
+        if constexpr (C::STRIPS > 1) {
+          constexpr int CQ = KPG * 2;                               // float4 per pixel
+          if (iy0 < 0)
+            for (int i = gtid; i < C::HS_COLS * CQ; i += TPG)
+              *reinterpret_cast<float4*>(sH + (size_t)(i / CQ) * C::HS_STRIDE + grp * KPG * 8 + (i % CQ) * 4) =
+                  make_float4(0.f, 0.f, 0.f, 0.f);
+          if (iy0 + C::RWIN - 1 > C::W - 1)
+            for (int i = gtid; i < C::HS_COLS * CQ; i += TPG)
+              *reinterpret_cast<float4*>(sH + (size_t)((C::RWIN - 1) * C::HS_COLS + i / CQ) * C::HS_STRIDE +
+                                         grp * KPG * 8 + (i % CQ) * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        issue_g1(wg < slabs1, acc1[0], wg, w0);
+        gemm1_epi1(0, w0);
+      }
+      // Chunk c runs from its depthwise pass to EPI1 of chunk c + 1, so that no MMA is in flight across the loop's
+      // back edge: ptxas would serialise every MMA otherwise.
+      for (int c = 0; c < C::NCHUNK; ++c, ++g) {
+        const int slot = C::WSTREAM ? (int)(g % C::WSTAGES) : c;
+        const uint8_t* wch = sWch + slot * C::CHUNK_BYTES;
+        const float* dwc = reinterpret_cast<const float*>(wch + C::CH_DW);
+        // the hidden window of this chunk is complete, and no warpgroup reads A2 any more
+        group_bar_sync<TPG>(grp);
         SYN_TRACE(0, c, 4);
+        // the first GEMM1 slab of the next chunk runs under the depthwise pass (an empty group after the last chunk)
+        const bool more = c + 1 < C::NCHUNK;
+        const uint8_t* wn = wch;
+        if constexpr (!LATE_G1) {
+          if (more) wn = chunk_slot(g + 1, c + 1);
+          issue_g1(more && wg < slabs1, acc1[0], wg, wn);
+        }
+        // ---- DW: 3x3 depthwise on the window -> A2 operand ----------------------------------------
         if constexpr (C::DW3) {
           // Stride-1 60^2 / 30^2 / 15^2 maps.  The depthwise phase is bound by shared-memory wavefronts (every LDS.128 of
           // a warp costs four), so an item is register-blocked as far as the register file allows: ONE channel quad x
@@ -831,36 +892,41 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
           }
         }
         SYN_TRACE(0, c, 5);
+        if constexpr (LATE_G1) {
+          if (more) wn = chunk_slot(g + 1, c + 1);
+          issue_g1(more && wg < slabs1, acc1[0], wg, wn);
+        }
         fence_proxy_async_smem();
         group_bar_sync<TPG>(grp);   // A2 of this chunk is complete
         {
-          // ---- GEMM2: D2 += A2 * W3c^T on this warpgroup's items (accumulators stay in registers over the chunks)
-          const uint32_t w_lo = smem_desc_lo(smem_u32(sWch + slot * C::CHUNK_BYTES + C::CH_W3), LBO_W3);
+          // ---- GEMM2: D2 += A2 * W3c^T on this warpgroup's items (accumulators stay in registers over the chunks);
+          const uint32_t w_lo = smem_desc_lo(smem_u32(wch + C::CH_W3), LBO_W3);
           const int items2 = ((M2 + 63) >> 6) * NSPL;
-          wgmma_fence();
 #pragma unroll
-          for (int u = 0; u < IPW; ++u) {
+          for (int u = 0; u < IPW; ++u) {                            // one group per item (empty if it has none)
             const int it = wg + u * NWG;
             if (it < items2) {                                       // warpgroup-uniform
               const int s2 = it / NSPL, pc = it - s2 * NSPL;
               const uint32_t a_lo = smem_desc_lo(smem_u32(sA2 + (s2 >> 1) * (128 * C::NC * 2)) + (s2 & 1) * 1024, 2048);
               const uint32_t b_lo = w_lo + ((pc * (N2 / 8) * 128) >> 4);
-#pragma unroll
-              for (int pass = 0; pass < 3; ++pass) {
-                if (pass >= p.npass) break;
-#pragma unroll
-                for (int ks = 0; ks < C::NC / 16; ++ks)
-                  wgmma_f16<N2>(acc2[u], desc64(d_hi, a_lo + (((pass == 2 ? C::A2_PLANE : 0) + ks * 4096) >> 4)),
-                                desc64(d_hi, b_lo + (((pass == 1 ? C::W3_PLANE : 0) + ks * 2 * LBO_W3) >> 4)),
-                                (c > 0 || pass > 0 || ks > 0) ? 1u : 0u);
-              }
+              if (p.npass == 1) fused_mma_group<N2, C::NC / 16, 1>(acc2[u], d_hi, a_lo, C::A2_PLANE, 4096, b_lo, C::W3_PLANE, 2 * LBO_W3, c > 0);
+              else fused_mma_group<N2, C::NC / 16, 3>(acc2[u], d_hi, a_lo, C::A2_PLANE, 4096, b_lo, C::W3_PLANE, 2 * LBO_W3, c > 0);
+            } else {
+              wgmma_fence();
+              wgmma_commit();
             }
           }
-          wgmma_commit();
-          wgmma_wait<0>();
         }
+        // GEMM2 is retired at once: kept in flight under the next EPI1, ptxas serialises every MMA of the kernel (it
+        // cannot prove that EPI1 reads no register of the pending GEMM2)
+        wgmma_wait<0>();
         if constexpr (C::WSTREAM) mbar_arrive(smem_u32(&bar_wempty[slot]));   // the chunk's slot may be refilled
         SYN_TRACE(0, c, 6);
+        if (more) {
+          SYN_TRACE(0, c + 1, 0);
+          SYN_TRACE(0, c + 1, 1);
+          gemm1_epi1(c + 1, wn);
+        }
       }
       SYN_TRACE(0, 63, 1);
 
