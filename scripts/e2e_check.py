@@ -1,6 +1,5 @@
 #!/usr/bin/env python
-"""End-to-end host call, blocking vs two calls in flight, fp32 and uint8 crops (SYN_HOST_CHUNK / SYN_HOST_CHUNK0 select
-the chunking): faces/s over 40 steps of 1024 faces."""
+"""End-to-end host call, blocking vs two calls in flight, fp32 and uint8 crops: faces/s over 40 steps of 1024 faces."""
 import os
 import sys
 import time
@@ -38,7 +37,7 @@ def main():
                 eng.host_wait(prev)
             torch.cuda.synchronize()
             res[f'{kind}_{mode}'] = round(B * steps / (time.perf_counter() - t0))
-    print(f"chunk={os.environ.get('SYN_HOST_CHUNK', '512')}/{os.environ.get('SYN_HOST_CHUNK0', '512')}", res)
+    print(res)
 
 
 if __name__ == '__main__':

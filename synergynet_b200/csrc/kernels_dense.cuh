@@ -96,7 +96,6 @@ struct DenseArgs {
   float* out;                 // (B,3,nver)
   int batch, nver, n_vtiles, n_ftiles, transform;
   int affine;                 // apply the per-face crop -> image affine stored behind the pose rows
-  int stream_stores;          // 1: st.global.cs (evict-first), 0: plain write-back stores (L2 merges neighbouring 512-byte runs)
   long long* trace;           // debug (SYN_DENSE_TRACE): clock64 stamps of CTA 0, 8 events x 64 items x {team 0, unused, loader}
   int* err;
 };
@@ -262,9 +261,6 @@ __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_tc_kernel(const Den
 //   bar_mfull[slot]   meta rows of item i (slot i % 4) landed                         loader -> teams
 //   bar_bfull         alpha + pose tile of the CTA's face tile landed (once)
 constexpr int kFmPlane = 2 * kDnAPlane;                   // 32 KB: [hi|lo] of one coordinate of one vertex tile
-#ifndef SYN_FM_SPLIT
-#define SYN_FM_SPLIT 1                                    // bulk copies per plane (1, 2, 4, 8)
-#endif
 constexpr int kFmPSlots = 4, kFmMetaSlots = 4;
 constexpr int kFmTeams = 4;                               // one warpgroup each: faces 16t .. 16t+15 of the item
 constexpr int kFmSubFaces = 8;                            // faces staged per sub-round -> 24 rows
@@ -468,11 +464,8 @@ __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_fm_kernel(const Den
         if (kTrace && blockIdx.x == 0 && lane == 0 && v < 64) p.trace[(128 + v) * 8 + c] = clock64();
         if (elect_one()) {
           mbar_expect_tx(smem_u32(&bar_pfull[slot]), kFmPlane);
-#pragma unroll
-          for (int part = 0; part < SYN_FM_SPLIT; ++part)
-            bulk_g2s_hint(smem_u32(sP + slot * kFmPlane + part * (kFmPlane / SYN_FM_SPLIT)),
-                          p.basis_img + (size_t)(vt_lo + v) * kDnATile + (size_t)c * kFmPlane + part * (kFmPlane / SYN_FM_SPLIT),
-                          kFmPlane / SYN_FM_SPLIT, smem_u32(&bar_pfull[slot]), keep);
+          bulk_g2s_hint(smem_u32(sP + slot * kFmPlane), p.basis_img + (size_t)(vt_lo + v) * kDnATile + (size_t)c * kFmPlane,
+                        kFmPlane, smem_u32(&bar_pfull[slot]), keep);
           if (c == 0) {
             const int ms = v % kFmMetaSlots;
             mbar_expect_tx(smem_u32(&bar_mfull[ms]), kDnMetaTile);

@@ -18,9 +18,9 @@
 // resident in shared memory for the whole kernel (early blocks) or streamed chunk by chunk through a 2-3-slot
 // bulk-copy (TMA) ring (late blocks).
 //
-// Roles: warps 0..NWW-1 = workers (thread = GEMM row / pixel in the conversion, channel octets in EPI1 / DW, MMA
-// operand slabs per warpgroup), warp NWW = weight loader and stem-row stager (converged warp, bulk copies under
-// elect.sync).  smem operand tiles use the canonical K-major no-swizzle layout of tc_common.cuh (SBO 128 B,
+// Roles: warps 0..kFusedWorkerWarps-1 = workers (thread = GEMM row / pixel in the conversion, channel octets in EPI1 /
+// DW, MMA operand slabs per warpgroup), warp kFusedWorkerWarps = weight loader and stem-row stager (converged warp, bulk
+// copies under elect.sync).  smem operand tiles use the canonical K-major no-swizzle layout of tc_common.cuh (SBO 128 B,
 // LBO = rows/8 * 128 B).
 #pragma once
 #include "common.cuh"
@@ -28,73 +28,12 @@
 
 namespace syn {
 
+// Worker warps of a fused CTA (whole warpgroups).  8 rather than 16: on an H100 a 1024-face step measured 5.13 ms
+// against 5.76 ms with 16, whose 17-warp CTAs leave 96 registers per thread and spill.
+constexpr int kFusedWorkerWarps = 8;
+static_assert(kFusedWorkerWarps % 4 == 0, "worker warps form whole warpgroups");
+
 __host__ __device__ constexpr int ceil_div_c(int a, int b) { return (a + b - 1) / b; }
-// tile shapes / chunk widths / batching depths worth re-measuring when the kernel changes: build variants
-// with -D... (scripts/build_variant.sh) and compare them with scripts/quick_variant_check.py
-#ifndef SYN_RO_STEM
-#define SYN_RO_STEM 6
-#endif
-#ifndef SYN_RO_B2
-#define SYN_RO_B2 6
-#endif
-#ifndef SYN_PREP_BATCH
-#define SYN_PREP_BATCH 4
-#endif
-#ifndef SYN_NC_B4
-#define SYN_NC_B4 16
-#endif
-#ifndef SYN_NC_B2
-#define SYN_NC_B2 32
-#endif
-// block 3: 48-channel chunks (3 chunks per tile: fewer per-chunk barrier round trips).  Strip heights of blocks 3-6
-// are bounded by shared memory: the block input (XA) is staged there next to the hidden window.
-#ifndef SYN_NC_B3
-#define SYN_NC_B3 48
-#endif
-#ifndef SYN_RO_B3
-#define SYN_RO_B3 6
-#endif
-#ifndef SYN_RO_B4
-#define SYN_RO_B4 5
-#endif
-#ifndef SYN_RO_B56
-#define SYN_RO_B56 5
-#endif
-// programmatic dependent launch over the fused launches: a block's prologue overlaps the previous block's tail
-#ifndef SYN_PDL
-#define SYN_PDL 1
-#endif
-#ifndef SYN_DW2_SMALL
-#define SYN_DW2_SMALL 1
-#endif
-// SYN_DW3: depthwise items of one channel quad x 2 output rows x 5 output columns on the stride-1 60^2 / 30^2 / 15^2 maps
-// (15.2 shared-memory loads per 16 outputs instead of 26 + conflicted tap loads, DESIGN.md section 5)
-#ifndef SYN_DW3
-#define SYN_DW3 0      // off: one long item per thread serialises the depthwise phase
-#endif
-// output columns of a DW3 item: 3 (76 live registers; 17 warps leave 96 per thread: 5 warps share one sub-partition's
-// 16 K registers) or 5 (fewer loads per output, needs ~105 registers: spills unless the CTA has <= 16 warps)
-#ifndef SYN_DW3_S
-#define SYN_DW3_S 3
-#endif
-#ifndef SYN_DW2_MAXW
-#define SYN_DW2_MAXW 30
-#endif
-#ifndef SYN_NC_B56
-#define SYN_NC_B56 64
-#endif
-#ifndef SYN_NC_B7
-#define SYN_NC_B7 64
-#endif
-#ifndef SYN_NC_B12
-#define SYN_NC_B12 32
-#endif
-#ifndef SYN_NC_B14
-#define SYN_NC_B14 32
-#endif
-#ifndef SYN_NC_B17
-#define SYN_NC_B17 32
-#endif
 __host__ __device__ constexpr int round_up_c(int a, int b) { return ceil_div_c(a, b) * b; }
 
 template <int CIN_, int CHID_, int NC_, int COUT_, int W_, int STRIDE_, int RO_, int FACES_, bool RES_, bool STEM_,
@@ -113,17 +52,10 @@ struct FusedCfg {
   static constexpr int ROWS_MAX = (RWIN < W_ ? RWIN : W_);               // valid input rows per face
   static constexpr int M1_MAX = FACES_ * ROWS_MAX * W_;
   static constexpr int MT1 = ceil_div_c(M1_MAX, 128);
-  // DW3 (register-blocked 2 x 5 depthwise items, lanes = NS column segments x NR row pairs): the lane mapping is
-  // bank-conflict free only for certain row pitches of the hidden window (HS_COLS) and of the GEMM2 operand (WOP)
-  static constexpr int DW3_S = SYN_DW3_S;                                // output columns per item (odd)
-  static constexpr bool DW3 = SYN_DW3 && STRIDE_ == 1 && (WO % 15 == 0);                  // 60, 30, 15
-  static constexpr int DW3_NS = (WO >= 60) ? 4 : 2, DW3_NR = 8 / DW3_NS;
-  // pitch of an output row in the GEMM2 M index (pad columns are computed by the MMA and never read)
-  static constexpr int WOP = !DW3 ? WO : (DW3_NS == 4 ? WO + ((6 - WO % 4) % 4) : WO | 1);
-  static constexpr int M2F = RO_ * WOP;                                  // GEMM2 rows per face
+  static constexpr int M2F = RO_ * WO;                                   // GEMM2 rows per face
   static constexpr int M2_MAX = FACES_ * M2F;
   static constexpr int MT2 = ceil_div_c(M2_MAX, 128);
-  static constexpr int HS_COLS = (DW3 && DW3_NS == 2) ? ((W_ + 2) | 1) : W_ + 2;      // DW3 with 4 row-pair lanes: odd pitch
+  static constexpr int HS_COLS = W_ + 2;                                 // hidden window row incl. the halo columns
   static constexpr int HS_FACE = RWIN * HS_COLS, HS_PIX = FACES_ * HS_FACE, HS_STRIDE = NC_ + 4;
   static constexpr int DWS = NC_ + 4;     // floats between the tap rows of a chunk: mirrored lanes of the 2x2 depthwise read
                                           // taps kx and 2-kx, which must not lie a multiple of 128 bytes apart
@@ -159,13 +91,6 @@ struct FusedCfg {
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
   static_assert(NC_ <= 256, "MMA N");
   static_assert(WSTREAM_ == 0 || (WSTREAM_ >= 2 && WSTREAM_ <= 4 && NCHUNK >= WSTREAM_), "weight ring");
-  // DW3 bank-conflict conditions.  Window loads: lane (s, r) of a quarter-warp reads 16 bytes at group offset
-  // S*G*s + 2*HS_COLS*G*r (S = DW3_S, G = HS_STRIDE/4, both odd) and the eight offsets must differ mod 8; operand stores: 8-byte halves
-  // at 16-byte slot (S*s + 2*WOP*r) mod 8.  NS=4,NR=2 needs the row-pair term = 4 (mod 8), NS=2,NR=4 needs it = 2 or 6.
-  static_assert(!DW3 || ((HS_STRIDE / 4) % 2 == 1), "pixel pitch must be an odd number of 16-byte groups");
-  static_assert(!DW3 || (DW3_NS == 4 ? (2 * HS_COLS * (HS_STRIDE / 4)) % 8 == 4 : (2 * HS_COLS * (HS_STRIDE / 4)) % 4 == 2), "window row pitch");
-  static_assert(!DW3 || (DW3_NS == 4 ? (2 * WOP) % 8 == 4 : (2 * WOP) % 4 == 2), "operand row pitch");
-  static_assert(!DW3 || FACES_ == 1 || WOP == WO, "padded output rows only with one face per tile");
 };
 
 struct FusedArgs {
@@ -233,12 +158,11 @@ __device__ __forceinline__ void fused_mma_group(float* acc, uint32_t d_hi, uint3
   tc::wgmma_commit();
 }
 
-// NWW = worker warps (multiple of 4: whole warpgroups); the loader is warp NWW.
-template <class C, int NWW>
-__global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const FusedArgs p) {
+template <class C>
+__global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_kernel(const FusedArgs p) {
+  constexpr int NWW = kFusedWorkerWarps;
   constexpr int NWT = NWW * 32;          // worker threads
   constexpr int NWG = NWW / 4;           // worker warpgroups
-  static_assert(NWW % 4 == 0 && NWW >= 4 && NWW <= 24, "worker warps");
   // EPI1 and the depthwise conv are separated by a barrier of all workers (every warpgroup's GEMM1 slabs hold all
   // NC channels of their rows), so the depthwise items are spread over all workers as one channel group
   constexpr int NKG_ = C::NC / 8;
@@ -278,9 +202,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
     }
   };
 
-#if SYN_PDL
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // the next kernel's prologue may overlap this one's tail
-#endif
   if (tid == 0) {
     mbar_init(smem_u32(&bar_w), 1);
     for (int i = 0; i < 4; ++i) {
@@ -404,7 +326,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
         constexpr int KG = C::CIN_P / 8;
         constexpr int NXG = NWT / 64;                                    // thread groups of 64 = one slab's rows
         constexpr int ITERS = (C::SLABS1 * KG + NXG - 1) / NXG;          // items per thread
-        constexpr int PB = ITERS < SYN_PREP_BATCH ? ITERS : SYN_PREP_BATCH;
+        constexpr int PB = ITERS < 4 ? ITERS : 4;                        // items per batch of loads
         const int r64 = tid & 63, xg = tid >> 6;
         const int n_items = ((M1 + 63) >> 6) * KG;
         for (int e0 = xg; e0 < n_items; e0 += PB * NXG) {
@@ -505,12 +427,10 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
           asm volatile("prefetch.global.L2 [%0];" ::"l"(base + o));
       }
     };
-#if SYN_PDL
     // Programmatic dependent launch: everything above (barriers, the zeroed window, the weight image) does not
     // depend on the previous kernel; its output -- this kernel's input -- is first touched below, and this kernel's
     // first global store comes later still.
     asm volatile("griddepcontrol.wait;" ::: "memory");
-#endif
     if ((int)blockIdx.x < ntiles) prep(blockIdx.x);
     prefetch_x(blockIdx.x + gridDim.x);
 
@@ -616,89 +536,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
           issue_g1(more && wg < slabs1, acc1[0], wg, wn);
         }
         // ---- DW: 3x3 depthwise on the window -> A2 operand ----------------------------------------
-        if constexpr (C::DW3) {
-          // Stride-1 60^2 / 30^2 / 15^2 maps.  The depthwise phase is bound by shared-memory wavefronts (every LDS.128 of
-          // a warp costs four), so an item is register-blocked as far as the register file allows: ONE channel quad x
-          // TWO output rows x S = 3 (5) output columns = 4 x (S + 2) window loads + 10 tap loads per 8 S outputs: 20 (15.2)
-          // per 16 outputs; the 2 x 2 items below need 26 and their mirrored tap loads used to conflict.  A unit of 16
-          // threads = 8 lanes (NS column segments x NR row pairs) x the two quads of a channel octet.  Segments
-          // are S pixels = an odd number of 16-byte groups apart, row pairs 2 * HS_COLS pixels: with the row pitches
-          // FusedCfg asserts, the eight window addresses of a quarter-warp and the sixteen 8-byte operand stores of a
-          // half-warp fall on different banks.
-          constexpr int NS = C::DW3_NS, NR = C::DW3_NR, S = C::DW3_S, NSEG = C::WO / S, RP2 = (C::RO + 1) / 2;
-          constexpr int XGU = (NSEG + NS - 1) / NS, RPGU = (RP2 + NR - 1) / NR, UPK = XGU * RPGU;   // units per (face, octet)
-          const int l8 = tid & 7, qh = (tid >> 3) & 1;
-          const int ls = l8 % NS, lr = l8 / NS;
-          const int units = KPG * nfaces * UPK;
-          for (int u = gtid >> 4; u < units; u += TPG / 16) {
-            const int kgl = u / (nfaces * UPK), r1 = u - kgl * (nfaces * UPK);
-            const int f = r1 / UPK, r2 = r1 - f * UPK;
-            const int rpg = r2 / XGU, xg = r2 - rpg * XGU;
-            const int kg = grp * KPG + kgl, j0 = kg * 8 + qh * 4;
-            const int seg = xg * NS + ls, oy = 2 * (rpg * NR + lr);
-            if (seg >= NSEG || oy >= C::RO) continue;
-            const int ox0 = S * seg;
-            const bool two = (oy + 1 < C::RO);
-            const float* wq = dwc + j0;
-            float2 w[3][3][2];                                             // [ky][kx][channel pair]
-#pragma unroll
-            for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-              for (int kx = 0; kx < 3; ++kx) {
-                const float4 t4 = *reinterpret_cast<const float4*>(wq + (ky * 3 + kx) * C::DWS);
-                w[ky][kx][0] = make_float2(t4.x, t4.y); w[ky][kx][1] = make_float2(t4.z, t4.w);
-              }
-            float2 acc[2][S][2];                                           // [output row][output column][channel pair]
-            {
-              const float4 b4 = *reinterpret_cast<const float4*>(wq + 9 * C::DWS);
-#pragma unroll
-              for (int ro = 0; ro < 2; ++ro)
-#pragma unroll
-                for (int a = 0; a < S; ++a) { acc[ro][a][0] = make_float2(b4.x, b4.y); acc[ro][a][1] = make_float2(b4.z, b4.w); }
-            }
-            // window columns ox0-1 .. ox0+S are Hs columns ox0 .. ox0+S+1; window rows oy .. oy+3
-            const float* hb = sH + (size_t)(f * C::HS_FACE + oy * C::HS_COLS + ox0) * C::HS_STRIDE + j0;
-#pragma unroll
-            for (int ic = 0; ic < S + 2; ++ic) {
-              float2 d[4][2];
-#pragma unroll
-              for (int r = 0; r < 4; ++r) {
-                if (r == 3 && !two) continue;                              // row only the absent second output row needs
-                const float4 t4 = *reinterpret_cast<const float4*>(hb + (r * C::HS_COLS + ic) * C::HS_STRIDE);
-                d[r][0] = make_float2(t4.x, t4.y); d[r][1] = make_float2(t4.z, t4.w);
-              }
-#pragma unroll
-              for (int a = 0; a < S; ++a) {
-                const int kx = ic - a;
-                if (kx < 0 || kx > 2) continue;
-#pragma unroll
-                for (int ky = 0; ky < 3; ++ky) {
-#pragma unroll
-                  for (int j = 0; j < 2; ++j) acc[0][a][j] = ffma2(d[ky][j], w[ky][kx][j], acc[0][a][j]);
-                  if (two) {
-#pragma unroll
-                    for (int j = 0; j < 2; ++j) acc[1][a][j] = ffma2(d[ky + 1][j], w[ky][kx][j], acc[1][a][j]);
-                  }
-                }
-              }
-            }
-            constexpr float kOut = 6.0f * kActScale;
-#pragma unroll
-            for (int ro = 0; ro < 2; ++ro) {
-              if (ro == 1 && !two) continue;
-#pragma unroll
-              for (int a = 0; a < S; ++a) {
-                const int m2 = f * C::M2F + (oy + ro) * C::WOP + ox0 + a;
-                uint32_t h0, l0, h1, l1;
-                split2_f16<false>(__saturatef(acc[ro][a][0].x) * kOut, __saturatef(acc[ro][a][0].y) * kOut, h0, l0);
-                split2_f16<false>(__saturatef(acc[ro][a][1].x) * kOut, __saturatef(acc[ro][a][1].y) * kOut, h1, l1);
-                uint8_t* dst = sA2 + (m2 >> 7) * (128 * C::NC * 2) + ((m2 & 127) >> 3) * 128 + kg * 2048 + (m2 & 7) * 16 + qh * 8;
-                *reinterpret_cast<uint2*>(dst) = make_uint2(h0, h1);
-                *reinterpret_cast<uint2*>(dst + C::A2_PLANE) = make_uint2(l0, l1);
-              }
-            }
-          }
-        } else if constexpr (C::STRIDE == 1 && ((C::WO >= 15 && C::WO <= SYN_DW2_MAXW) || (SYN_DW2_SMALL && C::WO == 8))) {
+        if constexpr (C::STRIDE == 1 && ((C::WO >= 15 && C::WO <= 30) || C::WO == 8)) {
           // Stride-1 30^2, 15^2 and 8^2 maps (on the 60^2 map of block 1 the units do not divide evenly between
           // the channel groups and the row-pair items below are faster): the window loads of the depthwise
           // conv are what the shared-memory pipe spends its time on, so an item is register-blocked over a 2 x 2 output patch
@@ -709,9 +547,8 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
           // an even number of 16-byte bank groups apart, and the mirror image shifts lanes 4-7 onto the odd
           // groups: every window load (quarter-warp) and every 8-byte operand store (half-warp) is
           // bank-conflict free.
-          // 8x8 maps (SYN_DW2_SMALL): the 8 lanes
-          // are 4 column pairs x 2 row pairs; the second row pair lies 2 window rows = 4 bank groups further
-          // and is the mirrored half.
+          // 8x8 maps: the 8 lanes are 4 column pairs x 2 row pairs; the second row pair lies 2 window rows = 4 bank
+          // groups further and is the mirrored half.
           constexpr int XL = (C::WO >= 15) ? 8 : 4, YL = 8 / XL;           // lanes of a unit along x / along row pairs
           constexpr int CPR = (C::WO + 1) / 2, XG2 = (CPR + XL - 1) / XL, RP2 = (C::RO + 1) / 2;
           constexpr int RPU = (RP2 + YL - 1) / YL, UPK = RPU * XG2;        // units per (face, channel octet)
@@ -779,7 +616,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
               for (int a = 0; a < 2; ++a) {
                 const int col = ox + (mir ? 1 - a : a);
                 if (col >= C::WO) continue;                                // odd width: the last pair has one column
-                const int m2 = f * C::M2F + (oy + ro) * C::WOP + col;
+                const int m2 = f * C::M2F + (oy + ro) * C::WO + col;
                 uint32_t h0, l0, h1, l1;
                 split2_f16<false>(__saturatef(acc[ro][a][0].x) * kOut, __saturatef(acc[ro][a][0].y) * kOut, h0, l0);
                 split2_f16<false>(__saturatef(acc[ro][a][1].x) * kOut, __saturatef(acc[ro][a][1].y) * kOut, h1, l1);
@@ -865,7 +702,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
                   }
                 }
                 constexpr float kOut = 6.0f * kActScale;                   // relu6(x) * kActScale = sat(x/6) * 384
-                const int m2 = f * C::M2F + oy * C::WOP + ox;
+                const int m2 = f * C::M2F + oy * C::WO + ox;
                 {
                   uint32_t h[4], l[4];
   #pragma unroll
@@ -876,7 +713,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
                   *reinterpret_cast<uint4*>(dst + C::A2_PLANE) = swz ? make_uint4(l[2], l[3], l[0], l[1]) : make_uint4(l[0], l[1], l[2], l[3]);
                 }
                 if (two) {
-                  const int m3 = m2 + C::WOP;
+                  const int m3 = m2 + C::WO;
                   uint32_t h[4], l[4];
   #pragma unroll
                   for (int j = 0; j < 4; ++j)
@@ -934,12 +771,10 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
       prefetch_x(tile + 2 * (int)gridDim.x);
       // ---- EPI2: s3*D2 + b3 (+ skip) -> global NHWC --------------------------------------------------
       SYN_TRACE(0, 63, 2);
-      // GEMM2 row m2 -> output pixel of the tile (rows are padded to WOP pixels when DW3 needs it); -1 = no pixel
+      // GEMM2 row m2 -> output pixel of the tile (tiles are contiguous in NHWC memory); -1 = no pixel
       auto out_pixel = [&](int m2) -> int {
         if (m2 >= M2) return -1;
-        if constexpr (C::WOP == C::WO) return m2;                  // tiles are contiguous in NHWC memory
-        const int oyl = m2 / C::WOP, oxl = m2 - oyl * C::WOP;
-        return oxl < C::WO ? oyl * C::WO + oxl : -1;
+        return m2;
       };
       const int items2 = ((M2 + 63) >> 6) * NSPL;
 #pragma unroll
@@ -1024,9 +859,7 @@ __global__ void __launch_bounds__((NWW + 1) * 32, 1) fused_mbconv_kernel(const F
           bulk_g2s(smem_u32(sIn + (ci * C::IN_ROWS + r_lo) * C::IN_STRIDE),
                    p.x + ((size_t)(fgq * 3 + ci) * kImg + iy_first + r_lo) * kImg, bytes, smem_u32(&bar_in));
       };
-#if SYN_PDL
       asm volatile("griddepcontrol.wait;" ::: "memory");   // the crop rows are inputs; the rule is kept uniform
-#endif
       stage_rows(blockIdx.x);
       __syncwarp();
       uint32_t n_x = 0;
@@ -1056,20 +889,22 @@ inline void fused_tile_plan(int batch, int sms, int& split, int& face_groups) {
 }
 
 // ---- the instantiations used by the backbone (SURVEY.md section 8(a) shape table) -------------------
+// Block 3 takes 48-channel chunks (3 per tile: fewer per-chunk barrier round trips).  The strip heights of blocks 3-6
+// are bounded by shared memory: the block input (XA) is staged there next to the hidden window.
 //                          CIN CHID NC COUT  W  S  RO FACES RES    STEM   weight ring slots (0 = resident)
-using FusedStemB1 = FusedCfg<27, 32, 32, 16, 60, 1, SYN_RO_STEM, 1, false, true, 0>;    // features[0] + features[1]
-using FusedB2 = FusedCfg<16, 96, SYN_NC_B2, 24, 60, 2, SYN_RO_B2, 1, false, false, 0>;       // features[2]
-using FusedB3 = FusedCfg<24, 144, SYN_NC_B3, 24, 30, 1, SYN_RO_B3, 1, true, false, 0>;      // features[3]
-using FusedB4 = FusedCfg<24, 144, SYN_NC_B4, 32, 30, 2, SYN_RO_B4, 1, false, false, 0>;      // features[4]
-using FusedB56 = FusedCfg<32, 192, SYN_NC_B56, 32, 15, 1, SYN_RO_B56, 1, true, false, 0>;     // features[5], [6]
-using FusedB7 = FusedCfg<32, 192, SYN_NC_B7, 64, 15, 2, 8, 1, false, false, 0>;      // features[7]
+using FusedStemB1 = FusedCfg<27, 32, 32, 16, 60, 1, 6, 1, false, true, 0>;    // features[0] + features[1]
+using FusedB2 = FusedCfg<16, 96, 32, 24, 60, 2, 6, 1, false, false, 0>;       // features[2]
+using FusedB3 = FusedCfg<24, 144, 48, 24, 30, 1, 6, 1, true, false, 0>;      // features[3]
+using FusedB4 = FusedCfg<24, 144, 16, 32, 30, 2, 5, 1, false, false, 0>;      // features[4]
+using FusedB56 = FusedCfg<32, 192, 64, 32, 15, 1, 5, 1, true, false, 0>;     // features[5], [6]
+using FusedB7 = FusedCfg<32, 192, 64, 64, 15, 2, 8, 1, false, false, 0>;      // features[7]
 using FusedB8 = FusedCfg<64, 384, 64, 64, 8, 1, 8, 2, true, false, 3>;         // features[8..10]
 using FusedB11 = FusedCfg<64, 384, 64, 96, 8, 1, 8, 2, false, false, 2>;       // features[11]
-using FusedB12 = FusedCfg<96, 576, SYN_NC_B12, 96, 8, 1, 8, 2, true, false, SYN_NC_B12 == 32 ? 3 : 2>;        // features[12], [13]
-using FusedB14 = FusedCfg<96, 576, SYN_NC_B14, 160, 8, 2, 4, 2, false, false, SYN_NC_B14 == 32 ? 3 : 2>;      // features[14]
+using FusedB12 = FusedCfg<96, 576, 32, 96, 8, 1, 8, 2, true, false, 3>;        // features[12], [13]
+using FusedB14 = FusedCfg<96, 576, 32, 160, 8, 2, 4, 2, false, false, 3>;      // features[14]
 // blocks 15-17: four faces per tile (64 GEMM rows = one MMA slab), so that the 64 x COUT fp32 D2 accumulator fits the
 // registers of the worker warpgroups
 using FusedB15 = FusedCfg<160, 960, 32, 160, 4, 1, 4, 4, true, false, 3>;      // features[15], [16]
-using FusedB17 = FusedCfg<160, 960, SYN_NC_B17, 320, 4, 1, 4, 4, false, false, SYN_NC_B17 == 16 ? 3 : 2>;     // features[17]
+using FusedB17 = FusedCfg<160, 960, 32, 320, 4, 1, 4, 4, false, false, 2>;     // features[17]
 
 }  // namespace syn

@@ -386,9 +386,6 @@ int run_reconstruct_tc(syn_handle* h, const float* params, int batch, int dense,
   const int items = a.n_vtiles * a.n_ftiles;
   // dense mesh: face-major walk with streamed basis planes (long contiguous output runs per CTA); the 68-landmark
   // basis is one vertex tile, where the two kernels do the same work -- keep the simpler one there.
-  static const bool fm_off = getenv("SYN_DENSE_VERTEX_MAJOR") != nullptr;      // A/B switches for measurements
-  static const bool wb_stores = getenv("SYN_DENSE_WB_STORES") != nullptr;
-  a.stream_stores = wb_stores ? 0 : 1;
   a.trace = nullptr;
   static long long* d_dense_trace = nullptr;                                   // debug: SYN_DENSE_TRACE=file dumps CTA 0's timeline
   static const char* trace_fp = getenv("SYN_DENSE_TRACE");
@@ -397,7 +394,7 @@ int run_reconstruct_tc(syn_handle* h, const float* params, int batch, int dense,
     cudaMemsetAsync(d_dense_trace, 0, 192 * 8 * sizeof(long long), st);
     a.trace = d_dense_trace;
   }
-  if (dense && !fm_off) {
+  if (dense) {
     // grid = face tiles x vertex bands (see the kernel): as many whole bands as fit the SMs
     const int n_bands = std::max(1, h->sm_count / a.n_ftiles);
     const int grid = a.n_ftiles * std::min(n_bands, a.n_vtiles);
@@ -543,68 +540,13 @@ void pack_fused(std::vector<uint8_t>& img, const float* w1, int K, const float* 
   }
 }
 
-// Worker warps of the fused kernel: 8 by default (H100, 1024-face step: 5.13 ms against 5.76 ms with 16, whose
-// 17-warp CTAs leave 96 registers per thread and spill); SYN_FUSED_WARPS=8|12|16 selects another instantiation for
-// tuning runs.
-inline int fused_worker_warps(int block) {
-  static const struct Table {
-    int v[18];
-    Table() {
-      const char* e = getenv("SYN_FUSED_WARPS");
-      const int n = e ? atoi(e) : 8;
-      const int all = (n == 8 || n == 12 || n == 16 || n == 20 || n == 24) ? n : 8;
-      for (int i = 0; i < 18; ++i) v[i] = all;
-      // per block: SYN_FUSED_WARPS_MAP="1:24,2:20" (tuning runs)
-      const char* m = getenv("SYN_FUSED_WARPS_MAP");
-      while (m && *m) {
-        const int b = atoi(m);
-        const char* c = strchr(m, ':');
-        if (!c) break;
-        const int w = atoi(c + 1);
-        if (b >= 1 && b <= 17 && (w == 8 || w == 12 || w == 16 || w == 20 || w == 24)) v[b] = w;
-        m = strchr(c, ',');
-        if (m) ++m;
-      }
-    }
-  } t;
-  return t.v[block];
-}
-
-template <class C, int NWW>
-int launch_fused_nww(syn_handle* h, const FusedArgs& a, int grid, cudaStream_t st) {
-  static bool attr_set[16] = {};
-  if (!attr_set[h->device & 15]) {
-    SYN_CUDA(cudaFuncSetAttribute(fused_mbconv_kernel<C, NWW>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-    attr_set[h->device & 15] = true;
-    if (getenv("SYN_DEBUG_OCC") != nullptr) {
-      int nb = -1;
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fused_mbconv_kernel<C, NWW>, (NWW + 1) * 32, C::SMEM_BYTES);
-      fprintf(stderr, "[syn] fused CIN=%d CHID=%d W=%d: %d worker warps, %d B smem -> %d CTA(s)/SM\n",
-              C::CIN, C::CHID, C::W, NWW, C::SMEM_BYTES, nb);
-    }
-  }
-#if SYN_PDL
-  // programmatic dependent launch (experimental, see kernels_fused.cuh): the kernel may start while its
-  // predecessor in the stream drains; it waits (griddepcontrol.wait) before touching the predecessor's output
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3((NWW + 1) * 32);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  SYN_CUDA(cudaLaunchKernelEx(&cfg, fused_mbconv_kernel<C, NWW>, a));
-#else
-  fused_mbconv_kernel<C, NWW><<<grid, (NWW + 1) * 32, C::SMEM_BYTES, st>>>(a);
-#endif
-  return SYN_OK;
-}
-
 template <class C>
 int launch_fused(syn_handle* h, const float* x, int block, float* y, int batch, cudaStream_t st, const uint8_t* x_u8) {
+  static bool attr_set[16] = {};
+  if (!attr_set[h->device & 15]) {
+    SYN_CUDA(cudaFuncSetAttribute(fused_mbconv_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    attr_set[h->device & 15] = true;
+  }
   FusedArgs a;
   a.x_u8 = x_u8;
   a.x = x; a.wimg = h->d_fused + h->fused_off[block]; a.y = y; a.batch = batch; a.err = h->d_err; a.sat = h->d_sat; a.npass = h->npass(); a.border = h->center_crop;
@@ -613,18 +555,19 @@ int launch_fused(syn_handle* h, const float* x, int block, float* y, int batch, 
 #endif
   fused_tile_plan<C>(batch, h->sm_count, a.split, a.face_groups);
   const int ntiles = a.face_groups * C::STRIPS;
-  const int grid = std::min(ntiles, h->sm_count);
-  int rc;
-  switch (fused_worker_warps(block)) {
-    case 8: rc = launch_fused_nww<C, 8>(h, a, grid, st); break;
-    case 12: rc = launch_fused_nww<C, 12>(h, a, grid, st); break;
-#ifdef SYN_MORE_WARPS
-    case 20: rc = launch_fused_nww<C, 20>(h, a, grid, st); break;
-    case 24: rc = launch_fused_nww<C, 24>(h, a, grid, st); break;
-#endif
-    default: rc = launch_fused_nww<C, 16>(h, a, grid, st); break;
-  }
-  if (rc != SYN_OK) return rc;
+  // programmatic dependent launch: the kernel may start while its predecessor in the stream drains; it waits
+  // (griddepcontrol.wait) before touching the predecessor's output
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(std::min(ntiles, h->sm_count));
+  cfg.blockDim = dim3((kFusedWorkerWarps + 1) * 32);
+  cfg.dynamicSmemBytes = C::SMEM_BYTES;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  SYN_CUDA(cudaLaunchKernelEx(&cfg, fused_mbconv_kernel<C>, a));
   SYN_LAUNCH_CHECK("fused_mbconv_kernel");
   static const char* const names[18] = {"", "fused_stem_block1", "fused_block2", "fused_block3", "fused_block4",
                                         "fused_block5", "fused_block6", "fused_block7", "fused_block8", "fused_block9",
@@ -1097,33 +1040,11 @@ int syn_forward_landmarks_u8(syn_handle_t* h, const uint8_t* x_u8, int batch, fl
 
 // Faces per pipeline chunk: large enough that the 8x8 / 4x4 blocks still fill the 132 SMs, small enough that the copies
 // hide behind compute.  The FIRST chunk is small: its host->device copy is the only one nothing can overlap.
-// SYN_HOST_CHUNK / SYN_HOST_CHUNK0 override both for measurements.
-static int host_chunk_faces() {
-  static const int v = [] {
-    const char* e = getenv("SYN_HOST_CHUNK");
-    const int c = e ? atoi(e) : 0;
-    return c > 0 ? c : 512;
-  }();
-  return v;
-}
-static int host_submit_chunk_faces() {
-  static const int v = [] {
-    const char* e = getenv("SYN_HOST_CHUNK_SUBMIT");
-    const int c = e ? atoi(e) : 0;
-    return c > 0 ? c : 1024;
-  }();
-  return v;
-}
-static int host_first_chunk_faces() {
-  static const int v = [] {
-    const char* e = getenv("SYN_HOST_CHUNK0");
-    const int c = e ? atoi(e) : 0;
-    return c > 0 ? c : 512;
-  }();
-  return v;
-}
+// A blocking call can only overlap its own chunks (512 + 512); a submitted call overlaps with its neighbours in the
+// queue, so it runs whole 1024-face launches.
+constexpr int kHostChunkFaces = 512, kHostSubmitChunkFaces = 1024, kHostFirstChunkFaces = 512;
 
-// Shared host pipeline: chunks of host_chunk_faces() faces, H2D on s_copy overlapped with compute on s_compute.
+// Shared host pipeline: chunks of kHostChunkFaces faces, H2D on s_copy overlapped with compute on s_compute.
 // Everything is stream-ordered, so a second call may be submitted while the first one computes: its H2D copies then run
 // under the first call's kernels (the staging slots and their events persist across calls; the result staging buffers
 // are reused in s_compute order, after the previous call's D2H).  At most two calls are in flight.
@@ -1133,9 +1054,7 @@ static int host_submit_impl(syn_handle_t* h, const void* x_host, int is_u8, int 
   DeviceGuard g(h->device);
   const unsigned long long seq = h->host_calls;
   if (seq >= 2) SYN_CUDA(cudaEventSynchronize(h->ev_call[seq & 1]));   // ticket seq - 2 owns this event: it must be done
-  // A blocking call can only overlap its own chunks (512 + 512); a submitted call overlaps with its neighbours in the
-  // queue, so it runs whole 1024-face launches.
-  const int chunk = std::min(batch, blocking ? host_chunk_faces() : host_submit_chunk_faces());
+  const int chunk = std::min(batch, blocking ? kHostChunkFaces : kHostSubmitChunkFaces);
   const size_t x_face = (size_t)3 * kImg * kImg;
   const size_t elt = is_u8 ? 1 : sizeof(float);
   const size_t lmk_face = (size_t)3 * h->n_pts;
@@ -1177,7 +1096,7 @@ static int host_submit_impl(syn_handle_t* h, const void* x_host, int is_u8, int 
   int issued = 0;
   for (int b0 = 0, nb = 0; b0 < batch; b0 += nb, h->host_slot ^= 1, ++h->host_chunks, ++issued) {
     const int slot = h->host_slot;
-    nb = std::min(issued == 0 && blocking ? std::min(chunk, host_first_chunk_faces()) : chunk, batch - b0);
+    nb = std::min(issued == 0 && blocking ? std::min(chunk, kHostFirstChunkFaces) : chunk, batch - b0);
     if (h->host_chunks >= 2) SYN_CUDA(cudaStreamWaitEvent(h->s_copy, h->ev_done[slot], 0));   // the slot's last reader
     SYN_CUDA(cudaMemcpyAsync(stage[slot], (const uint8_t*)x_host + (size_t)b0 * x_face * elt, nb * x_face * elt,
                              cudaMemcpyHostToDevice, h->s_copy));

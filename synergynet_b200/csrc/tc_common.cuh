@@ -94,20 +94,13 @@ __device__ __forceinline__ bool mbar_wait_spin(uint32_t bar, uint32_t parity, in
 __device__ __noinline__ bool mbar_wait_slow(uint32_t bar, uint32_t parity, int* err_flag) {
   return mbar_wait_spin(bar, parity, err_flag);
 }
-// SYN_MBAR_INLINE: a real call in a kernel makes ptxas keep the global-memory descriptor in a vector register and copy it
-// to a uniform register pair (2 x R2UR) in front of every LDG / STG; the spin loop inlined costs less code than that.
-#ifndef SYN_MBAR_INLINE
-#define SYN_MBAR_INLINE 0
-#endif
 __device__ __forceinline__ bool mbar_wait(uint32_t bar, uint32_t parity, int* err_flag) {
   if (mbar_try_wait(bar, parity)) return true;
-#if SYN_MBAR_INLINE
-  return mbar_wait_spin(bar, parity, err_flag);
-#else
   return mbar_wait_slow(bar, parity, err_flag);
-#endif
 }
-// always-inline flavour for kernels whose hot loop is made of global stores (dense_recon_fm_kernel)
+// always-inline flavour for kernels whose hot loop is made of global stores (dense_recon_fm_kernel): a real call in a
+// kernel makes ptxas keep the global-memory descriptor in a vector register and copy it to a uniform register pair
+// (2 x R2UR) in front of every LDG / STG; the spin loop inlined costs less code than that.
 __device__ __forceinline__ bool mbar_wait_inl(uint32_t bar, uint32_t parity, int* err_flag) {
   if (mbar_try_wait(bar, parity)) return true;
   return mbar_wait_spin(bar, parity, err_flag);
