@@ -158,6 +158,77 @@ def reparametrize_pointnet(sd: Dict[str, torch.Tensor], seed: int, lo: int, hi: 
     return out
 
 
+def reparametrize_3dmm(pack: dict, seed: int, lo: int, hi: int) -> dict:
+    """The same morphable model with a wide spread of coefficient scales: basis column k (shape and expression) is
+    multiplied by 2^e_k and the whitening mean / std of coefficient k divided by it, e_k an integer in [lo, hi] (one
+    coefficient at each end).  Every product W_ck alpha_k is unchanged, so the fp32 reference is bit-identical, while the
+    library's alpha scales and basis row scales move."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    e = rng.integers(lo, hi + 1, 50)
+    ends = rng.permutation(50)[:2]
+    e[ends[0]], e[ends[1]] = lo, hi
+    f = np.exp2(e).astype(np.float32)
+    out = dict(pack)
+    out['w_shp'] = pack['w_shp'] * f[:40]
+    out['w_exp'] = pack['w_exp'] * f[40:]
+    for key in ('param_mean', 'param_std'):
+        out[key] = pack[key].copy()
+        out[key][12:62] /= f
+    return out
+
+
+STRESS_ZERO_COEF = 45            # the coefficient of stress_3dmm with mean = std = 0
+
+
+def stress_3dmm(pack: dict, seed: int = 0) -> dict:
+    """A morphable model (make_3dmm format) with the rows the basis packing treats specially, in both the dense and
+    the keypoint (sparse) rows: rows with u = 0, all-zero basis rows (row scale 1), rows where one column is 2^20 times
+    the others, and one coefficient (``STRESS_ZERO_COEF``) with mean = std = 0, whose alpha scale is then 2^10."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    kp = pack['keypoints']
+    n3 = pack['w_shp'].shape[0]
+    pick = lambda n: np.concatenate([rng.choice(kp, n, replace=False), rng.choice(n3, 4 * n, replace=False)])
+    u_shp, u_exp = pack['u_shp'].copy(), pack['u_exp'].copy()
+    w = np.concatenate([pack['w_shp'], pack['w_exp']], 1)
+    zero_u, zero_w, spike = pick(12), pick(12), pick(12)
+    u_shp[zero_u], u_exp[zero_u] = 0.0, 0.0
+    w[zero_w] = 0.0
+    cols = rng.integers(0, 50, len(spike))
+    w[spike, cols] *= np.float32(2.0 ** 20)
+    out = dict(pack, u_shp=u_shp, u_exp=u_exp, w_shp=np.ascontiguousarray(w[:, :40]),
+               w_exp=np.ascontiguousarray(w[:, 40:]))
+    for key in ('param_mean', 'param_std'):
+        out[key] = pack[key].copy()
+        out[key][12 + STRESS_ZERO_COEF] = 0.0
+    return out
+
+
+def basis_arrays(n: int, seed: int):
+    """(u (3n, 1), w_shp (3n, 40), w_exp (3n, 10)) fp32 with the statistics of synthetic.make_3dmm, for bases of any
+    size (make_3dmm needs at least 68 vertices)."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    d = rng.standard_normal((n, 3))
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    u = (d * np.array([7.0e4, 9.0e4, 6.0e4])).reshape(-1, 1) + rng.standard_normal((3 * n, 1)) * 2.0e2
+    return (u.astype(np.float32), rng.standard_normal((3 * n, 40)).astype(np.float32),
+            rng.standard_normal((3 * n, 10)).astype(np.float32))
+
+
+def recon_pack(base: dict, dense=None, sparse=None) -> dict:
+    """Reconstruction pack (reference_port.gather_sparse_basis format) of the make_3dmm-format ``base``, with the dense
+    and / or sparse basis replaced by (u, w_shp, w_exp) arrays."""
+    from oracle import reference_port as rp
+    out = rp.gather_sparse_basis(base)
+    if dense is not None:
+        out['u'], out['w_shp'], out['w_exp'] = dense
+    if sparse is not None:
+        out['u_base'], out['w_shp_base'], out['w_exp_base'] = sparse
+    return out
+
+
 @torch.no_grad()
 def _calibrate_pointnet(sd: Dict[str, torch.Tensor], pooled: torch.Tensor, seed: int) -> None:
     """Same treatment for the BatchNorm1d layers of forwardDirection / reverseDirection (reference

@@ -14,7 +14,8 @@
 //     warps 0-15: four warpgroups; warpgroup w runs the MMAs (3 planes x 3 passes x 4 K-steps, N = 32) of
 //                 vertices 64 (w & 1) .. +63 x faces 32 (w >> 1) .. +31 of every item and their epilogue
 // Split-16x3 precision scheme of kernels_tc.cuh; basis rows are pre-scaled per vertex row and alpha
-// per coefficient (both powers of two, folded back exactly in the epilogue / the basis image).
+// per coefficient (both powers of two, folded back exactly in the epilogue / the basis image); a face whose scaled
+// coefficients leave the fp16 range is further divided by a per-face power of two (dense_alpha_kernel).
 #pragma once
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -27,7 +28,7 @@ constexpr int kDnAPlane = 128 * kDnK * 2;                 // 16 KB: one plane (h
 constexpr int kDnATile = 3 * 2 * kDnAPlane;               // 96 KB per 128-vertex tile: [x|y|z][hi|lo]
 constexpr int kDnBPlane = kDnFaces * kDnK * 2;            // 8 KB
 constexpr int kDnBTile = 2 * kDnBPlane;                   // 16 KB per face tile: [hi|lo]
-constexpr int kDnPoseStride = 20;                        // floats per face: [R|t] (12), crop->image affine kx, sx, ky, sy, kz, pad
+constexpr int kDnPoseStride = 20;                        // floats per face: [R|t] (12), crop->image affine kx, sx, ky, sy, kz, face scale fs, pad
 constexpr int kDnPoseTile = kDnFaces * kDnPoseStride * 4; // 5 KB
 constexpr int kDnBSlot = kDnBTile + kDnPoseTile;
 constexpr int kDnMetaTile = 128 * 6 * 4;                  // per vertex tile: u[3][128], 1/rowscale[3][128]
@@ -61,7 +62,29 @@ __global__ void __launch_bounds__(kDnAlphaThreads) dense_alpha_kernel(const floa
     }
     return v;
   };
-  // pose row: float4 #kg of [R|t] (kg 0..2), crop -> image affine kx,sx,ky,sy (3), kz,0,0,0 (4)
+  float a[8], amax = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int k = kg * 8 + j;
+    a[j] = (k < kNumAlpha) ? param(12 + k) * ascale[k] : 0.f;
+    amax = fmaxf(amax, fabsf(a[j]));
+  }
+  // Face scale: ascale bounds |alpha_k * ascale_k| by 2^10 within 8 sigma of the mean, but a face further out (or raw
+  // coefficients with whitening off) would hit split2_f16's clamp at 60000.  Such a face is divided by a power of two
+  // fs that brings its largest scaled coefficient into [2^14, 2^15); the epilogues multiply the accumulator by fs
+  // (exact).  Faces inside the clamp keep fs = 1 and their results bit for bit.
+  __shared__ float s_amax[kDnK / 8][kDnFaces];
+  s_amax[kg][f] = amax;
+  __syncthreads();
+#pragma unroll
+  for (int g = 0; g < kDnK / 8; ++g) amax = fmaxf(amax, s_amax[g][f]);
+  float fs = 1.f, fs_inv = 1.f;
+  if (amax > 60000.f && isfinite(amax)) {
+    const int ex = ((__float_as_int(amax) >> 23) & 0xff) - 126;     // amax in [2^(ex-1), 2^ex)
+    fs = __int_as_float((ex - 15 + 127) << 23);
+    fs_inv = __int_as_float((127 - ex + 15) << 23);
+  }
+  // pose row: float4 #kg of [R|t] (kg 0..2), crop -> image affine kx,sx,ky,sy (3), kz,fs,0,0 (4)
   // (utils/inference.py:127-138: x*kx+sx, y*ky+sy, z*kz; identity if absent)
   if (kg < kDnPoseStride / 4) {
     float4 v;
@@ -71,18 +94,13 @@ __global__ void __launch_bounds__(kDnAlphaThreads) dense_alpha_kernel(const floa
       const bool has = roi5 != nullptr && live;
       const float* r = roi5 + (size_t)b * 5;
       if (kg == 3) v = make_float4(has ? r[0] : 1.f, has ? r[1] : 0.f, has ? r[2] : 1.f, has ? r[3] : 0.f);
-      else v = make_float4(has ? r[4] : 1.f, 0.f, 0.f, 0.f);
+      else v = make_float4(has ? r[4] : 1.f, fs, 0.f, 0.f);
     }
     *reinterpret_cast<float4*>(pose + (size_t)(tile * kDnFaces + f) * kDnPoseStride + 4 * kg) = v;
   }
   uint32_t h[4], l[4];
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const int k0 = kg * 8 + 2 * j, k1 = k0 + 1;
-    const float a0 = (k0 < kNumAlpha) ? param(12 + k0) * ascale[k0] : 0.f;
-    const float a1 = (k1 < kNumAlpha) ? param(12 + k1) * ascale[k1] : 0.f;
-    tc::split2_f16(a0, a1, h[j], l[j]);
-  }
+  for (int j = 0; j < 4; ++j) tc::split2_f16(a[2 * j] * fs_inv, a[2 * j + 1] * fs_inv, h[j], l[j]);
   uint8_t* hi = aimg + (size_t)tile * kDnBTile + kg * 1024 + f * 16;   // (f >> 3) * 128 + (f & 7) * 16 = f * 16
   *reinterpret_cast<uint4*>(hi) = make_uint4(h[0], h[1], h[2], h[3]);
   *reinterpret_cast<uint4*>(hi + kDnBPlane) = make_uint4(l[0], l[1], l[2], l[3]);
@@ -180,7 +198,9 @@ __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_tc_kernel(const Den
           const float4 r0 = *reinterpret_cast<const float4*>(pose);
           const float4 r1 = *reinterpret_cast<const float4*>(pose + 4);
           const float4 r2 = *reinterpret_cast<const float4*>(pose + 8);
-          const float X = fmaf(acc[0][q], ox[h], ux[h]), Y = fmaf(acc[1][q], oy[h], uy[h]), Z = fmaf(acc[2][q], oz[h], uz[h]);
+          const float fs = pose[17];                             // face scale (dense_alpha_kernel)
+          const float X = fmaf(acc[0][q] * fs, ox[h], ux[h]), Y = fmaf(acc[1][q] * fs, oy[h], uy[h]),
+                      Z = fmaf(acc[2][q] * fs, oz[h], uz[h]);
           float vx = fmaf(r0.x, X, fmaf(r0.y, Y, fmaf(r0.z, Z, r0.w)));
           float vy = fmaf(r1.x, X, fmaf(r1.y, Y, fmaf(r1.z, Z, r1.w)));
           float vz = fmaf(r2.x, X, fmaf(r2.y, Y, fmaf(r2.z, Z, r2.w)));
@@ -385,6 +405,20 @@ __global__ void __launch_bounds__(kDnThreads, 1) dense_recon_fm_kernel(const Den
       wgmma_wait<0>();
 #pragma unroll
       for (int c = 0; c < 3; ++c) mbar_arrive(smem_u32(&bar_pempty[(3 * i + c) % kFmPSlots]));   // planes may be refilled
+      // face scales (dense_alpha_kernel) of this thread's four faces, applied to the accumulators before the epilogue
+      // (exact: powers of two; the same values as fmaf(acc * fs, ox, ux) in dense_recon_tc_kernel)
+#pragma unroll
+      for (int sr = 0; sr < 2; ++sr)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float fs = pose_tile[(f0 + sr * kFmSubFaces + 2 * (t & 3) + e) * kDnPoseStride + 17];
+#pragma unroll
+          for (int c = 0; c < 3; ++c)
+#pragma unroll
+            for (int sl = 0; sl < 2; ++sl)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) acc[c][sl][4 * sr + 2 * h + e] *= fs;
+        }
       if (tr) p.trace[i * 8 + 2] = clock64();
       const bool first = i == 0, last = i == n_items - 1;
       const bool edge = first || last || (ft + 1) * kDnFaces > p.batch;     // CTA-uniform
