@@ -303,6 +303,20 @@ int  syn_fb_commit(syn_fb_t* f);
  * `self.net(img)` returns, P = syn_faceboxes_num_priors(height, width); feed them to syn_faceboxes_decode + syn_nms. */
 int  syn_fb_forward(syn_fb_t* f, const uint8_t* image_dev, int height, int width, float* loc_dev, float* conf_dev, void* stream);
 int64_t syn_fb_launch_count(const syn_fb_t* f);
+/* Per-stage tests of the detector network.  Runs syn_fb_forward's launch sequence unchanged and returns right after launch
+ * `stage` (0..38), having copied (on the stream) the whole tensor that launch wrote to out_dev, which holds out_numel
+ * floats (SYN_ERR_SHAPE if that is not the tensor's size).  NHWC maps of an h x w image, n3/n4/n5 = the pixels of the
+ * stride-32/64/128 maps, P = syn_faceboxes_num_priors(h, w):
+ *   0 conv1 (CReLU, 48 ch)   1 max-pool (48 ch)   2 conv2 (CReLU, 128 ch)   3 max-pool (128 ch: inception1's input)
+ *   4 + 8b .. 11 + 8b, inception b = 0..2: branch1x1 -> block output (all 128 ch; it owns 0..31), avg-pool of the
+ *     block input (128 ch), branch1x1_2 -> block output (owns 32..63), branch3x3_reduce (24 ch), branch3x3 -> block
+ *     output (owns 64..95), branch3x3_reduce_2 (24 ch), branch3x3_2 (32 ch), branch3x3_3 -> block output (owns 96..127)
+ *   28 conv3_1 (128 ch)   29 conv3_2 (256 ch)   30 conv4_1 (128 ch)   31 conv4_2 (256 ch)
+ *   32..34 loc.0..2 -> the whole loc_dev (P*4; loc.k owns offsets from 0, n3*84, n3*84 + n4*4)
+ *   35..37 conf.0..2 -> the whole conf_dev (P*2 logits; offsets 0, n3*42, n3*42 + n4*2)   38 softmax -> conf_dev (P*2)
+ * The block input is stage 3 for inception1 and the previous block's stage 11 + 8b otherwise. */
+int  syn_fb_debug_forward_until(syn_fb_t* f, const uint8_t* image_dev, int height, int width, int stage, float* out_dev,
+                                int64_t out_numel, float* loc_dev, float* conf_dev, void* stream);
 
 /* ---- introspection ---------------------------------------------------------------------------*/
 /* Number of kernels this handle has launched since creation (bench.py "gpu_launches"). */

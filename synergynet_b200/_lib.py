@@ -104,6 +104,7 @@ SIGNATURES = {
     'syn_fb_commit': (_I, [_P]),
     'syn_fb_forward': (_I, [_P, _F, _I, _I, _F, _F, _P]),
     'syn_fb_launch_count': (_L, [_P]),
+    'syn_fb_debug_forward_until': (_I, [_P, _F, _I, _I, _I, _F, _L, _F, _F, _P]),
     'syn_faceboxes_decode': (_I, [_F, _F, _I, _I, C.c_float, C.c_float, C.c_float, C.c_float, _I, _F, _F, _F, _P]),
     'syn_launch_count': (_L, [_P]),
     'syn_set_timing': (_I, [_P, _I]),
@@ -125,7 +126,8 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_mesh_incidence_host', 'syn_mesh_normals', 'syn_mesh_lighting', 'syn_rasterize', 'syn_nms',
                                              'syn_crop_resize_plan_size', 'syn_crop_resize_plan_host', 'syn_crop_resize',
                                              'syn_faceboxes_num_priors', 'syn_faceboxes_decode', 'syn_fb_num_layers', 'syn_fb_layer_desc', 'syn_fb_create',
-                                             'syn_fb_destroy', 'syn_fb_set_layer', 'syn_fb_commit', 'syn_fb_forward', 'syn_fb_launch_count')}
+                                             'syn_fb_destroy', 'syn_fb_set_layer', 'syn_fb_commit', 'syn_fb_forward', 'syn_fb_launch_count',
+                                             'syn_fb_debug_forward_until')}
 
 
 def declared_symbols(header: str = HEADER_PATH):

@@ -303,6 +303,111 @@ int fb_conv(syn_fb* f, int idx, const float* x, const uint8_t* x_u8, int h, int 
   return SYN_OK;
 }
 
+// A debug run (syn_fb_debug_forward_until): the production launch sequence, stopped right after launch `stage`, whose
+// whole destination tensor is copied to `out` on the same stream.  Production calls pass nullptr.
+constexpr int kFbStages = 39;
+struct FbStop {
+  int stage;
+  float* out;
+  int64_t numel;
+};
+
+int fb_stop_copy(const FbStop* d, const float* src, size_t n, cudaStream_t st) {
+  if (d->numel != (int64_t)n)
+    return fail(SYN_ERR_SHAPE, "syn_fb_debug_forward_until: stage %d writes %lld floats, out_numel is %lld", d->stage,
+                (long long)n, (long long)d->numel);
+  SYN_CUDA(cudaMemcpyAsync(d->out, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return SYN_OK;
+}
+
+// after launch s: return from the enclosing function if a debug run stops there
+#define SYN_FB_STOP(d, s, src, n, st) \
+  do { if ((d) != nullptr && (d)->stage == (s)) return fb_stop_copy((d), (src), (n), (st)); } while (0)
+
+// syn_fb_forward's launch sequence; `stop` (nullable) ends it early.  Stages are the launches in order, see the table
+// at syn_fb_debug_forward_until in include/synergy_b200.h.
+int fb_forward_body(syn_fb* f, const uint8_t* image_dev, int height, int width, float* loc_dev, float* conf_dev,
+                    cudaStream_t st, const FbStop* stop, const char* who) {
+  if (!f || !image_dev || !loc_dev || !conf_dev || height <= 0 || width <= 0) return fail(SYN_ERR_INVALID, "%s: bad argument", who);
+  if (!f->committed) return fail(SYN_ERR_STATE, "%s before syn_fb_commit", who);
+  SYN_CUDA(cudaSetDevice(f->device));
+  if (int rc = fb_workspace(f, height, width)) return rc;
+  const FbGeom g = fb_geom(height, width);
+  if (g.h3 != fb_cells(height, 32) || g.w3 != fb_cells(width, 32) || g.h4 != fb_cells(height, 64) || g.w4 != fb_cells(width, 64) ||
+      g.h5 != fb_cells(height, 128) || g.w5 != fb_cells(width, 128))
+    return fail(SYN_ERR_SHAPE, "%s: feature maps of a %dx%d input do not match the prior grid", who, height, width);
+  auto pool_grid = [](size_t n) { return (unsigned)((n + 255) / 256); };
+  const size_t n1 = (size_t)g.h1 * g.w1, np1 = (size_t)g.hp1 * g.wp1, n2 = (size_t)g.h2 * g.w2;
+  const size_t n3 = (size_t)g.h3 * g.w3, n4 = (size_t)g.h4 * g.w4, n5 = (size_t)g.h5 * g.w5;
+  const int np = (int)(n3 * 21 + n4 + n5);
+  // conv1 (CReLU) -> max-pool -> conv2 (CReLU) -> max-pool                                          faceboxes.py:120-123
+  if (int rc = fb_conv(f, 0, nullptr, image_dev, height, width, 3, 0, f->c1, 48, 0, st)) return rc;
+  SYN_FB_STOP(stop, 0, f->c1, n1 * 48, st);
+  fb_maxpool_kernel<<<pool_grid(np1 * 48), 256, 0, st>>>(f->c1, g.h1, g.w1, 48, f->p1, g.hp1, g.wp1);
+  SYN_LAUNCH_CHECK("fb_maxpool_kernel");
+  ++f->launches;
+  SYN_FB_STOP(stop, 1, f->p1, np1 * 48, st);
+  if (int rc = fb_conv(f, 1, f->p1, nullptr, g.hp1, g.wp1, 48, 0, f->c2, 128, 0, st)) return rc;
+  SYN_FB_STOP(stop, 2, f->c2, n2 * 128, st);
+  fb_maxpool_kernel<<<pool_grid(n3 * 128), 256, 0, st>>>(f->c2, g.h2, g.w2, 128, f->xa, g.h3, g.w3);
+  SYN_LAUNCH_CHECK("fb_maxpool_kernel");
+  ++f->launches;
+  SYN_FB_STOP(stop, 3, f->xa, n3 * 128, st);
+  // three inception blocks: every branch writes its 32-channel slice of the next 128-channel tensor     :124-126, :33-47
+  float *x = f->xa, *y = f->xb;
+  for (int blk = 0; blk < 3; ++blk) {
+    const int L0 = 2 + 7 * blk, s0 = 4 + 8 * blk;
+    if (int rc = fb_conv(f, L0 + 0, x, nullptr, g.h3, g.w3, 128, 0, y, 128, 0, st)) return rc;
+    SYN_FB_STOP(stop, s0 + 0, y, n3 * 128, st);
+    fb_avgpool_kernel<<<pool_grid(n3 * 128), 256, 0, st>>>(x, g.h3, g.w3, 128, f->avg);
+    SYN_LAUNCH_CHECK("fb_avgpool_kernel");
+    ++f->launches;
+    SYN_FB_STOP(stop, s0 + 1, f->avg, n3 * 128, st);
+    if (int rc = fb_conv(f, L0 + 1, f->avg, nullptr, g.h3, g.w3, 128, 0, y, 128, 32, st)) return rc;
+    SYN_FB_STOP(stop, s0 + 2, y, n3 * 128, st);
+    if (int rc = fb_conv(f, L0 + 2, x, nullptr, g.h3, g.w3, 128, 0, f->r1, 24, 0, st)) return rc;
+    SYN_FB_STOP(stop, s0 + 3, f->r1, n3 * 24, st);
+    if (int rc = fb_conv(f, L0 + 3, f->r1, nullptr, g.h3, g.w3, 24, 0, y, 128, 64, st)) return rc;
+    SYN_FB_STOP(stop, s0 + 4, y, n3 * 128, st);
+    if (int rc = fb_conv(f, L0 + 4, x, nullptr, g.h3, g.w3, 128, 0, f->r2, 24, 0, st)) return rc;
+    SYN_FB_STOP(stop, s0 + 5, f->r2, n3 * 24, st);
+    if (int rc = fb_conv(f, L0 + 5, f->r2, nullptr, g.h3, g.w3, 24, 0, f->t3, 32, 0, st)) return rc;
+    SYN_FB_STOP(stop, s0 + 6, f->t3, n3 * 32, st);
+    if (int rc = fb_conv(f, L0 + 6, f->t3, nullptr, g.h3, g.w3, 32, 0, y, 128, 96, st)) return rc;
+    SYN_FB_STOP(stop, s0 + 7, y, n3 * 128, st);
+    float* t = x; x = y; y = t;
+  }
+  // x = inception3 output (detection source 0); conv3_x, conv4_x give sources 1 and 2                  :127-135
+  if (int rc = fb_conv(f, 23, x, nullptr, g.h3, g.w3, 128, 0, f->c31, 128, 0, st)) return rc;
+  SYN_FB_STOP(stop, 28, f->c31, n3 * 128, st);
+  if (int rc = fb_conv(f, 24, f->c31, nullptr, g.h3, g.w3, 128, 0, f->c32, 256, 0, st)) return rc;
+  SYN_FB_STOP(stop, 29, f->c32, n4 * 256, st);
+  if (int rc = fb_conv(f, 25, f->c32, nullptr, g.h4, g.w4, 256, 0, f->c41, 128, 0, st)) return rc;
+  SYN_FB_STOP(stop, 30, f->c41, n4 * 128, st);
+  if (int rc = fb_conv(f, 26, f->c41, nullptr, g.h4, g.w4, 128, 0, f->c42, 256, 0, st)) return rc;
+  SYN_FB_STOP(stop, 31, f->c42, n5 * 256, st);
+  // heads: NHWC output of each source IS permute(0,2,3,1).view(-1) (:137-142); the three sources are concatenated by offset
+  if (int rc = fb_conv(f, 27, x, nullptr, g.h3, g.w3, 128, 0, loc_dev, 84, 0, st)) return rc;
+  SYN_FB_STOP(stop, 32, loc_dev, (size_t)np * 4, st);
+  if (int rc = fb_conv(f, 28, f->c32, nullptr, g.h4, g.w4, 256, 0, loc_dev + n3 * 84, 4, 0, st)) return rc;
+  SYN_FB_STOP(stop, 33, loc_dev, (size_t)np * 4, st);
+  if (int rc = fb_conv(f, 29, f->c42, nullptr, g.h5, g.w5, 256, 0, loc_dev + n3 * 84 + n4 * 4, 4, 0, st)) return rc;
+  SYN_FB_STOP(stop, 34, loc_dev, (size_t)np * 4, st);
+  if (int rc = fb_conv(f, 30, x, nullptr, g.h3, g.w3, 128, 0, conf_dev, 42, 0, st)) return rc;
+  SYN_FB_STOP(stop, 35, conf_dev, (size_t)np * 2, st);
+  if (int rc = fb_conv(f, 31, f->c32, nullptr, g.h4, g.w4, 256, 0, conf_dev + n3 * 42, 2, 0, st)) return rc;
+  SYN_FB_STOP(stop, 36, conf_dev, (size_t)np * 2, st);
+  if (int rc = fb_conv(f, 32, f->c42, nullptr, g.h5, g.w5, 256, 0, conf_dev + n3 * 42 + n4 * 2, 2, 0, st)) return rc;
+  SYN_FB_STOP(stop, 37, conf_dev, (size_t)np * 2, st);
+  fb_softmax2_kernel<<<(np + 255) / 256, 256, 0, st>>>(conf_dev, np);
+  SYN_LAUNCH_CHECK("fb_softmax2_kernel");
+  ++f->launches;
+  SYN_FB_STOP(stop, 38, conf_dev, (size_t)np * 2, st);
+  return SYN_OK;
+}
+
+#undef SYN_FB_STOP
+
 }  // namespace
 
 extern "C" {
@@ -386,58 +491,16 @@ int syn_fb_commit(syn_fb_t* f) {
 int64_t syn_fb_launch_count(const syn_fb_t* f) { return f ? f->launches : 0; }
 
 int syn_fb_forward(syn_fb_t* f, const uint8_t* image_dev, int height, int width, float* loc_dev, float* conf_dev, void* stream) {
-  if (!f || !image_dev || !loc_dev || !conf_dev || height <= 0 || width <= 0) return fail(SYN_ERR_INVALID, "syn_fb_forward: bad argument");
-  if (!f->committed) return fail(SYN_ERR_STATE, "syn_fb_forward before syn_fb_commit");
-  SYN_CUDA(cudaSetDevice(f->device));
-  if (int rc = fb_workspace(f, height, width)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  const FbGeom g = fb_geom(height, width);
-  if (g.h3 != fb_cells(height, 32) || g.w3 != fb_cells(width, 32) || g.h4 != fb_cells(height, 64) || g.w4 != fb_cells(width, 64) ||
-      g.h5 != fb_cells(height, 128) || g.w5 != fb_cells(width, 128))
-    return fail(SYN_ERR_SHAPE, "syn_fb_forward: feature maps of a %dx%d input do not match the prior grid", height, width);
-  auto pool_grid = [](size_t n) { return (unsigned)((n + 255) / 256); };
-  // conv1 (CReLU) -> max-pool -> conv2 (CReLU) -> max-pool                                          faceboxes.py:120-123
-  if (int rc = fb_conv(f, 0, nullptr, image_dev, height, width, 3, 0, f->c1, 48, 0, st)) return rc;
-  fb_maxpool_kernel<<<pool_grid((size_t)g.hp1 * g.wp1 * 48), 256, 0, st>>>(f->c1, g.h1, g.w1, 48, f->p1, g.hp1, g.wp1);
-  SYN_LAUNCH_CHECK("fb_maxpool_kernel");
-  if (int rc = fb_conv(f, 1, f->p1, nullptr, g.hp1, g.wp1, 48, 0, f->c2, 128, 0, st)) return rc;
-  fb_maxpool_kernel<<<pool_grid((size_t)g.h3 * g.w3 * 128), 256, 0, st>>>(f->c2, g.h2, g.w2, 128, f->xa, g.h3, g.w3);
-  SYN_LAUNCH_CHECK("fb_maxpool_kernel");
-  f->launches += 2;
-  // three inception blocks: every branch writes its 32-channel slice of the next 128-channel tensor     :124-126, :33-47
-  float *x = f->xa, *y = f->xb;
-  for (int blk = 0; blk < 3; ++blk) {
-    const int L0 = 2 + 7 * blk;
-    if (int rc = fb_conv(f, L0 + 0, x, nullptr, g.h3, g.w3, 128, 0, y, 128, 0, st)) return rc;
-    fb_avgpool_kernel<<<pool_grid((size_t)g.h3 * g.w3 * 128), 256, 0, st>>>(x, g.h3, g.w3, 128, f->avg);
-    SYN_LAUNCH_CHECK("fb_avgpool_kernel");
-    ++f->launches;
-    if (int rc = fb_conv(f, L0 + 1, f->avg, nullptr, g.h3, g.w3, 128, 0, y, 128, 32, st)) return rc;
-    if (int rc = fb_conv(f, L0 + 2, x, nullptr, g.h3, g.w3, 128, 0, f->r1, 24, 0, st)) return rc;
-    if (int rc = fb_conv(f, L0 + 3, f->r1, nullptr, g.h3, g.w3, 24, 0, y, 128, 64, st)) return rc;
-    if (int rc = fb_conv(f, L0 + 4, x, nullptr, g.h3, g.w3, 128, 0, f->r2, 24, 0, st)) return rc;
-    if (int rc = fb_conv(f, L0 + 5, f->r2, nullptr, g.h3, g.w3, 24, 0, f->t3, 32, 0, st)) return rc;
-    if (int rc = fb_conv(f, L0 + 6, f->t3, nullptr, g.h3, g.w3, 32, 0, y, 128, 96, st)) return rc;
-    float* t = x; x = y; y = t;
-  }
-  // x = inception3 output (detection source 0); conv3_x, conv4_x give sources 1 and 2                  :127-135
-  if (int rc = fb_conv(f, 23, x, nullptr, g.h3, g.w3, 128, 0, f->c31, 128, 0, st)) return rc;
-  if (int rc = fb_conv(f, 24, f->c31, nullptr, g.h3, g.w3, 128, 0, f->c32, 256, 0, st)) return rc;
-  if (int rc = fb_conv(f, 25, f->c32, nullptr, g.h4, g.w4, 256, 0, f->c41, 128, 0, st)) return rc;
-  if (int rc = fb_conv(f, 26, f->c41, nullptr, g.h4, g.w4, 128, 0, f->c42, 256, 0, st)) return rc;
-  // heads: NHWC output of each source IS permute(0,2,3,1).view(-1) (:137-142); the three sources are concatenated by offset
-  const size_t n3 = (size_t)g.h3 * g.w3, n4 = (size_t)g.h4 * g.w4, n5 = (size_t)g.h5 * g.w5;
-  if (int rc = fb_conv(f, 27, x, nullptr, g.h3, g.w3, 128, 0, loc_dev, 84, 0, st)) return rc;
-  if (int rc = fb_conv(f, 28, f->c32, nullptr, g.h4, g.w4, 256, 0, loc_dev + n3 * 84, 4, 0, st)) return rc;
-  if (int rc = fb_conv(f, 29, f->c42, nullptr, g.h5, g.w5, 256, 0, loc_dev + n3 * 84 + n4 * 4, 4, 0, st)) return rc;
-  if (int rc = fb_conv(f, 30, x, nullptr, g.h3, g.w3, 128, 0, conf_dev, 42, 0, st)) return rc;
-  if (int rc = fb_conv(f, 31, f->c32, nullptr, g.h4, g.w4, 256, 0, conf_dev + n3 * 42, 2, 0, st)) return rc;
-  if (int rc = fb_conv(f, 32, f->c42, nullptr, g.h5, g.w5, 256, 0, conf_dev + n3 * 42 + n4 * 2, 2, 0, st)) return rc;
-  const int np = (int)(n3 * 21 + n4 + n5);
-  fb_softmax2_kernel<<<(np + 255) / 256, 256, 0, st>>>(conf_dev, np);
-  SYN_LAUNCH_CHECK("fb_softmax2_kernel");
-  ++f->launches;
-  return SYN_OK;
+  return fb_forward_body(f, image_dev, height, width, loc_dev, conf_dev, (cudaStream_t)stream, nullptr, "syn_fb_forward");
+}
+
+int syn_fb_debug_forward_until(syn_fb_t* f, const uint8_t* image_dev, int height, int width, int stage, float* out_dev,
+                               int64_t out_numel, float* loc_dev, float* conf_dev, void* stream) {
+  if (stage < 0 || stage >= kFbStages)
+    return fail(SYN_ERR_INVALID, "syn_fb_debug_forward_until: stage %d outside 0..%d", stage, kFbStages - 1);
+  if (!f || !out_dev) return fail(SYN_ERR_INVALID, "syn_fb_debug_forward_until: null handle or output");
+  const FbStop stop{stage, out_dev, out_numel};
+  return fb_forward_body(f, image_dev, height, width, loc_dev, conf_dev, (cudaStream_t)stream, &stop, "syn_fb_debug_forward_until");
 }
 
 }  // extern "C"

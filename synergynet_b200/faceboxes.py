@@ -103,6 +103,48 @@ class FaceBoxesNet:
                                                 torch.cuda.current_stream(self.device).cuda_stream))
         return loc, conf
 
+    def debug_forward_until(self, image: torch.Tensor, stage: int) -> torch.Tensor:
+        """Run :meth:`forward`'s launch sequence up to launch ``stage`` (0..38, table at ``syn_fb_debug_forward_until`` in
+        include/synergy_b200.h) and return the whole tensor that launch wrote: an NHWC ``(h, w, channels)`` map, or the
+        flat ``loc`` (P*4) / ``conf`` (P*2) for stages 32..38.  ``loc`` / ``conf`` start as NaN, so what a head did not
+        write reads NaN.  Per-stage tests only."""
+        if image.dtype != torch.uint8 or image.dim() != 3 or image.shape[2] != 3 or image.device != self.device or not image.is_contiguous():
+            raise ValueError('image must be a contiguous uint8 (H,W,3) tensor on the detector device')
+        h, w = int(image.shape[0]), int(image.shape[1])
+        p = detect.num_priors(h, w)
+        loc = torch.full((p * 4,), float('nan'), dtype=torch.float32, device=self.device)
+        conf = torch.full((p * 2,), float('nan'), dtype=torch.float32, device=self.device)
+        shape = debug_stage_shape(stage, h, w)
+        out = torch.empty(shape, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.syn_fb_debug_forward_until(self._h, image.data_ptr(), h, w, stage, out.data_ptr(), out.numel(),
+                                                            loc.data_ptr(), conf.data_ptr(),
+                                                            torch.cuda.current_stream(self.device).cuda_stream))
+        return out
+
+
+def _conv_out(n: int, k: int, s: int, p: int) -> int:
+    return (n + 2 * p - k) // s + 1
+
+
+def debug_stage_shape(stage: int, h: int, w: int) -> tuple:
+    """Shape of the tensor launch ``stage`` of the detector writes, for an h x w image (see ``debug_forward_until``)."""
+    if not 0 <= stage < 39:
+        raise ValueError(f'detector stage {stage} outside 0..38')
+    h1, w1 = _conv_out(h, 7, 4, 3), _conv_out(w, 7, 4, 3)
+    hp, wp = _conv_out(h1, 3, 2, 1), _conv_out(w1, 3, 2, 1)
+    h2, w2 = _conv_out(hp, 5, 2, 2), _conv_out(wp, 5, 2, 2)
+    h3, w3 = _conv_out(h2, 3, 2, 1), _conv_out(w2, 3, 2, 1)
+    h4, w4 = _conv_out(h3, 3, 2, 1), _conv_out(w3, 3, 2, 1)
+    h5, w5 = _conv_out(h4, 3, 2, 1), _conv_out(w4, 3, 2, 1)
+    if stage >= 32:
+        return (detect.num_priors(h, w) * (4 if stage < 35 else 2),)
+    fixed = {0: (h1, w1, 48), 1: (hp, wp, 48), 2: (h2, w2, 128), 3: (h3, w3, 128),
+             28: (h3, w3, 128), 29: (h4, w4, 256), 30: (h4, w4, 128), 31: (h5, w5, 256)}
+    if stage in fixed:
+        return fixed[stage]
+    return (h3, w3, {3: 24, 5: 24, 6: 32}.get((stage - 4) % 8, 128))         # inception: r1, r2, t3, else 128 channels
+
 
 class FaceBoxes:
     """``FaceBoxes.FaceBoxes`` (FaceBoxes/FaceBoxes.py:46-143).  ``weights``: a state dict, a checkpoint path, or None for
