@@ -334,8 +334,12 @@ int syn_poll_error(syn_handle_t* h, int* flag_out);
 /* The same flag WITHOUT synchronising or clearing (it lives in mapped host memory): cheap enough to
  * call after any host-side synchronisation point. */
 int syn_peek_error(const syn_handle_t* h, int* flag_out);
-/* Synchronise and report (then clear) the "activation clamped" flag: the split-fp16 engines scale
- * block inputs by 64 and clamp to the fp16 range, i.e. |x| > ~937 saturates; the fp32 engine
+/* Synchronise and report (then clear) the sticky "activation clamped" flag of this handle: the
+ * split-fp16 engines scale an activation by 64 and clamp it to +-60000 before the fp16 hi/lo split, so
+ * an input with |x| > 937.5, +-Inf or NaN is changed (NaN is read as -937.5).  The flag is raised
+ * wherever that happens: the fused block kernel's input (the fp32 crop at the stem and the inputs of
+ * blocks 2-17; engines 2, 3), the tail kernel's input (the block-17 output; engines 2, 3) and the input
+ * of every expand conv and of conv 51 on the unfused tensor-core engine (engine 1).  The fp32 engine
  * (SYN_ENGINE_SIMT_FP32) has no such limit.  *flag_out != 0: results of engines 1-3 are suspect. */
 int syn_poll_saturation(syn_handle_t* h, int* flag_out);
 /* Run the backbone on x_dev but stop after convolution `layer` (0..51) and copy its NHWC

@@ -107,15 +107,17 @@ def conv(sd: Dict[str, torch.Tensor], index: int, x: torch.Tensor, skip: Optiona
     return _conv(sd, index, x, torch.zeros_like(x), None if skip is None else skip.double())
 
 
-def block(sd: Dict[str, torch.Tensor], b: int, x: torch.Tensor) -> Pair:
+def block(sd: Dict[str, torch.Tensor], b: int, x: torch.Tensor, skip: Optional[torch.Tensor] = None) -> Pair:
     """Inverted-residual block ``b`` (1..17) as one stage, the unit of the fused engine; block 1 includes the stem and
-    takes the NCHW image.  The rounding of the hidden tensors inside the block is carried in S."""
+    takes the NCHW image.  The rounding of the hidden tensors inside the block is carried in S.  ``skip`` is what a
+    residual block adds to its output (default ``x``): the fused kernel adds its fp32 input even where the expand GEMM
+    read a clamped copy of it."""
     x = x.double()
+    skip = x if skip is None else skip.double()
     idx = [s.index for s in _PLAN if s.block == b or (b == 1 and s.kind == 'stem')]
     y, s = x, torch.zeros_like(x)
     for i in idx:
-        skip = x if _PLAN[i].residual else None
-        y, s = _conv(sd, i, y, s, skip)
+        y, s = _conv(sd, i, y, s, skip if _PLAN[i].residual else None)
     return y, s
 
 

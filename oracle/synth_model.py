@@ -100,6 +100,37 @@ def reparametrize_streams(sd: Dict[str, torch.Tensor], seed: int, lo: int, hi: i
     return out
 
 
+STREAMS = (16, 24, 32, 64, 96, 160, 320)         # channels of the block streams, in network order
+
+
+def stream_blocks(stream: int):
+    """(blocks whose project conv writes the stream, blocks whose input it is; 18 stands for the tail, features.18)."""
+    writers = [s.block for s in conv_plan() if s.kind == 'project' and s.cout == stream]
+    readers = [s.block for s in conv_plan() if s.kind in ('expand', 'last') and s.cin == stream]
+    assert writers and readers == [b + 1 for b in writers], (stream, writers, readers)
+    return writers, readers
+
+
+@torch.no_grad()
+def scale_stream_channel(sd: Dict[str, torch.Tensor], stream: int, channel: int, factor: float) -> Dict[str, torch.Tensor]:
+    """The same network with channel ``channel`` of one block stream multiplied by ``factor`` (> 0): gamma and beta of
+    every project BatchNorm that writes the stream are multiplied by the fp32 factor, and input column ``channel`` of
+    every conv that reads it (the following expands, or features.18 for the 320 stream) is divided by it -- the
+    arithmetic of ``reparametrize_streams`` for one channel and any factor.  Exact in function; in fp32 only for a
+    power of two, otherwise within the rounding of the rescaled weights."""
+    out = {k: v.clone() for k, v in sd.items()}
+    pre = 'I2P.backbone.'
+    f = torch.tensor(factor, dtype=torch.float32)
+    assert f > 0, factor
+    for spec in conv_plan():
+        if spec.kind == 'project' and spec.cout == stream:
+            out[pre + spec.bn_key + '.weight'][channel] *= f
+            out[pre + spec.bn_key + '.bias'][channel] *= f
+        if spec.kind in ('expand', 'last') and spec.cin == stream:
+            out[pre + spec.conv_key + '.weight'][:, channel] /= f
+    return out
+
+
 def _pow2_factors(n: int, g: torch.Generator, lo: int, hi: int) -> torch.Tensor:
     """n factors 2^k, k an integer drawn from [lo, hi], with one channel at each end of the range."""
     k = torch.randint(lo, hi + 1, (n,), generator=g)

@@ -389,10 +389,10 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
             if (e < n_items) {
               const int t = e / KG, kg = e - t * KG;
               uint32_t h[4], l[4];
-              float vmax = 0.f;
+              bool out_of_range = false;                            // |x| > 937.5, +-Inf or NaN
 #pragma unroll
-              for (int j = 0; j < 8; ++j) vmax = fmaxf(vmax, fabsf(v[u][j]));
-              if (vmax * kActScale > 60000.f) *p.sat = 1;          // the clamp below changes a value: tell the host (sticky)
+              for (int j = 0; j < 8; ++j) out_of_range |= act_clamped(v[u][j]);
+              if (out_of_range) *p.sat = 1;                         // the clamp below changes a value: tell the host (sticky)
 #pragma unroll
               for (int j = 0; j < 4; ++j) split2_f16(v[u][2 * j] * kActScale, v[u][2 * j + 1] * kActScale, h[j], l[j]);
               // canonical K-major operand: row of this thread in slab t, 8 K values = one 16-byte core-matrix row

@@ -32,6 +32,7 @@ struct TailArgs {
   int batch;
   int ctas_per_slice;
   int* err;
+  int* sat;              // sticky flag: an input value was clamped by the fp16 split (|x| > 937.5, +-Inf or NaN)
   int npass;             // 3 = split-fp16 x3, 1 = single fp16 pass
 };
 
@@ -62,6 +63,7 @@ __global__ void __launch_bounds__(kTailThreads, 1) tail_conv_pool_kernel(const T
     // ------------------------------ producers -----------------------------------------------------
     const int row = tid & 127, half = tid >> 7;            // pixel row of the tile, which 4 of the 8 k-groups
     uint32_t g = 0;
+    bool out_of_range = false;                             // the split below clamps a value: |x| > 937.5, +-Inf or NaN
     for (int i = 0; i < my_tiles; ++i) {
       const int tile = pi + i * p.ctas_per_slice;
       const int f0 = tile * kTailFaces;
@@ -79,6 +81,9 @@ __global__ void __launch_bounds__(kTailThreads, 1) tail_conv_pool_kernel(const T
             a = *reinterpret_cast<const float4*>(xrow + kc * kTailKC + kg * 8);
             e = *reinterpret_cast<const float4*>(xrow + kc * kTailKC + kg * 8 + 4);
           }
+          const float v[8] = {a.x, a.y, a.z, a.w, e.x, e.y, e.z, e.w};
+#pragma unroll
+          for (int j = 0; j < 8; ++j) out_of_range |= act_clamped(v[j]);
           uint32_t h[4], l[4];
           split2_f16(a.x * kActScale, a.y * kActScale, h[0], l[0]);
           split2_f16(a.z * kActScale, a.w * kActScale, h[1], l[1]);
@@ -91,6 +96,7 @@ __global__ void __launch_bounds__(kTailThreads, 1) tail_conv_pool_kernel(const T
         mbar_arrive(smem_u32(&bar_xfull[s]));
       }
     }
+    if (out_of_range) *p.sat = 1;                           // sticky, cleared by syn_poll_saturation
   } else {
     // ------------------------------ MMA + pooling: warpgroup wg owns channels 64 wg .. 64 wg + 63 of the slice ----
     const int t = tid & 127, wg = (tid >> 7) - 2;

@@ -49,6 +49,7 @@ struct TcPointwiseArgs {
   int nr;                  // channels per n-range (multiple of 16, <= 256)
   int relu6;
   int* err;
+  int* sat;                // sticky flag: an A value was clamped by the fp16 split (|x| > 937.5, +-Inf or NaN)
 };
 
 __global__ void __launch_bounds__(kTcThreads, 1) tc_pointwise_kernel(const TcPointwiseArgs p) {
@@ -88,6 +89,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_pointwise_kernel(const TcPoi
   float acc[128];
 #pragma unroll
   for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+  bool out_of_range = false;                             // the split below clamps a value: |x| > 937.5, +-Inf or NaN
   for (int c = 0; c < nchunks; ++c) {
     const int s = c & 1, use = c >> 1;
     const int k0 = c * kTcKChunk;
@@ -114,6 +116,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_pointwise_kernel(const TcPoi
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[j] = 0.f;
       }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) out_of_range |= act_clamped(v[j]);
       uint32_t h[4], l[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) split2_f16(v[2 * j] * kActScale, v[2 * j + 1] * kActScale, h[j], l[j]);
@@ -139,6 +143,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_pointwise_kernel(const TcPoi
     wgmma_wait<0>();
     mbar_arrive(smem_u32(&bar_empty[s]));                  // slot s may be refilled
   }
+  if (out_of_range) *p.sat = 1;                            // sticky, cleared by syn_poll_saturation
   // ------------------------------ epilogue from the accumulators ------------------------------------
   const int ncols = min(p.nr, p.N - n0);                   // valid channels of this range
 #pragma unroll

@@ -194,7 +194,7 @@ int launch_pointwise_tc(syn_handle* h, const float* A, int layer, const float* r
   TcPointwiseArgs a;
   a.A = A; a.Wimg = h->d_tcw + h->tc_off[layer]; a.bias = h->dconv[layer].bias; a.oscale = h->d_tc_oscale + h->tc_osc_off[layer]; a.residual = residual;
   a.out = out; a.M = M; a.K = c.cin; a.N = c.cout; a.Kp = h->tc_kp[layer]; a.nr = h->tc_nr[layer];
-  a.relu6 = c.relu6; a.err = h->d_err;
+  a.relu6 = c.relu6; a.err = h->d_err; a.sat = h->d_sat;
   dim3 grid((M + 127) / 128, h->tc_nranges[layer]);
   tc_pointwise_kernel<<<grid, kTcThreads, kTcSmemBytes, st>>>(a);
   SYN_LAUNCH_CHECK("tc_pointwise_kernel");
@@ -290,7 +290,7 @@ int run_backbone(syn_handle* h, const float* x, int batch, float* params, float*
       float* pooled = pool ? pool : h->d_pool_tmp;
       TailArgs t;
       t.x = h->buf_io[cur]; t.wimg = h->d_tail_w; t.bias = h->dconv[51].bias; t.oscale = h->d_tail_osc;
-      t.pooled = pooled; t.batch = batch; t.err = h->d_err; t.npass = h->npass();
+      t.pooled = pooled; t.batch = batch; t.err = h->d_err; t.sat = h->d_sat; t.npass = h->npass();
       const int ntiles = (batch + kTailFaces - 1) / kTailFaces;
       t.ctas_per_slice = std::max(1, std::min(ntiles, h->sm_count / 10));
       tail_conv_pool_kernel<<<10 * t.ctas_per_slice, kTailThreads, kTailSmem, st>>>(t);

@@ -259,6 +259,9 @@ __device__ __forceinline__ void split_f16(float x, __half& hi, __half& lo) {
   hi = __float2half_rn(x);
   lo = __float2half_rn(x - __half2float(hi));
 }
+// true when the clamp of an activation split (x * kActScale to +-60000) would change x: |x| > 937.5, +-Inf or NaN.
+// Scaling by a power of two is exact, so the test is made on x itself (no multiply); NaN fails every comparison.
+__device__ __forceinline__ bool act_clamped(float x) { return !(fabsf(x) <= 60000.f / kActScale); }
 __device__ __forceinline__ uint32_t pack_f16x2(__half a, __half b) {
   return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
 }

@@ -160,8 +160,10 @@ class Engine:
                                           '(Engine.poll_error() reports and clears the flag)')
 
     def poll_saturation(self, warn: bool = True) -> int:
-        """Device sync + sticky "a block input was clamped to the fp16 range" flag of the split-fp16 engines
-        (|x| > ~937 at a block input).  Non-zero: use ``set_engine(0)`` (fp32) for this checkpoint."""
+        """Device sync + sticky "an activation was clamped to the fp16 range" flag of the split-fp16 engines, then
+        clear it.  Raised when |x| > 937.5, +-Inf or NaN reaches a clamp: the fused kernel's input (fp32 crop and
+        block inputs, engines 2 and 3), the tail kernel's input (engines 2 and 3) or an expand / conv 51 input (engine
+        1).  Non-zero: use ``set_engine(0)`` (fp32) for this checkpoint, or check the input for Inf / NaN."""
         fn = getattr(self._lib, 'syn_poll_saturation', None)
         if fn is None:
             return 0

@@ -7,7 +7,8 @@ from oracle import block64, synth_model, tile_cover
 from oracle import reference_port as rp
 from synergynet_b200 import _lib, synthetic
 from synergynet_b200.backbone import conv_plan
-from test_gpu_blocks import TAU, WIDE
+from oracle.stage_check import TAU
+from test_gpu_blocks import WIDE
 from test_gpu_parity import LAYER_TOL
 
 PLAN = conv_plan()

@@ -6,47 +6,18 @@ conv by conv (52 convs), the fused engine block by block (17 blocks, conv index 
 the 62 params.  The batches come from the device's SM count and cover every tile plan of the fused kernels
 (oracle/tile_cover.py); the faces checked cover every tile kind of those plans.  H100 only.
 """
-import types
-
 import pytest
 import torch
 
-from oracle import block64, synth_model, tile_cover
+from oracle import stage_check, synth_model, tile_cover
 from oracle import reference_port as rp
+from oracle.stage_check import ENGINES, make_model as _make_model, report as _report, stage_ratios, tau as _tau
 from synergynet_b200 import _lib, synthetic
-from synergynet_b200.backbone import conv_plan
 
 pytestmark = pytest.mark.gpu
 
-# The bar: |got - want| <= TAU * S at every element.  S is a first-order bound, and a bound carried through the three
-# convs of a fused block is far more pessimistic than the bound of one conv (it adds |W| * S of every hidden element,
-# while real rounding errors cancel), so one TAU for both would leave the fused blocks ~40x of slack.  TAU is therefore
-# set per engine and stage kind, at most 4x the worst ratio measured on an H100 80GB HBM3 (132 SMs, 700 W power limit)
-# over the three batches of this file and the rescaled checkpoint (worst in the comment):
-TAU = {
-    'simt_fp32': {'conv': 1.3e-6,        # 3.29e-07 (conv 6)
-                  'pool': 8e-7,          # 2.10e-07
-                  'params': 8e-8},       # 2.00e-08
-    'tc_bf16x3': {'conv': 4.9e-6,        # 1.24e-06 (conv 44, rescaled checkpoint; 1.235e-06 on the original)
-                  'pool': 9e-7,          # 2.38e-07
-                  'params': 9e-8},       # 2.27e-08
-    'tc_fused': {'block': 1.4e-7,        # 3.54e-08 (block 2)
-                 'pool': 6.9e-7,         # 1.75e-07 (tail kernel)
-                 'params': 8.8e-8},      # 2.22e-08
-}
-# The single-pass engine measures 2.06e-06 (block 15) to 3.40e-05 (block 1) and 2.46e-05 at the tail: >= 14x the bar.
-ENGINES = {'simt_fp32': _lib.ENGINE_SIMT_FP32, 'tc_bf16x3': _lib.ENGINE_TC_BF16X3, 'tc_fused': _lib.ENGINE_TC_FUSED}
 TOL = 1e-4
 WIDE = dict(seed=7, lo=-6, hi=4)         # channel factors 2^-6 .. 2^4 on every block stream
-
-
-def _make_model(sd):
-    from synergynet_b200 import model_building
-    args = types.SimpleNamespace(arch='mobilenet_v2', img_size=120, devices_id=[0])
-    m = model_building.SynergyNet(args)
-    m.load_state_dict(sd, strict=True)
-    m.eval()
-    return m
 
 
 @pytest.fixture(scope='module')
@@ -79,50 +50,6 @@ def _engine(model, kind):
     return model._engine(torch.device('cuda', 0))
 
 
-def stage_ratios(eng, fused, sd, x, faces):
-    """{stage: (worst |got - want| / S, (face, y, x, channel))} over the given faces of batch ``x`` (on the GPU)."""
-    fidx = torch.tensor(faces, device='cuda')
-    pick = lambda t: t.index_select(0, fidx).cpu().double()
-    img = pick(x)
-    out = {}
-    if fused:
-        prev = img
-        for b in range(1, 18):
-            got = pick(eng.debug_forward_until(x, 3 * b - 1))
-            out[f'block{b}'] = block64.worst(got, *block64.block(sd, b, prev))
-            prev = got
-        pool_want = block64.tail(sd, prev)
-    else:
-        got = {}
-        for spec in conv_plan():
-            got[spec.index] = pick(eng.debug_forward_until(x, spec.index))
-            src = img if spec.index == 0 else got[spec.index - 1]
-            skip = got[spec.index - 3] if spec.residual else None        # the block input, before its expand
-            out[f'conv{spec.index}'] = block64.worst(got[spec.index], *block64.conv(sd, spec.index, src, skip))
-        pool_want = block64.avgpool(got[len(got) - 1])
-    params, pool = eng.forward(x, want_pool=True)
-    pool = pick(pool)
-    out['pool'] = block64.worst(pool, *pool_want)
-    out['params'] = block64.worst(pick(params), *block64.heads(sd, pool))
-    assert eng.poll_error() == 0
-    assert eng.poll_saturation(warn=False) == 0
-    return out
-
-
-def _tau(engine, stage):
-    return TAU[engine][stage.rstrip('0123456789')]
-
-
-def _over(engine, ratios):
-    return {k: v for k, v in ratios.items() if v[0] > _tau(engine, k)}
-
-
-def _report(tag, ratios):
-    name, (r, where) = max(ratios.items(), key=lambda kv: kv[1][0])
-    print(f'\n[{tag}] worst {r:.3e} at {name} {where}')
-    print('  ' + '  '.join(f'{k}={v[0]:.2e}' for k, v in ratios.items()))
-
-
 def _batch(sms, kind):
     batch = tile_cover.choose_batches(sms)[kind]
     tile_cover.check_plan(kind, batch, sms)
@@ -140,7 +67,7 @@ def test_every_stage_matches_float64_oracle(model, sd, sms, engine, plan):
     finally:
         model.set_engine(_lib.ENGINE_TC_FUSED)
     _report(f'{engine} B={x.shape[0]} {plan} faces={len(faces)}', ratios)
-    bad = _over(engine, ratios)
+    bad = stage_check.over(engine, ratios)
     assert not bad, bad
 
 
@@ -187,5 +114,5 @@ def test_rescaled_checkpoint_every_stage(model_wide, sd_wide, sms, engine):
     finally:
         model_wide.set_engine(_lib.ENGINE_TC_FUSED)
     _report(f'{engine} rescaled B={x.shape[0]} faces={len(faces)}', ratios)
-    bad = _over(engine, ratios)
+    bad = stage_check.over(engine, ratios)
     assert not bad, bad
