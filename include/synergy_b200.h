@@ -196,6 +196,30 @@ int syn_resnet_commit(syn_handle_t* h);                      /* after syn_commit
 int syn_resnet50_forward(syn_handle_t* h, const float* x_dev, int batch, float* out102_dev, float* pool2048_dev,
                          void* stream);
 
+/* ---- MobileNetV1 backbones (backbone_nets/mobilenetv1_backbone.py:21-140, prelu=False) ------------------------------
+ * Five widths, named by widen_code = 100 x the widen factor: SYN_MBV1_2 (200, mobilenet_2), SYN_MBV1_1 (100),
+ * SYN_MBV1_075 (75), SYN_MBV1_05 (50), SYN_MBV1_025 (25); every channel count is int(c * widen).  27 convolutions in
+ * execution order: 0 = conv1 (3x3/s2, 3 -> 32w), then per DepthWiseBlock dw2_1 .. dw6 its conv_dw (3x3 depthwise,
+ * stride 1 or 2) and its conv_sep (1x1) -- syn_mbv1_conv_desc gives each one's geometry (groups = cin for a depthwise).
+ * syn_mbv1_set_widen selects the width of the handle and forgets the MobileNetV1 weights set so far; then every conv
+ * takes OIHW fp32 weights + eval BatchNorm2d as for syn_resnet_set_conv, and the heads the four Linear layers
+ * concatenated in the reference's OUTPUT order fc_ori | fc_shape | fc_exp | fc_tex -> (102, 1024w) weights, (102)
+ * bias (:95-98, :132-138).  syn_mbv1_commit comes after syn_commit (the shared library state); BatchNorm is folded in
+ * float64.  syn_mbv1_forward: x_dev (B,3,120,120) NCHW fp32 crops, or raw uint8 crops when x_is_u8 (normalised as
+ * (v - 127.5) / 128, with the syn_set_center_crop frame), -> out102_dev (B,102) = what MobileNet.forward returns;
+ * pool_dev (B,1024w) = the flattened avgpool, may be NULL.  (The reference's I2P unpacks two values from this backbone
+ * along dim 0; the Python shim adapts as for ResNet-50: params = out[:, :62], pool = the 1024w-d feature.) */
+enum { SYN_MBV1_2 = 200, SYN_MBV1_1 = 100, SYN_MBV1_075 = 75, SYN_MBV1_05 = 50, SYN_MBV1_025 = 25 };
+int syn_mbv1_num_convs(void);                                /* 27 */
+int syn_mbv1_conv_desc(int widen_code, int idx, syn_conv_desc_t* out);
+int syn_mbv1_set_widen(syn_handle_t* h, int widen_code);
+int syn_mbv1_set_conv(syn_handle_t* h, int idx, const float* w_host, int64_t w_numel, const float* bn_weight_host,
+                      const float* bn_bias_host, const float* bn_mean_host, const float* bn_var_host, float eps);
+int syn_mbv1_set_heads(syn_handle_t* h, const float* w102xC_host, const float* b102_host);
+int syn_mbv1_commit(syn_handle_t* h);                        /* after syn_commit */
+int syn_mbv1_forward(syn_handle_t* h, const void* x_dev, int x_is_u8, int batch, float* out102_dev, float* pool_dev,
+                     void* stream);
+
 /* ---- Sim3DR: vertex normals, lighting, z-buffer rasterisation (SURVEY.md section 8 row f2) -------------------------
  * Handle-free; every pointer is caller-owned device memory unless it says _host.  B meshes share one triangle list
  * tri_dev (ntri,3) int32, 0-based (utils/render.py:32-33).  Vertices are read in place through element strides:
@@ -356,6 +380,11 @@ int syn_debug_forward_until(syn_handle_t* h, const float* x_dev, int batch, int 
  * (B x 2048), 55 heads (B x 102, no row maxima). */
 int syn_debug_resnet_until(syn_handle_t* h, const float* x_dev, int batch, int stage, float* out_dev, unsigned* rowmax_dev,
                            void* stream);
+/* MobileNetV1 (NHWC rows, one per pixel; C_i = cout of conv i of syn_mbv1_conv_desc): 0 stem (B*3600 x C_0),
+ * 2j - 1 / 2j conv_dw / conv_sep of block j = 1..13 (B*HO*HO x C_i; every stage records row maxima except the conv_seps
+ * of blocks 1..12), 27 avgpool (B x 1024w), 28 heads (B x 102, no row maxima).  x_dev: fp32 crops. */
+int syn_debug_mbv1_until(syn_handle_t* h, const float* x_dev, int batch, int stage, float* out_dev, unsigned* rowmax_dev,
+                         void* stream);
 /* PointNet heads (rows = B*68 point-major, or B): net 0 = MLP_for: 0..4 conv1..conv5 (64, 64, 64, 128, 1024 columns;
  * conv5 is written only by this call, without row maxima), 5 the max-pooled global features (B x 1024), 6 the face vector
  * (B x 2360), 7 conv6's face part (B x 512, no row maxima), 8 conv6's point part (512), 9 conv7 (256), 10 conv8 (128),

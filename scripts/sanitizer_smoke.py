@@ -50,6 +50,12 @@ def main():
     rn.load_state_dict({'I2P.backbone.' + k: v for k, v in synth_model.build_resnet50_state_dict(0).items()}, strict=False)
     rn.eval()
     rn.forward_test(x[:2])
+    from oracle import synth_mbv1
+    v1 = model_building.SynergyNet(types.SimpleNamespace(arch='mobilenet_075', img_size=120, devices_id=[0]))
+    v1.load_state_dict({'I2P.backbone.' + k: v for k, v in synth_mbv1.build_mobilenet_v1_state_dict(0, 'mobilenet_075').items()},
+                       strict=False)
+    v1.eval()
+    v1._engine(dev).forward_mobilenet_v1(u8[:2].cuda())                # uint8 stem, every depthwise band plan
     torch.cuda.synchronize()
     eng.raise_if_error()
     print('sanitizer smoke done:', float(dense.abs().max()), {k: float(v.mean()) for k, v in loss.items()})

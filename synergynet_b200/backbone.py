@@ -258,3 +258,89 @@ def resnet50_conv_keys():
 
 def resnet50(pretrained: bool = False, **_):
     return ResNet50Params()
+
+
+# ---- MobileNetV1 backbones (reference backbone_nets/mobilenetv1_backbone.py:21-140, prelu=False) ---------------------------
+
+MBV1_BLOCKS = (('dw2_1', 64, 1), ('dw2_2', 128, 2), ('dw3_1', 128, 1), ('dw3_2', 256, 2), ('dw4_1', 256, 1),
+               ('dw4_2', 512, 2), ('dw5_1', 512, 1), ('dw5_2', 512, 1), ('dw5_3', 512, 1), ('dw5_4', 512, 1),
+               ('dw5_5', 512, 1), ('dw5_6', 1024, 2), ('dw6', 1024, 1))      # (name, out channels at width 1, stride)
+MBV1_WIDTHS = {'mobilenet_2': 2.0, 'mobilenet_1': 1.0, 'mobilenet_075': 0.75, 'mobilenet_05': 0.5, 'mobilenet_025': 0.25}
+
+
+class _DepthWiseBlock(nn.Module):
+    """Keys of ``DepthWiseBlock`` (conv_dw, bn_dw, conv_sep, bn_sep; :21-33)."""
+
+    def __init__(self, inplanes, planes, stride=1):
+        super().__init__()
+        inplanes, planes = int(inplanes), int(planes)
+        self.conv_dw = nn.Conv2d(inplanes, inplanes, 3, stride, 1, groups=inplanes, bias=False)
+        self.bn_dw = nn.BatchNorm2d(inplanes)
+        self.conv_sep = nn.Conv2d(inplanes, planes, 1, bias=False)
+        self.bn_sep = nn.BatchNorm2d(planes)
+
+
+class MobileNetV1Params(nn.Module):
+    """Key schema of ``mobilenetv1_backbone.MobileNet(widen)`` (conv1/bn1, dw2_1 .. dw6, fc_ori/fc_shape/fc_exp/fc_tex);
+    parameter container, the forward pass runs in the sm_90a library."""
+
+    def __init__(self, widen: float = 1.0, num_classes: int = 62, input_channel: int = 3):
+        super().__init__()
+        if input_channel != 3:
+            raise RuntimeError('the sm_90a MobileNetV1 stem is built for 3-channel crops')
+        self.widen_factor = float(widen)
+        self.conv1 = nn.Conv2d(input_channel, int(32 * widen), 3, 2, 1, bias=False)
+        self.bn1 = nn.BatchNorm2d(int(32 * widen))
+        cin = 32
+        for name, cout, stride in MBV1_BLOCKS:
+            setattr(self, name, _DepthWiseBlock(cin * widen, cout * widen, stride))
+            cin = cout
+        self.feature_dim = int(1024 * widen)
+        self.num_ori, self.num_shape, self.num_exp, self.num_texture = 12, 40, 10, 40
+        self.fc_ori = nn.Linear(self.feature_dim, 12)
+        self.fc_shape = nn.Linear(self.feature_dim, 40)
+        self.fc_exp = nn.Linear(self.feature_dim, 10)
+        self.fc_tex = nn.Linear(self.feature_dim, 40)
+        for m in self.modules():                                            # mobilenetv1_backbone.py:100-106
+            if isinstance(m, nn.Conv2d):
+                n = m.kernel_size[0] * m.kernel_size[1] * m.out_channels
+                m.weight.data.normal_(0, (2. / n) ** 0.5)
+            elif isinstance(m, nn.BatchNorm2d):
+                m.weight.data.fill_(1)
+                m.bias.data.zero_()
+
+    @property
+    def widen_code(self) -> int:
+        """100 x the widen factor: the width argument of the C ABI (syn_mbv1_set_widen)."""
+        return int(round(self.widen_factor * 100))
+
+    def forward(self, *a, **k):  # pragma: no cover
+        raise RuntimeError('MobileNetV1Params is a parameter container; the forward pass runs in the sm_90a library')
+
+
+def mobilenet_v1_conv_keys():
+    """(conv key, bn key) of the 27 convolutions in the execution order of the C ABI (syn_mbv1_set_conv)."""
+    keys = [('conv1', 'bn1')]
+    for name, _, _ in MBV1_BLOCKS:
+        keys += [(f'{name}.conv_dw', f'{name}.bn_dw'), (f'{name}.conv_sep', f'{name}.bn_sep')]
+    return keys
+
+
+def mobilenet_2(num_classes=62, input_channel=3):
+    return MobileNetV1Params(2.0, num_classes, input_channel)
+
+
+def mobilenet_1(num_classes=62, input_channel=3):
+    return MobileNetV1Params(1.0, num_classes, input_channel)
+
+
+def mobilenet_075(num_classes=62, input_channel=3):
+    return MobileNetV1Params(0.75, num_classes, input_channel)
+
+
+def mobilenet_05(num_classes=62, input_channel=3):
+    return MobileNetV1Params(0.5, num_classes, input_channel)
+
+
+def mobilenet_025(num_classes=62, input_channel=3):
+    return MobileNetV1Params(0.25, num_classes, input_channel)

@@ -17,6 +17,7 @@
 #include "kernels_gemm.cuh"
 #include "kernels_loss.cuh"
 #include "kernels_resnet.cuh"
+#include "kernels_mbv1.cuh"
 
 using namespace syn;
 
@@ -39,11 +40,14 @@ struct syn_heads;       // PointNet refinement heads (heads_host.inl)
 void syn_heads_destroy(syn_heads* s);
 struct syn_resnet;      // ResNet-50 backbone variant (resnet_host.inl)
 void syn_resnet_destroy(syn_resnet* s);
+struct syn_mbv1;        // MobileNetV1 backbones (mbv1_host.inl)
+void syn_mbv1_destroy(syn_mbv1* s);
 
 struct syn_handle {
   int device = 0;
   syn_heads* heads = nullptr;
   syn_resnet* resnet = nullptr;
+  syn_mbv1* mbv1 = nullptr;
   int sm_count = 0;
   int engine = SYN_ENGINE_TC_FUSED;            // default: fused tensor-core engine; 0/1 remain for cross-checks
   int center_crop = 0;                         // CenterCrop margin applied by the uint8 entry points (syn_set_center_crop)
@@ -688,6 +692,7 @@ void syn_destroy(syn_handle_t* h) {
   cudaDeviceSynchronize();
   syn_heads_destroy(h->heads);
   syn_resnet_destroy(h->resnet);
+  syn_mbv1_destroy(h->mbv1);
   cudaFree(h->d_weights); cudaFree(h->d_head_w); cudaFree(h->d_head_b); cudaFree(h->d_mean);
   cudaFree(h->d_std); cudaFree(h->d_sparse); cudaFree(h->d_dense); cudaFree(h->d_tcw); cudaFreeHost(h->d_err); cudaFree(h->d_sat); cudaFree(h->d_fused); cudaFree(h->d_tc_oscale);
   cudaFree(h->buf_io[0]); cudaFree(h->buf_io[1]); cudaFree(h->buf_hid); cudaFree(h->buf_dw);
@@ -1257,3 +1262,4 @@ int syn_debug_forward_until(syn_handle_t* h, const float* x, int batch, int laye
 
 #include "heads_host.inl"
 #include "resnet_host.inl"
+#include "mbv1_host.inl"

@@ -40,6 +40,7 @@ class Engine:
         self._h = h
         self.n_pts = 0
         self.n_vert = 0
+        self._mbv1_feat = 0                  # pooled feature width of the committed MobileNetV1 (1024 x widen)
         self._keep = []
         # The C handle is not re-entrant and all calls share one activation workspace: serialise the host threads
         # (nn.DataParallel replicas use one engine per device, but user threads may share a model) and order
@@ -411,6 +412,66 @@ class Engine:
             _lib.check(self._lib.syn_resnet50_forward(self._h, x.data_ptr(), b, out.data_ptr(), pool.data_ptr(), self._stream()))
             self._done()
         return out, pool
+
+    # ---- MobileNetV1 backbones (backbone_nets/mobilenetv1_backbone.py, the five mobilenet_* factories) -----------
+    def load_mobilenet_v1(self, sd: Dict[str, torch.Tensor], arch: str, prefix: str = '') -> None:
+        """Hand a ``mobilenetv1_backbone.<arch>()`` state dict to the library (27 conv+BN pairs in execution order, the four
+        Linear heads concatenated in the reference's output order ori | shape | exp | tex, mobilenetv1_backbone.py:132-138)."""
+        from .backbone import MBV1_WIDTHS, mobilenet_v1_conv_keys
+        if arch not in MBV1_WIDTHS:
+            raise RuntimeError(f"arch '{arch}': MobileNetV1 widths are {', '.join(MBV1_WIDTHS)}")
+        with self._lock:
+            _lib.check(self._lib.syn_mbv1_set_widen(self._h, int(round(MBV1_WIDTHS[arch] * 100))))
+            for i, (ck, bk) in enumerate(mobilenet_v1_conv_keys()):
+                w = _host_f32(sd[f'{prefix}{ck}.weight'])
+                bn = [_host_f32(sd[f'{prefix}{bk}.{k}']) for k in ('weight', 'bias', 'running_mean', 'running_var')]
+                _lib.check(self._lib.syn_mbv1_set_conv(self._h, i, w.data_ptr(), w.numel(), *[t.data_ptr() for t in bn], 1e-5))
+            order = ('fc_ori', 'fc_shape', 'fc_exp', 'fc_tex')
+            w = torch.cat([_host_f32(sd[f'{prefix}{k}.weight']) for k in order]).contiguous()
+            b = torch.cat([_host_f32(sd[f'{prefix}{k}.bias']) for k in order]).contiguous()
+            if w.shape[0] != 102:
+                raise RuntimeError(f'MobileNetV1 heads: expected 102 output rows, got {w.shape[0]}')
+            _lib.check(self._lib.syn_mbv1_set_heads(self._h, w.data_ptr(), b.data_ptr()))
+            _lib.check(self._lib.syn_mbv1_commit(self._h))
+            self._mbv1_feat = w.shape[1]
+
+    def forward_mobilenet_v1(self, x: torch.Tensor):
+        """MobileNet.forward (mobilenetv1_backbone.py:108-140): (B,3,120,120) fp32 normalised crops or raw uint8 crops ->
+        ((B,102) ori|shape|exp|tex, (B,1024w) pooled)."""
+        if x.dtype == torch.uint8:
+            if x.dim() != 4 or tuple(x.shape[1:]) != (3, 120, 120) or x.device != self.device:
+                raise RuntimeError(f'expected uint8 (B,3,120,120) on {self.device}, got {tuple(x.shape)} on {x.device}')
+            x = x.contiguous()
+        else:
+            x = self._check_x(x)
+        b = x.shape[0]
+        out = torch.empty((b, 102), device=self.device, dtype=torch.float32)
+        pool = torch.empty((b, self._mbv1_feat), device=self.device, dtype=torch.float32)
+        with self._lock:
+            _lib.check(self._lib.syn_mbv1_forward(self._h, x.data_ptr(), int(x.dtype == torch.uint8), b, out.data_ptr(),
+                                                  pool.data_ptr(), self._stream()))
+            self._done()
+        return out, pool
+
+    def debug_mobilenet_v1_until(self, x: torch.Tensor, stage: int):
+        """MobileNetV1 run up to ``stage`` (0 stem, 2j - 1 / 2j conv_dw / conv_sep of block j = 1..13, 27 avgpool, 28
+        heads): (that stage's output as (rows, channels) -- one row per NHWC pixel, or per face --, its row maxima as int32
+        fp32 bit patterns, or None for a stage that records none)."""
+        x = self._check_x(x)
+        b = x.shape[0]
+        if stage <= 26:
+            d = _lib.ConvDesc()
+            widen = int(round(self._mbv1_feat / 1024 * 100))
+            _lib.check(self._lib.syn_mbv1_conv_desc(widen, stage, C.byref(d)))
+            rows, cols, rm = b * d.h_out * d.h_out, d.cout, stage == 0 or stage % 2 == 1 or stage == 26
+        else:
+            rows, cols, rm = b, self._mbv1_feat if stage == 27 else 102, stage == 27
+        out, rmax = self._debug_out(rows, cols, rm)
+        with self._lock:
+            _lib.check(self._lib.syn_debug_mbv1_until(self._h, x.data_ptr(), b, stage, out.data_ptr(),
+                                                      rmax.data_ptr() if rm else None, self._stream()))
+            self._done()
+        return out, rmax
 
     # ---- per-stage debug runs of the GEMM layers (include/synergy_b200.h syn_debug_*_until / syn_debug_gemm) ----
     RESNET_STAGES = 56

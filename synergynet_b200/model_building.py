@@ -102,12 +102,24 @@ class I2P(nn.Module):
             # fact 4).  Adapter used here (and by the oracle / golden vectors): params = out[:, :62] (ori|shape|exp),
             # avgpool = the 2048-d pooled feature.
             self.backbone = mobilenetv2_backbone.resnet50(pretrained=False)
+        elif 'mobilenet' in self.args.arch:
+            # the reference sends every other 'mobilenet*' arch to mobilenetv1_backbone (model_building.py:42-43).  Like
+            # ResNet-50, MobileNet.forward returns ONE (B,102) tensor (mobilenetv1_backbone.py:138-140) and the reference's
+            # I2P unpacks two values from it along dim 0: it raises for B != 2, and for B = 2 it silently takes face 0's
+            # row as the params of both faces and face 1's as the pool.  Same adapter as resnet50: params = out[:, :62]
+            # (ori|shape|exp), avgpool = the 1024w-d pooled feature.
+            if self.args.arch not in mobilenetv2_backbone.MBV1_WIDTHS:
+                raise RuntimeError(f"arch '{args.arch}': the MobileNetV1 backbones are "
+                                   f"{', '.join(mobilenetv2_backbone.MBV1_WIDTHS)}")
+            self.backbone = getattr(mobilenetv2_backbone, args.arch)()
         elif any(k in self.args.arch for k in ('mobilenet', 'resnet', 'ghostnet', 'resnest')):
             raise RuntimeError(f"arch '{args.arch}': mobilenet_v2 and resnet50 are built for sm_90a "
                                '(SURVEY.md section 8; the other backbones are not on the hot path)')
         else:
             raise RuntimeError("Please choose [mobilenet_v2, mobilenet_1, resnet50, or ghostnet]")
         self._is_resnet = self.args.arch == 'resnet50'
+        self._is_mbv1 = self.args.arch in mobilenetv2_backbone.MBV1_WIDTHS
+        self._adapted = self._is_resnet or self._is_mbv1      # one (B,102) output: params = out[:, :62]
         object.__setattr__(self, '_rt', _Runtime())
         object.__setattr__(self, '_basis_provider', None)
 
@@ -118,6 +130,8 @@ class I2P(nn.Module):
     def _engine(self, device) -> Engine:
         if self._is_resnet:
             return self._resnet_engine(device)
+        if self._is_mbv1:
+            return self._mbv1_engine(device)
         return self._rt.get(device, self._backbone_sd, self._basis_provider)
 
     def _resnet_engine(self, device) -> Engine:
@@ -138,6 +152,29 @@ class I2P(nn.Module):
                 eng._resnet_commit_of = rt._sig.get(eng.device.index)
         return eng
 
+    def _mbv1_engine(self, device) -> Engine:
+        """Engine with the MobileNetV1 weights, built the way ``_resnet_engine`` builds its engine."""
+        rt = self._rt
+        if not hasattr(rt, '_mbv2_stub'):
+            rt._mbv2_stub = {k: v for k, v in mobilenetv2_backbone.mobilenet_v2().state_dict().items()
+                             if not k.endswith('num_batches_tracked')}
+        eng = rt.get(device, lambda: rt._mbv2_stub, self._basis_provider)
+        sd = self._backbone_sd()
+        sig = rt._signature(list(sd.values()))
+        key = (eng.device.index, self.args.arch)
+        with rt._lock:
+            if rt._pn_sig.get(key) != sig or getattr(eng, '_mbv1_commit_of', None) is not rt._sig.get(eng.device.index):
+                eng.load_mobilenet_v1(sd, self.args.arch)
+                rt._pn_sig[key] = sig
+                eng._mbv1_commit_of = rt._sig.get(eng.device.index)
+        return eng
+
+    def _forward_adapted(self, x: torch.Tensor):
+        """(out102, pool) of the resnet50 / mobilenet_* backbone on ``x`` (fp32 crops; uint8 crops for mobilenet_*),
+        which lives on the compute device."""
+        eng = self._engine(x.device)
+        return eng.forward_mobilenet_v1(x) if self._is_mbv1 else eng.forward_resnet50(x)
+
     def _compute_device(self, t: Optional[torch.Tensor] = None) -> torch.device:
         """Where the library runs for tensor ``t``: its own GPU, else the GPU the backbone lives on, else the current
         CUDA device -- the reference wrappers are built on the CPU (synergy3DMM.py:71-77) and still usable as is."""
@@ -154,8 +191,8 @@ class I2P(nn.Module):
         """Testing time forward -> (param62, avgpool1280) (model_building.py:59-62).  A CPU input is moved to the
         compute GPU and the results come back on the CPU, as the reference's CPU model would return them."""
         dev = self._compute_device(input)
-        if self._is_resnet:
-            out, pool = self._engine(dev).forward_resnet50(input.to(dev))
+        if self._adapted:
+            out, pool = self._forward_adapted(input.to(dev))
             params = out[:, :62].contiguous()
         else:
             params, pool = self._engine(dev).forward(input.to(dev), want_pool=True)
@@ -241,7 +278,7 @@ class _SynergyBase(nn.Module):
 
     def forward_test(self, input):
         """test time forward (model_building.py:159-162): whitened (B,62) parameters (on the input's device)."""
-        if self.I2P._is_resnet:
+        if self.I2P._adapted:
             return self.I2P.forward_test(input)[0]
         dev = self._compute_device(input)
         out = self._engine(dev).forward(input.to(dev))
@@ -249,7 +286,7 @@ class _SynergyBase(nn.Module):
 
     def forward_landmarks(self, input):
         """forward_test + reconstruct_vertex_62(dense=False) in one library call."""
-        if self.I2P._is_resnet:
+        if self.I2P._adapted:
             return self.reconstruct_vertex_62(self.forward_test(input))
         dev = self._compute_device(input)
         out = self._engine(dev).forward_landmarks(input.to(dev))
@@ -266,6 +303,11 @@ class _SynergyBase(nn.Module):
         autograd): backbone -> landmarks of prediction and ground truth -> WingLoss / ParamLoss -> MLP_for refinement
         -> MLP_rev -> the two cycle losses.  Returns the same dict of five (weighted) losses; the intermediate
         tensors are kept in ``self.last_forward`` for inspection."""
+        if self.I2P._is_mbv1:
+            raise RuntimeError(f'SynergyNet.forward: MLP_for.conv6 is hard-wired to a 1280-d image feature '
+                               '(pointnet_backbone.py:15,58: 2418 = 64 + 1024 + 1280 + 40 + 10); the '
+                               f'{self.I2P.args.arch} backbone pools {self.I2P.backbone.feature_dim} channels, so the '
+                               'refinement head cannot follow it.  Use forward_test() / reconstruct_vertex_62() with it.')
         dev = self._compute_device(input)
         eng = self._engine(dev)
         _3D_attr, avgpool = self.I2P.forward_test(input.to(dev))
@@ -323,7 +365,10 @@ class _SynergyBase(nn.Module):
         eng = self._engine(dev)
         image = torch.from_numpy(np.ascontiguousarray(input, dtype=np.uint8)).to(dev)    # crop_img's uint8 crops
         batch = crop_resize_device(image, boxes, (120, 120), interp)
-        _, params = eng.forward_landmarks(batch, want_params=True)
+        if self.I2P._is_mbv1:                       # that backbone, on the uint8 crops; then the same image-space stages
+            params = eng.forward_mobilenet_v1(batch)[0][:, :62].contiguous()
+        else:
+            _, params = eng.forward_landmarks(batch, want_params=True)
         roi5 = torch.from_numpy(roi_affine(boxes)).to(dev)
         lmk = eng.reconstruct_image(params, roi5, dense=False).cpu().numpy()
         mesh = eng.reconstruct_image(params, roi5, dense=True).cpu().numpy()
