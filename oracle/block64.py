@@ -19,9 +19,9 @@ number; for small x, lo falls into fp16's subnormals, whose spacing 2^-24 is abs
 activation units.  The two bounds meet at |x| = ACT_FLOOR = 2^-24 / kActScale / 2^-22 = 2^-8, so every operand enters
 S as |x| + ACT_FLOOR: the fixed-scale absolute error is charged at the same rate tau as the relative one.
 
-BatchNorm is folded here, in float64, from the state dict (not from the library's folded weights).  Pointwise convs are
-matmuls over NHWC and the depthwise 3x3 is nine shifted multiply-adds on a zero-padded tensor.  Tensors are NHWC, the
-layout ``syn_debug_forward_until`` returns; the stem takes the NCHW image.
+BatchNorm is folded here, in float64, from the state dict (``check64.fold_bn``, not the library's folded weights).
+Pointwise convs are matmuls over NHWC and the depthwise 3x3 is nine shifted multiply-adds on a zero-padded tensor.
+Tensors are NHWC, the layout ``syn_debug_forward_until`` returns; the stem takes the NCHW image.
 """
 from __future__ import annotations
 
@@ -30,25 +30,20 @@ from typing import Dict, Optional, Tuple
 import torch
 import torch.nn.functional as F
 
+from oracle.check64 import Pair, fold_bn, linear_heads, worst  # noqa: F401  (worst: the check the stage tests apply)
 from synergynet_b200.backbone import conv_plan
 
-BN_EPS = 1e-5
 ACT_SCALE = 64.0                         # tc::kActScale (csrc/tc_common.cuh)
 ACT_FLOOR = 2.0 ** -24 / ACT_SCALE / 2.0 ** -22
 PREFIX = 'I2P.backbone.'
 
-Pair = Tuple[torch.Tensor, torch.Tensor]          # (value, error scale S), both float64
 _PLAN = conv_plan()
 
 
 def fold(sd: Dict[str, torch.Tensor], index: int) -> Tuple[torch.Tensor, torch.Tensor]:
     """Conv ``index`` of the plan with its eval-mode BatchNorm folded in float64 -> (weight, bias)."""
     spec = _PLAN[index]
-    g = lambda s: sd[PREFIX + s].double()
-    w = g(spec.conv_key + '.weight')
-    scale = g(spec.bn_key + '.weight') / torch.sqrt(g(spec.bn_key + '.running_var') + BN_EPS)
-    bias = g(spec.bn_key + '.bias') - g(spec.bn_key + '.running_mean') * scale
-    return w * scale.view(-1, 1, 1, 1), bias
+    return fold_bn(sd, PREFIX + spec.bn_key, sd[PREFIX + spec.conv_key + '.weight'])
 
 
 def _pointwise(a: torch.Tensor, s_a: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> Pair:
@@ -136,20 +131,5 @@ def tail(sd: Dict[str, torch.Tensor], x: torch.Tensor) -> Pair:
 def heads(sd: Dict[str, torch.Tensor], pool: torch.Tensor) -> Pair:
     """The three linear heads on the pooled feature -> (N, 62) params."""
     pool = pool.double()
-    keys = ('classifier_ori', 'classifier_shape', 'classifier_exp')
-    w = torch.cat([sd[f'{PREFIX}{k}.1.weight'].double() for k in keys])
-    b = torch.cat([sd[f'{PREFIX}{k}.1.bias'].double() for k in keys])
+    w, b = linear_heads(sd, [f'{PREFIX}{k}.1' for k in ('classifier_ori', 'classifier_shape', 'classifier_exp')])
     return _pointwise(pool, torch.zeros_like(pool), w, b)
-
-
-def ratio(got: torch.Tensor, want: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
-    """|got - want| / S per element (0 where they are equal, inf where S = 0 and they differ)."""
-    d = (got.double() - want).abs()
-    return torch.where(d == 0, torch.zeros_like(d), d / s)
-
-
-def worst(got: torch.Tensor, want: torch.Tensor, s: torch.Tensor) -> Tuple[float, tuple]:
-    """Largest |got - want| / S and the index (face, y, x, channel) where it occurs."""
-    r = ratio(got, want, s)
-    i = int(torch.argmax(r))
-    return float(r.reshape(-1)[i]), tuple(int(v) for v in torch.unravel_index(torch.tensor(i), r.shape))

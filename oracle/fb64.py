@@ -4,8 +4,8 @@ TEST INFRASTRUCTURE.
 
 The contract is that of ``block64.py`` / ``gemm64.py``: every stage is fed the exact fp32 tensor the GPU stage was fed
 (the GPU's own output of the stages before it, as ``FaceBoxesNet.debug_forward_until`` returns them) and returns
-``(want, S)``; a stage passes when |got - want| <= tau * S at every element (``gemm64.worst``).  BatchNorm is folded here,
-in float64, from the reference-schema state dict (eps 1e-5), not from the library's folded weights.
+``(want, S)``; a stage passes when |got - want| <= tau * S at every element (``check64.worst``).  BatchNorm is folded
+here, in float64, from the reference-schema state dict (``check64.fold_bn``), not from the library's folded weights.
 
 Every convolution runs on CUDA cores in fp32 FMA (``fb_conv_kernel``, ``fb_conv_smalln_kernel``, csrc/kernels_detect.cuh),
 so S = sum_k |a_k||w_k| + |b| (``gemm64.simt``).  conv1's operand is u8 - mean, exact in fp32.  CReLU writes relu(v) to
@@ -23,12 +23,10 @@ import torch
 import torch.nn.functional as F
 
 from oracle import gemm64
+from oracle.check64 import Pair, fold_bn, strip_prefix
 
-BN_EPS = 1e-5
 MEAN_BGR = (104.0, 117.0, 123.0)                 # FaceBoxes.py:92
 FB_BM = 64                                       # output pixels per CTA of fb_conv_kernel
-
-Pair = Tuple[torch.Tensor, torch.Tensor]
 
 # ---- the network -------------------------------------------------------------------------------------------------------
 
@@ -128,9 +126,9 @@ def owned(stage: int, t: torch.Tensor, h: int, w: int) -> torch.Tensor:
 def fold(sd, index: int) -> Tuple[torch.Tensor, torch.Tensor]:
     """Layer ``index`` with its BatchNorm folded in float64: (W (cout, k*k*cin) in the kernel's (ky, kx, c) order, bias)."""
     L = LAYERS[index]
-    sd = {(k[7:] if k.startswith('module.') else k): v for k, v in sd.items()}
+    sd = strip_prefix(sd, 'module.')
     if L.bn:
-        w, b = gemm64._bn_fold(sd, f'{L.name}.bn', sd[f'{L.name}.conv.weight'], None)
+        w, b = fold_bn(sd, f'{L.name}.bn', sd[f'{L.name}.conv.weight'])
     else:
         w, b = sd[f'{L.name}.weight'].double(), sd[f'{L.name}.bias'].double()
     return w.permute(0, 2, 3, 1).reshape(L.cout, -1), b

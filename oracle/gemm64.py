@@ -3,7 +3,8 @@ INFRASTRUCTURE.
 
 The contract is that of ``block64.py``: every stage is fed the exact fp32 tensor the GPU stage was fed (normally the
 GPU's own output of the previous stage) and returns ``(want, S)``; a stage passes when |got - want| <= tau * S at every
-element.  BatchNorm is folded here, in float64, from the state dict (not from the library's folded weights).
+element.  BatchNorm is folded here, in float64, from the state dict (``check64.fold_bn``, not the library's folded
+weights).
 
 Tensor-core stages (``tc_gemm_kernel``, csrc/kernels_gemm.cuh).  Every operand is split into fp16 hi + lo after a
 power-of-two scale: row m of A by 2^e so that its max |a| (``rowmax``) lands in [2^13, 2^14), output channel n of W by
@@ -31,17 +32,17 @@ Rows are what the GPU stores: one per NHWC pixel for ResNet-50, one per point (f
 """
 from __future__ import annotations
 
-from typing import Dict, Optional, Tuple
+from typing import Optional, Tuple
 
 import torch
 import torch.nn.functional as F
 
-BN_EPS = 1e-5
+from oracle.check64 import Pair, fold_bn, linear_heads, strip_prefix, worst  # noqa: F401  (the tests' check)
+
 PTS = 68
 RESNET_PREFIX = 'I2P.backbone.'
+HEADS = ('fc_ori', 'fc_shape', 'fc_exp', 'fc_tex')          # the four linear heads of ResNet-50 and MobileNetV1
 FACE_VEC_LD = 2360                      # kFaceVecLd (csrc/heads_host.inl): 1024 + 1280 + 40 + 10 = 2354, padded
-
-Pair = Tuple[torch.Tensor, torch.Tensor]
 
 
 # ---- floors and the two forms of S ----------------------------------------------------------------------------------
@@ -96,28 +97,14 @@ def patches(x: torch.Tensor, ksize: int, stride: int, pad: int) -> torch.Tensor:
     return cols.reshape(-1, ksize * ksize * c)
 
 
-# ---- BatchNorm folding ------------------------------------------------------------------------------------------------
-
-def _bn_fold(sd, bn: str, w: torch.Tensor, conv_bias: Optional[torch.Tensor]) -> Tuple[torch.Tensor, torch.Tensor]:
-    g = lambda k: sd[f'{bn}.{k}'].double()
-    scale = g('weight') / torch.sqrt(g('running_var') + BN_EPS)
-    cb = conv_bias.double() if conv_bias is not None else torch.zeros_like(scale)
-    return w.double() * scale.view(-1, *([1] * (w.dim() - 1))), (cb - g('running_mean')) * scale + g('bias')
-
-
 # ---- ResNet-50 (rows = NHWC pixels) ---------------------------------------------------------------------------------
-
-def _resnet_sd(sd):
-    return {k[len(RESNET_PREFIX):]: v for k, v in sd.items() if k.startswith(RESNET_PREFIX)} \
-        if any(k.startswith(RESNET_PREFIX) for k in sd) else sd
-
 
 def resnet_fold(sd, index: int) -> Tuple[torch.Tensor, torch.Tensor]:
     """Conv ``index`` of the 53-conv execution plan with BN folded: (W (N, K) in the GEMM's k order, bias)."""
     from synergynet_b200.backbone import resnet50_conv_keys
-    sd = _resnet_sd(sd)
+    sd = strip_prefix(sd, RESNET_PREFIX)
     ck, bk = resnet50_conv_keys()[index]
-    w, b = _bn_fold(sd, bk, sd[ck + '.weight'], None)
+    w, b = fold_bn(sd, bk, sd[ck + '.weight'])
     if index == 0:                                                   # the stem keeps the OIHW order (c, ky, kx)
         return w.reshape(w.shape[0], -1), b
     return w.permute(0, 2, 3, 1).reshape(w.shape[0], -1), b          # (ky, kx, c)
@@ -156,20 +143,15 @@ def avgpool(x: torch.Tensor, batch: int) -> Pair:
 
 
 def resnet_heads(sd, pooled: torch.Tensor) -> Pair:
-    sd = _resnet_sd(sd)
-    keys = ('fc_ori', 'fc_shape', 'fc_exp', 'fc_tex')
-    w = torch.cat([sd[f'{k}.weight'].double() for k in keys])
-    b = torch.cat([sd[f'{k}.bias'].double() for k in keys])
-    return gemm(pooled, w, b, False)
+    return gemm(pooled, *linear_heads(strip_prefix(sd, RESNET_PREFIX), HEADS), False)
 
 
 # ---- PointNet heads (rows = B*68 points, face-major) ---------------------------------------------------------------
 
 def pn_fold(sd, prefix: str, conv: str) -> Tuple[torch.Tensor, torch.Tensor]:
     """Conv1d(k=1) ``conv`` of ``prefix`` ('forwardDirection.' / 'reverseDirection.') with its BatchNorm folded."""
-    bn = 'bn' + conv[4:]
-    sub = {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
-    return _bn_fold(sub, bn, sub[conv + '.weight'][:, :, 0], sub[conv + '.bias'])
+    sub = strip_prefix(sd, prefix)
+    return fold_bn(sub, 'bn' + conv[4:], sub[conv + '.weight'][:, :, 0], sub[conv + '.bias'])
 
 
 def lmk_rows(lmk: torch.Tensor) -> torch.Tensor:
@@ -255,19 +237,25 @@ def check_pointnet_batches(batches=POINTNET_BATCHES) -> None:
     assert any(64 < r < 80 for r in rems) and any(r >= 80 for r in rems), rems
 
 
-def resnet_faces(batch: int) -> list:
-    """Faces to check at this batch: the first and the last face and, at every map size, the face that straddles the
-    edge of the last tile and the first face wholly inside that tile (where one fits)."""
+def tile_edge_faces(batch: int, maps, tile: int = TILE) -> list:
+    """Faces to check at this batch of GEMMs that hold p rows per face, p each map size of ``maps``: the first and the
+    last face and, at every map size, the face that straddles the edge of the last tile and the first face wholly inside
+    that tile (where one fits)."""
     faces = {0, batch - 1}
-    for p in RESNET_MAPS:
+    for p in maps:
         m = batch * p
-        t0 = (m - 1) // TILE * TILE                      # first row of the last tile
+        t0 = (m - 1) // tile * tile                      # first row of the last tile
         if t0 > 0:
             faces |= {(t0 - 1) // p, t0 // p}
         inside = -(-t0 // p)
         if inside < batch:
             faces.add(inside)
     return sorted(faces)
+
+
+def resnet_faces(batch: int) -> list:
+    """``tile_edge_faces`` over the four ResNet-50 map sizes."""
+    return tile_edge_faces(batch, RESNET_MAPS)
 
 
 def check_resnet_faces(batch: int, faces) -> None:
@@ -284,19 +272,6 @@ def check_resnet_faces(batch: int, faces) -> None:
 
 
 # ---- checking --------------------------------------------------------------------------------------------------------
-
-def ratio(got: torch.Tensor, want: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
-    """|got - want| / S per element (0 where they are equal, inf where S = 0 and they differ)."""
-    d = (got.double() - want).abs()
-    return torch.where(d == 0, torch.zeros_like(d), d / s)
-
-
-def worst(got: torch.Tensor, want: torch.Tensor, s: torch.Tensor) -> Tuple[float, tuple]:
-    """Largest |got - want| / S and its index (row, column)."""
-    r = ratio(got, want, s)
-    i = int(torch.argmax(r))
-    return float(r.reshape(-1)[i]), tuple(int(v) for v in torch.unravel_index(torch.tensor(i), r.shape))
-
 
 def rowmax_bits(x: torch.Tensor) -> torch.Tensor:
     """max |x| of every row as fp32 bit patterns (int32), what a producer must record."""

@@ -2,7 +2,8 @@
 
 The contract is that of ``gemm64.py`` (whose docstring defines both forms of S): every stage is fed the exact fp32 tensor
 the GPU stage was fed (normally the GPU's own output of the previous stage) and returns ``(want, S)``; a stage passes when
-|got - want| <= tau * S at every element.  BatchNorm is folded here, in float64, from the state dict.
+|got - want| <= tau * S at every element.  BatchNorm is folded here, in float64, from the state dict
+(``check64.fold_bn``).
 
   * conv_sep (1x1) and the heads run on ``tc_gemm_kernel``: the split-GEMM form of ``gemm64.gemm``, with the row scale
     taken from the true max |a| of each row -- which is what the depthwise kernel and the pool record.
@@ -21,10 +22,10 @@ import torch
 import torch.nn.functional as F
 
 from oracle import gemm64
+from oracle.check64 import Pair, fold_bn, linear_heads, strip_prefix
+from oracle.gemm64 import HEADS
 
-Pair = Tuple[torch.Tensor, torch.Tensor]
 PREFIX = 'I2P.backbone.'
-HEADS = ('fc_ori', 'fc_shape', 'fc_exp', 'fc_tex')
 NUM_STAGES = 29
 
 
@@ -49,18 +50,12 @@ def stage_table(arch: str) -> List[tuple]:
     return out
 
 
-def _sd(sd):
-    return {k[len(PREFIX):]: v for k, v in sd.items() if k.startswith(PREFIX)} if any(k.startswith(PREFIX) for k in sd) else sd
-
-
 def fold(sd, index: int) -> Tuple[torch.Tensor, torch.Tensor]:
     """Conv ``index`` of the 27-conv plan with BN folded in float64: (W (cout, cin/groups, k, k), bias)."""
     from synergynet_b200.backbone import mobilenet_v1_conv_keys
-    sd = _sd(sd)
+    sd = strip_prefix(sd, PREFIX)
     ck, bk = mobilenet_v1_conv_keys()[index]
-    g = lambda k: sd[f'{bk}.{k}'].double()
-    scale = g('weight') / torch.sqrt(g('running_var') + gemm64.BN_EPS)
-    return sd[ck + '.weight'].double() * scale.view(-1, 1, 1, 1), g('bias') - g('running_mean') * scale
+    return fold_bn(sd, bk, sd[ck + '.weight'])
 
 
 def _nchw(rows: torch.Tensor, batch: int) -> torch.Tensor:
@@ -97,16 +92,9 @@ def pointwise(sd, index: int, x: torch.Tensor) -> Pair:
     return gemm64.gemm(x, w.reshape(w.shape[0], -1), b, True)
 
 
-def avgpool(x: torch.Tensor, batch: int) -> Pair:
-    return gemm64.avgpool(x, batch)
-
-
 def heads(sd, pooled: torch.Tensor) -> Pair:
     """fc_ori | fc_shape | fc_exp | fc_tex on the pooled features -> (B, 102) (tensor-core stage, no activation)."""
-    sd = _sd(sd)
-    w = torch.cat([sd[f'{k}.weight'].double() for k in HEADS])
-    b = torch.cat([sd[f'{k}.bias'].double() for k in HEADS])
-    return gemm64.gemm(pooled, w, b, False)
+    return gemm64.gemm(pooled, *linear_heads(strip_prefix(sd, PREFIX), HEADS), False)
 
 
 def stage(sd, index: int, inp: torch.Tensor, batch: int) -> Pair:
@@ -115,7 +103,7 @@ def stage(sd, index: int, inp: torch.Tensor, batch: int) -> Pair:
         return stem(sd, inp)
     if index <= 26:
         return depthwise(sd, index, inp, batch) if index % 2 == 1 else pointwise(sd, index, inp)
-    return avgpool(inp, batch) if index == 27 else heads(sd, inp)
+    return gemm64.avgpool(inp, batch) if index == 27 else heads(sd, inp)
 
 
 @torch.no_grad()
@@ -125,7 +113,7 @@ def forward64(sd, x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     cur = stem(sd, x)[0]
     for i in range(1, 27):
         cur = stage(sd, i, cur, b)[0]
-    pooled = avgpool(cur, b)[0]
+    pooled = gemm64.avgpool(cur, b)[0]
     return heads(sd, pooled)[0], pooled
 
 
@@ -166,15 +154,5 @@ def check_mbv1_batches(batches=BATCHES) -> None:
 
 
 def faces(batch: int) -> list:
-    """Faces to check at this batch: the first and the last face and, at every map size, the face that straddles the
-    edge of the last tile and the first face wholly inside that tile (where one fits)."""
-    out = {0, batch - 1}
-    for p in MAPS:
-        m = batch * p
-        t0 = (m - 1) // gemm64.TILE * gemm64.TILE
-        if t0 > 0:
-            out |= {(t0 - 1) // p, t0 // p}
-        inside = -(-t0 // p)
-        if inside < batch:
-            out.add(inside)
-    return sorted(out)
+    """``gemm64.tile_edge_faces`` over the five MobileNetV1 map sizes."""
+    return gemm64.tile_edge_faces(batch, MAPS)

@@ -1,9 +1,9 @@
 """Float64 oracle of the 3DMM reconstruction (reference model_building.py:106-139 and the crop -> image affine of
-utils/inference.py:127-138), with a per-element error scale, and mirrors of the work plans of the two tensor-core
-reconstruction kernels.  TEST INFRASTRUCTURE.
+utils/inference.py:127-138), with a per-element error scale, mirrors of the work plans of the two tensor-core
+reconstruction kernels and the seeded parameters its tests feed them.  TEST INFRASTRUCTURE.
 
 The contract is that of ``block64.py`` / ``gemm64.py``: ``reconstruct`` returns ``(want, S)`` and an output passes when
-|got - want| <= tau * S at every element (``gemm64.worst``).
+|got - want| <= tau * S at every element (``check64.worst``).
 
 The tensor-core scheme (csrc/kernels_dense.cuh, ``syn_commit`` / ``pack_recon_tc`` in synergy_b200.cu).  Coefficient
 k is multiplied by ascale_k = 2^(10 - e_k), where 2^e_k bounds |mean_k| + 8 |std_k| (2^10 when that bound is 0), and
@@ -37,6 +37,8 @@ from __future__ import annotations
 from typing import Dict, Optional, Tuple
 
 import numpy as np
+
+from oracle.check64 import worst  # noqa: F401  (the check the reconstruction tests apply)
 
 IMG = 120
 N_ALPHA = 50
@@ -138,18 +140,68 @@ def reconstruct_chunked(params, pack, chunk: int = 64, **kw) -> Tuple[np.ndarray
     return np.concatenate([q[0] for q in parts]), np.concatenate([q[1] for q in parts])
 
 
-def ratio(got: np.ndarray, want: np.ndarray, s: np.ndarray) -> np.ndarray:
-    """|got - want| / S per element (0 where equal, inf where S = 0 and they differ)."""
-    d = np.abs(np.asarray(got, np.float64) - want)
-    with np.errstate(divide='ignore', invalid='ignore'):
-        return np.where(d == 0, 0.0, d / s)
+# ---- inputs -----------------------------------------------------------------------------------------------------------
+
+RESNET_SCALED = 23010.0                   # |alpha * ascale| the random ResNet-50 checkpoint reaches
 
 
-def worst(got, want, s) -> Tuple[float, tuple]:
-    """Largest |got - want| / S and its (face, coordinate, vertex)."""
-    r = ratio(got, want, s)
-    i = int(np.argmax(r))
-    return float(r.reshape(-1)[i]), tuple(int(v) for v in np.unravel_index(i, r.shape))
+def random_params(b, seed, spread=1.0):
+    """Whitened parameters: distinct faces within a few sigma."""
+    return (np.random.default_rng(seed).standard_normal((b, 62)) * spread).astype(np.float32)
+
+
+def roi_rows(b, seed):
+    rng = np.random.default_rng(seed)
+    k = rng.uniform(0.3, 4.0, (b, 3))
+    s = rng.uniform(-50.0, 800.0, (b, 2))
+    return np.stack([k[:, 0], s[:, 0], k[:, 1], s[:, 1], k[:, 2]], 1).astype(np.float32)
+
+
+def _whiten(p_raw, pack):
+    mean, std = pack['param_mean'][:62].astype(np.float64), pack['param_std'][:62].astype(np.float64)
+    return ((p_raw - mean) / np.where(std == 0, 1.0, std)).astype(np.float32)
+
+
+def magnitude_params(pack, beyond):
+    """(params, whitening) with coefficients at the magnitudes the alpha scale has to cover.  ``beyond`` = False: the
+    mean, +-8 sigma, the ResNet-50 magnitude, just below the fp16 clamp 60000 / ascale_k, and translations that put the
+    vertices around y = 121 (the flip cancels).  ``beyond`` = True: just above the clamp, one coefficient far above it
+    next to tiny ones, and raw coefficients (whitening off) far beyond it, including the coefficient of the stress
+    model whose mean and std are 0."""
+    from oracle.synth_model import STRESS_ZERO_COEF
+    mean, std = pack['param_mean'][:62].astype(np.float64), pack['param_std'][:62].astype(np.float64)
+    lim = CLAMP / ascale(mean, std)                                     # |alpha_k| at the clamp
+    sign = np.where(np.arange(50) % 2, -1.0, 1.0)
+    base = random_params(8, 91, 0.5).astype(np.float64)
+    rows = []
+
+    def face(alpha, i):
+        p = base[i % 8].copy() * std + mean
+        p[12:62] = alpha
+        return p
+
+    if not beyond:
+        rows += [face(mean[12:62], 0), face(mean[12:62] + 8 * std[12:62], 1), face(mean[12:62] - 8 * std[12:62], 2)]
+        rows += [face(sign * RESNET_SCALED / ascale(mean, std), 3), face(0.999 * sign * lim, 4),
+                 face(-0.999 * sign * lim, 5)]
+        for i in range(4):
+            p = face(mean[12:62] + 2 * std[12:62] * np.random.default_rng(i).standard_normal(50), 6 + i)
+            p[7] = 121.0 + 8.0 * i                                      # t_y: vy = 121 within the face
+            rows.append(p)
+        return _whiten(np.stack(rows), pack), True
+    rows += [face(1.001 * sign * lim, 0), face(-1.5 * sign * lim, 1)]
+    p = face(mean[12:62] + 1e-3 * std[12:62], 2)
+    p[12] = 4.0 * lim[0]                                                # huge next to tiny
+    rows.append(p)
+    p = face(mean[12:62] + 1e-6 * std[12:62], 3)
+    p[12 + 40] = -1e3 * lim[40]
+    rows.append(p)
+    rows += [face(3.0 * sign * lim, 4), face(-40.0 * lim, 5)]
+    for i, a in enumerate((100.0, -1000.0, 58.0, 1e5)):
+        p = face(mean[12:62], 6 + i)
+        p[12 + STRESS_ZERO_COEF] = a                                    # ascale 2^10 when mean = std = 0
+        rows.append(p)
+    return np.stack(rows).astype(np.float32), False
 
 
 # ---- work plans -----------------------------------------------------------------------------------------------------

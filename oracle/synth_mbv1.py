@@ -15,6 +15,7 @@ from typing import Dict
 import torch
 import torch.nn.functional as F
 
+from oracle.synth_model import _pow2_factors
 from synergynet_b200 import synthetic
 
 _CACHE: Dict[tuple, Dict[str, torch.Tensor]] = {}
@@ -46,14 +47,6 @@ def build_mobilenet_v1_state_dict(seed: int = 0, arch: str = 'mobilenet_1') -> D
         x = ((y - p('running_mean')) / torch.sqrt(p('running_var') + 1e-5) * p('weight') + p('bias')).clamp_min(0.0)
     _CACHE[key] = sd
     return sd
-
-
-def _pow2_factors(n: int, g: torch.Generator, lo: int, hi: int) -> torch.Tensor:
-    """n factors 2^k, k an integer drawn from [lo, hi], with one channel at each end of the range."""
-    k = torch.randint(lo, hi + 1, (n,), generator=g)
-    ends = torch.randperm(n, generator=g)[:2]
-    k[ends[0]], k[ends[1]] = lo, hi
-    return torch.pow(2.0, k.double()).float()
 
 
 @torch.no_grad()

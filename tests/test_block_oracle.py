@@ -5,11 +5,9 @@ import torch
 
 from oracle import block64, synth_model, tile_cover
 from oracle import reference_port as rp
+from oracle.stage_check import LAYER_TOL, TAU, WIDE
 from synergynet_b200 import _lib, synthetic
 from synergynet_b200.backbone import conv_plan
-from oracle.stage_check import TAU
-from test_gpu_blocks import WIDE
-from test_gpu_parity import LAYER_TOL
 
 PLAN = conv_plan()
 
@@ -54,7 +52,7 @@ def test_checker_flags_a_small_channel_that_max_rel_err_misses(sd, x8):
     """A channel whose values are a few percent of the tensor's maximum (a block output of the rescaled checkpoint),
     scaled by 1 + 1e-3: the per-element check flags it, while max_rel_err under the per-layer bar of test_gpu_parity
     passes the same tensor."""
-    wide = synth_model.reparametrize_streams(sd, **WIDE)
+    wide = synth_model.reparametrize_streams(sd, **WIDE['block64'])
     _, _, c = rp.mobilenetv2_forward(wide, x8[:2], return_convs=True)
     b = 9
     want, s = block64.block(wide, b, c[3 * b - 4].permute(0, 2, 3, 1))
@@ -73,7 +71,7 @@ def test_checker_flags_a_small_channel_that_max_rel_err_misses(sd, x8):
 def test_rescaled_checkpoint_is_exact_and_wide(sd, x8):
     """reparametrize_streams computes bit for bit the same params in fp32; every block input spreads its per-channel
     maxima over at least 2^8 and stays far inside the fp16 range of the split engines (|x| < ~937)."""
-    wide = synth_model.reparametrize_streams(sd, **WIDE)
+    wide = synth_model.reparametrize_streams(sd, **WIDE['block64'])
     p0, _, c0 = rp.mobilenetv2_forward(sd, x8, return_convs=True)
     p1, _, c1 = rp.mobilenetv2_forward(wide, x8, return_convs=True)
     assert torch.equal(p0, p1)

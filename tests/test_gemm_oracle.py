@@ -5,9 +5,9 @@ import torch
 
 from oracle import gemm64, synth_model
 from oracle import reference_port as rp
+from oracle.stage_check import HEAD_TOL, TAU, WIDE
 from synergynet_b200 import synthetic
 from synergynet_b200.backbone import resnet50_conv_keys
-from test_gpu_gemm_layers import HEAD_TOL, TAU, WIDE
 
 KEYS = resnet50_conv_keys()
 NOISE = 2e-6                # fp32 port against the float64 chain, relative to the largest output
@@ -95,7 +95,7 @@ def test_pointnet_oracle_agrees_with_fp32_reference(sd, heads_in):
 def test_rescaled_checkpoints_are_exact_and_wide(rsd, sd, x3, heads_in):
     """The reparametrizations compute bit for bit the same fp32 outputs, and they spread the per-channel maxima of the
     hidden tensors they rescale over at least 2^8 inside each row's set of channels."""
-    rw = synth_model.reparametrize_resnet(rsd, prefix='I2P.backbone.', **WIDE)
+    rw = synth_model.reparametrize_resnet(rsd, prefix='I2P.backbone.', **WIDE['gemm64'])
     a0, p0 = rp.resnet50_forward(rsd, x3)
     a1, p1 = rp.resnet50_forward(rw, x3)
     assert torch.equal(a0, a1) and torch.equal(p0, p1)
@@ -103,7 +103,7 @@ def test_rescaled_checkpoints_are_exact_and_wide(rsd, sd, x3, heads_in):
     assert float(f.max() / f.min()) == 2.0 ** 10
     assert torch.equal(f, torch.exp2(torch.round(torch.log2(f))))
     lmk, pool, attr = heads_in
-    pw = synth_model.reparametrize_pointnet(sd, **WIDE)
+    pw = synth_model.reparametrize_pointnet(sd, **WIDE['gemm64'])
     assert torch.equal(rp.mlp_for_forward(sd, lmk, pool, attr[:, 12:52], attr[:, 52:62]),
                        rp.mlp_for_forward(pw, lmk, pool, attr[:, 12:52], attr[:, 52:62]))
     assert torch.equal(rp.mlp_rev_forward(sd, lmk), rp.mlp_rev_forward(pw, lmk))
@@ -149,7 +149,7 @@ def test_checker_flags_a_small_channel_that_max_rel_err_misses(sd, heads_in):
     """A channel of conv5's output (rescaled MLP_for) whose values are 1-10 % of the tensor's maximum, scaled by
     1 + 1e-3: the per-element check flags it, while max_rel_err under HEAD_TOL passes the same tensor."""
     lmk, pool, attr = heads_in
-    pw = synth_model.reparametrize_pointnet(sd, **WIDE)
+    pw = synth_model.reparametrize_pointnet(sd, **WIDE['gemm64'])
     pre = 'forwardDirection.'
     h, _ = gemm64.pn_conv1(pw, pre, lmk)
     for i in range(2, 5):
@@ -163,5 +163,5 @@ def test_checker_flags_a_small_channel_that_max_rel_err_misses(sd, heads_in):
     bad[:, c] *= 1 + 1e-3
     assert rp.max_rel_err(bad.numpy(), want.numpy()) < HEAD_TOL
     r, where = gemm64.worst(bad, want, s)
-    assert r > 10 * TAU['gemm'] and where[1] == c, (r, where)
-    assert gemm64.worst(want.float(), want, s)[0] < TAU['gemm']
+    assert r > 10 * TAU['gemm64']['gemm'] and where[1] == c, (r, where)
+    assert gemm64.worst(want.float(), want, s)[0] < TAU['gemm64']['gemm']

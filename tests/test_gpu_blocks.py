@@ -11,13 +11,11 @@ import torch
 
 from oracle import stage_check, synth_model, tile_cover
 from oracle import reference_port as rp
-from oracle.stage_check import ENGINES, make_model as _make_model, report as _report, stage_ratios, tau as _tau
+from oracle.stage_check import (ENGINES, TOL, WIDE, make_model as _make_model, report as _report, seeded_crops,
+                                stage_ratios, tau as _tau)
 from synergynet_b200 import _lib, synthetic
 
 pytestmark = pytest.mark.gpu
-
-TOL = 1e-4
-WIDE = dict(seed=7, lo=-6, hi=4)         # channel factors 2^-6 .. 2^4 on every block stream
 
 
 @pytest.fixture(scope='module')
@@ -27,7 +25,7 @@ def sd():
 
 @pytest.fixture(scope='module')
 def sd_wide(sd):
-    return synth_model.reparametrize_streams(sd, **WIDE)
+    return synth_model.reparametrize_streams(sd, **WIDE['block64'])
 
 
 @pytest.fixture(scope='module')
@@ -53,8 +51,7 @@ def _engine(model, kind):
 def _batch(sms, kind):
     batch = tile_cover.choose_batches(sms)[kind]
     tile_cover.check_plan(kind, batch, sms)
-    x = synthetic.normalize_crops(synthetic.make_structured_crops_u8(batch, seed=900 + batch)).cuda()
-    return x, tile_cover.faces_to_check(batch, sms, seed=batch)
+    return seeded_crops(batch, 900 + batch), tile_cover.faces_to_check(batch, sms, seed=batch)
 
 
 @pytest.mark.parametrize('plan', ['mixed_pairs', 'odd_pairs', 'ragged_quads'])

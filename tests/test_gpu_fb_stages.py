@@ -8,43 +8,15 @@ inception branch and every head must write its slice of the shared tensor and no
 import pytest
 import torch
 
-from oracle import fb64, gemm64
+from oracle import fb64
+from oracle.stage_check import TAU, Ratios, over, report, same_bits
 from synergynet_b200 import faceboxes, synthetic
 
 pytestmark = pytest.mark.gpu
 
-# The bar: |got - want| <= TAU * S at every element, per stage kind, at most 4x the worst ratio measured on an H100
-# 80GB HBM3 (132 SMs, 400 W power limit) over the sizes of fb64.choose_sizes() (worst in the comment):
-TAU = {'conv': 1.5e-6,      # 4.37e-07: fp32 FMA on CUDA cores, conv3_2 (K = 1152) at 720 x 1080
-       'avgpool': 1e-6,     # 2.57e-07: inception2's average pool at 720 x 1080
-       'softmax': 4.5e-7}   # 1.25e-07: at 193 x 961
-# Negative control (conv weights rounded to bf16 before upload, 250 x 333): 1.27e-04 at its smallest (conf.1) and
-# 1.15e-03 at its largest (inception3.branch3x3_reduce), 85x and 770x the bar.
+BARS = TAU['fb64']
 NONZERO = 0.25              # every ReLU stage: the float64 chain measures 37-69 % nonzero on these scenes at every size
 SIZES = fb64.choose_sizes()
-
-
-class Worst:
-    """Largest ratio per stage kind, with where it occurred."""
-
-    def __init__(self):
-        self.by_kind = {}
-
-    def add(self, kind, where, got, want_s):
-        r, ix = gemm64.worst(got, *want_s)
-        if r >= self.by_kind.get(kind, (-1.0,))[0]:
-            self.by_kind[kind] = (r, where, ix)
-        return r
-
-    def over(self):
-        return {k: v for k, v in self.by_kind.items() if v[0] > TAU[k]}
-
-    def report(self, tag):
-        print(f'\n[{tag}] ' + '  '.join(f'{k}: {r:.3e} at {w} {ix}' for k, (r, w, ix) in self.by_kind.items()))
-
-
-def _same_bits(a, b):
-    return torch.equal(a.float().contiguous().view(torch.int32), b.float().contiguous().view(torch.int32))
 
 
 def _name(i):
@@ -73,9 +45,9 @@ def run_stages(net, img):
     return got
 
 
-def stage_ratios(sd, img, got, worst=None, per_stage=None):
-    """Hold every stage to the oracle on the GPU's own inputs: rounding stages to TAU (into ``worst`` and, by stage, into
-    ``per_stage``), max-pools bit for bit.  Returns the fraction of nonzero elements of every ReLU stage."""
+def stage_ratios(sd, img, got, ratios):
+    """Hold every stage to the oracle on the GPU's own inputs: rounding stages into ``ratios``, max-pools bit for bit.
+    Returns the fraction of nonzero elements of every ReLU stage."""
     h, w = int(img.shape[0]), int(img.shape[1])
     image = img.cpu()
     nonzero = {}
@@ -83,14 +55,9 @@ def stage_ratios(sd, img, got, worst=None, per_stage=None):
         r = fb64.stage(sd, i, [image if s == 'image' else got[s] for s in st.inputs])
         part = fb64.owned(i, got[i], h, w)
         if st.kind == 'maxpool':
-            assert _same_bits(part, r), f'{(h, w)} {_name(i)}'
+            assert same_bits(part, r), f'{(h, w)} {_name(i)}'
             continue
-        if worst is not None:
-            ratio = worst.add(st.kind, ((h, w), _name(i)), part, r)
-        else:
-            ratio = gemm64.worst(part, *r)[0]
-        if per_stage is not None:
-            per_stage[i] = ratio
+        ratios.add(st.kind, _name(i), part, r)
         if st.kind == 'conv' and fb64.LAYERS[st.layer].act:
             nonzero[i] = float((part != 0).double().mean())
     return nonzero
@@ -109,19 +76,19 @@ def check_slices(got, h, w):
             keep = torch.ones(128, dtype=torch.bool)
             keep[lo:hi] = False
             if before is not None:
-                assert _same_bits(got[s][..., keep], before[..., keep]), f'{(h, w)} {_name(s)} wrote outside {lo}..{hi}'
-            assert _same_bits(got[last][..., lo:hi], got[s][..., lo:hi]), f'{(h, w)} block {b + 1} slice {lo}..{hi}'
+                assert same_bits(got[s][..., keep], before[..., keep]), f'{(h, w)} {_name(s)} wrote outside {lo}..{hi}'
+            assert same_bits(got[last][..., lo:hi], got[s][..., lo:hi]), f'{(h, w)} block {b + 1} slice {lo}..{hi}'
             before = got[s]
     for head, last in fb64.HEAD_LAST.items():
         before = None
         for s in range(last - 2, last + 1):
             e0, e1 = fb64.head_range(s, h, w)
             t = got[s]
-            assert _same_bits(got[last][e0:e1], t[e0:e1]), f'{(h, w)} {head} head {_name(s)}'
+            assert same_bits(got[last][e0:e1], t[e0:e1]), f'{(h, w)} {head} head {_name(s)}'
             assert not torch.isnan(t[e0:e1]).any(), f'{(h, w)} {_name(s)} left part of its slice unwritten'
             assert torch.isnan(t[e1:]).all(), f'{(h, w)} {_name(s)} wrote past its slice'
             if before is not None:
-                assert _same_bits(t[:e0], before[:e0]), f'{(h, w)} {_name(s)} wrote before its slice'
+                assert same_bits(t[:e0], before[:e0]), f'{(h, w)} {_name(s)} wrote before its slice'
             before = t
 
 
@@ -131,17 +98,18 @@ def test_every_stage_matches_float64_oracle(sd, net, hw):
     h, w = hw
     img = _scene(h, w)
     got = run_stages(net, img)
-    worst = Worst()
-    nonzero = stage_ratios(sd, img, got, worst)
-    worst.report(f'faceboxes {h}x{w}')
-    assert not worst.over(), worst.over()
+    ratios = Ratios()
+    nonzero = stage_ratios(sd, img, got, ratios)
+    report(f'faceboxes {h}x{w}', ratios)
+    bad = over('fb64', ratios)
+    assert not bad, bad
     check_slices(got, h, w)
     low = {_name(i): f for i, f in nonzero.items() if f < NONZERO}
     assert not low, low
     loc, conf = net.forward(img)                        # the debug stops run the production sequence
     torch.cuda.synchronize()
-    assert _same_bits(loc.cpu().reshape(-1), got[fb64.HEAD_LAST['loc']])
-    assert _same_bits(conf.cpu().reshape(-1), got[len(fb64.STAGES) - 1])
+    assert same_bits(loc.cpu().reshape(-1), got[fb64.HEAD_LAST['loc']])
+    assert same_bits(conf.cpu().reshape(-1), got[len(fb64.STAGES) - 1])
 
 
 def test_workspace_reallocation_keeps_results(sd):
@@ -155,7 +123,7 @@ def test_workspace_reallocation_keeps_results(sd):
             first = (loc.cpu(), conf.cpu())
     loc, conf = net.forward(_scene(*SIZES[0]))
     torch.cuda.synchronize()
-    assert _same_bits(loc.cpu(), first[0]) and _same_bits(conf.cpu(), first[1])
+    assert same_bits(loc.cpu(), first[0]) and same_bits(conf.cpu(), first[1])
     net.close()
 
 
@@ -189,10 +157,10 @@ def test_bf16_weights_fail_the_bar(sd):
     net = faceboxes.FaceBoxesNet(bad, torch.device('cuda', 0))
     h, w = fb64.GOLDEN[0]
     img = _scene(h, w)
-    per_stage = {}
-    stage_ratios(sd, img, run_stages(net, img), per_stage=per_stage)
-    conv = {_name(i): r for i, r in per_stage.items() if fb64.STAGES[i].kind == 'conv'}
+    ratios = Ratios()
+    stage_ratios(sd, img, run_stages(net, img), ratios)
+    conv = {s: v[0] for s, v in ratios.items() if v[2] == 'conv'}
     lo, hi = min(conv, key=conv.get), max(conv, key=conv.get)
     print(f'\n[bf16 weights] smallest {conv[lo]:.3e} at {lo}, largest {conv[hi]:.3e} at {hi}')
-    assert conv[lo] > TAU['conv'] and conv[hi] >= 10 * TAU['conv'], conv
+    assert conv[lo] > BARS['conv'] and conv[hi] >= 10 * BARS['conv'], conv
     net.close()

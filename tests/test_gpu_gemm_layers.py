@@ -7,67 +7,23 @@ every row maximum a producer records are compared bit for bit.  The batches put 
 in each of its shapes (oracle/gemm64.py check_*_batches); the ResNet faces checked include the last face, faces that
 straddle the last tile's edge and faces wholly inside it.  H100 only.
 """
-import types
-
 import pytest
 import torch
 
 from oracle import gemm64, synth_model
 from oracle import reference_port as rp
+from oracle.stage_check import (HEAD_TOL, TAU, TOL, WIDE, Ratios, check_rowmax, face_picker, make_model, over, report,
+                                same_bits, seeded_crops)
 from synergynet_b200 import synthetic
 from synergynet_b200.backbone import resnet50_conv_keys
 
 pytestmark = pytest.mark.gpu
 
-# The bar: |got - want| <= TAU * S at every element, per stage kind, at most 4x the worst ratio measured on an H100
-# 80GB HBM3 (132 SMs, 700 W power limit) over the batches, both checkpoints and the kernel-level cases of this file
-# (worst in the comment):
-TAU = {'gemm': 8e-6,        # 3.13e-06: tc_gemm_kernel, ResNet layer4.0.conv2 (K = 4608) at B = 19; PointNet 1.67e-06
-       'simt': 2e-6,        # 7.18e-07: fp32 CUDA cores, ResNet stem (K = 147); PointNet conv1 9.96e-08
-       'pool': 8e-7}        # 2.39e-07: fp32 average pool
-# The ratio grows with K (the fp32 accumulation over k): 1.98e-06 for K = 2360, 2.52e-06 for a 3x3 conv with K = 2304.
-# Negative control: rowmax_in / 8 measures 2.21e-01 and rowmax_in * 2^24 2.13e-04, >= 26x the bar.
-WIDE = dict(seed=11, lo=-6, hi=4)         # hidden-channel factors 2^-6 .. 2^4
-TOL = 1e-4
-HEAD_TOL = 3e-4                           # tests/test_gpu_heads.py
+BARS = TAU['gemm64']
 KEYS = resnet50_conv_keys()
 
 
-class Worst:
-    """Largest ratio per stage kind, with where it occurred."""
-
-    def __init__(self):
-        self.by_kind = {}
-
-    def add(self, kind, stage, got, want_s, where_fn=lambda ix: ix):
-        r, ix = gemm64.worst(got, *want_s)
-        if r >= self.by_kind.get(kind, (-1.0,))[0]:
-            self.by_kind[kind] = (r, stage, where_fn(ix))
-        return r
-
-    def over(self):
-        return {k: v for k, v in self.by_kind.items() if v[0] > TAU[k]}
-
-    def report(self, tag):
-        print(f'\n[{tag}] ' + '  '.join(f'{k}: {r:.3e} at {s} {w}' for k, (r, s, w) in self.by_kind.items()))
-
-
-def _same_bits(a, b):
-    return torch.equal(a.float().contiguous().view(torch.int32), b.float().contiguous().view(torch.int32))
-
-
-def _check_rowmax(out, rm, stage):
-    assert rm is not None and torch.equal(rm, gemm64.rowmax_bits(out)), f'rowmax of {stage}'
-
-
 # ---- ResNet-50 ------------------------------------------------------------------------------------------------------
-
-def _resnet_model(sd):
-    from synergynet_b200 import model_building
-    m = model_building.SynergyNet(types.SimpleNamespace(arch='resnet50', img_size=120, devices_id=[0]))
-    m.load_state_dict({'I2P.backbone.' + k: v for k, v in sd.items()}, strict=False)
-    return m.eval()
-
 
 @pytest.fixture(scope='module')
 def rsd():
@@ -76,43 +32,39 @@ def rsd():
 
 @pytest.fixture(scope='module')
 def rsd_wide(rsd):
-    return synth_model.reparametrize_resnet(rsd, **WIDE)
+    return synth_model.reparametrize_resnet(rsd, **WIDE['gemm64'])
 
 
 @pytest.fixture(scope='module')
 def rs_model(synth_pack, rsd):
-    return _resnet_model(rsd)
+    return make_model(rsd, 'resnet50', strict=False)
 
 
 @pytest.fixture(scope='module')
 def rs_model_wide(synth_pack, rsd_wide):
-    return _resnet_model(rsd_wide)
+    return make_model(rsd_wide, 'resnet50', strict=False)
 
 
-def resnet_ratios(eng, sd, x, faces, worst):
+def resnet_ratios(eng, sd, x, faces, ratios):
     """Run every stage of ResNet-50 on batch ``x`` and hold the given faces to the oracle."""
-    b, nf = x.shape[0], len(faces)
-    fidx = torch.tensor(faces, device=x.device)
-    pick = lambda t: t.view(b, -1, t.shape[1]).index_select(0, fidx).reshape(-1, t.shape[1]).cpu()
-
-    def where(per_face):
-        return lambda ix: (faces[ix[0] // per_face], ix[0] % per_face, ix[1])
+    nf = len(faces)
+    pick, where = face_picker(x.shape[0], faces, x.device)
 
     def run(stage, name):
         out, rm = eng.debug_resnet_until(x, stage)
         if rm is not None:
-            _check_rowmax(out, rm, name)
+            check_rowmax(out, rm, name)
         return pick(out)
 
     stem = run(0, 'stem')
-    worst.add('simt', 'stem', stem, gemm64.resnet_stem(sd, x.index_select(0, fidx).cpu()), where(3600))
+    ratios.add('simt', 'stem', stem, gemm64.resnet_stem(sd, x[faces].cpu()), where(3600))
     pool = run(1, 'maxpool')
-    assert _same_bits(pool, gemm64.resnet_maxpool(stem, nf)), 'maxpool'
+    assert same_bits(pool, gemm64.resnet_maxpool(stem, nf)), 'maxpool'
 
     def conv(i, inp, residual=None):
         got = run(1 + i, KEYS[i][0])
         want = gemm64.resnet_conv(sd, i, inp, nf, residual)
-        worst.add('gemm', KEYS[i][0], got, want, where(got.shape[0] // nf))
+        ratios.add('gemm', KEYS[i][0], got, want, where(got.shape[0] // nf))
         return got
 
     X, i = pool, 1
@@ -124,14 +76,10 @@ def resnet_ratios(eng, sd, x, faces, worst):
         X = conv(i + 2, c2, ident)
         i += 4 if has_ds else 3
     pooled = run(54, 'avgpool')
-    worst.add('pool', 'avgpool', pooled, gemm64.avgpool(X, nf), where(1))
+    ratios.add('pool', 'avgpool', pooled, gemm64.avgpool(X, nf), where(1))
     heads = run(55, 'heads')
-    worst.add('gemm', 'heads', heads, gemm64.resnet_heads(sd, pooled), where(1))
+    ratios.add('gemm', 'heads', heads, gemm64.resnet_heads(sd, pooled), where(1))
     assert eng.poll_error() == 0
-
-
-def _crops(batch, seed):
-    return synthetic.normalize_crops(synthetic.make_structured_crops_u8(batch, seed=seed)).cuda()
 
 
 @pytest.mark.parametrize('batch', gemm64.RESNET_BATCHES)
@@ -140,10 +88,11 @@ def test_resnet_every_stage_matches_float64_oracle(rs_model, rsd, batch):
     faces = gemm64.resnet_faces(batch)
     gemm64.check_resnet_faces(batch, faces)
     eng = rs_model._engine(torch.device('cuda', 0))
-    w = Worst()
-    resnet_ratios(eng, rsd, _crops(batch, 500 + batch), faces, w)
-    w.report(f'resnet50 B={batch} faces={faces}')
-    assert not w.over(), w.over()
+    ratios = Ratios()
+    resnet_ratios(eng, rsd, seeded_crops(batch, 500 + batch), faces, ratios)
+    report(f'resnet50 B={batch} faces={faces}', ratios)
+    bad = over('gemm64', ratios)
+    assert not bad, bad
 
 
 def test_resnet_rescaled_checkpoint(rs_model_wide, rsd_wide):
@@ -157,10 +106,12 @@ def test_resnet_rescaled_checkpoint(rs_model_wide, rsd_wide):
     print(f'\n[resnet50 rescaled] out102 err {err:.3e}')
     assert err < TOL
     batch = gemm64.RESNET_BATCHES[0]
-    w = Worst()
-    resnet_ratios(eng, rsd_wide, _crops(batch, 500 + batch), gemm64.resnet_faces(batch), w)
-    w.report(f'resnet50 rescaled B={batch}')
-    assert not w.over(), w.over()
+    faces = gemm64.resnet_faces(batch)
+    ratios = Ratios()
+    resnet_ratios(eng, rsd_wide, seeded_crops(batch, 500 + batch), faces, ratios)
+    report(f'resnet50 rescaled B={batch}', ratios)
+    bad = over('gemm64', ratios)
+    assert not bad, bad
 
 
 # ---- PointNet heads ---------------------------------------------------------------------------------------------------
@@ -172,17 +123,17 @@ def sd():
 
 @pytest.fixture(scope='module')
 def sd_wide(sd):
-    return synth_model.reparametrize_pointnet(sd, **WIDE)
+    return synth_model.reparametrize_pointnet(sd, **WIDE['gemm64'])
 
 
 @pytest.fixture(scope='module')
 def pn_model(synth_pack, sd):
-    return _mobilenet_model(sd)
+    return make_model(sd)
 
 
 @pytest.fixture(scope='module')
 def pn_model_wide(synth_pack, sd_wide):
-    return _mobilenet_model(sd_wide)
+    return make_model(sd_wide)
 
 
 @pytest.fixture(scope='module')
@@ -194,14 +145,7 @@ def pn_inputs(synth_pack, sd):
     return lmk, pool, attr
 
 
-def _mobilenet_model(sd):
-    from synergynet_b200 import model_building
-    m = model_building.SynergyNet(types.SimpleNamespace(arch='mobilenet_v2', img_size=120, devices_id=[0]))
-    m.load_state_dict(sd, strict=True)
-    return m.eval()
-
-
-def pointnet_ratios(model, sd, lmk, pool, params, worst):
+def pointnet_ratios(model, sd, lmk, pool, params, ratios):
     b = lmk.shape[0]
     lmk, pool, params = lmk.cuda(), pool.cuda(), params.cuda()
     eng = model._pointnet_engine(lmk, 0)                  # hands both heads' weights to the engine
@@ -213,34 +157,34 @@ def pointnet_ratios(model, sd, lmk, pool, params, worst):
         def run(stage, name):
             out, rm = eng.debug_pointnet_until(net, lmk, stage, pool, params)
             if rm is not None:
-                _check_rowmax(out, rm, f'{tag} {name}')
+                check_rowmax(out, rm, f'{tag} {name}')
             return out.cpu()
 
         got = run(0, 'conv1')
-        worst.add('simt', f'{tag} conv1', got, gemm64.pn_conv1(sd, pre, lmk.cpu()), where(68))
+        ratios.add('simt', f'{tag} conv1', got, gemm64.pn_conv1(sd, pre, lmk.cpu()), where(68))
         outs = [got]
         for i in range(2, 6):
             got = run(i - 1, f'conv{i}')
-            worst.add('gemm', f'{tag} conv{i}', got, gemm64.pn_conv(sd, pre, f'conv{i}', outs[-1]), where(68))
+            ratios.add('gemm', f'{tag} conv{i}', got, gemm64.pn_conv(sd, pre, f'conv{i}', outs[-1]), where(68))
             outs.append(got)
         glob = run(5, 'global features')
-        assert _same_bits(glob, gemm64.pn_pool(outs[4])), f'{tag} max-pool'
+        assert same_bits(glob, gemm64.pn_pool(outs[4])), f'{tag} max-pool'
         if net == 1:
             heads = run(6, 'heads')
-            worst.add('gemm', 'rev heads', heads, gemm64.rev_heads(sd, glob), where(1))
+            ratios.add('gemm', 'rev heads', heads, gemm64.rev_heads(sd, glob), where(1))
             continue
         fv = run(6, 'face vector')
-        assert _same_bits(fv, gemm64.face_vector(glob, pool.cpu(), params.cpu())), 'face vector'
+        assert same_bits(fv, gemm64.face_vector(glob, pool.cpu(), params.cpu())), 'face vector'
         face = run(7, 'conv6 face')
-        worst.add('gemm', 'for conv6 face', face, gemm64.conv6_face(sd, fv), where(1))
+        ratios.add('gemm', 'for conv6 face', face, gemm64.conv6_face(sd, fv), where(1))
         got = run(8, 'conv6 point')
-        worst.add('gemm', 'for conv6 point', got, gemm64.conv6_point(sd, outs[1], face), where(68))
+        ratios.add('gemm', 'for conv6 point', got, gemm64.conv6_point(sd, outs[1], face), where(68))
         for i in (7, 8, 9):
             nxt = run(i + 2, f'conv{i}')
-            worst.add('gemm', f'for conv{i}', nxt, gemm64.pn_conv(sd, pre, f'conv{i}', got), where(68))
+            ratios.add('gemm', f'for conv{i}', nxt, gemm64.pn_conv(sd, pre, f'conv{i}', got), where(68))
             got = nxt
         res = run(12, 'residual')
-        assert _same_bits(res.view(b, 3, 68), gemm64.residual_from_rows(got)), 'point_residual'
+        assert same_bits(res.view(b, 3, 68), gemm64.residual_from_rows(got)), 'point_residual'
     assert eng.poll_error() == 0
 
 
@@ -248,10 +192,11 @@ def pointnet_ratios(model, sd, lmk, pool, params, worst):
 def test_pointnet_every_stage_matches_float64_oracle(pn_model, sd, pn_inputs, batch):
     gemm64.check_pointnet_batches()
     lmk, pool, attr = (t[:batch] for t in pn_inputs)
-    w = Worst()
-    pointnet_ratios(pn_model, sd, lmk, pool, attr, w)
-    w.report(f'pointnet B={batch}')
-    assert not w.over(), w.over()
+    ratios = Ratios()
+    pointnet_ratios(pn_model, sd, lmk, pool, attr, ratios)
+    report(f'pointnet B={batch}', ratios)
+    bad = over('gemm64', ratios)
+    assert not bad, bad
 
 
 def test_pointnet_rescaled_checkpoint(pn_model_wide, sd_wide, pn_inputs):
@@ -268,10 +213,11 @@ def test_pointnet_rescaled_checkpoint(pn_model_wide, sd_wide, pn_inputs):
     assert rp.max_rel_err(t['point_residual'].cpu().numpy(), gold['fwd_point_residual']) < HEAD_TOL
     assert rp.max_rel_err(t['_3D_attr_S2'].cpu().numpy(), gold['fwd_3D_attr_S2']) < HEAD_TOL
     lmk, pool, attr = (t[:37] for t in pn_inputs)
-    w = Worst()
-    pointnet_ratios(model, sd_wide, lmk, pool, attr, w)
-    w.report('pointnet rescaled B=37')
-    assert not w.over(), w.over()
+    ratios = Ratios()
+    pointnet_ratios(model, sd_wide, lmk, pool, attr, ratios)
+    report('pointnet rescaled B=37', ratios)
+    bad = over('gemm64', ratios)
+    assert not bad, bad
 
 
 # ---- tc_gemm_kernel alone ---------------------------------------------------------------------------------------------
@@ -313,12 +259,12 @@ def _kernel_case(eng, a, w, bias, act, rowmax_in=None, conv=None, residual=None,
     add = None if addend is None else addend.repeat_interleave(addend_group, dim=0)[:rows.shape[0]]
     want = gemm64.gemm(rows, w, bias, act == 2, addend=add, residual=residual)
     out_c = out.cpu()
-    _check_rowmax(out, rmo, name)
+    check_rowmax(out, rmo, name)
     if cm is not None:
         m = out_c.shape[0]
         pad_rows = -m % colmax_group
         full = torch.cat([out_c, torch.zeros((pad_rows, out_c.shape[1]))]).view(-1, colmax_group, out_c.shape[1])
-        assert _same_bits(full.amax(dim=1), cm.cpu().view(torch.float32)), f'colmax {name}'
+        assert same_bits(full.amax(dim=1), cm.cpu().view(torch.float32)), f'colmax {name}'
     return gemm64.worst(out_c, *want)
 
 
@@ -343,7 +289,7 @@ def test_gemm_kernel_shapes(eng, case):
     r, ix = _kernel_case(eng, a, w, bias, act, residual=res, addend=add, addend_group=ex.get('addend', 1),
                          colmax_group=ex.get('colmax', 0), name=name)
     print(f'\n[gemm {name}] worst {r:.3e} at {ix}')
-    assert r <= TAU['gemm'], (name, r, ix)
+    assert r <= BARS['gemm'], (name, r, ix)
 
 
 CONV_CASES = (   # (name, B, H, W, C, N, ksize, stride, pad, residual)
@@ -364,7 +310,7 @@ def test_gemm_kernel_conv_mode(eng, case):
     res = torch.randn((b * ho * wo, n), generator=torch.Generator().manual_seed(5)) if with_res else None
     r, ix = _kernel_case(eng, a, w, bias, 2, conv=(ks, st, pad, ho, wo), residual=res, name=name)
     print(f'\n[gemm conv {name}] worst {r:.3e} at {ix}')
-    assert r <= TAU['gemm'], (name, r, ix)
+    assert r <= BARS['gemm'], (name, r, ix)
 
 
 def test_gemm_kernel_row_magnitudes(eng):
@@ -381,7 +327,7 @@ def test_gemm_kernel_row_magnitudes(eng):
     w, _ = _layer(n, k, seed=9)
     r, ix = _kernel_case(eng, a, w, torch.zeros(n), 0, name='magnitudes')
     print(f'\n[gemm row magnitudes] worst {r:.3e} at {ix}')
-    assert r <= TAU['gemm'], (r, ix)
+    assert r <= BARS['gemm'], (r, ix)
 
 
 def test_wrong_row_scale_fails_the_bar(eng):
@@ -396,5 +342,5 @@ def test_wrong_row_scale_fails_the_bar(eng):
     r_lo, _ = _kernel_case(eng, a, w, bias, 0, rowmax_in=true_max / 8, name='rowmax / 8')
     r_hi, _ = _kernel_case(eng, a, w, bias, 0, rowmax_in=true_max * 2.0 ** 24, name='rowmax * 2^24')
     print(f'\n[negative control] true {r_ok:.3e}  rowmax/8 {r_lo:.3e}  rowmax*2^24 {r_hi:.3e}')
-    assert r_ok <= TAU['gemm']
-    assert r_lo >= 10 * TAU['gemm'] and r_hi >= 10 * TAU['gemm'], (r_lo, r_hi)
+    assert r_ok <= BARS['gemm']
+    assert r_lo >= 10 * BARS['gemm'] and r_hi >= 10 * BARS['gemm'], (r_lo, r_hi)

@@ -15,30 +15,16 @@ import torch.nn as nn
 
 from oracle import gemm64, mbv1_64, synth_mbv1
 from oracle import reference_port as rp
+from oracle.stage_check import (TAU, TOL, WIDE, Ratios, check_rowmax, face_picker, make_model, over, report, same_bits,
+                                seeded_crops)
 from synergynet_b200 import backbone, synthetic
-from test_gpu_gemm_layers import TAU as GEMM_TAU
 
 pytestmark = pytest.mark.gpu
 
 DEV = torch.device('cuda', 0)
 ARCHS = tuple(backbone.MBV1_WIDTHS)
-# The bar per stage kind.  'gemm' and 'pool' are those of tests/test_gpu_gemm_layers.py; 'dw' holds the fp32 CUDA-core
-# stages (stem, K = 27, and the depthwise convs, K = 9), at most 4x the worst ratio measured on an H100 80GB HBM3
-# (132 SMs, 700 W power limit) over the five widths, the batches and both checkpoints (worst in the comment):
-TAU = {'gemm': GEMM_TAU['gemm'], 'pool': GEMM_TAU['pool'],     # here: 1.96e-06 (mobilenet_2 dw6 conv_sep), 2.25e-07
-       'dw': 1.4e-6}        # 3.56e-07: the stem of mobilenet_1 at B = 33; the depthwise convs alone 2.25e-07
-# Negative controls (test_negative_controls_fail_the_bar): bf16 conv_sep weights measure 6.92e-04 (86x the gemm bar),
-# rowmax_in / 8 8.93e-02 (11161x).
-WIDE = dict(seed=11, lo=-6, hi=4)         # hidden-channel factors 2^-6 .. 2^4
-TOL = 1e-4
+BARS = TAU['mbv1_64']
 GOLD_FACES, GOLD_SEED = 4, 31             # tests/golden/make_golden_mbv1.py
-
-
-def _model(arch, sd):
-    from synergynet_b200 import model_building
-    m = model_building.SynergyNet(types.SimpleNamespace(arch=arch, img_size=120, devices_id=[0]))
-    m.load_state_dict({'I2P.backbone.' + k: v for k, v in sd.items()}, strict=False)
-    return m.eval()
 
 
 @pytest.fixture(scope='module')
@@ -49,50 +35,23 @@ def gold():
 
 @pytest.fixture(scope='module')
 def models(synth_pack):
-    return {a: _model(a, synth_mbv1.build_mobilenet_v1_state_dict(0, a)) for a in ARCHS}
+    return {a: make_model(synth_mbv1.build_mobilenet_v1_state_dict(0, a), a, strict=False) for a in ARCHS}
 
 
-def _crops(batch, seed):
-    return synthetic.normalize_crops(synthetic.make_structured_crops_u8(batch, seed=seed)).to(DEV)
-
-
-def _same_bits(a, b):
-    return torch.equal(a.float().contiguous().view(torch.int32), b.float().contiguous().view(torch.int32))
-
-
-class Worst:
-    def __init__(self):
-        self.by_kind = {}
-
-    def add(self, kind, stage, got, want_s, where_fn):
-        r, ix = gemm64.worst(got, *want_s)
-        if r >= self.by_kind.get(kind, (-1.0,))[0]:
-            self.by_kind[kind] = (r, stage, where_fn(ix))
-
-    def over(self):
-        return {k: v for k, v in self.by_kind.items() if v[0] > TAU[k]}
-
-    def report(self, tag):
-        print(f'\n[{tag}] ' + '  '.join(f'{k}: {r:.3e} at stage {s} {w}' for k, (r, s, w) in self.by_kind.items()))
-
-
-def mbv1_ratios(eng, sd, x, faces, worst):
+def mbv1_ratios(eng, sd, x, faces, ratios):
     """Run every stage on batch ``x`` and hold the given faces to the oracle; row maxima bit for bit."""
-    b, nf = x.shape[0], len(faces)
-    fidx = torch.tensor(faces, device=x.device)
-    pick = lambda t: t.view(b, -1, t.shape[1]).index_select(0, fidx).reshape(-1, t.shape[1]).cpu()
-    inp = x.index_select(0, fidx).cpu()
+    nf = len(faces)
+    pick, where = face_picker(x.shape[0], faces, x.device)
+    inp = x[faces].cpu()
     for s in range(mbv1_64.NUM_STAGES):
         out, rm = eng.debug_mobilenet_v1_until(x, s)
         if s in (0, 26, 27) or (s <= 26 and s % 2 == 1):
-            assert rm is not None and torch.equal(rm, gemm64.rowmax_bits(out)), f'rowmax of stage {s}'
+            check_rowmax(out, rm, f'stage {s}')
         else:
             assert rm is None
         got = pick(out)
         kind = 'dw' if s == 0 or (s <= 26 and s % 2 == 1) else 'pool' if s == 27 else 'gemm'
-        per_face = got.shape[0] // nf
-        worst.add(kind, s, got, mbv1_64.stage(sd, s, inp, nf),
-                  lambda ix, p=per_face: (faces[ix[0] // p], ix[0] % p, ix[1]))
+        ratios.add(kind, s, got, mbv1_64.stage(sd, s, inp, nf), where(got.shape[0] // nf))
         inp = got
     assert eng.poll_error() == 0
 
@@ -103,28 +62,30 @@ def test_every_stage_matches_float64_oracle(models, arch, batch):
     mbv1_64.check_mbv1_batches()
     sd = synth_mbv1.build_mobilenet_v1_state_dict(0, arch)
     eng = models[arch]._engine(DEV)
-    w = Worst()
-    mbv1_ratios(eng, sd, _crops(batch, 700 + batch), mbv1_64.faces(batch), w)
-    w.report(f'{arch} B={batch}')
-    assert not w.over(), w.over()
+    ratios = Ratios()
+    mbv1_ratios(eng, sd, seeded_crops(batch, 700 + batch), mbv1_64.faces(batch), ratios)
+    report(f'{arch} B={batch}', ratios)
+    bad = over('mbv1_64', ratios)
+    assert not bad, bad
 
 
 @pytest.mark.parametrize('arch', ARCHS)
 def test_rescaled_checkpoint(synth_pack, gold, arch):
     """Hidden channels spread over 2^10: the same function (out102 of the reference within TOL) and every stage under the
     same bar, with the GEMMs' row scales spread as widely."""
-    sd = synth_mbv1.reparametrize_mobilenet_v1(synth_mbv1.build_mobilenet_v1_state_dict(0, arch), **WIDE)
-    m = _model(arch, sd)
+    sd = synth_mbv1.reparametrize_mobilenet_v1(synth_mbv1.build_mobilenet_v1_state_dict(0, arch), **WIDE['mbv1_64'])
+    m = make_model(sd, arch, strict=False)
     eng = m._engine(DEV)
-    out, _ = eng.forward_mobilenet_v1(_crops(GOLD_FACES, GOLD_SEED))
+    out, _ = eng.forward_mobilenet_v1(seeded_crops(GOLD_FACES, GOLD_SEED))
     err = rp.max_rel_err(out.cpu().numpy(), gold[f'{arch}_out102'])
     print(f'\n[{arch} rescaled] out102 err {err:.3e}')
     assert err < TOL
     batch = 33
-    w = Worst()
-    mbv1_ratios(eng, sd, _crops(batch, 700 + batch), mbv1_64.faces(batch), w)
-    w.report(f'{arch} rescaled B={batch}')
-    assert not w.over(), w.over()
+    ratios = Ratios()
+    mbv1_ratios(eng, sd, seeded_crops(batch, 700 + batch), mbv1_64.faces(batch), ratios)
+    report(f'{arch} rescaled B={batch}', ratios)
+    bad = over('mbv1_64', ratios)
+    assert not bad, bad
 
 
 def test_negative_controls_fail_the_bar(models):
@@ -134,7 +95,7 @@ def test_negative_controls_fail_the_bar(models):
     arch, batch, idx = 'mobilenet_1', 2, 14
     sd = synth_mbv1.build_mobilenet_v1_state_dict(0, arch)
     eng = models[arch]._engine(DEV)
-    x = _crops(batch, 5)
+    x = seeded_crops(batch, 5)
     a, rm = eng.debug_mobilenet_v1_until(x, idx - 1)
     w4, b = mbv1_64.fold(sd, idx)
     w = w4.reshape(w4.shape[0], -1).float()
@@ -143,10 +104,10 @@ def test_negative_controls_fail_the_bar(models):
     r_ok = ratio(w, rm)
     r_bf16 = ratio(w.bfloat16().float(), rm)
     r_div8 = ratio(w, (rm.view(torch.float32) / 8).view(torch.int32))
-    print(f'\n[negative controls] true {r_ok:.3e}  bf16 weights {r_bf16:.3e} ({r_bf16 / TAU["gemm"]:.0f}x the bar)  '
-          f'rowmax/8 {r_div8:.3e} ({r_div8 / TAU["gemm"]:.0f}x the bar)')
-    assert r_ok <= TAU['gemm']
-    assert r_bf16 >= 10 * TAU['gemm'] and r_div8 >= 10 * TAU['gemm'], (r_bf16, r_div8)
+    print(f'\n[negative controls] true {r_ok:.3e}  bf16 weights {r_bf16:.3e} ({r_bf16 / BARS["gemm"]:.0f}x the bar)  '
+          f'rowmax/8 {r_div8:.3e} ({r_div8 / BARS["gemm"]:.0f}x the bar)')
+    assert r_ok <= BARS['gemm']
+    assert r_bf16 >= 10 * BARS['gemm'] and r_div8 >= 10 * BARS['gemm'], (r_bf16, r_div8)
 
 
 @pytest.mark.parametrize('arch', ARCHS)
@@ -163,11 +124,11 @@ def test_end_to_end_matches_reference(models, gold, arch):
     assert e_out < TOL and e_lmk < TOL
     assert pool.shape == (GOLD_FACES, int(1024 * backbone.MBV1_WIDTHS[arch]))
     out_u8, pool_u8 = eng.forward_mobilenet_v1(u8)                     # (v - 127.5) / 128 in the stem: the same bits
-    assert _same_bits(out_u8, out) and _same_bits(pool_u8, pool)
+    assert same_bits(out_u8, out) and same_bits(pool_u8, pool)
     again, _ = eng.forward_mobilenet_v1(x)
-    assert _same_bits(again, out)
+    assert same_bits(again, out)
     params = m.forward_test(x)
-    assert _same_bits(params, out[:, :62])
+    assert same_bits(params, out[:, :62])
     assert eng.poll_error() == 0
 
 
@@ -181,7 +142,7 @@ def test_ragged_batches_are_bit_identical_per_face(models, arch):
     for b in (1, 2, 7, 129):
         for f0 in (0, big - b):
             o, p = eng.forward_mobilenet_v1(x[f0:f0 + b])
-            assert _same_bits(o, full[f0:f0 + b]) and _same_bits(p, pool[f0:f0 + b]), (b, f0)
+            assert same_bits(o, full[f0:f0 + b]) and same_bits(p, pool[f0:f0 + b]), (b, f0)
     assert eng.poll_error() == 0
 
 
@@ -202,7 +163,7 @@ def test_reference_caller_sequences(synth_pack, gold):
     params = dp.module.forward_test(x.to(DEV))
     assert rp.max_rel_err(params.cpu().numpy(), gold[f'{arch}_out102'][:, :62]) < TOL
     p_cpu = model.forward_test(x)                                          # CPU tensor in, CPU tensor out
-    assert not p_cpu.is_cuda and _same_bits(p_cpu, params.cpu())
+    assert not p_cpu.is_cuda and same_bits(p_cpu, params.cpu())
     lmk = model.reconstruct_vertex_62(params)
     assert rp.max_rel_err(lmk.cpu().numpy(), gold[f'{arch}_lmk']) < TOL
     # a new checkpoint in the same model rebuilds the engine; the old one back gives the old bits
@@ -210,9 +171,9 @@ def test_reference_caller_sequences(synth_pack, gold):
     model.load_state_dict({'I2P.backbone.' + k: v for k, v in sd1.items()}, strict=False)
     p1 = model.forward_test(x.to(DEV))
     want1, _ = mbv1_64.forward64(sd1, x)
-    assert rp.max_rel_err(p1.cpu().numpy(), want1[:, :62].numpy()) < TOL and not _same_bits(p1, params)
+    assert rp.max_rel_err(p1.cpu().numpy(), want1[:, :62].numpy()) < TOL and not same_bits(p1, params)
     model.load_state_dict({'I2P.backbone.' + k: v for k, v in sd0.items()}, strict=False)
-    assert _same_bits(model.forward_test(x.to(DEV)), params)
+    assert same_bits(model.forward_test(x.to(DEV)), params)
     with pytest.raises(RuntimeError, match='1280-d image feature'):
         model(x.to(DEV), params)
     # get_all_outputs: this backbone on the device-made uint8 crops, then the image-space stages
@@ -238,22 +199,19 @@ def test_mobilenet_v2_unchanged_by_a_mobilenet_v1_model(synth_pack):
     """A mobilenet_v2 model's landmarks on the same device are bit-identical before and after a MobileNetV1 model is
     created and run in the same process."""
     from oracle import synth_model
-    from synergynet_b200 import model_building
-    m2 = model_building.SynergyNet(types.SimpleNamespace(arch='mobilenet_v2', img_size=120, devices_id=[0]))
-    m2.load_state_dict(synth_model.build_state_dict(0), strict=True)
-    m2.eval()
-    x = _crops(9, 3)
+    m2 = make_model(synth_model.build_state_dict(0))
+    x = seeded_crops(9, 3)
     before = m2.forward_landmarks(x).clone()
-    m1 = _model('mobilenet_2', synth_mbv1.build_mobilenet_v1_state_dict(0, 'mobilenet_2'))
-    m1.forward_landmarks(_crops(130, 4))
+    m1 = make_model(synth_mbv1.build_mobilenet_v1_state_dict(0, 'mobilenet_2'), 'mobilenet_2', strict=False)
+    m1.forward_landmarks(seeded_crops(130, 4))
     torch.cuda.synchronize()
-    assert _same_bits(m2.forward_landmarks(x), before)
+    assert same_bits(m2.forward_landmarks(x), before)
 
 
 def test_timing_names(models):
     eng = models['mobilenet_05']._engine(DEV)
     eng.set_timing(True)
-    eng.forward_mobilenet_v1(_crops(3, 2))
+    eng.forward_mobilenet_v1(seeded_crops(3, 2))
     names = [n for n, _ in eng.timings()]
     eng.set_timing(False)
     assert names == (['mbv1_stem_kernel'] + ['mbv1_dw3x3', 'mbv1_conv_sep'] * 12 + ['mbv1_dw3x3', 'mbv1_conv_sep_last',

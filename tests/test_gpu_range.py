@@ -25,8 +25,8 @@ import pytest
 import torch
 
 from oracle import block64, stage_check, synth_model, tile_cover
-from oracle.stage_check import make_model, report, stage_ratios, tau
-from synergynet_b200 import _lib, synthetic
+from oracle.stage_check import make_model, report, seeded_crops, stage_ratios, tau
+from synergynet_b200 import _lib
 
 pytestmark = pytest.mark.gpu
 
@@ -51,8 +51,7 @@ def batch():
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     b = tile_cover.choose_batches(sms)['odd_pairs']
     tile_cover.check_plan('odd_pairs', b, sms)
-    x = synthetic.normalize_crops(synthetic.make_structured_crops_u8(b, seed=900 + b)).cuda()
-    return x, tile_cover.faces_to_check(b, sms, seed=b)
+    return seeded_crops(b, 900 + b), tile_cover.faces_to_check(b, sms, seed=b)
 
 
 def _engine(model, kind):
@@ -184,7 +183,7 @@ def test_just_outside_the_range(synth_pack, sd, peaks, batch, stream):
 
 
 def _crops():
-    return synthetic.normalize_crops(synthetic.make_structured_crops_u8(CROP_BATCH, seed=77)).cuda()
+    return seeded_crops(CROP_BATCH, 77)
 
 
 def _with_pixel(x, pixel, value):

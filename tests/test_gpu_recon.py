@@ -11,103 +11,33 @@ import pytest
 import torch
 
 from oracle import recon64, synth_model
+from oracle.recon64 import magnitude_params, random_params, roi_rows
+from oracle.stage_check import TAU, WIDE, Ratios, report as print_report
 from synergynet_b200 import _lib, synthetic
 
 pytestmark = pytest.mark.gpu
 
-# The bar: |got - want| <= TAU * S at every element, at most 4x the worst ratio measured on an H100 80GB HBM3 (132 SMs,
-# 400 W power limit) over this file (worst in the comment):
-TAU = {'tc': 2.5e-6,        # 8.83e-07: tensor-core path, dense, a face 1.5x beyond the fp16 clamp (face scale 2)
-       'fp32': 2e-6}        # 7.18e-07: reconstruct_kernel (engine 0), dense, the same magnitude set
-# In range the tensor-core path measures 5.3e-7 (coefficients just below the clamp) and 2.5e-7 for random faces.
-# Negative control (tests/test_recon_oracle.py, numpy emulation): one of the three passes dropped measures >= 3.7e-5,
-# coefficients clamped at 60000 instead of face-scaled 0.998: >= 15x the bar.
-WIDE = dict(seed=5, lo=-8, hi=8)          # coefficient scales 2^-8 .. 2^8
-RESNET_SCALED = 23010.0                   # |alpha * ascale| the random ResNet-50 checkpoint reaches
 PATH = {_lib.ENGINE_SIMT_FP32: 'fp32', _lib.ENGINE_TC_FUSED: 'tc'}
-
-_worst = {}
+RATIOS = Ratios()
 
 
 def check(tag, path, got, want_s):
     got = got.cpu().numpy() if isinstance(got, torch.Tensor) else got
-    r, ix = recon64.worst(got, *want_s)
-    if r >= _worst.get((path, tag), (-1.0,))[0]:
-        _worst[(path, tag)] = (r, ix)
-    assert r <= TAU[path], f'{tag} ({path}): |got - want| / S = {r:.3e} at {ix}'
+    r, ix = RATIOS.add(path, f'{path} {tag}', got, want_s)
+    assert r <= TAU['recon64'][path], f'{tag} ({path}): |got - want| / S = {r:.3e} at {ix}'
 
 
 @pytest.fixture(scope='module', autouse=True)
 def report():
     yield
-    for (path, tag), (r, ix) in sorted(_worst.items()):
-        print(f'worst {path:4s} {tag:34s} {r:.3e} at {ix}')
+    print_report('reconstruction', RATIOS)
 
 
 # ---- inputs ---------------------------------------------------------------------------------------------------------
 
-def random_params(b, seed, spread=1.0):
-    """Whitened parameters: distinct faces within a few sigma."""
-    return (np.random.default_rng(seed).standard_normal((b, 62)) * spread).astype(np.float32)
-
-
-def roi_rows(b, seed):
-    rng = np.random.default_rng(seed)
-    k = rng.uniform(0.3, 4.0, (b, 3))
-    s = rng.uniform(-50.0, 800.0, (b, 2))
-    return np.stack([k[:, 0], s[:, 0], k[:, 1], s[:, 1], k[:, 2]], 1).astype(np.float32)
-
-
 def raw(params, pack):
     """The de-whitened fp32 parameters (to call with whitening off)."""
     return (params * pack['param_std'][:62] + pack['param_mean'][:62]).astype(np.float32)
-
-
-def whiten(p_raw, pack):
-    mean, std = pack['param_mean'][:62].astype(np.float64), pack['param_std'][:62].astype(np.float64)
-    return ((p_raw - mean) / np.where(std == 0, 1.0, std)).astype(np.float32)
-
-
-def magnitude_params(pack, beyond):
-    """(params, whitening) with coefficients at the magnitudes the alpha scale has to cover.  ``beyond`` = False: the
-    mean, +-8 sigma, the ResNet-50 magnitude, just below the fp16 clamp 60000 / ascale_k, and translations that put the
-    vertices around y = 121 (the flip cancels).  ``beyond`` = True: just above the clamp, one coefficient far above it
-    next to tiny ones, and raw coefficients (whitening off) far beyond it, including the coefficient of the stress
-    model whose mean and std are 0."""
-    mean, std = pack['param_mean'][:62].astype(np.float64), pack['param_std'][:62].astype(np.float64)
-    lim = recon64.CLAMP / recon64.ascale(mean, std)                     # |alpha_k| at the clamp
-    sign = np.where(np.arange(50) % 2, -1.0, 1.0)
-    base = random_params(8, 91, 0.5).astype(np.float64)
-    rows = []
-
-    def face(alpha, i):
-        p = base[i % 8].copy() * std + mean
-        p[12:62] = alpha
-        return p
-
-    if not beyond:
-        rows += [face(mean[12:62], 0), face(mean[12:62] + 8 * std[12:62], 1), face(mean[12:62] - 8 * std[12:62], 2)]
-        rows += [face(sign * RESNET_SCALED / recon64.ascale(mean, std), 3), face(0.999 * sign * lim, 4),
-                 face(-0.999 * sign * lim, 5)]
-        for i in range(4):
-            p = face(mean[12:62] + 2 * std[12:62] * np.random.default_rng(i).standard_normal(50), 6 + i)
-            p[7] = 121.0 + 8.0 * i                                      # t_y: vy = 121 within the face
-            rows.append(p)
-        return whiten(np.stack(rows), pack), True
-    rows += [face(1.001 * sign * lim, 0), face(-1.5 * sign * lim, 1)]
-    p = face(mean[12:62] + 1e-3 * std[12:62], 2)
-    p[12] = 4.0 * lim[0]                                                # huge next to tiny
-    rows.append(p)
-    p = face(mean[12:62] + 1e-6 * std[12:62], 3)
-    p[12 + 40] = -1e3 * lim[40]
-    rows.append(p)
-    rows += [face(3.0 * sign * lim, 4), face(-40.0 * lim, 5)]
-    k = synth_model.STRESS_ZERO_COEF
-    for i, a in enumerate((100.0, -1000.0, 58.0, 1e5)):
-        p = face(mean[12:62], 6 + i)
-        p[12 + k] = a                                                   # ascale 2^10 when mean = std = 0
-        rows.append(p)
-    return np.stack(rows).astype(np.float32), False
 
 
 # ---- fixtures -------------------------------------------------------------------------------------------------------
@@ -320,7 +250,7 @@ def _magnitude_case(eng, pack, beyond, engine, tag):
 @pytest.fixture(scope='module')
 def packs(base3dmm, prod):
     return {'synthetic': prod,
-            'wide': synth_model.recon_pack(synth_model.reparametrize_3dmm(base3dmm, **WIDE)),
+            'wide': synth_model.recon_pack(synth_model.reparametrize_3dmm(base3dmm, **WIDE['recon64'])),
             'stress': synth_model.recon_pack(synth_model.stress_3dmm(base3dmm))}
 
 

@@ -6,8 +6,9 @@ import pytest
 
 from oracle import recon64, synth_model
 from oracle import reference_port as rp
+from oracle.recon64 import magnitude_params, random_params, roi_rows
+from oracle.stage_check import TAU, WIDE
 from synergynet_b200 import synthetic
-from test_gpu_recon import TAU, WIDE, magnitude_params, random_params, roi_rows
 
 NOISE = 4e-6               # the fp32 reference (numpy sgemm, K = 50) against the float64 oracle, in units of S
 F32, F16 = np.float32, np.float16
@@ -21,7 +22,7 @@ def base3dmm():
 @pytest.fixture(scope='module')
 def packs(base3dmm):
     return {'synthetic': synth_model.recon_pack(base3dmm),
-            'wide': synth_model.recon_pack(synth_model.reparametrize_3dmm(base3dmm, **WIDE)),
+            'wide': synth_model.recon_pack(synth_model.reparametrize_3dmm(base3dmm, **WIDE['recon64'])),
             'stress': synth_model.recon_pack(synth_model.stress_3dmm(base3dmm))}
 
 
@@ -44,12 +45,12 @@ def test_oracle_agrees_with_fp32_reference(packs, model):
 
 
 def test_reparametrized_model_is_bit_identical(base3dmm):
-    wide = synth_model.reparametrize_3dmm(base3dmm, **WIDE)
+    wide = synth_model.reparametrize_3dmm(base3dmm, **WIDE['recon64'])
     a, b = synth_model.recon_pack(base3dmm), synth_model.recon_pack(wide)
     assert not np.array_equal(recon64.ascale(a['param_mean'], a['param_std']),
                               recon64.ascale(b['param_mean'], b['param_std']))
     e = np.log2(recon64.ascale(b['param_mean'], b['param_std']) / recon64.ascale(a['param_mean'], a['param_std']))
-    assert e.min() == WIDE['lo'] and e.max() == WIDE['hi']
+    assert e.min() == WIDE['recon64']['lo'] and e.max() == WIDE['recon64']['hi']
     p = random_params(8, 4, 2.0)
     for dense in (False, True):
         assert np.array_equal(rp.reconstruct_vertex_62(p, a, True, dense), rp.reconstruct_vertex_62(p, b, True, dense))
@@ -142,10 +143,10 @@ def test_emulated_kernel_passes_and_broken_ones_fail(packs, model):
             roi = roi_rows(len(params), 1) if whitening else None
             want = recon64.reconstruct(params, pack, dense, whitening, roi5=roi)
             r, ix = recon64.worst(emulate_tc(params, pack, dense, whitening, roi5=roi), *want)
-            assert r < TAU['tc'], (model, dense, r, ix)
+            assert r < TAU['recon64']['tc'], (model, dense, r, ix)
             for drop in ('hh', 'hl', 'lh'):
                 bad, _ = recon64.worst(emulate_tc(params, pack, dense, whitening, roi5=roi, drop=drop), *want)
-                assert bad > 10 * TAU['tc'], (model, dense, drop, bad)
+                assert bad > 10 * TAU['recon64']['tc'], (model, dense, drop, bad)
             if np.any(recon64.face_scales(params, pack['param_mean'], pack['param_std'], whitening) > 1):
                 bad, _ = recon64.worst(emulate_tc(params, pack, dense, whitening, roi5=roi, clamp=True), *want)
-                assert bad > 10 * TAU['tc'], (model, dense, 'clamp', bad)
+                assert bad > 10 * TAU['recon64']['tc'], (model, dense, 'clamp', bad)
