@@ -195,6 +195,24 @@ int syn_resnet_set_heads(syn_handle_t* h, const float* w102x2048_host, const flo
 int syn_resnet_commit(syn_handle_t* h);                      /* after syn_commit */
 int syn_resnet50_forward(syn_handle_t* h, const float* x_dev, int batch, float* out102_dev, float* pool2048_dev,
                          void* stream);
+/* The other ResNet factories the reference's I2P builds (model_building.py:44-45; resnet_backbone.py:282-391), named by
+ * (depth, width_per_group): resnet18 (18, 64), resnet34 (34, 64), resnet50 (50, 64), resnet101 (101, 64), resnet152
+ * (152, 64), wide_resnet50_2 (50, 128), wide_resnet101_2 (101, 128).  18 / 34 use BasicBlock (:50-88: conv1 3x3 carries
+ * the stride, conv2 3x3 adds the shortcut), the others Bottleneck (:90-136, width = planes * width_per_group / 64).
+ * Convolutions in state-dict order: 0 = conv1 (7x7/s2); then per block conv1, conv2 (, conv3) and, where the block has
+ * one (stride != 1 or inplanes != planes * expansion, :210-214), downsample.0.  `residual` marks the conv that adds the
+ * shortcut.  Anything but the seven pairs is SYN_ERR_INVALID; syn_resnet_arch_num_convs then returns -1.
+ * syn_resnet_select picks the arch of the handle and forgets the ResNet weights set so far; a handle that never calls it
+ * holds resnet50.  syn_resnet_set_conv / _set_heads / _commit act on the selected arch; the heads are (102, 512) for
+ * 18 / 34 and (102, 2048) otherwise.  syn_resnet50_forward refuses any other committed arch.
+ * syn_resnet_forward: x_dev (B,3,120,120) NCHW fp32 crops, or raw uint8 crops when x_is_u8 (normalised in the stem as
+ * (v - 127.5) / 128, with the syn_set_center_crop frame), -> out102_dev (B,102) = what ResNet._forward_impl returns;
+ * pool_dev (B,512 or 2048) = the flattened avgpool, may be NULL. */
+int syn_resnet_arch_num_convs(int depth, int width_per_group);
+int syn_resnet_arch_conv_desc(int depth, int width_per_group, int idx, syn_conv_desc_t* out);
+int syn_resnet_select(syn_handle_t* h, int depth, int width_per_group);
+int syn_resnet_forward(syn_handle_t* h, const void* x_dev, int x_is_u8, int batch, float* out102_dev, float* pool_dev,
+                       void* stream);
 
 /* ---- MobileNetV1 backbones (backbone_nets/mobilenetv1_backbone.py:21-140, prelu=False) ------------------------------
  * Five widths, named by widen_code = 100 x the widen factor: SYN_MBV1_2 (200, mobilenet_2), SYN_MBV1_1 (100),
@@ -377,7 +395,9 @@ int syn_debug_forward_until(syn_handle_t* h, const float* x_dev, int batch, int 
  * GEMM scales its rows by) to rowmax_dev (nullable; left untouched for a stage that records none).
  * ResNet-50 (NHWC rows, one per pixel): 0 stem (B*3600 x 64), 1 max-pool (B*900 x 64), 1 + i conv i of
  * syn_resnet_conv_desc (i = 1..52; a block's downsample runs before its conv3 and records no row maxima), 54 avgpool
- * (B x 2048), 55 heads (B x 102, no row maxima). */
+ * (B x 2048), 55 heads (B x 102, no row maxima).  For the selected arch with n convs (syn_resnet_arch_num_convs):
+ * 1 + i conv i of syn_resnet_arch_conv_desc (i = 1..n-1; a downsample runs before the conv that adds it), n + 1 avgpool
+ * (B x 512 or 2048), n + 2 heads.  x_dev: fp32 crops. */
 int syn_debug_resnet_until(syn_handle_t* h, const float* x_dev, int batch, int stage, float* out_dev, unsigned* rowmax_dev,
                            void* stream);
 /* MobileNetV1 (NHWC rows, one per pixel; C_i = cout of conv i of syn_mbv1_conv_desc): 0 stem (B*3600 x C_0),

@@ -56,6 +56,12 @@ def main():
                        strict=False)
     v1.eval()
     v1._engine(dev).forward_mobilenet_v1(u8[:2].cuda())                # uint8 stem, every depthwise band plan
+    from oracle import synth_resnet
+    r18 = model_building.SynergyNet(types.SimpleNamespace(arch='resnet18', img_size=120, devices_id=[0]))
+    r18.load_state_dict({'I2P.backbone.' + k: v for k, v in synth_resnet.build_resnet_state_dict(0, 'resnet18').items()},
+                        strict=False)
+    r18.eval()
+    r18._engine(dev).forward_resnet(u8[:2].cuda())                     # uint8 ResNet stem, BasicBlocks, plan-sized workspace
     torch.cuda.synchronize()
     eng.raise_if_error()
     print('sanitizer smoke done:', float(dense.abs().max()), {k: float(v.mean()) for k, v in loss.items()})

@@ -85,6 +85,10 @@ SIGNATURES = {
     'syn_resnet_commit': (_I, [_P]),
     'syn_resnet50_forward': (_I, [_P, _F, _I, _F, _F, _P]),
     'syn_debug_resnet_until': (_I, [_P, _F, _I, _I, _F, _P, _P]),
+    'syn_resnet_arch_num_convs': (_I, [_I, _I]),
+    'syn_resnet_arch_conv_desc': (_I, [_I, _I, _I, C.POINTER(ConvDesc)]),
+    'syn_resnet_select': (_I, [_P, _I, _I]),
+    'syn_resnet_forward': (_I, [_P, _F, _I, _I, _F, _F, _P]),
     'syn_mbv1_num_convs': (_I, []),
     'syn_mbv1_conv_desc': (_I, [_I, _I, C.POINTER(ConvDesc)]),
     'syn_mbv1_set_widen': (_I, [_P, _I]),
@@ -130,6 +134,7 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_pointnet_commit', 'syn_mlp_for', 'syn_mlp_rev', 'syn_wing_loss',
                                              'syn_param_loss', 'syn_reconstruct_image', 'syn_pose_decode', 'syn_set_center_crop', 'syn_resnet_num_convs', 'syn_resnet_conv_desc',
                                              'syn_resnet_set_conv', 'syn_resnet_set_heads', 'syn_resnet_commit', 'syn_resnet50_forward', 'syn_debug_resnet_until',
+                                             'syn_resnet_arch_num_convs', 'syn_resnet_arch_conv_desc', 'syn_resnet_select', 'syn_resnet_forward',
                                              'syn_mbv1_num_convs', 'syn_mbv1_conv_desc', 'syn_mbv1_set_widen', 'syn_mbv1_set_conv',
                                              'syn_mbv1_set_heads', 'syn_mbv1_commit', 'syn_mbv1_forward', 'syn_debug_mbv1_until',
                                              'syn_debug_pointnet_until', 'syn_debug_gemm',

@@ -194,46 +194,75 @@ class MLP_rev(_PointMLPParams):
         return out if x.is_cuda else out.to(x.device)
 
 
-# ---- ResNet-50 backbone variant (reference backbone_nets/resnet_backbone.py:120-249; BASELINE.json configs[4]) -------
+# ---- ResNet backbones (reference backbone_nets/resnet_backbone.py:50-391; BASELINE.json configs[4] is resnet50) ----------
+
+# The seven factories the reference's I2P can build (model_building.py:44-45): name -> (depth, width_per_group)
+RESNET_ARCHS = {'resnet18': (18, 64), 'resnet34': (34, 64), 'resnet50': (50, 64), 'resnet101': (101, 64),
+                'resnet152': (152, 64), 'wide_resnet50_2': (50, 128), 'wide_resnet101_2': (101, 128)}
+RESNET_LAYERS = {18: (2, 2, 2, 2), 34: (3, 4, 6, 3), 50: (3, 4, 6, 3), 101: (3, 4, 23, 3), 152: (3, 8, 36, 3)}
+
+
+class _BasicBlock(nn.Module):
+    """Keys of ``BasicBlock`` (conv1/bn1 3x3 with the stride, conv2/bn2 3x3, downsample; :50-88)."""
+    expansion = 1
+
+    def __init__(self, inplanes, planes, stride=1, downsample=None, width_per_group=64):
+        super().__init__()
+        self.conv1 = nn.Conv2d(inplanes, planes, 3, stride, 1, bias=False)
+        self.bn1 = nn.BatchNorm2d(planes)
+        self.conv2 = nn.Conv2d(planes, planes, 3, 1, 1, bias=False)
+        self.bn2 = nn.BatchNorm2d(planes)
+        self.downsample = downsample
+
 
 class _Bottleneck(nn.Module):
+    """Keys of ``Bottleneck`` (conv1 1x1, conv2 3x3 with the stride, conv3 1x1, downsample; :90-136)."""
     expansion = 4
 
-    def __init__(self, inplanes, planes, stride=1, downsample=None):
+    def __init__(self, inplanes, planes, stride=1, downsample=None, width_per_group=64):
         super().__init__()
-        self.conv1 = nn.Conv2d(inplanes, planes, 1, bias=False)
-        self.bn1 = nn.BatchNorm2d(planes)
-        self.conv2 = nn.Conv2d(planes, planes, 3, stride, 1, bias=False)
-        self.bn2 = nn.BatchNorm2d(planes)
-        self.conv3 = nn.Conv2d(planes, planes * 4, 1, bias=False)
+        width = planes * width_per_group // 64                              # :104
+        self.conv1 = nn.Conv2d(inplanes, width, 1, bias=False)
+        self.bn1 = nn.BatchNorm2d(width)
+        self.conv2 = nn.Conv2d(width, width, 3, stride, 1, bias=False)
+        self.bn2 = nn.BatchNorm2d(width)
+        self.conv3 = nn.Conv2d(width, planes * 4, 1, bias=False)
         self.bn3 = nn.BatchNorm2d(planes * 4)
         self.downsample = downsample
 
 
-class ResNet50Params(nn.Module):
-    """Key schema of ``resnet_backbone.resnet50()`` (conv1/bn1, layer1..4.{i}.conv{1,2,3}/bn{1,2,3}/downsample.{0,1},
-    fc_tex/fc_ori/fc_shape/fc_exp); parameter container, the forward pass runs in the sm_90a library."""
-    feature_dim = 2048
+class ResNetParams(nn.Module):
+    """Key schema of ``resnet_backbone.ResNet`` for one of the seven factories of RESNET_ARCHS (conv1/bn1,
+    layer1..4.{i}.conv{1,2[,3]}/bn{1,2[,3]}[/downsample.{0,1}], fc_tex/fc_ori/fc_shape/fc_exp); parameter container, the
+    forward pass runs in the sm_90a library."""
 
-    def __init__(self):
+    def __init__(self, depth: int = 50, width_per_group: int = 64):
         super().__init__()
+        if depth not in RESNET_LAYERS or width_per_group not in (64, 128) or (width_per_group == 128 and depth not in (50, 101)):
+            raise RuntimeError(f'no ResNet ({depth}, {width_per_group}); the sm_90a library builds '
+                               + ', '.join(f'{a} {v}' for a, v in RESNET_ARCHS.items()))
+        self.depth, self.width_per_group = depth, width_per_group
+        block = _BasicBlock if depth < 50 else _Bottleneck
         self.conv1 = nn.Conv2d(3, 64, 7, 2, 3, bias=False)
         self.bn1 = nn.BatchNorm2d(64)
         inplanes = 64
-        for li, (planes, blocks, stride) in enumerate(((64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2)), 1):
+        for li, (planes, blocks, stride) in enumerate(zip((64, 128, 256, 512), RESNET_LAYERS[depth], (1, 2, 2, 2)), 1):
             layers = []
-            for j in range(blocks):
+            for j in range(blocks):                                         # :203-225
+                st = stride if j == 0 else 1
                 ds = None
-                if j == 0:
-                    ds = nn.Sequential(nn.Conv2d(inplanes, planes * 4, 1, stride, bias=False), nn.BatchNorm2d(planes * 4))
-                layers.append(_Bottleneck(inplanes, planes, stride if j == 0 else 1, ds))
-                inplanes = planes * 4
+                if st != 1 or inplanes != planes * block.expansion:
+                    ds = nn.Sequential(nn.Conv2d(inplanes, planes * block.expansion, 1, st, bias=False),
+                                       nn.BatchNorm2d(planes * block.expansion))
+                layers.append(block(inplanes, planes, st, ds, width_per_group))
+                inplanes = planes * block.expansion
             setattr(self, f'layer{li}', nn.Sequential(*layers))
-        self.fc_tex = nn.Linear(2048, 40)
-        self.fc_ori = nn.Linear(2048, 12)
-        self.fc_shape = nn.Linear(2048, 40)
-        self.fc_exp = nn.Linear(2048, 10)
-        for m in self.modules():                                            # resnet_backbone.py:184-189
+        self.feature_dim = 512 * block.expansion
+        self.fc_tex = nn.Linear(self.feature_dim, 40)
+        self.fc_ori = nn.Linear(self.feature_dim, 12)
+        self.fc_shape = nn.Linear(self.feature_dim, 40)
+        self.fc_exp = nn.Linear(self.feature_dim, 10)
+        for m in self.modules():                                            # resnet_backbone.py:186-191
             if isinstance(m, nn.Conv2d):
                 nn.init.kaiming_normal_(m.weight, mode='fan_out', nonlinearity='relu')
             elif isinstance(m, nn.BatchNorm2d):
@@ -241,23 +270,63 @@ class ResNet50Params(nn.Module):
                 nn.init.constant_(m.bias, 0)
 
     def forward(self, *a, **k):  # pragma: no cover
-        raise RuntimeError('ResNet50Params is a parameter container; the forward pass runs in the sm_90a library')
+        raise RuntimeError(f'{type(self).__name__} is a parameter container; the forward pass runs in the sm_90a library')
 
 
-def resnet50_conv_keys():
-    """(conv key, bn key) of the 53 convolutions in the execution order of the C ABI (syn_resnet_set_conv)."""
+class ResNet50Params(ResNetParams):
+    """Key schema of ``resnet_backbone.resnet50()``."""
+    feature_dim = 2048
+
+    def __init__(self):
+        super().__init__(50, 64)
+
+
+def resnet_conv_keys(arch: str = 'resnet50'):
+    """(conv key, bn key) of the convolutions of ``arch`` in the state-dict order of the C ABI (syn_resnet_set_conv):
+    conv1, then per block conv1, conv2 (, conv3) and its downsample if it has one."""
+    depth, _ = RESNET_ARCHS[arch]
+    names = ('1', '2') if depth < 50 else ('1', '2', '3')
     keys = [('conv1', 'bn1')]
-    for li, blocks in enumerate((3, 4, 6, 3), 1):
+    for li, blocks in enumerate(RESNET_LAYERS[depth], 1):
         for j in range(blocks):
             pre = f'layer{li}.{j}'
-            keys += [(f'{pre}.conv1', f'{pre}.bn1'), (f'{pre}.conv2', f'{pre}.bn2'), (f'{pre}.conv3', f'{pre}.bn3')]
-            if j == 0:
+            keys += [(f'{pre}.conv{c}', f'{pre}.bn{c}') for c in names]
+            if j == 0 and (li > 1 or depth >= 50):                          # stride 2, or 64 -> 256 channels in layer1
                 keys.append((f'{pre}.downsample.0', f'{pre}.downsample.1'))
     return keys
 
 
+def resnet50_conv_keys():
+    """(conv key, bn key) of the 53 convolutions in the execution order of the C ABI (syn_resnet_set_conv)."""
+    return resnet_conv_keys('resnet50')
+
+
+def resnet18(pretrained: bool = False, **_):
+    return ResNetParams(18, 64)
+
+
+def resnet34(pretrained: bool = False, **_):
+    return ResNetParams(34, 64)
+
+
 def resnet50(pretrained: bool = False, **_):
     return ResNet50Params()
+
+
+def resnet101(pretrained: bool = False, **_):
+    return ResNetParams(101, 64)
+
+
+def resnet152(pretrained: bool = False, **_):
+    return ResNetParams(152, 64)
+
+
+def wide_resnet50_2(pretrained: bool = False, **_):
+    return ResNetParams(50, 128)
+
+
+def wide_resnet101_2(pretrained: bool = False, **_):
+    return ResNetParams(101, 128)
 
 
 # ---- MobileNetV1 backbones (reference backbone_nets/mobilenetv1_backbone.py:21-140, prelu=False) ---------------------------

@@ -1,6 +1,6 @@
-// CUDA-core pieces of the ResNet-50 backbone variant (reference backbone_nets/resnet_backbone.py:227-249; BASELINE.json
-// configs[4]): the 7x7/s2 stem convolution (K = 147 is too thin for an MMA tile), the 3x3/s2 max-pool and the global
-// average pool.  All 52 other convolutions and the four Linear heads run on tc_gemm_kernel (kernels_gemm.cuh).
+// CUDA-core pieces of the ResNet backbones (reference backbone_nets/resnet_backbone.py:227-249; BASELINE.json configs[4]
+// is resnet50): the 7x7/s2 stem convolution (K = 147 is too thin for an MMA tile), the 3x3/s2 max-pool and the global
+// average pool.  Every other convolution and the four Linear heads run on tc_gemm_kernel (kernels_gemm.cuh).
 // Activations are NHWC fp32; every kernel also records max|x| per pixel row for the next GEMM's dynamic scaling.
 #pragma once
 #include "common.cuh"
@@ -9,11 +9,14 @@ namespace syn {
 
 // conv1 7x7 stride 2 pad 3 (3 -> 64) + folded BN + ReLU: (B,3,120,120) NCHW -> (B,60,60,64) NHWC.
 // One CTA per (face, output row): 7 input rows x 3 channels staged with the zero padding, weights [147][64] in smem,
-// thread = (output pixel, 16-channel group).
+// thread = (output pixel, 16-channel group).  The input is the fp32 crop or, when x_u8 is set, the raw uint8 crop,
+// normalised while staging as (v - 127.5) / 128 -- exact in fp32, so both inputs give the same bits.  `border` zeroes the
+// uint8 frame like normalize_u8_kernel (syn_set_center_crop).
 constexpr int kRsStemThreads = 256;
-__global__ void __launch_bounds__(kRsStemThreads) resnet_stem_kernel(const float* __restrict__ x, const float* __restrict__ Wkn,
-                                                                      const float* __restrict__ bias, float* __restrict__ y,
-                                                                      unsigned* __restrict__ rowmax, int batch) {
+__global__ void __launch_bounds__(kRsStemThreads) resnet_stem_kernel(const float* __restrict__ x, const uint8_t* __restrict__ x_u8,
+                                                                      const float* __restrict__ Wkn, const float* __restrict__ bias,
+                                                                      float* __restrict__ y, unsigned* __restrict__ rowmax, int batch,
+                                                                      int border) {
   __shared__ float s_in[3][7][kImg + 6];
   __shared__ __align__(16) float s_w[147 * 64];
   __shared__ unsigned s_max[60];
@@ -23,7 +26,17 @@ __global__ void __launch_bounds__(kRsStemThreads) resnet_stem_kernel(const float
   for (int i = tid; i < 3 * 7 * (kImg + 6); i += kRsStemThreads) {
     const int col = i % (kImg + 6), r = (i / (kImg + 6)) % 7, ci = i / (7 * (kImg + 6));
     const int iy = oy * 2 - 3 + r, ix = col - 3;
-    s_in[ci][r][col] = (iy >= 0 && iy < kImg && ix >= 0 && ix < kImg) ? x[((size_t)(b * 3 + ci) * kImg + iy) * kImg + ix] : 0.f;
+    float v = 0.f;
+    if (iy >= 0 && iy < kImg && ix >= 0 && ix < kImg) {
+      const size_t off = ((size_t)(b * 3 + ci) * kImg + iy) * kImg + ix;
+      if (x_u8 != nullptr) {
+        const bool out = iy < border || iy >= kImg - border || ix < border || ix >= kImg - border;
+        v = ((float)(out ? 0 : x_u8[off]) - 127.5f) / 128.0f;
+      } else {
+        v = x[off];
+      }
+    }
+    s_in[ci][r][col] = v;
   }
   if (tid < 60) s_max[tid] = 0u;
   __syncthreads();

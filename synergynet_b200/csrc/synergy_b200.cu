@@ -38,7 +38,7 @@ struct DevConv {
 
 struct syn_heads;       // PointNet refinement heads (heads_host.inl)
 void syn_heads_destroy(syn_heads* s);
-struct syn_resnet;      // ResNet-50 backbone variant (resnet_host.inl)
+struct syn_resnet;      // ResNet backbones (resnet_host.inl)
 void syn_resnet_destroy(syn_resnet* s);
 struct syn_mbv1;        // MobileNetV1 backbones (mbv1_host.inl)
 void syn_mbv1_destroy(syn_mbv1* s);

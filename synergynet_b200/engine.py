@@ -14,10 +14,9 @@ import numpy as np
 import torch
 
 from . import _lib
-from .backbone import HEAD_DIMS, conv_plan, resnet50_conv_keys
+from .backbone import HEAD_DIMS, RESNET_ARCHS, conv_plan, resnet_conv_keys
 
 N_PARAMS = 62
-_RESNET_DOWNSAMPLES = {i for i, (ck, _) in enumerate(resnet50_conv_keys()) if 'downsample' in ck}
 
 
 def _host_f32(t) -> torch.Tensor:
@@ -41,6 +40,7 @@ class Engine:
         self.n_pts = 0
         self.n_vert = 0
         self._mbv1_feat = 0                  # pooled feature width of the committed MobileNetV1 (1024 x widen)
+        self._resnet_arch = 'resnet50'       # the ResNet the handle holds (syn_resnet_select; resnet50 until selected)
         self._keep = []
         # The C handle is not re-entrant and all calls share one activation workspace: serialise the host threads
         # (nn.DataParallel replicas use one engine per device, but user threads may share a model) and order
@@ -105,12 +105,13 @@ class Engine:
     def set_timing(self, on: bool) -> None:
         _lib.check(self._lib.syn_set_timing(self._h, int(on)))
 
-    def timings(self):
-        """[(kernel label, ms)] of the last device-buffer call (needs set_timing(True) before it)."""
-        ms = (C.c_float * 64)()
-        names = (C.c_char_p * 64)()
+    def timings(self, max_entries: int = 64):
+        """[(kernel label, ms)] of the last device-buffer call (needs set_timing(True) before it), at most
+        ``max_entries`` launches."""
+        ms = (C.c_float * max_entries)()
+        names = (C.c_char_p * max_entries)()
         n = C.c_int(0)
-        _lib.check(self._lib.syn_get_timings(self._h, ms, names, 64, C.byref(n)))
+        _lib.check(self._lib.syn_get_timings(self._h, ms, names, max_entries, C.byref(n)))
         return [(names[i].decode(), float(ms[i])) for i in range(n.value)]
 
     def poll_error(self) -> int:
@@ -386,21 +387,55 @@ class Engine:
             self._done()
         return out
 
-    # ---- ResNet-50 backbone variant (BASELINE.json configs[4]) ---------------------------------------------------
-    def load_resnet50(self, sd: Dict[str, torch.Tensor], prefix: str = '') -> None:
-        """Hand a ``resnet_backbone.resnet50()`` state dict to the library (53 conv+BN pairs in execution order, the four
-        Linear heads concatenated in the reference's output order ori | shape | exp | tex, resnet_backbone.py:242-246)."""
-        from .backbone import resnet50_conv_keys
+    # ---- ResNet backbones (backbone_nets/resnet_backbone.py; BASELINE.json configs[4] is resnet50) -------------------
+    def load_resnet(self, sd: Dict[str, torch.Tensor], arch: str, prefix: str = '') -> None:
+        """Hand a ``resnet_backbone.<arch>()`` state dict to the library: select the arch, then its conv+BN pairs in
+        state-dict order and the four Linear heads concatenated in the reference's output order ori | shape | exp | tex
+        (resnet_backbone.py:242-246)."""
+        if arch not in RESNET_ARCHS:
+            raise RuntimeError(f"arch '{arch}': the ResNet backbones are {', '.join(RESNET_ARCHS)}")
         with self._lock:
-            for i, (ck, bk) in enumerate(resnet50_conv_keys()):
+            _lib.check(self._lib.syn_resnet_select(self._h, *RESNET_ARCHS[arch]))
+            self._resnet_arch = arch
+            for i, (ck, bk) in enumerate(resnet_conv_keys(arch)):
                 w = _host_f32(sd[f'{prefix}{ck}.weight'])
                 bn = [_host_f32(sd[f'{prefix}{bk}.{k}']) for k in ('weight', 'bias', 'running_mean', 'running_var')]
                 _lib.check(self._lib.syn_resnet_set_conv(self._h, i, w.data_ptr(), w.numel(), *[t.data_ptr() for t in bn], 1e-5))
             order = ('fc_ori', 'fc_shape', 'fc_exp', 'fc_tex')
             w = torch.cat([_host_f32(sd[f'{prefix}{k}.weight']) for k in order]).contiguous()
             b = torch.cat([_host_f32(sd[f'{prefix}{k}.bias']) for k in order]).contiguous()
+            if tuple(w.shape) != (102, self.resnet_feature_dim):
+                raise RuntimeError(f'{arch} heads: expected (102, {self.resnet_feature_dim}) weights, got {tuple(w.shape)}')
             _lib.check(self._lib.syn_resnet_set_heads(self._h, w.data_ptr(), b.data_ptr()))
             _lib.check(self._lib.syn_resnet_commit(self._h))
+
+    def load_resnet50(self, sd: Dict[str, torch.Tensor], prefix: str = '') -> None:
+        """Hand a ``resnet_backbone.resnet50()`` state dict to the library (53 conv+BN pairs in execution order, the four
+        Linear heads concatenated in the reference's output order ori | shape | exp | tex, resnet_backbone.py:242-246)."""
+        self.load_resnet(sd, 'resnet50', prefix)
+
+    @property
+    def resnet_feature_dim(self) -> int:
+        """Pooled feature width of the selected ResNet: 512 (resnet18 / 34) or 2048."""
+        return 512 if RESNET_ARCHS[self._resnet_arch][0] < 50 else 2048
+
+    def forward_resnet(self, x: torch.Tensor):
+        """ResNet._forward_impl (resnet_backbone.py:227-249) of the loaded arch: (B,3,120,120) fp32 normalised crops or raw
+        uint8 crops -> ((B,102) ori|shape|exp|tex, (B,512 or 2048) pooled)."""
+        if x.dtype == torch.uint8:
+            if x.dim() != 4 or tuple(x.shape[1:]) != (3, 120, 120) or x.device != self.device:
+                raise RuntimeError(f'expected uint8 (B,3,120,120) on {self.device}, got {tuple(x.shape)} on {x.device}')
+            x = x.contiguous()
+        else:
+            x = self._check_x(x)
+        b = x.shape[0]
+        out = torch.empty((b, 102), device=self.device, dtype=torch.float32)
+        pool = torch.empty((b, self.resnet_feature_dim), device=self.device, dtype=torch.float32)
+        with self._lock:
+            _lib.check(self._lib.syn_resnet_forward(self._h, x.data_ptr(), int(x.dtype == torch.uint8), b, out.data_ptr(),
+                                                    pool.data_ptr(), self._stream()))
+            self._done()
+        return out, pool
 
     def forward_resnet50(self, x: torch.Tensor):
         """ResNet._forward_impl (resnet_backbone.py:227-249): (B,3,120,120) -> ((B,102) ori|shape|exp|tex, (B,2048) pooled)."""
@@ -485,21 +520,23 @@ class Engine:
         return out, rm
 
     def debug_resnet_until(self, x: torch.Tensor, stage: int):
-        """ResNet-50 run up to ``stage`` (0 stem, 1 max-pool, 1 + i conv i of the plan, 54 avgpool, 55 heads): (that
-        stage's output as (rows, channels) -- one row per NHWC pixel, or per face --, its row maxima as int32 fp32 bit
-        patterns, or None for a stage that records none)."""
+        """Run of the loaded ResNet up to ``stage`` (0 stem, 1 max-pool, 1 + i conv i of the plan, n + 1 avgpool, n + 2
+        heads, n convs; 54 / 55 for resnet50): (that stage's output as (rows, channels) -- one row per NHWC pixel, or per
+        face --, its row maxima as int32 fp32 bit patterns, or None for a stage that records none)."""
         x = self._check_x(x)
         b = x.shape[0]
+        keys = resnet_conv_keys(self._resnet_arch)
+        n = len(keys)
         if stage == 0:
             rows, cols, rm = b * 3600, 64, True
         elif stage == 1:
             rows, cols, rm = b * 900, 64, True
-        elif stage <= 53:
+        elif stage <= n:
             d = _lib.ConvDesc()
-            _lib.check(self._lib.syn_resnet_conv_desc(stage - 1, C.byref(d)))
-            rows, cols, rm = b * d.h_out * d.h_out, d.cout, stage - 1 not in _RESNET_DOWNSAMPLES
+            _lib.check(self._lib.syn_resnet_arch_conv_desc(*RESNET_ARCHS[self._resnet_arch], stage - 1, C.byref(d)))
+            rows, cols, rm = b * d.h_out * d.h_out, d.cout, 'downsample' not in keys[stage - 1][0]
         else:
-            rows, cols, rm = b, 2048 if stage == 54 else 102, stage == 54
+            rows, cols, rm = b, self.resnet_feature_dim if stage == n + 1 else 102, stage == n + 1
         out, rmax = self._debug_out(rows, cols, rm)
         with self._lock:
             _lib.check(self._lib.syn_debug_resnet_until(self._h, x.data_ptr(), b, stage, out.data_ptr(),

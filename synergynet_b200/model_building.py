@@ -96,12 +96,6 @@ class I2P(nn.Module):
         self.args = args
         if 'mobilenet_v2' in self.args.arch:
             self.backbone = getattr(mobilenetv2_backbone, args.arch)(pretrained=False)
-        elif self.args.arch == 'resnet50':
-            # BASELINE.json configs[4].  The reference's own I2P cannot run this backbone: ResNet._forward_impl returns
-            # ONE (B,102) tensor (resnet_backbone.py:242-249) and I2P unpacks two (model_building.py:55,61; SURVEY.md
-            # fact 4).  Adapter used here (and by the oracle / golden vectors): params = out[:, :62] (ori|shape|exp),
-            # avgpool = the 2048-d pooled feature.
-            self.backbone = mobilenetv2_backbone.resnet50(pretrained=False)
         elif 'mobilenet' in self.args.arch:
             # the reference sends every other 'mobilenet*' arch to mobilenetv1_backbone (model_building.py:42-43).  Like
             # ResNet-50, MobileNet.forward returns ONE (B,102) tensor (mobilenetv1_backbone.py:138-140) and the reference's
@@ -112,12 +106,23 @@ class I2P(nn.Module):
                 raise RuntimeError(f"arch '{args.arch}': the MobileNetV1 backbones are "
                                    f"{', '.join(mobilenetv2_backbone.MBV1_WIDTHS)}")
             self.backbone = getattr(mobilenetv2_backbone, args.arch)()
-        elif any(k in self.args.arch for k in ('mobilenet', 'resnet', 'ghostnet', 'resnest')):
+        elif 'resnet' in self.args.arch:
+            # the reference builds any 'resnet' arch with getattr(resnet_backbone, arch)(pretrained=False)
+            # (model_building.py:44-45): the seven factories of RESNET_ARCHS; resnet50 is BASELINE.json configs[4].  The
+            # reference's own I2P cannot run these backbones: ResNet._forward_impl returns ONE (B,102) tensor
+            # (resnet_backbone.py:242-249) and I2P unpacks two (model_building.py:55,61; SURVEY.md fact 4).  Adapter used
+            # here (and by the oracle / golden vectors): params = out[:, :62] (ori|shape|exp), avgpool = the pooled
+            # feature (2048-d; 512-d for resnet18 / 34).
+            if self.args.arch not in mobilenetv2_backbone.RESNET_ARCHS:
+                raise RuntimeError(f"arch '{args.arch}': the ResNet backbones are "
+                                   f"{', '.join(mobilenetv2_backbone.RESNET_ARCHS)}")
+            self.backbone = getattr(mobilenetv2_backbone, args.arch)(pretrained=False)
+        elif any(k in self.args.arch for k in ('ghostnet', 'resnest')):
             raise RuntimeError(f"arch '{args.arch}': mobilenet_v2 and resnet50 are built for sm_90a "
                                '(SURVEY.md section 8; the other backbones are not on the hot path)')
         else:
             raise RuntimeError("Please choose [mobilenet_v2, mobilenet_1, resnet50, or ghostnet]")
-        self._is_resnet = self.args.arch == 'resnet50'
+        self._is_resnet = self.args.arch in mobilenetv2_backbone.RESNET_ARCHS
         self._is_mbv1 = self.args.arch in mobilenetv2_backbone.MBV1_WIDTHS
         self._adapted = self._is_resnet or self._is_mbv1      # one (B,102) output: params = out[:, :62]
         object.__setattr__(self, '_rt', _Runtime())
@@ -135,8 +140,9 @@ class I2P(nn.Module):
         return self._rt.get(device, self._backbone_sd, self._basis_provider)
 
     def _resnet_engine(self, device) -> Engine:
-        """Engine with the ResNet-50 weights: the shared library state (error flag, 3DMM bases for reconstruct) comes from
-        a commit of the MobileNetV2 path with a zero checkpoint of the right schema, then the ResNet layers are handed over."""
+        """Engine with the weights of the ResNet backbone: the shared library state (error flag, 3DMM bases for reconstruct)
+        comes from a commit of the MobileNetV2 path with a zero checkpoint of the right schema, then the ResNet layers are
+        handed over."""
         rt = self._rt
         if not hasattr(rt, '_mbv2_stub'):
             rt._mbv2_stub = {k: v for k, v in mobilenetv2_backbone.mobilenet_v2().state_dict().items()
@@ -144,10 +150,10 @@ class I2P(nn.Module):
         eng = rt.get(device, lambda: rt._mbv2_stub, self._basis_provider)
         sd = self._backbone_sd()
         sig = rt._signature(list(sd.values()))
-        key = (eng.device.index, 'resnet50')
+        key = (eng.device.index, self.args.arch)
         with rt._lock:
             if rt._pn_sig.get(key) != sig or getattr(eng, '_resnet_commit_of', None) is not rt._sig.get(eng.device.index):
-                eng.load_resnet50(sd)
+                eng.load_resnet(sd, self.args.arch)
                 rt._pn_sig[key] = sig
                 eng._resnet_commit_of = rt._sig.get(eng.device.index)
         return eng
@@ -170,10 +176,10 @@ class I2P(nn.Module):
         return eng
 
     def _forward_adapted(self, x: torch.Tensor):
-        """(out102, pool) of the resnet50 / mobilenet_* backbone on ``x`` (fp32 crops; uint8 crops for mobilenet_*),
-        which lives on the compute device."""
+        """(out102, pool) of the ResNet / mobilenet_* backbone on ``x`` (fp32 crops or uint8 crops), which lives on the
+        compute device."""
         eng = self._engine(x.device)
-        return eng.forward_mobilenet_v1(x) if self._is_mbv1 else eng.forward_resnet50(x)
+        return eng.forward_mobilenet_v1(x) if self._is_mbv1 else eng.forward_resnet(x)
 
     def _compute_device(self, t: Optional[torch.Tensor] = None) -> torch.device:
         """Where the library runs for tensor ``t``: its own GPU, else the GPU the backbone lives on, else the current
@@ -313,9 +319,10 @@ class _SynergyBase(nn.Module):
         _3D_attr, avgpool = self.I2P.forward_test(input.to(dev))
         if avgpool.shape[1] != 1280:
             raise RuntimeError('SynergyNet.forward: MLP_for.conv6 is hard-wired to a 1280-d image feature '
-                               '(pointnet_backbone.py:15,58: 2418 = 64 + 1024 + 1280 + 40 + 10); the resnet50 backbone pools '
-                               f'{avgpool.shape[1]} channels, so the refinement head cannot follow it (the reference fails '
-                               'here too, SURVEY.md fact 4).  Use forward_test() / reconstruct_vertex_62() with resnet50.')
+                               f'(pointnet_backbone.py:15,58: 2418 = 64 + 1024 + 1280 + 40 + 10); the {self.I2P.args.arch} '
+                               f'backbone pools {avgpool.shape[1]} channels, so the refinement head cannot follow it (the '
+                               'reference fails here too, SURVEY.md fact 4).  Use forward_test() / reconstruct_vertex_62() '
+                               f'with {self.I2P.args.arch}.')
         _3D_attr_GT = target.to(device=dev, dtype=torch.float32)
         vertex_lmk = eng.reconstruct(_3D_attr, dense=False)
         vertex_GT_lmk = eng.reconstruct(_3D_attr_GT, dense=False)
@@ -365,8 +372,9 @@ class _SynergyBase(nn.Module):
         eng = self._engine(dev)
         image = torch.from_numpy(np.ascontiguousarray(input, dtype=np.uint8)).to(dev)    # crop_img's uint8 crops
         batch = crop_resize_device(image, boxes, (120, 120), interp)
-        if self.I2P._is_mbv1:                       # that backbone, on the uint8 crops; then the same image-space stages
-            params = eng.forward_mobilenet_v1(batch)[0][:, :62].contiguous()
+        if self.I2P._adapted:                       # that backbone, on the uint8 crops; then the same image-space stages
+            out = eng.forward_mobilenet_v1(batch)[0] if self.I2P._is_mbv1 else eng.forward_resnet(batch)[0]
+            params = out[:, :62].contiguous()
         else:
             _, params = eng.forward_landmarks(batch, want_params=True)
         roi5 = torch.from_numpy(roi_affine(boxes)).to(dev)
