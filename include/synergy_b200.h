@@ -186,7 +186,10 @@ int syn_param_loss(syn_handle_t* h, const float* input_dev, const float* target_
  * fc_ori | fc_shape | fc_exp | fc_tex -> (102, 2048) weights, (102) bias (:242-246).
  * syn_resnet50_forward: x_dev (B,3,120,120) NCHW -> out102_dev (B,102) exactly what ResNet._forward_impl returns;
  * pool2048_dev (B,2048) = the flattened avgpool, may be NULL.  (The reference's I2P unpacks two values from this
- * backbone and fails, SURVEY.md fact 4; the Python shim adapts: params = out[:, :62], pool = the 2048-d feature.) */
+ * backbone and fails, SURVEY.md fact 4; the Python shim adapts: params = out[:, :62], pool = the 2048-d feature.)
+ * Every forward and debug run of the ResNet and MobileNetV1 backbones (syn_resnet50_forward, syn_resnet_forward,
+ * syn_mbv1_forward, syn_debug_resnet_until, syn_debug_mbv1_until) takes 1 <= B <= 65535 faces per call, and returns
+ * SYN_ERR_INVALID before any launch otherwise. */
 int syn_resnet_num_convs(void);                              /* 53 */
 int syn_resnet_conv_desc(int idx, syn_conv_desc_t* out);
 int syn_resnet_set_conv(syn_handle_t* h, int idx, const float* w_host, int64_t w_numel, const float* bn_weight_host,

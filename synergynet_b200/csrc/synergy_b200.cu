@@ -1261,5 +1261,6 @@ int syn_debug_forward_until(syn_handle_t* h, const float* x, int batch, int laye
 }  // extern "C"
 
 #include "heads_host.inl"
+#include "convbn_host.inl"
 #include "resnet_host.inl"
 #include "mbv1_host.inl"

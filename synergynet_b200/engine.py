@@ -14,7 +14,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .backbone import HEAD_DIMS, RESNET_ARCHS, conv_plan, resnet_conv_keys
+from .backbone import HEAD_DIMS, MBV1_WIDTHS, RESNET_ARCHS, conv_plan, mobilenet_v1_conv_keys, resnet_conv_keys
 
 N_PARAMS = 62
 
@@ -39,8 +39,9 @@ class Engine:
         self._h = h
         self.n_pts = 0
         self.n_vert = 0
-        self._mbv1_feat = 0                  # pooled feature width of the committed MobileNetV1 (1024 x widen)
-        self._resnet_arch = 'resnet50'       # the ResNet the handle holds (syn_resnet_select; resnet50 until selected)
+        # the conv+BN backbone each family's part of the handle holds: family -> (arch, pooled feature width); the ResNet
+        # part holds resnet50 until syn_resnet_select
+        self._backbones: Dict[str, Tuple[str, int]] = {'resnet': ('resnet50', 2048)}
         self._keep = []
         # The C handle is not re-entrant and all calls share one activation workspace: serialise the host threads
         # (nn.DataParallel replicas use one engine per device, but user threads may share a model) and order
@@ -387,27 +388,70 @@ class Engine:
             self._done()
         return out
 
-    # ---- ResNet backbones (backbone_nets/resnet_backbone.py; BASELINE.json configs[4] is resnet50) -------------------
+    # ---- conv+BN backbones: ResNet and MobileNetV1, one (B,102) output ori | shape | exp | tex ---------------------
+    def _load_convbn(self, family: str, arch: str, select, conv_keys, feat: int, sd: Dict[str, torch.Tensor],
+                     prefix: str) -> None:
+        """``select()`` the plan of ``arch``, then hand over its conv+BN pairs in plan order and the four Linear heads
+        concatenated in the reference's output order as (102, feat) weights, and commit."""
+        set_conv, set_heads, commit = (getattr(self._lib, f'syn_{family}_{n}') for n in ('set_conv', 'set_heads', 'commit'))
+        with self._lock:
+            _lib.check(select())
+            self._backbones[family] = (arch, feat)
+            for i, (ck, bk) in enumerate(conv_keys):
+                w = _host_f32(sd[f'{prefix}{ck}.weight'])
+                bn = [_host_f32(sd[f'{prefix}{bk}.{k}']) for k in ('weight', 'bias', 'running_mean', 'running_var')]
+                _lib.check(set_conv(self._h, i, w.data_ptr(), w.numel(), *[t.data_ptr() for t in bn], 1e-5))
+            order = ('fc_ori', 'fc_shape', 'fc_exp', 'fc_tex')
+            w = torch.cat([_host_f32(sd[f'{prefix}{k}.weight']) for k in order]).contiguous()
+            b = torch.cat([_host_f32(sd[f'{prefix}{k}.bias']) for k in order]).contiguous()
+            if tuple(w.shape) != (102, feat):
+                raise RuntimeError(f'{arch} heads: expected (102, {feat}) weights, got {tuple(w.shape)}')
+            _lib.check(set_heads(self._h, w.data_ptr(), b.data_ptr()))
+            _lib.check(commit(self._h))
+
+    def _backbone(self, family: str) -> Tuple[str, int]:
+        if family not in self._backbones:
+            raise RuntimeError(f'no {family} backbone loaded on this engine')
+        return self._backbones[family]
+
+    def _forward_convbn(self, family: str, x: torch.Tensor):
+        """(B,3,120,120) fp32 normalised crops or raw uint8 crops -> ((B,102) out, (B,feat) pooled)."""
+        if x.dtype == torch.uint8:
+            if x.dim() != 4 or tuple(x.shape[1:]) != (3, 120, 120) or x.device != self.device:
+                raise RuntimeError(f'expected uint8 (B,3,120,120) on {self.device}, got {tuple(x.shape)} on {x.device}')
+            x = x.contiguous()
+        else:
+            x = self._check_x(x)
+        b = x.shape[0]
+        out = torch.empty((b, 102), device=self.device, dtype=torch.float32)
+        pool = torch.empty((b, self._backbone(family)[1]), device=self.device, dtype=torch.float32)
+        forward = getattr(self._lib, f'syn_{family}_forward')
+        with self._lock:
+            _lib.check(forward(self._h, x.data_ptr(), int(x.dtype == torch.uint8), b, out.data_ptr(), pool.data_ptr(),
+                               self._stream()))
+            self._done()
+        return out, pool
+
+    def _debug_run(self, fn, x: torch.Tensor, stage: int, rows: int, cols: int, rowmax: bool):
+        """One syn_debug_*_until run of a conv+BN backbone on fp32 crops ``x`` into (rows, cols) and, if the stage records
+        them, (rows,) row maxima."""
+        out, rmax = self._debug_out(rows, cols, rowmax)
+        with self._lock:
+            _lib.check(fn(self._h, x.data_ptr(), x.shape[0], stage, out.data_ptr(), rmax.data_ptr() if rowmax else None,
+                          self._stream()))
+            self._done()
+        return out, rmax
+
+    # ResNet backbones (backbone_nets/resnet_backbone.py; BASELINE.json configs[4] is resnet50)
     def load_resnet(self, sd: Dict[str, torch.Tensor], arch: str, prefix: str = '') -> None:
         """Hand a ``resnet_backbone.<arch>()`` state dict to the library: select the arch, then its conv+BN pairs in
         state-dict order and the four Linear heads concatenated in the reference's output order ori | shape | exp | tex
         (resnet_backbone.py:242-246)."""
         if arch not in RESNET_ARCHS:
             raise RuntimeError(f"arch '{arch}': the ResNet backbones are {', '.join(RESNET_ARCHS)}")
-        with self._lock:
-            _lib.check(self._lib.syn_resnet_select(self._h, *RESNET_ARCHS[arch]))
-            self._resnet_arch = arch
-            for i, (ck, bk) in enumerate(resnet_conv_keys(arch)):
-                w = _host_f32(sd[f'{prefix}{ck}.weight'])
-                bn = [_host_f32(sd[f'{prefix}{bk}.{k}']) for k in ('weight', 'bias', 'running_mean', 'running_var')]
-                _lib.check(self._lib.syn_resnet_set_conv(self._h, i, w.data_ptr(), w.numel(), *[t.data_ptr() for t in bn], 1e-5))
-            order = ('fc_ori', 'fc_shape', 'fc_exp', 'fc_tex')
-            w = torch.cat([_host_f32(sd[f'{prefix}{k}.weight']) for k in order]).contiguous()
-            b = torch.cat([_host_f32(sd[f'{prefix}{k}.bias']) for k in order]).contiguous()
-            if tuple(w.shape) != (102, self.resnet_feature_dim):
-                raise RuntimeError(f'{arch} heads: expected (102, {self.resnet_feature_dim}) weights, got {tuple(w.shape)}')
-            _lib.check(self._lib.syn_resnet_set_heads(self._h, w.data_ptr(), b.data_ptr()))
-            _lib.check(self._lib.syn_resnet_commit(self._h))
+        feat = 512 if RESNET_ARCHS[arch][0] < 50 else 2048
+        self._load_convbn('resnet', arch, lambda: self._lib.syn_resnet_select(self._h, *RESNET_ARCHS[arch]),
+                          resnet_conv_keys(arch), feat, sd, prefix)
 
     def load_resnet50(self, sd: Dict[str, torch.Tensor], prefix: str = '') -> None:
         """Hand a ``resnet_backbone.resnet50()`` state dict to the library (53 conv+BN pairs in execution order, the four
@@ -417,25 +461,12 @@ class Engine:
     @property
     def resnet_feature_dim(self) -> int:
         """Pooled feature width of the selected ResNet: 512 (resnet18 / 34) or 2048."""
-        return 512 if RESNET_ARCHS[self._resnet_arch][0] < 50 else 2048
+        return self._backbone('resnet')[1]
 
     def forward_resnet(self, x: torch.Tensor):
         """ResNet._forward_impl (resnet_backbone.py:227-249) of the loaded arch: (B,3,120,120) fp32 normalised crops or raw
         uint8 crops -> ((B,102) ori|shape|exp|tex, (B,512 or 2048) pooled)."""
-        if x.dtype == torch.uint8:
-            if x.dim() != 4 or tuple(x.shape[1:]) != (3, 120, 120) or x.device != self.device:
-                raise RuntimeError(f'expected uint8 (B,3,120,120) on {self.device}, got {tuple(x.shape)} on {x.device}')
-            x = x.contiguous()
-        else:
-            x = self._check_x(x)
-        b = x.shape[0]
-        out = torch.empty((b, 102), device=self.device, dtype=torch.float32)
-        pool = torch.empty((b, self.resnet_feature_dim), device=self.device, dtype=torch.float32)
-        with self._lock:
-            _lib.check(self._lib.syn_resnet_forward(self._h, x.data_ptr(), int(x.dtype == torch.uint8), b, out.data_ptr(),
-                                                    pool.data_ptr(), self._stream()))
-            self._done()
-        return out, pool
+        return self._forward_convbn('resnet', x)
 
     def forward_resnet50(self, x: torch.Tensor):
         """ResNet._forward_impl (resnet_backbone.py:227-249): (B,3,120,120) -> ((B,102) ori|shape|exp|tex, (B,2048) pooled)."""
@@ -448,45 +479,41 @@ class Engine:
             self._done()
         return out, pool
 
-    # ---- MobileNetV1 backbones (backbone_nets/mobilenetv1_backbone.py, the five mobilenet_* factories) -----------
+    def debug_resnet_until(self, x: torch.Tensor, stage: int):
+        """Run of the loaded ResNet up to ``stage`` (0 stem, 1 max-pool, 1 + i conv i of the plan, n + 1 avgpool, n + 2
+        heads, n convs; 54 / 55 for resnet50): (that stage's output as (rows, channels) -- one row per NHWC pixel, or per
+        face --, its row maxima as int32 fp32 bit patterns, or None for a stage that records none)."""
+        x = self._check_x(x)
+        b = x.shape[0]
+        arch, feat = self._backbone('resnet')
+        keys = resnet_conv_keys(arch)
+        n = len(keys)
+        if stage == 0:
+            rows, cols, rm = b * 3600, 64, True
+        elif stage == 1:
+            rows, cols, rm = b * 900, 64, True
+        elif stage <= n:
+            d = _lib.ConvDesc()
+            _lib.check(self._lib.syn_resnet_arch_conv_desc(*RESNET_ARCHS[arch], stage - 1, C.byref(d)))
+            rows, cols, rm = b * d.h_out * d.h_out, d.cout, 'downsample' not in keys[stage - 1][0]
+        else:
+            rows, cols, rm = b, feat if stage == n + 1 else 102, stage == n + 1
+        return self._debug_run(self._lib.syn_debug_resnet_until, x, stage, rows, cols, rm)
+
+    # MobileNetV1 backbones (backbone_nets/mobilenetv1_backbone.py, the five mobilenet_* factories)
     def load_mobilenet_v1(self, sd: Dict[str, torch.Tensor], arch: str, prefix: str = '') -> None:
         """Hand a ``mobilenetv1_backbone.<arch>()`` state dict to the library (27 conv+BN pairs in execution order, the four
         Linear heads concatenated in the reference's output order ori | shape | exp | tex, mobilenetv1_backbone.py:132-138)."""
-        from .backbone import MBV1_WIDTHS, mobilenet_v1_conv_keys
         if arch not in MBV1_WIDTHS:
             raise RuntimeError(f"arch '{arch}': MobileNetV1 widths are {', '.join(MBV1_WIDTHS)}")
-        with self._lock:
-            _lib.check(self._lib.syn_mbv1_set_widen(self._h, int(round(MBV1_WIDTHS[arch] * 100))))
-            for i, (ck, bk) in enumerate(mobilenet_v1_conv_keys()):
-                w = _host_f32(sd[f'{prefix}{ck}.weight'])
-                bn = [_host_f32(sd[f'{prefix}{bk}.{k}']) for k in ('weight', 'bias', 'running_mean', 'running_var')]
-                _lib.check(self._lib.syn_mbv1_set_conv(self._h, i, w.data_ptr(), w.numel(), *[t.data_ptr() for t in bn], 1e-5))
-            order = ('fc_ori', 'fc_shape', 'fc_exp', 'fc_tex')
-            w = torch.cat([_host_f32(sd[f'{prefix}{k}.weight']) for k in order]).contiguous()
-            b = torch.cat([_host_f32(sd[f'{prefix}{k}.bias']) for k in order]).contiguous()
-            if w.shape[0] != 102:
-                raise RuntimeError(f'MobileNetV1 heads: expected 102 output rows, got {w.shape[0]}')
-            _lib.check(self._lib.syn_mbv1_set_heads(self._h, w.data_ptr(), b.data_ptr()))
-            _lib.check(self._lib.syn_mbv1_commit(self._h))
-            self._mbv1_feat = w.shape[1]
+        code = int(round(MBV1_WIDTHS[arch] * 100))
+        self._load_convbn('mbv1', arch, lambda: self._lib.syn_mbv1_set_widen(self._h, code), mobilenet_v1_conv_keys(),
+                          1024 * code // 100, sd, prefix)
 
     def forward_mobilenet_v1(self, x: torch.Tensor):
         """MobileNet.forward (mobilenetv1_backbone.py:108-140): (B,3,120,120) fp32 normalised crops or raw uint8 crops ->
         ((B,102) ori|shape|exp|tex, (B,1024w) pooled)."""
-        if x.dtype == torch.uint8:
-            if x.dim() != 4 or tuple(x.shape[1:]) != (3, 120, 120) or x.device != self.device:
-                raise RuntimeError(f'expected uint8 (B,3,120,120) on {self.device}, got {tuple(x.shape)} on {x.device}')
-            x = x.contiguous()
-        else:
-            x = self._check_x(x)
-        b = x.shape[0]
-        out = torch.empty((b, 102), device=self.device, dtype=torch.float32)
-        pool = torch.empty((b, self._mbv1_feat), device=self.device, dtype=torch.float32)
-        with self._lock:
-            _lib.check(self._lib.syn_mbv1_forward(self._h, x.data_ptr(), int(x.dtype == torch.uint8), b, out.data_ptr(),
-                                                  pool.data_ptr(), self._stream()))
-            self._done()
-        return out, pool
+        return self._forward_convbn('mbv1', x)
 
     def debug_mobilenet_v1_until(self, x: torch.Tensor, stage: int):
         """MobileNetV1 run up to ``stage`` (0 stem, 2j - 1 / 2j conv_dw / conv_sep of block j = 1..13, 27 avgpool, 28
@@ -494,19 +521,14 @@ class Engine:
         fp32 bit patterns, or None for a stage that records none)."""
         x = self._check_x(x)
         b = x.shape[0]
+        arch, feat = self._backbone('mbv1')
         if stage <= 26:
             d = _lib.ConvDesc()
-            widen = int(round(self._mbv1_feat / 1024 * 100))
-            _lib.check(self._lib.syn_mbv1_conv_desc(widen, stage, C.byref(d)))
+            _lib.check(self._lib.syn_mbv1_conv_desc(int(round(MBV1_WIDTHS[arch] * 100)), stage, C.byref(d)))
             rows, cols, rm = b * d.h_out * d.h_out, d.cout, stage == 0 or stage % 2 == 1 or stage == 26
         else:
-            rows, cols, rm = b, self._mbv1_feat if stage == 27 else 102, stage == 27
-        out, rmax = self._debug_out(rows, cols, rm)
-        with self._lock:
-            _lib.check(self._lib.syn_debug_mbv1_until(self._h, x.data_ptr(), b, stage, out.data_ptr(),
-                                                      rmax.data_ptr() if rm else None, self._stream()))
-            self._done()
-        return out, rmax
+            rows, cols, rm = b, feat if stage == 27 else 102, stage == 27
+        return self._debug_run(self._lib.syn_debug_mbv1_until, x, stage, rows, cols, rm)
 
     # ---- per-stage debug runs of the GEMM layers (include/synergy_b200.h syn_debug_*_until / syn_debug_gemm) ----
     RESNET_STAGES = 56
@@ -518,31 +540,6 @@ class Engine:
         out = torch.empty((rows, cols), device=self.device, dtype=torch.float32)
         rm = torch.zeros((rows,), device=self.device, dtype=torch.int32) if rowmax else None
         return out, rm
-
-    def debug_resnet_until(self, x: torch.Tensor, stage: int):
-        """Run of the loaded ResNet up to ``stage`` (0 stem, 1 max-pool, 1 + i conv i of the plan, n + 1 avgpool, n + 2
-        heads, n convs; 54 / 55 for resnet50): (that stage's output as (rows, channels) -- one row per NHWC pixel, or per
-        face --, its row maxima as int32 fp32 bit patterns, or None for a stage that records none)."""
-        x = self._check_x(x)
-        b = x.shape[0]
-        keys = resnet_conv_keys(self._resnet_arch)
-        n = len(keys)
-        if stage == 0:
-            rows, cols, rm = b * 3600, 64, True
-        elif stage == 1:
-            rows, cols, rm = b * 900, 64, True
-        elif stage <= n:
-            d = _lib.ConvDesc()
-            _lib.check(self._lib.syn_resnet_arch_conv_desc(*RESNET_ARCHS[self._resnet_arch], stage - 1, C.byref(d)))
-            rows, cols, rm = b * d.h_out * d.h_out, d.cout, 'downsample' not in keys[stage - 1][0]
-        else:
-            rows, cols, rm = b, self.resnet_feature_dim if stage == n + 1 else 102, stage == n + 1
-        out, rmax = self._debug_out(rows, cols, rm)
-        with self._lock:
-            _lib.check(self._lib.syn_debug_resnet_until(self._h, x.data_ptr(), b, stage, out.data_ptr(),
-                                                        rmax.data_ptr() if rm else None, self._stream()))
-            self._done()
-        return out, rmax
 
     def debug_pointnet_until(self, net: int, lmk: torch.Tensor, stage: int, pool: Optional[torch.Tensor] = None,
                              params: Optional[torch.Tensor] = None):

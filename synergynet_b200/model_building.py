@@ -133,16 +133,14 @@ class I2P(nn.Module):
                 if not k.endswith('num_batches_tracked')}
 
     def _engine(self, device) -> Engine:
-        if self._is_resnet:
-            return self._resnet_engine(device)
-        if self._is_mbv1:
-            return self._mbv1_engine(device)
+        if self._adapted:
+            return self._adapted_engine(device)
         return self._rt.get(device, self._backbone_sd, self._basis_provider)
 
-    def _resnet_engine(self, device) -> Engine:
-        """Engine with the weights of the ResNet backbone: the shared library state (error flag, 3DMM bases for reconstruct)
-        comes from a commit of the MobileNetV2 path with a zero checkpoint of the right schema, then the ResNet layers are
-        handed over."""
+    def _adapted_engine(self, device) -> Engine:
+        """Engine with the weights of the ResNet or MobileNetV1 backbone: the shared library state (error flag, 3DMM bases
+        for reconstruct) comes from a commit of the MobileNetV2 path with a zero checkpoint of the right schema, then the
+        backbone's layers are handed over."""
         rt = self._rt
         if not hasattr(rt, '_mbv2_stub'):
             rt._mbv2_stub = {k: v for k, v in mobilenetv2_backbone.mobilenet_v2().state_dict().items()
@@ -152,27 +150,11 @@ class I2P(nn.Module):
         sig = rt._signature(list(sd.values()))
         key = (eng.device.index, self.args.arch)
         with rt._lock:
-            if rt._pn_sig.get(key) != sig or getattr(eng, '_resnet_commit_of', None) is not rt._sig.get(eng.device.index):
-                eng.load_resnet(sd, self.args.arch)
+            if rt._pn_sig.get(key) != sig or getattr(eng, '_adapted_commit_of', None) is not rt._sig.get(eng.device.index):
+                load = eng.load_mobilenet_v1 if self._is_mbv1 else eng.load_resnet
+                load(sd, self.args.arch)
                 rt._pn_sig[key] = sig
-                eng._resnet_commit_of = rt._sig.get(eng.device.index)
-        return eng
-
-    def _mbv1_engine(self, device) -> Engine:
-        """Engine with the MobileNetV1 weights, built the way ``_resnet_engine`` builds its engine."""
-        rt = self._rt
-        if not hasattr(rt, '_mbv2_stub'):
-            rt._mbv2_stub = {k: v for k, v in mobilenetv2_backbone.mobilenet_v2().state_dict().items()
-                             if not k.endswith('num_batches_tracked')}
-        eng = rt.get(device, lambda: rt._mbv2_stub, self._basis_provider)
-        sd = self._backbone_sd()
-        sig = rt._signature(list(sd.values()))
-        key = (eng.device.index, self.args.arch)
-        with rt._lock:
-            if rt._pn_sig.get(key) != sig or getattr(eng, '_mbv1_commit_of', None) is not rt._sig.get(eng.device.index):
-                eng.load_mobilenet_v1(sd, self.args.arch)
-                rt._pn_sig[key] = sig
-                eng._mbv1_commit_of = rt._sig.get(eng.device.index)
+                eng._adapted_commit_of = rt._sig.get(eng.device.index)
         return eng
 
     def _forward_adapted(self, x: torch.Tensor):

@@ -314,3 +314,29 @@ def test_launches_and_timing_names(models, arch):
     eng.set_timing(False)
     assert launches == n + 3 and names == want
     assert eng.poll_error() == 0
+
+
+def test_backbone_entry_points_reject_65536_faces(synth_pack):
+    """All five forward and debug entry points of the conv+BN backbones refuse 65536 faces with SYN_ERR_INVALID before
+    they launch anything (the bound dw3x3_kernel's grid.y sets, shared by every entry point)."""
+    from oracle import synth_mbv1
+    rn = make_model(synth_resnet.build_resnet_state_dict(0, 'resnet50'), 'resnet50', strict=False)._engine(DEV)
+    v1 = make_model(synth_mbv1.build_mobilenet_v1_state_dict(0, 'mobilenet_025'), 'mobilenet_025', strict=False)._engine(DEV)
+    x = torch.zeros((1, 3, 120, 120), device=DEV)
+    out = torch.empty((1, 2048), device=DEV)
+    rm = torch.zeros((1,), device=DEV, dtype=torch.int32)
+    b = 65536
+    calls = [(rn, lambda L, h: L.syn_resnet50_forward(h, x.data_ptr(), b, out.data_ptr(), out.data_ptr(), None)),
+             (rn, lambda L, h: L.syn_resnet_forward(h, x.data_ptr(), 0, b, out.data_ptr(), out.data_ptr(), None)),
+             (rn, lambda L, h: L.syn_debug_resnet_until(h, x.data_ptr(), b, 2, out.data_ptr(), rm.data_ptr(), None)),
+             (v1, lambda L, h: L.syn_mbv1_forward(h, x.data_ptr(), 0, b, out.data_ptr(), out.data_ptr(), None)),
+             (v1, lambda L, h: L.syn_debug_mbv1_until(h, x.data_ptr(), b, 1, out.data_ptr(), rm.data_ptr(), None))]
+    for i, (eng, call) in enumerate(calls):
+        n0 = eng.launch_count
+        assert call(eng._lib, eng._h) == 1, i                                     # SYN_ERR_INVALID
+        assert b'65535' in eng._lib.syn_last_error(), i
+        assert eng.launch_count == n0, i
+    rn.forward_resnet50(x)                                          # both handles still run
+    v1.forward_mobilenet_v1(x)
+    torch.cuda.synchronize()
+    assert rn.poll_error() == 0 and v1.poll_error() == 0
