@@ -289,6 +289,13 @@ enum {
  * the index list either reference function returns, bit for bit.  mask_ws_dev: n * ceil(n/64) uint64. */
 int syn_nms(const float* dets_dev, int n, double thresh, int mode, uint64_t* mask_ws_dev, int32_t* keep_dev, int32_t* n_keep_dev,
             void* stream);
+/* The same greedy loop (FaceBoxes.py:122-127) for n_frames frames in two launches, with no host round trip after the
+ * decode: dets_dev (n_frames, rows_per_frame, 5), frame f's first min(n_dev[f], rows_per_frame) rows are its boxes
+ * (n_dev: the device counts syn_faceboxes_decode_batch wrote).  keep_dev (n_frames, rows_per_frame) int32 and n_keep_dev
+ * (n_frames) receive every frame's list and count, each what syn_nms returns for that frame alone (a frame with no box:
+ * count 0).  mask_ws_dev: n_frames * rows_per_frame * ceil(rows_per_frame/64) uint64.  n_frames <= SYN_FB_MAX_FRAMES. */
+int syn_nms_batch(const float* dets_dev, const int32_t* n_dev, int n_frames, int rows_per_frame, double thresh, int mode,
+                  uint64_t* mask_ws_dev, int32_t* keep_dev, int32_t* n_keep_dev, void* stream);
 /* Number of prior boxes for an im_height x im_width network input (utils/prior_box.py:19-43); -1 on bad sizes. */
 int syn_faceboxes_num_priors(int im_height, int im_width);
 /* FaceBoxes.__call__ between the network and the NMS (FaceBoxes/FaceBoxes.py:98-121): priors, decode
@@ -298,6 +305,13 @@ int syn_faceboxes_num_priors(int im_height, int im_width);
 int syn_faceboxes_decode(const float* loc_dev, const float* conf_dev, int im_height, int im_width, float box_scale_w,
                          float box_scale_h, float scale, float conf_thresh, int top_k, int32_t* cand_ws_dev, float* dets_dev,
                          int32_t* n_dets_dev, void* stream);
+/* FaceBoxes.py:98-121 for n_frames network inputs of one size in two launches: loc_dev (n_frames,P,4), conf_dev
+ * (n_frames,P,2) as syn_fb_forward_batch writes them.  Every frame has its own candidates, its own ranking (same tie
+ * rule), its own (top_k,5) block of dets_dev (n_frames,top_k,5) and its own count in n_dets_dev (n_frames).
+ * cand_ws_dev: n_frames * (P+1) int32.  n_frames <= SYN_FB_MAX_FRAMES. */
+int syn_faceboxes_decode_batch(const float* loc_dev, const float* conf_dev, int n_frames, int im_height, int im_width,
+                               float box_scale_w, float box_scale_h, float scale, float conf_thresh, int top_k, int32_t* cand_ws_dev,
+                               float* dets_dev, int32_t* n_dets_dev, void* stream);
 
 /* ---- crop + resize of uint8 BGR images (crop_img + cv2.resize) ---------------------------------------------------------
  * The face crops of get_all_outputs (utils/inference.py:95-125 crop_img, then cv2.resize to 120x120: INTER_LANCZOS4 in
@@ -322,8 +336,19 @@ int syn_crop_resize_plan_host(const int32_t* rois_host, int batch, int out_h, in
 int syn_crop_resize(const uint8_t* image_dev, int height, int width, int channels, const void* plan_dev, int batch, int out_h,
                     int out_w, int mode, uint8_t* out_dev, int64_t stride_roi, int64_t stride_y, int64_t stride_x, int64_t stride_c,
                     void* stream);
+/* The same stage for a stack of equally sized frames in ONE launch: the crops of every face of every frame
+ * (synergy3DMM.py:186-188 once per face per image), or the detector's shrink of every frame (FaceBoxes.py:62-79; ROI =
+ * the whole frame, interleaved output).  The planner also takes frames_host (B): ROI b is cut out of frame
+ * frames_host[b] of n_frames (outside 0..n_frames-1: SYN_ERR_SHAPE); the plan has syn_crop_resize_plan_size bytes and
+ * the same tables.  images_dev (n_frames,height,width,3).  Output bytes are those of syn_crop_resize on each frame. */
+int syn_crop_resize_plan_frames_host(const int32_t* rois_host, const int32_t* frames_host, int n_frames, int batch, int out_h,
+                                     int out_w, int mode, void* plan_out, int64_t plan_bytes);
+int syn_crop_resize_batch(const uint8_t* images_dev, int n_frames, int height, int width, int channels, const void* plan_dev,
+                          int batch, int out_h, int out_w, int mode, uint8_t* out_dev, int64_t stride_roi, int64_t stride_y,
+                          int64_t stride_x, int64_t stride_c, void* stream);
 
-/* The detector network (FaceBoxes/models/faceboxes.py:68-150, FaceBoxesNet in 'test' phase) on ONE image of any size.
+/* The detector network (FaceBoxes/models/faceboxes.py:68-150, FaceBoxesNet in 'test' phase) on ONE image of any size
+ * (syn_fb_forward), or on a stack of frames of one size (syn_fb_forward_batch).
  * A separate handle: the detector has its own weights and workspace and does not touch syn_handle_t.  Like syn_handle_t
  * it is bound to one device and is not re-entrant (its activation workspace is shared by consecutive calls, which are
  * ordered by the stream they are enqueued on; a change of image size synchronises the device and reallocates).
@@ -348,6 +373,15 @@ int  syn_fb_commit(syn_fb_t* f);
  * `self.net(img)` returns, P = syn_faceboxes_num_priors(height, width); feed them to syn_faceboxes_decode + syn_nms. */
 int  syn_fb_forward(syn_fb_t* f, const uint8_t* image_dev, int height, int width, float* loc_dev, float* conf_dev, void* stream);
 int64_t syn_fb_launch_count(const syn_fb_t* f);
+/* FaceBoxes.__call__ lines 88-96 for n_frames images of one size in the SAME 39 launches (syn_fb_launch_count grows by 39
+ * whatever n_frames is): images_dev (n_frames,height,width,3) uint8 BGR -> loc_dev (n_frames,P,4), conf_dev
+ * (n_frames,P,2).  Rows of every convolution's implicit GEMM run over frame * pixels + pixel; each output element is
+ * computed by the one-image kernel's arithmetic in its order, so frame i's outputs are, bit for bit, syn_fb_forward's for
+ * image i.  The workspace grows to n_frames times the one-image maps (15.5 MB per 720 x 1080 frame, so about 1 GB at
+ * SYN_FB_MAX_FRAMES); more frames per call are SYN_ERR_INVALID, callers split the stack. */
+#define SYN_FB_MAX_FRAMES 64
+int  syn_fb_forward_batch(syn_fb_t* f, const uint8_t* images_dev, int n_frames, int height, int width, float* loc_dev,
+                          float* conf_dev, void* stream);
 /* Per-stage tests of the detector network.  Runs syn_fb_forward's launch sequence unchanged and returns right after launch
  * `stage` (0..38), having copied (on the stream) the whole tensor that launch wrote to out_dev, which holds out_numel
  * floats (SYN_ERR_SHAPE if that is not the tensor's size).  NHWC maps of an h x w image, n3/n4/n5 = the pixels of the
@@ -362,6 +396,10 @@ int64_t syn_fb_launch_count(const syn_fb_t* f);
  * The block input is stage 3 for inception1 and the previous block's stage 11 + 8b otherwise. */
 int  syn_fb_debug_forward_until(syn_fb_t* f, const uint8_t* image_dev, int height, int width, int stage, float* out_dev,
                                 int64_t out_numel, float* loc_dev, float* conf_dev, void* stream);
+/* syn_fb_forward_batch stopped after launch `stage` of the same table: out_dev receives the (n_frames,h,w,c) stack of that
+ * launch's maps, or the whole (n_frames,P*4) loc / (n_frames,P*2) conf for stages 32..38. */
+int  syn_fb_debug_forward_batch_until(syn_fb_t* f, const uint8_t* images_dev, int n_frames, int height, int width, int stage,
+                                      float* out_dev, int64_t out_numel, float* loc_dev, float* conf_dev, void* stream);
 
 /* ---- introspection ---------------------------------------------------------------------------*/
 /* Number of kernels this handle has launched since creation (bench.py "gpu_launches"). */

@@ -1,0 +1,36 @@
+#!/usr/bin/env python
+"""The frame-batch path for `compute-sanitizer --tool memcheck` (needs an H100): one batched detector pass on frames whose
+maps make 64-row tiles straddle frames, one ``detect_batch`` with the device shrink, one ``get_all_outputs_batch`` with
+ROIs over the frame edges and a frame without a face.  scripts/sanitizer_smoke.py covers the one-image kernels."""
+import os
+import sys
+import types
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from oracle import synth_model  # noqa: E402
+from synergynet_b200 import faceboxes, model_building, synthetic  # noqa: E402
+from synergynet_b200.params import ParamsPack, set_param_pack  # noqa: E402
+
+
+def main():
+    set_param_pack(ParamsPack(arrays=synthetic.make_3dmm(seed=0)))
+    det = faceboxes.FaceBoxes(weights=synthetic.make_faceboxes_state_dict(0), device='cuda:0')
+    frames = np.stack([synthetic.make_scene_u8(193, 258, s) for s in range(3)])
+    loc, conf = det.net.forward_batch(torch.from_numpy(frames).cuda())
+    boxes = det.detect_batch(frames)
+    big = det.detect_batch(np.stack([synthetic.make_scene_u8(750, 1100, s) for s in range(2)]))     # shrunk on the device
+    m = model_building.SynergyNet(types.SimpleNamespace(arch='mobilenet_v2', img_size=120, devices_id=[0]))
+    m.load_state_dict(synth_model.build_state_dict(0), strict=True)
+    m.eval()
+    rects = [[[-10.0, -5.0, 50.0, 55.0, 0.9], [150.0, 120.0, 300.0, 230.0, 0.8]], [], [[40.0, 20.0, 100.0, 80.0, 0.7]]]
+    out = m.get_all_outputs_batch(frames, rects=rects)
+    torch.cuda.synchronize()
+    m._engine(torch.device('cuda', 0)).raise_if_error()
+    print('sanitizer frames done:', tuple(loc.shape), [len(b) for b in boxes], [len(b) for b in big], [len(t[0]) for t in out])
+
+
+if __name__ == '__main__':
+    main()

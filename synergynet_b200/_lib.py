@@ -43,6 +43,7 @@ class FbLayerDesc(C.Structure):
 
 
 NMS_CPU_NMS, NMS_PY_CPU_NMS = 0, 1
+FB_MAX_FRAMES = 64            # SYN_FB_MAX_FRAMES: frames per batched detector call
 
 _P, _F, _I, _L = C.c_void_p, C.c_void_p, C.c_int, C.c_int64
 # name -> (restype, argtypes); float*/void* travel as integer addresses (tensor.data_ptr()).
@@ -118,6 +119,12 @@ SIGNATURES = {
     'syn_fb_launch_count': (_L, [_P]),
     'syn_fb_debug_forward_until': (_I, [_P, _F, _I, _I, _I, _F, _L, _F, _F, _P]),
     'syn_faceboxes_decode': (_I, [_F, _F, _I, _I, C.c_float, C.c_float, C.c_float, C.c_float, _I, _F, _F, _F, _P]),
+    'syn_fb_forward_batch': (_I, [_P, _F, _I, _I, _I, _F, _F, _P]),
+    'syn_fb_debug_forward_batch_until': (_I, [_P, _F, _I, _I, _I, _I, _F, _L, _F, _F, _P]),
+    'syn_faceboxes_decode_batch': (_I, [_F, _F, _I, _I, _I, C.c_float, C.c_float, C.c_float, C.c_float, _I, _F, _F, _F, _P]),
+    'syn_nms_batch': (_I, [_F, _F, _I, _I, C.c_double, _I, _F, _F, _F, _P]),
+    'syn_crop_resize_plan_frames_host': (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _L]),
+    'syn_crop_resize_batch': (_I, [_P, _I, _I, _I, _I, _P, _I, _I, _I, _I, _P, _L, _L, _L, _L, _P]),
     'syn_launch_count': (_L, [_P]),
     'syn_set_timing': (_I, [_P, _I]),
     'syn_get_timings': (_I, [_P, C.POINTER(C.c_float), C.POINTER(C.c_char_p), _I, C.POINTER(C.c_int)]),
@@ -142,7 +149,9 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_crop_resize_plan_size', 'syn_crop_resize_plan_host', 'syn_crop_resize',
                                              'syn_faceboxes_num_priors', 'syn_faceboxes_decode', 'syn_fb_num_layers', 'syn_fb_layer_desc', 'syn_fb_create',
                                              'syn_fb_destroy', 'syn_fb_set_layer', 'syn_fb_commit', 'syn_fb_forward', 'syn_fb_launch_count',
-                                             'syn_fb_debug_forward_until')}
+                                             'syn_fb_debug_forward_until', 'syn_fb_forward_batch', 'syn_fb_debug_forward_batch_until',
+                                             'syn_faceboxes_decode_batch', 'syn_nms_batch', 'syn_crop_resize_plan_frames_host',
+                                             'syn_crop_resize_batch')}
 
 
 def declared_symbols(header: str = HEADER_PATH):

@@ -42,17 +42,25 @@ __device__ inline void prior_of(int idx, int h, int w, float* p) {
   p[3] = (float)(ms / (double)h);
 }
 
-// cand[0] = number of priors whose face score conf[:, 1] exceeds the threshold (FaceBoxes.py:112), cand[1..] = their indices
+// cand[0] = number of priors whose face score conf[:, 1] exceeds the threshold (FaceBoxes.py:112), cand[1..] = their indices.
+// Frame axis (syn_faceboxes_decode_batch): grid.y = frame, every frame with its own (np,2) scores and np + 1 candidate slots.
 __global__ void faceboxes_select_kernel(const float* __restrict__ conf, int np, float thresh, int32_t* __restrict__ cand) {
+  conf += (size_t)blockIdx.y * np * 2;
+  cand += (size_t)blockIdx.y * (np + 1);
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < np && conf[2 * i + 1] > thresh) cand[1 + atomicAdd(cand, 1)] = i;
 }
 
 // Rank of every candidate in descending score order (ties: the higher prior index first = a stable ascending argsort
 // read backwards, :117), the first top_k decoded and written in that order as rows [x1 y1 x2 y2 score] (:121).
+// Frame axis: grid.y = frame, which ranks its own candidates into its own (top_k,5) block of dets and its own count.
 __global__ void faceboxes_rank_decode_kernel(const float* __restrict__ loc, const float* __restrict__ conf, int h, int w,
                                              float box_scale_w, float box_scale_h, float scale, int top_k,
                                              const int32_t* __restrict__ cand, float* __restrict__ dets, int32_t* __restrict__ n_dets) {
+  {
+    const size_t fr = blockIdx.y, np = faceboxes_num_priors(h, w);
+    loc += fr * np * 4; conf += fr * np * 2; cand += fr * (np + 1); dets += fr * top_k * 5; n_dets += fr;
+  }
   const int n = cand[0];
   if (blockIdx.x == 0 && threadIdx.x == 0) *n_dets = min(n, top_k);
   if ((int)(blockIdx.x * blockDim.x) >= n) return;                       // whole CTA: the grid is sized for every prior
@@ -98,7 +106,7 @@ __global__ void faceboxes_rank_decode_kernel(const float* __restrict__ loc, cons
 }  // namespace syn
 
 // ---- the detector network (FaceBoxes/models/faceboxes.py:8-150) -------------------------------------------------------
-// 33 small convolutions on one image of arbitrary size (0.7 GMAC at 720 x 1080).  A first, plain H100 path: fp32 FMA on
+// 33 small convolutions on one image of arbitrary size (0.7 GMAC at 720 x 1080), or on a stack of equally sized frames.  A first, plain H100 path: fp32 FMA on
 // CUDA cores as a shared-memory-tiled implicit GEMM (M = output pixels, N = output channels, K = kh*kw*cin), BatchNorm
 // folded into weights and bias on the host in float64, activation and the channel concatenations fused into the store
 // (every layer writes its slice of the NHWC tensor the next layer reads).  NHWC is also how the image arrives (H,W,3
@@ -116,19 +124,37 @@ struct FbConvArgs {
   int k, stride, pad;
   int act;                 // 0 linear, 1 ReLU, 2 CReLU: channel c gets relu(v), channel c + cout gets relu(-v)  (faceboxes.py:60-64)
   float mean[3];
+  // frame axis (FRAMES instantiations only): `frames` maps of the same geometry, x / x_u8 and y advance by x_fs / y_fs
+  // elements per frame (y_fs is the whole (P,4) / (P,2) row block for the heads, which write one slice of it)
+  int frames;
+  long long x_fs, y_fs;
 };
 
 constexpr int FB_BM = 64, FB_BN = 64, FB_BK = 16;
 
-// One input value of the implicit GEMM: element `kidx` = (kh, kw, ci) of output pixel m's patch (0 outside the image)
-__device__ __forceinline__ float fb_gather1(const FbConvArgs& a, int kidx, int m, int K, int M) {
-  if (kidx >= K || m >= M) return 0.f;
+// Row m of the implicit GEMM -> (frame, output pixel of that frame).  FRAMES: m = frame * M + pixel, so a 64-row tile may
+// hold the last pixels of one frame and the first of the next; each row gathers, pads and stores against its OWN frame.
+// One image: frame 0, pixel m, and every offset below folds to the one-image expression.
+template <bool FRAMES>
+__device__ __forceinline__ void fb_row(int m, int M, int& fr, int& pix) {
+  if (FRAMES) { fr = m / M; pix = m - fr * M; }
+  else { fr = 0; pix = m; }
+}
+
+// One input value of the implicit GEMM: element `kidx` = (kh, kw, ci) of output row m's patch (0 outside its frame);
+// MT = rows of the GEMM (M, or frames * M)
+template <bool FRAMES>
+__device__ __forceinline__ float fb_gather1(const FbConvArgs& a, int kidx, int m, int K, int M, int MT) {
+  if (kidx >= K || m >= MT) return 0.f;
+  int fr, pix;
+  fb_row<FRAMES>(m, M, fr, pix);
   const int ci = kidx % a.cin, t = kidx / a.cin, kw = t % a.k, kh = t / a.k;
-  const int oy = m / a.wo, ox = m - oy * a.wo;
+  const int oy = pix / a.wo, ox = pix - oy * a.wo;
   const int iy = oy * a.stride - a.pad + kh, ix = ox * a.stride - a.pad + kw;
   if (iy < 0 || iy >= a.h || ix < 0 || ix >= a.w) return 0.f;
-  if (a.x_u8) return (float)a.x_u8[((size_t)iy * a.w + ix) * 3 + ci] - (ci == 0 ? a.mean[0] : ci == 1 ? a.mean[1] : a.mean[2]);
-  return a.x[((size_t)iy * a.w + ix) * a.cin_stride + a.cin_off + ci];
+  const size_t fo = FRAMES ? (size_t)fr * a.x_fs : 0;
+  if (a.x_u8) return (float)a.x_u8[fo + ((size_t)iy * a.w + ix) * 3 + ci] - (ci == 0 ? a.mean[0] : ci == 1 ? a.mean[1] : a.mean[2]);
+  return a.x[fo + ((size_t)iy * a.w + ix) * a.cin_stride + a.cin_off + ci];
 }
 
 // VEC: cin, cin_stride, cin_off and cout are multiples of 4 (every layer but conv1 and the 42- / 2-channel heads): a
@@ -136,13 +162,15 @@ __device__ __forceinline__ float fb_gather1(const FbConvArgs& a, int kidx, int m
 // one float4 of the B tile per K step instead of four scalars each.  Either way the next step's operands are fetched
 // into registers before the current step's FMAs and stored to shared memory after them, so the global-load latency of
 // the long-K, small-M layers (conv2, the stride-2 3x3s, the heads: 72-144 K steps on a few dozen CTAs) is hidden.
-template <bool VEC>
+// FRAMES (syn_fb_forward_batch) only changes which frame a row addresses: the K order and the fmaf chain of every
+// accumulator are the one-image kernel's, so each output element has the one-image bits.
+template <bool VEC, bool FRAMES>
 __global__ void __launch_bounds__(256) fb_conv_kernel(const FbConvArgs a) {
   __shared__ __align__(16) float sA[FB_BK][FB_BM + 4];
   __shared__ __align__(16) float sB[FB_BK][FB_BN + 4];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;            // thread = 4 pixels (ty) x 4 channels (tx)
   const int m0 = blockIdx.x * FB_BM, n0 = blockIdx.y * FB_BN;
-  const int M = a.ho * a.wo, K = a.k * a.k * a.cin;
+  const int M = a.ho * a.wo, K = a.k * a.k * a.cin, MT = FRAMES ? M * a.frames : M;
   float acc[4][4];
 #pragma unroll
   for (int i = 0; i < 4; ++i)
@@ -153,16 +181,22 @@ __global__ void __launch_bounds__(256) fb_conv_kernel(const FbConvArgs a) {
   //              B -- K row tid / 16, channel quad tid % 16
   const int a_mm = tid >> 2, a_kq = tid & 3, b_kk = tid >> 4, b_nq = tid & 15;
   int v_oy = 0, v_ox = 0;
-  if (VEC) { const int m = m0 + a_mm; v_oy = m / a.wo; v_ox = m - v_oy * a.wo; }
+  const float* v_x = a.x;
+  if (VEC) {
+    int fr, pix;
+    fb_row<FRAMES>(m0 + a_mm, M, fr, pix);
+    v_oy = pix / a.wo; v_ox = pix - v_oy * a.wo;
+    if (FRAMES) v_x += (size_t)fr * a.x_fs;
+  }
   auto fetch = [&](int k0) {
     if (VEC) {
       float4 va = make_float4(0.f, 0.f, 0.f, 0.f), vb = make_float4(0.f, 0.f, 0.f, 0.f);
       const int kidx = k0 + a_kq * 4;
-      if (kidx < K && m0 + a_mm < M) {
+      if (kidx < K && m0 + a_mm < MT) {
         const int ci = kidx % a.cin, t = kidx / a.cin, kw = t % a.k, kh = t / a.k;
         const int iy = v_oy * a.stride - a.pad + kh, ix = v_ox * a.stride - a.pad + kw;
         if (iy >= 0 && iy < a.h && ix >= 0 && ix < a.w)
-          va = __ldg(reinterpret_cast<const float4*>(a.x + ((size_t)iy * a.w + ix) * a.cin_stride + a.cin_off + ci));
+          va = __ldg(reinterpret_cast<const float4*>(v_x + ((size_t)iy * a.w + ix) * a.cin_stride + a.cin_off + ci));
       }
       const int kb = k0 + b_kk, n = n0 + b_nq * 4;
       if (kb < K && n < a.cout) vb = __ldg(reinterpret_cast<const float4*>(a.wk + (size_t)kb * a.cout + n));
@@ -172,7 +206,7 @@ __global__ void __launch_bounds__(256) fb_conv_kernel(const FbConvArgs a) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int e = tid + j * 256, kk = e / FB_BM, mm = e - kk * FB_BM;
-        ra[j] = fb_gather1(a, k0 + kk, m0 + mm, K, M);
+        ra[j] = fb_gather1<FRAMES>(a, k0 + kk, m0 + mm, K, M, MT);
         const int kb = k0 + e / FB_BN, n = n0 + e % FB_BN;
         rb[j] = (kb < K && n < a.cout) ? a.wk[(size_t)kb * a.cout + n] : 0.f;
       }
@@ -217,8 +251,10 @@ __global__ void __launch_bounds__(256) fb_conv_kernel(const FbConvArgs a) {
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int m = m0 + ty * 4 + i;
-    if (m >= M) continue;
-    float* o = a.y + (size_t)m * a.cout_stride + a.cout_off;
+    if (m >= MT) continue;
+    int fr, pix;
+    fb_row<FRAMES>(m, M, fr, pix);
+    float* o = a.y + (FRAMES ? (size_t)fr * a.y_fs : 0) + (size_t)pix * a.cout_stride + a.cout_off;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int n = n0 + tx * 4 + j;
@@ -234,16 +270,18 @@ __global__ void __launch_bounds__(256) fb_conv_kernel(const FbConvArgs a) {
 // Layers with at most 8 output channels and a long K (the 4- / 2-channel heads on the stride-64 / -128 maps: K = 2304,
 // 204 or 54 pixels): a 64 x 64 tile would run 144 serial K steps on one or two CTAs.  Here a CTA of 128 threads owns ONE
 // output pixel, the threads stride over K and the partial sums meet in a warp-shuffle + shared-memory reduction.
+// FRAMES: blockIdx.x = frame * M + pixel; the K stride and the reduction tree are unchanged.
 constexpr int FB_SMALLN = 8;
+template <bool FRAMES>
 __global__ void __launch_bounds__(128) fb_conv_smalln_kernel(const FbConvArgs a) {
   __shared__ float red[4][FB_SMALLN];
   const int m = blockIdx.x, tid = threadIdx.x;
-  const int M = a.ho * a.wo, K = a.k * a.k * a.cin;
+  const int M = a.ho * a.wo, K = a.k * a.k * a.cin, MT = FRAMES ? M * a.frames : M;
   float acc[FB_SMALLN];
 #pragma unroll
   for (int n = 0; n < FB_SMALLN; ++n) acc[n] = 0.f;
   for (int k = tid; k < K; k += 128) {
-    const float v = fb_gather1(a, k, m, K, M);
+    const float v = fb_gather1<FRAMES>(a, k, m, K, M, MT);
     const float* wr = a.wk + (size_t)k * a.cout;
 #pragma unroll
     for (int n = 0; n < FB_SMALLN; ++n)
@@ -258,17 +296,21 @@ __global__ void __launch_bounds__(128) fb_conv_smalln_kernel(const FbConvArgs a)
   __syncthreads();
   if (tid < a.cout) {
     const float v = ((red[0][tid] + red[1][tid]) + (red[2][tid] + red[3][tid])) + a.bias[tid];
-    float* o = a.y + (size_t)m * a.cout_stride + a.cout_off;
+    int fr, pix;
+    fb_row<FRAMES>(m, M, fr, pix);
+    float* o = a.y + (FRAMES ? (size_t)fr * a.y_fs : 0) + (size_t)pix * a.cout_stride + a.cout_off;
     if (a.act == 0) o[tid] = v;
     else if (a.act == 1) o[tid] = fmaxf(v, 0.f);
     else { o[tid] = fmaxf(v, 0.f); o[tid + a.cout] = fmaxf(-v, 0.f); }
   }
 }
 
-// F.max_pool2d(x, 3, stride 2, padding 1) (faceboxes.py:121,123), NHWC
+// F.max_pool2d(x, 3, stride 2, padding 1) (faceboxes.py:121,123), NHWC; grid.y = frame of the contiguous (N,h,w,c) stack
 __global__ void fb_maxpool_kernel(const float* __restrict__ x, int h, int w, int c, float* __restrict__ y, int ho, int wo) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)ho * wo * c) return;
+  x += (size_t)blockIdx.y * h * w * c;
+  y += (size_t)blockIdx.y * ho * wo * c;
   const int ch = (int)(i % c), ox = (int)((i / c) % wo), oy = (int)(i / ((size_t)c * wo));
   float m = -INFINITY;
   for (int dy = 0; dy < 3; ++dy)
@@ -279,10 +321,13 @@ __global__ void fb_maxpool_kernel(const float* __restrict__ x, int h, int w, int
   y[i] = m;
 }
 
-// F.avg_pool2d(x, 3, stride 1, padding 1) (faceboxes.py:37): count_include_pad defaults to True, the divisor is always 9
+// F.avg_pool2d(x, 3, stride 1, padding 1) (faceboxes.py:37): count_include_pad defaults to True, the divisor is always 9;
+// grid.y = frame of the contiguous (N,h,w,c) stack
 __global__ void fb_avgpool_kernel(const float* __restrict__ x, int h, int w, int c, float* __restrict__ y) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)h * w * c) return;
+  x += (size_t)blockIdx.y * h * w * c;
+  y += (size_t)blockIdx.y * h * w * c;
   const int ch = (int)(i % c), ox = (int)((i / c) % w), oy = (int)(i / ((size_t)c * w));
   float s = 0.f;
   for (int dy = -1; dy <= 1; ++dy)
@@ -293,7 +338,7 @@ __global__ void fb_avgpool_kernel(const float* __restrict__ x, int h, int w, int
   y[i] = s / 9.0f;
 }
 
-// nn.Softmax(dim=-1) over the (P, 2) class scores (faceboxes.py:92,143)
+// nn.Softmax(dim=-1) over the (P, 2) class scores (faceboxes.py:92,143); a frame stack is np = N * P rows
 __global__ void fb_softmax2_kernel(float* __restrict__ conf, int np) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= np) return;

@@ -208,7 +208,22 @@ __global__ void raster_resolve_kernel(MeshView m, const int32_t* __restrict__ tr
 // dets (n, 5) fp32 [x1 y1 x2 y2 score], ALREADY in the order the greedy loop visits them (descending score).
 // mask[i][j / 64] bit (j % 64) = box j (> i) is suppressed by box i.  ge != 0: `ovr >= thresh` in double (cpu_nms.pyx:65,
 // thresh is a C double there); ge == 0: py_cpu_nms keeps `ovr <= thresh` in float32, i.e. suppresses on `ovr > thresh`.
-__global__ void nms_mask_kernel(const float* __restrict__ dets, int n, double thresh, int ge, unsigned long long* __restrict__ mask) {
+// Segmented (syn_nms_batch): n_dev != nullptr, grid.z = frame.  Frame f owns rows [f * n, (f + 1) * n) of dets and a mask
+// block sized for n rows, of which its own count n_dev[f] <= n are valid and laid out with ITS OWN word count, so the
+// bits (and the scan below) are those of a one-image call with that count.  The grid is sized for n.
+__device__ __forceinline__ int nms_segment(const int32_t* n_dev, int& n, int fr) {      // -> rows per frame; n = the frame's count
+  const int cap = n;
+  if (n_dev) n = max(0, min(n_dev[fr], cap));
+  return cap;
+}
+
+__global__ void nms_mask_kernel(const float* __restrict__ dets, int n, double thresh, int ge, unsigned long long* __restrict__ mask,
+                                const int32_t* __restrict__ n_dev) {
+  {
+    const int cap = nms_segment(n_dev, n, blockIdx.z);
+    dets += (size_t)blockIdx.z * cap * 5;
+    mask += (size_t)blockIdx.z * cap * ((cap + 63) / 64);
+  }
   const int words = (n + 63) / 64;
   const int i = blockIdx.y * blockDim.y + threadIdx.y, wj = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n || wj >= words) return;
@@ -237,12 +252,20 @@ __global__ void nms_mask_kernel(const float* __restrict__ dets, int n, double th
 //   B  all threads OR the rows of the boxes that survived into `removed` for the words to the right of the block, four
 //      independent loads in flight per thread (a box-by-box scan would pay one dependent L2 round trip per kept box).
 // keep (n) int32 receives the kept indices in visiting order, *n_keep their number: the serial greedy list, exactly.
+// Segmented: one CTA per frame (blockIdx.x), frame f's keep list at keep + f * n and its count at n_keep[f].
 constexpr int kNmsScanThreads = 1024;
 __global__ void __launch_bounds__(kNmsScanThreads) nms_scan_kernel(const unsigned long long* __restrict__ mask, int n,
-                                                                   int32_t* __restrict__ keep, int32_t* __restrict__ n_keep) {
+                                                                   int32_t* __restrict__ keep, int32_t* __restrict__ n_keep,
+                                                                   const int32_t* __restrict__ n_dev) {
   extern __shared__ unsigned long long removed[];          // words entries
   __shared__ int rows[64];
   __shared__ int n_rows, total;
+  {
+    const int cap = nms_segment(n_dev, n, blockIdx.x);
+    mask += (size_t)blockIdx.x * cap * ((cap + 63) / 64);
+    keep += (size_t)blockIdx.x * cap;
+    n_keep += blockIdx.x;
+  }
   const int words = (n + 63) / 64, tid = threadIdx.x, lane = tid & 31;
   for (int wq = tid; wq < words; wq += kNmsScanThreads) removed[wq] = 0ull;
   if (tid == 0) total = 0;

@@ -14,16 +14,18 @@ namespace syn {
 
 constexpr int kResizeBX = 32, kResizeBY = 8;
 
-// out[b*sb + oy*sy + ox*sx + c*sc] (element strides): planar (B,3,h,w) crops or an interleaved (h,w,3) image
+// out[b*sb + oy*sy + ox*sx + c*sc] (element strides): planar (B,3,h,w) crops or an interleaved (h,w,3) image.
+// frames > 0 (syn_crop_resize_batch): img is a stack of `frames` images and ROI b reads the one its plan header names.
 template <int K>
 __global__ void __launch_bounds__(kResizeBX * kResizeBY) crop_resize_kernel(const uint8_t* __restrict__ img, int height, int width,
                                                                             const void* __restrict__ plan, int batch, int out_h,
                                                                             int out_w, uint8_t* __restrict__ out, long long sb,
-                                                                            long long sy, long long sx, long long sc) {
+                                                                            long long sy, long long sx, long long sc, int frames) {
   const int ox = blockIdx.x * kResizeBX + threadIdx.x, oy = blockIdx.y * kResizeBY + threadIdx.y, b = blockIdx.z;
   if (ox >= out_w || oy >= out_h) return;
   const rsz::PlanView v = rsz::plan_view(plan, batch, out_h, out_w, K);
   uint8_t px[3];
+  if (frames > 0) img += (size_t)rsz::clampi(v.hdr[b].frame, 0, frames - 1) * height * width * 3;
   rsz::resize_pixel<K>(img, height, width, v, b, out_h, out_w, oy, ox, px);
   uint8_t* o = out + b * sb + oy * sy + ox * sx;
   o[0] = px[0];

@@ -21,6 +21,49 @@ int check_mesh(const float* v, long long sb, int sv, int sc, int batch, int nver
   return SYN_OK;
 }
 
+// the host planner of both crop entries; frames_host == nullptr: one image
+int crop_plan(const int32_t* rois_host, const int32_t* frames_host, int n_frames, int batch, int out_h, int out_w, int mode,
+              void* plan_out, int64_t plan_bytes, const char* who) {
+  if (!rois_host || !plan_out || batch <= 0) return fail(SYN_ERR_INVALID, "%s: null pointer or empty batch", who);
+  if (out_h < 1 || out_w < 1) return fail(SYN_ERR_INVALID, "%s: output size %dx%d", who, out_h, out_w);
+  if (mode != SYN_INTER_LINEAR && mode != SYN_INTER_LANCZOS4)
+    return fail(SYN_ERR_UNSUPPORTED, "%s: interpolation %d (only INTER_LINEAR = 1 and INTER_LANCZOS4 = 4)", who, mode);
+  for (int b = 0; b < batch; ++b) {
+    const int32_t* r = rois_host + 4 * b;
+    if (r[2] <= r[0] || r[3] <= r[1])        // crop_img would return an empty array, which cv2.resize rejects
+      return fail(SYN_ERR_SHAPE, "%s: ROI %d (%d,%d,%d,%d) is empty", who, b, r[0], r[1], r[2], r[3]);
+    if (frames_host && (frames_host[b] < 0 || frames_host[b] >= n_frames))
+      return fail(SYN_ERR_SHAPE, "%s: ROI %d names frame %d of %d", who, b, frames_host[b], n_frames);
+  }
+  if (plan_bytes < syn_crop_resize_plan_size(batch, out_h, out_w, mode))
+    return fail(SYN_ERR_SHAPE, "%s: plan buffer of %lld bytes, %lld needed", who, (long long)plan_bytes,
+                (long long)syn_crop_resize_plan_size(batch, out_h, out_w, mode));
+  rsz::build_plan(rois_host, batch, out_h, out_w, mode, plan_out, frames_host);
+  return SYN_OK;
+}
+
+// the launch of both crop entries; n_frames == 0: one image, the plan's frame indices are not read
+int crop_launch(const uint8_t* image_dev, int n_frames, int height, int width, int channels, const void* plan_dev, int batch,
+                int out_h, int out_w, int mode, uint8_t* out_dev, int64_t stride_roi, int64_t stride_y, int64_t stride_x,
+                int64_t stride_c, cudaStream_t st, const char* who) {
+  if (!image_dev || !plan_dev || !out_dev || batch <= 0) return fail(SYN_ERR_INVALID, "%s: null pointer or empty batch", who);
+  if (height < 1 || width < 1 || out_h < 1 || out_w < 1)
+    return fail(SYN_ERR_INVALID, "%s: image %dx%d, output %dx%d", who, height, width, out_h, out_w);
+  if (channels != 3) return fail(SYN_ERR_UNSUPPORTED, "%s: %d channels (BGR images only)", who, channels);
+  if (mode != SYN_INTER_LINEAR && mode != SYN_INTER_LANCZOS4)
+    return fail(SYN_ERR_UNSUPPORTED, "%s: interpolation %d (only INTER_LINEAR = 1 and INTER_LANCZOS4 = 4)", who, mode);
+  if (batch > 65535) return fail(SYN_ERR_SHAPE, "%s: %d ROIs exceed one launch's grid", who, batch);
+  const dim3 grid((out_w + kResizeBX - 1) / kResizeBX, (out_h + kResizeBY - 1) / kResizeBY, batch), block(kResizeBX, kResizeBY);
+  if (mode == SYN_INTER_LANCZOS4)
+    crop_resize_kernel<8><<<grid, block, 0, st>>>(image_dev, height, width, plan_dev, batch, out_h, out_w, out_dev, stride_roi,
+                                                  stride_y, stride_x, stride_c, n_frames);
+  else
+    crop_resize_kernel<2><<<grid, block, 0, st>>>(image_dev, height, width, plan_dev, batch, out_h, out_w, out_dev, stride_roi,
+                                                  stride_y, stride_x, stride_c, n_frames);
+  SYN_LAUNCH_CHECK("crop_resize_kernel");
+  return SYN_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -116,11 +159,32 @@ int syn_nms(const float* dets_dev, int n, double thresh, int mode, uint64_t* mas
   const int words = (n + 63) / 64;
   if ((size_t)words * 8 > 200 * 1024) return fail(SYN_ERR_SHAPE, "syn_nms: %d boxes exceed the scan kernel's shared memory", n);
   nms_mask_kernel<<<dim3((words + 31) / 32, (n + 7) / 8), dim3(32, 8), 0, st>>>(dets_dev, n, thresh, mode == SYN_NMS_CPU_NMS ? 1 : 0,
-                                                                               reinterpret_cast<unsigned long long*>(mask_ws_dev));
+                                                                               reinterpret_cast<unsigned long long*>(mask_ws_dev), nullptr);
   SYN_LAUNCH_CHECK("nms_mask_kernel");
   if (words * 8 > 48 * 1024)
     SYN_CUDA(cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, words * 8));
-  nms_scan_kernel<<<1, kNmsScanThreads, words * 8, st>>>(reinterpret_cast<const unsigned long long*>(mask_ws_dev), n, keep_dev, n_keep_dev);
+  nms_scan_kernel<<<1, kNmsScanThreads, words * 8, st>>>(reinterpret_cast<const unsigned long long*>(mask_ws_dev), n, keep_dev, n_keep_dev,
+                                                         nullptr);
+  SYN_LAUNCH_CHECK("nms_scan_kernel");
+  return SYN_OK;
+}
+
+int syn_nms_batch(const float* dets_dev, const int32_t* n_dev, int n_frames, int rows_per_frame, double thresh, int mode,
+                  uint64_t* mask_ws_dev, int32_t* keep_dev, int32_t* n_keep_dev, void* stream) {
+  if (!dets_dev || !n_dev || !mask_ws_dev || !keep_dev || !n_keep_dev || n_frames <= 0 || rows_per_frame <= 0)
+    return fail(SYN_ERR_INVALID, "syn_nms_batch: null pointer, no frame or no row");
+  if (n_frames > SYN_FB_MAX_FRAMES) return fail(SYN_ERR_INVALID, "syn_nms_batch: %d frames, at most %d per call", n_frames, SYN_FB_MAX_FRAMES);
+  if (mode != SYN_NMS_CPU_NMS && mode != SYN_NMS_PY_CPU_NMS) return fail(SYN_ERR_INVALID, "syn_nms_batch: unknown mode %d", mode);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int n = rows_per_frame, words = (n + 63) / 64;
+  if ((size_t)words * 8 > 200 * 1024) return fail(SYN_ERR_SHAPE, "syn_nms_batch: %d boxes exceed the scan kernel's shared memory", n);
+  nms_mask_kernel<<<dim3((words + 31) / 32, (n + 7) / 8, n_frames), dim3(32, 8), 0, st>>>(
+      dets_dev, n, thresh, mode == SYN_NMS_CPU_NMS ? 1 : 0, reinterpret_cast<unsigned long long*>(mask_ws_dev), n_dev);
+  SYN_LAUNCH_CHECK("nms_mask_kernel");
+  if (words * 8 > 48 * 1024)
+    SYN_CUDA(cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, words * 8));
+  nms_scan_kernel<<<n_frames, kNmsScanThreads, words * 8, st>>>(reinterpret_cast<const unsigned long long*>(mask_ws_dev), n, keep_dev,
+                                                                n_keep_dev, n_dev);
   SYN_LAUNCH_CHECK("nms_scan_kernel");
   return SYN_OK;
 }
@@ -132,42 +196,29 @@ int64_t syn_crop_resize_plan_size(int batch, int out_h, int out_w, int mode) {
 
 int syn_crop_resize_plan_host(const int32_t* rois_host, int batch, int out_h, int out_w, int mode, void* plan_out,
                               int64_t plan_bytes) {
-  if (!rois_host || !plan_out || batch <= 0) return fail(SYN_ERR_INVALID, "syn_crop_resize_plan_host: null pointer or empty batch");
-  if (out_h < 1 || out_w < 1) return fail(SYN_ERR_INVALID, "syn_crop_resize_plan_host: output size %dx%d", out_h, out_w);
-  if (mode != SYN_INTER_LINEAR && mode != SYN_INTER_LANCZOS4)
-    return fail(SYN_ERR_UNSUPPORTED, "syn_crop_resize_plan_host: interpolation %d (only INTER_LINEAR = 1 and INTER_LANCZOS4 = 4)", mode);
-  for (int b = 0; b < batch; ++b) {
-    const int32_t* r = rois_host + 4 * b;
-    if (r[2] <= r[0] || r[3] <= r[1])        // crop_img would return an empty array, which cv2.resize rejects
-      return fail(SYN_ERR_SHAPE, "syn_crop_resize_plan_host: ROI %d (%d,%d,%d,%d) is empty", b, r[0], r[1], r[2], r[3]);
-  }
-  if (plan_bytes < syn_crop_resize_plan_size(batch, out_h, out_w, mode))
-    return fail(SYN_ERR_SHAPE, "syn_crop_resize_plan_host: plan buffer of %lld bytes, %lld needed", (long long)plan_bytes,
-                (long long)syn_crop_resize_plan_size(batch, out_h, out_w, mode));
-  rsz::build_plan(rois_host, batch, out_h, out_w, mode, plan_out);
-  return SYN_OK;
+  return crop_plan(rois_host, nullptr, 0, batch, out_h, out_w, mode, plan_out, plan_bytes, "syn_crop_resize_plan_host");
+}
+
+int syn_crop_resize_plan_frames_host(const int32_t* rois_host, const int32_t* frames_host, int n_frames, int batch, int out_h,
+                                     int out_w, int mode, void* plan_out, int64_t plan_bytes) {
+  const char* who = "syn_crop_resize_plan_frames_host";
+  if (!frames_host || n_frames <= 0) return fail(SYN_ERR_INVALID, "%s: null frame list or no frame", who);
+  return crop_plan(rois_host, frames_host, n_frames, batch, out_h, out_w, mode, plan_out, plan_bytes, who);
 }
 
 int syn_crop_resize(const uint8_t* image_dev, int height, int width, int channels, const void* plan_dev, int batch, int out_h,
                     int out_w, int mode, uint8_t* out_dev, int64_t stride_roi, int64_t stride_y, int64_t stride_x, int64_t stride_c,
                     void* stream) {
-  if (!image_dev || !plan_dev || !out_dev || batch <= 0) return fail(SYN_ERR_INVALID, "syn_crop_resize: null pointer or empty batch");
-  if (height < 1 || width < 1 || out_h < 1 || out_w < 1)
-    return fail(SYN_ERR_INVALID, "syn_crop_resize: image %dx%d, output %dx%d", height, width, out_h, out_w);
-  if (channels != 3) return fail(SYN_ERR_UNSUPPORTED, "syn_crop_resize: %d channels (BGR images only)", channels);
-  if (mode != SYN_INTER_LINEAR && mode != SYN_INTER_LANCZOS4)
-    return fail(SYN_ERR_UNSUPPORTED, "syn_crop_resize: interpolation %d (only INTER_LINEAR = 1 and INTER_LANCZOS4 = 4)", mode);
-  if (batch > 65535) return fail(SYN_ERR_SHAPE, "syn_crop_resize: %d ROIs exceed one launch's grid", batch);
-  cudaStream_t st = (cudaStream_t)stream;
-  const dim3 grid((out_w + kResizeBX - 1) / kResizeBX, (out_h + kResizeBY - 1) / kResizeBY, batch), block(kResizeBX, kResizeBY);
-  if (mode == SYN_INTER_LANCZOS4)
-    crop_resize_kernel<8><<<grid, block, 0, st>>>(image_dev, height, width, plan_dev, batch, out_h, out_w, out_dev, stride_roi,
-                                                  stride_y, stride_x, stride_c);
-  else
-    crop_resize_kernel<2><<<grid, block, 0, st>>>(image_dev, height, width, plan_dev, batch, out_h, out_w, out_dev, stride_roi,
-                                                  stride_y, stride_x, stride_c);
-  SYN_LAUNCH_CHECK("crop_resize_kernel");
-  return SYN_OK;
+  return crop_launch(image_dev, 0, height, width, channels, plan_dev, batch, out_h, out_w, mode, out_dev, stride_roi, stride_y,
+                     stride_x, stride_c, (cudaStream_t)stream, "syn_crop_resize");
+}
+
+int syn_crop_resize_batch(const uint8_t* images_dev, int n_frames, int height, int width, int channels, const void* plan_dev,
+                          int batch, int out_h, int out_w, int mode, uint8_t* out_dev, int64_t stride_roi, int64_t stride_y,
+                          int64_t stride_x, int64_t stride_c, void* stream) {
+  if (n_frames <= 0) return fail(SYN_ERR_INVALID, "syn_crop_resize_batch: %d frames", n_frames);
+  return crop_launch(images_dev, n_frames, height, width, channels, plan_dev, batch, out_h, out_w, mode, out_dev, stride_roi,
+                     stride_y, stride_x, stride_c, (cudaStream_t)stream, "syn_crop_resize_batch");
 }
 
 int syn_faceboxes_num_priors(int im_height, int im_width) {
@@ -188,6 +239,27 @@ int syn_faceboxes_decode(const float* loc_dev, const float* conf_dev, int im_hei
   SYN_LAUNCH_CHECK("faceboxes_select_kernel");
   faceboxes_rank_decode_kernel<<<(np + 127) / 128, 128, 0, st>>>(loc_dev, conf_dev, im_height, im_width, box_scale_w, box_scale_h, scale,
                                                                 top_k, cand_ws_dev, dets_dev, n_dets_dev);
+  SYN_LAUNCH_CHECK("faceboxes_rank_decode_kernel");
+  return SYN_OK;
+}
+
+int syn_faceboxes_decode_batch(const float* loc_dev, const float* conf_dev, int n_frames, int im_height, int im_width,
+                               float box_scale_w, float box_scale_h, float scale, float conf_thresh, int top_k, int32_t* cand_ws_dev,
+                               float* dets_dev, int32_t* n_dets_dev, void* stream) {
+  if (!loc_dev || !conf_dev || !cand_ws_dev || !dets_dev || !n_dets_dev || n_frames <= 0 || im_height <= 0 || im_width <= 0 ||
+      top_k <= 0 || !(scale > 0.f))
+    return fail(SYN_ERR_INVALID, "syn_faceboxes_decode_batch: bad argument");
+  if (n_frames > SYN_FB_MAX_FRAMES)
+    return fail(SYN_ERR_INVALID, "syn_faceboxes_decode_batch: %d frames, at most %d per call", n_frames, SYN_FB_MAX_FRAMES);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int np = faceboxes_num_priors(im_height, im_width);
+  SYN_CUDA(cudaMemsetAsync(n_dets_dev, 0, sizeof(int32_t) * n_frames, st));
+  SYN_CUDA(cudaMemset2DAsync(cand_ws_dev, sizeof(int32_t) * (np + 1), 0, sizeof(int32_t), n_frames, st));   // every frame's count
+  faceboxes_select_kernel<<<dim3((np + 255) / 256, n_frames), 256, 0, st>>>(conf_dev, np, conf_thresh, cand_ws_dev);
+  SYN_LAUNCH_CHECK("faceboxes_select_kernel");
+  faceboxes_rank_decode_kernel<<<dim3((np + 127) / 128, n_frames), 128, 0, st>>>(loc_dev, conf_dev, im_height, im_width, box_scale_w,
+                                                                                box_scale_h, scale, top_k, cand_ws_dev, dets_dev,
+                                                                                n_dets_dev);
   SYN_LAUNCH_CHECK("faceboxes_rank_decode_kernel");
   return SYN_OK;
 }
@@ -231,8 +303,8 @@ struct syn_fb {
   float* d_w[33] = {};
   float* d_b[33] = {};
   bool committed = false;
-  // workspace for the current image size
-  int ws_h = 0, ws_w = 0;
+  // workspace for the current image size, ws_frames frames of it
+  int ws_h = 0, ws_w = 0, ws_frames = 0;
   float *c1 = nullptr, *p1 = nullptr, *c2 = nullptr, *xa = nullptr, *xb = nullptr, *avg = nullptr, *r1 = nullptr, *r2 = nullptr,
         *t3 = nullptr, *c31 = nullptr, *c32 = nullptr, *c41 = nullptr, *c42 = nullptr;
   int64_t launches = 0;
@@ -243,7 +315,7 @@ namespace {
 void fb_free_ws(syn_fb* f) {
   float** bufs[] = {&f->c1, &f->p1, &f->c2, &f->xa, &f->xb, &f->avg, &f->r1, &f->r2, &f->t3, &f->c31, &f->c32, &f->c41, &f->c42};
   for (float** q : bufs) { cudaFree(*q); *q = nullptr; }
-  f->ws_h = f->ws_w = 0;
+  f->ws_h = f->ws_w = f->ws_frames = 0;
 }
 
 struct FbGeom { int h1, w1, hp1, wp1, h2, w2, h3, w3, h4, w4, h5, w5; };
@@ -258,15 +330,17 @@ inline FbGeom fb_geom(int h, int w) {
   return g;
 }
 
-int fb_workspace(syn_fb* f, int h, int w) {
-  if (h == f->ws_h && w == f->ws_w) return SYN_OK;
+// nf frames of an h x w input: every buffer is the (nf, h', w', c) stack of its one-image map.  Grown (never shrunk for the
+// same size) with the device idle, like Workspace::ensure of the backbones.
+int fb_workspace(syn_fb* f, int h, int w, int nf) {
+  if (h == f->ws_h && w == f->ws_w && nf <= f->ws_frames) return SYN_OK;
   SYN_CUDA(cudaDeviceSynchronize());
   fb_free_ws(f);
   const FbGeom g = fb_geom(h, w);
-  const size_t n3 = (size_t)g.h3 * g.w3, n4 = (size_t)g.h4 * g.w4, n5 = (size_t)g.h5 * g.w5;
-  SYN_CUDA(cudaMalloc(&f->c1, sizeof(float) * g.h1 * g.w1 * 48));
-  SYN_CUDA(cudaMalloc(&f->p1, sizeof(float) * g.hp1 * g.wp1 * 48));
-  SYN_CUDA(cudaMalloc(&f->c2, sizeof(float) * g.h2 * g.w2 * 128));
+  const size_t n3 = (size_t)nf * g.h3 * g.w3, n4 = (size_t)nf * g.h4 * g.w4, n5 = (size_t)nf * g.h5 * g.w5;
+  SYN_CUDA(cudaMalloc(&f->c1, sizeof(float) * nf * g.h1 * g.w1 * 48));
+  SYN_CUDA(cudaMalloc(&f->p1, sizeof(float) * nf * g.hp1 * g.wp1 * 48));
+  SYN_CUDA(cudaMalloc(&f->c2, sizeof(float) * nf * g.h2 * g.w2 * 128));
   SYN_CUDA(cudaMalloc(&f->xa, sizeof(float) * n3 * 128));
   SYN_CUDA(cudaMalloc(&f->xb, sizeof(float) * n3 * 128));
   SYN_CUDA(cudaMalloc(&f->avg, sizeof(float) * n3 * 128));
@@ -277,12 +351,14 @@ int fb_workspace(syn_fb* f, int h, int w) {
   SYN_CUDA(cudaMalloc(&f->c32, sizeof(float) * n4 * 256));
   SYN_CUDA(cudaMalloc(&f->c41, sizeof(float) * n4 * 128));
   SYN_CUDA(cudaMalloc(&f->c42, sizeof(float) * n5 * 256));
-  f->ws_h = h; f->ws_w = w;
+  f->ws_h = h; f->ws_w = w; f->ws_frames = nf;
   return SYN_OK;
 }
 
+// frames == 0: the one-image kernels.  frames >= 1: their FRAMES instantiations on stacks of `frames` maps; y_fs = floats
+// from one frame's output to the next (0: the dense (frames, ho, wo, cout_stride) stack).
 int fb_conv(syn_fb* f, int idx, const float* x, const uint8_t* x_u8, int h, int w, int cin_stride, int cin_off, float* y,
-            int cout_stride, int cout_off, cudaStream_t st) {
+            int cout_stride, int cout_off, cudaStream_t st, int frames = 0, size_t y_fs = 0) {
   const FbLayer& L = kFbLayers[idx];
   FbConvArgs a;
   a.x = x; a.x_u8 = x_u8; a.wk = f->d_w[idx]; a.bias = f->d_b[idx]; a.y = y;
@@ -291,13 +367,23 @@ int fb_conv(syn_fb* f, int idx, const float* x, const uint8_t* x_u8, int h, int 
   a.cout = L.cout; a.cout_stride = cout_stride; a.cout_off = cout_off;
   a.k = L.k; a.stride = L.stride; a.pad = L.pad; a.act = L.act;
   a.mean[0] = 104.f; a.mean[1] = 117.f; a.mean[2] = 123.f;          // FaceBoxes.py:92
-  const int M = a.ho * a.wo;
+  const int M1 = a.ho * a.wo, M = M1 * (frames ? frames : 1);
+  a.frames = frames;
+  a.x_fs = (long long)h * w * (x_u8 ? 3 : cin_stride);
+  a.y_fs = y_fs ? (long long)y_fs : (long long)M1 * cout_stride;
   const dim3 grid((M + FB_BM - 1) / FB_BM, (L.cout + FB_BN - 1) / FB_BN);
   const bool vec = x_u8 == nullptr && L.cin % 4 == 0 && cin_stride % 4 == 0 && cin_off % 4 == 0 && L.cout % 4 == 0 &&
                    (reinterpret_cast<uintptr_t>(x) & 15) == 0;
-  if (L.cout <= FB_SMALLN && L.k * L.k * L.cin >= 512) fb_conv_smalln_kernel<<<M, 128, 0, st>>>(a);
-  else if (vec) fb_conv_kernel<true><<<grid, 256, 0, st>>>(a);
-  else fb_conv_kernel<false><<<grid, 256, 0, st>>>(a);
+  const bool smalln = L.cout <= FB_SMALLN && L.k * L.k * L.cin >= 512;
+  if (frames) {
+    if (smalln) fb_conv_smalln_kernel<true><<<M, 128, 0, st>>>(a);
+    else if (vec) fb_conv_kernel<true, true><<<grid, 256, 0, st>>>(a);
+    else fb_conv_kernel<false, true><<<grid, 256, 0, st>>>(a);
+  } else {
+    if (smalln) fb_conv_smalln_kernel<false><<<M, 128, 0, st>>>(a);
+    else if (vec) fb_conv_kernel<true, false><<<grid, 256, 0, st>>>(a);
+    else fb_conv_kernel<false, false><<<grid, 256, 0, st>>>(a);
+  }
   SYN_LAUNCH_CHECK("fb_conv_kernel");
   ++f->launches;
   return SYN_OK;
@@ -325,84 +411,87 @@ int fb_stop_copy(const FbStop* d, const float* src, size_t n, cudaStream_t st) {
   do { if ((d) != nullptr && (d)->stage == (s)) return fb_stop_copy((d), (src), (n), (st)); } while (0)
 
 // syn_fb_forward's launch sequence; `stop` (nullable) ends it early.  Stages are the launches in order, see the table
-// at syn_fb_debug_forward_until in include/synergy_b200.h.
-int fb_forward_body(syn_fb* f, const uint8_t* image_dev, int height, int width, float* loc_dev, float* conf_dev,
+// at syn_fb_debug_forward_until in include/synergy_b200.h.  frames == 0: one image.  frames >= 1 (syn_fb_forward_batch): the
+// same 39 launches, each over the stack of `frames` maps; loc / conf are (frames, P, 4) / (frames, P, 2).
+int fb_forward_body(syn_fb* f, const uint8_t* image_dev, int frames, int height, int width, float* loc_dev, float* conf_dev,
                     cudaStream_t st, const FbStop* stop, const char* who) {
   if (!f || !image_dev || !loc_dev || !conf_dev || height <= 0 || width <= 0) return fail(SYN_ERR_INVALID, "%s: bad argument", who);
+  if (frames < 0 || frames > SYN_FB_MAX_FRAMES) return fail(SYN_ERR_INVALID, "%s: %d frames, 1..%d per call", who, frames, SYN_FB_MAX_FRAMES);
   if (!f->committed) return fail(SYN_ERR_STATE, "%s before syn_fb_commit", who);
   SYN_CUDA(cudaSetDevice(f->device));
-  if (int rc = fb_workspace(f, height, width)) return rc;
+  const int nf = frames ? frames : 1;
+  if (int rc = fb_workspace(f, height, width, nf)) return rc;
   const FbGeom g = fb_geom(height, width);
   if (g.h3 != fb_cells(height, 32) || g.w3 != fb_cells(width, 32) || g.h4 != fb_cells(height, 64) || g.w4 != fb_cells(width, 64) ||
       g.h5 != fb_cells(height, 128) || g.w5 != fb_cells(width, 128))
     return fail(SYN_ERR_SHAPE, "%s: feature maps of a %dx%d input do not match the prior grid", who, height, width);
-  auto pool_grid = [](size_t n) { return (unsigned)((n + 255) / 256); };
+  auto pool_grid = [nf](size_t n) { return dim3((unsigned)((n + 255) / 256), nf); };
   const size_t n1 = (size_t)g.h1 * g.w1, np1 = (size_t)g.hp1 * g.wp1, n2 = (size_t)g.h2 * g.w2;
   const size_t n3 = (size_t)g.h3 * g.w3, n4 = (size_t)g.h4 * g.w4, n5 = (size_t)g.h5 * g.w5;
   const int np = (int)(n3 * 21 + n4 + n5);
   // conv1 (CReLU) -> max-pool -> conv2 (CReLU) -> max-pool                                          faceboxes.py:120-123
-  if (int rc = fb_conv(f, 0, nullptr, image_dev, height, width, 3, 0, f->c1, 48, 0, st)) return rc;
-  SYN_FB_STOP(stop, 0, f->c1, n1 * 48, st);
+  if (int rc = fb_conv(f, 0, nullptr, image_dev, height, width, 3, 0, f->c1, 48, 0, st, frames)) return rc;
+  SYN_FB_STOP(stop, 0, f->c1, nf * (n1 * 48), st);
   fb_maxpool_kernel<<<pool_grid(np1 * 48), 256, 0, st>>>(f->c1, g.h1, g.w1, 48, f->p1, g.hp1, g.wp1);
   SYN_LAUNCH_CHECK("fb_maxpool_kernel");
   ++f->launches;
-  SYN_FB_STOP(stop, 1, f->p1, np1 * 48, st);
-  if (int rc = fb_conv(f, 1, f->p1, nullptr, g.hp1, g.wp1, 48, 0, f->c2, 128, 0, st)) return rc;
-  SYN_FB_STOP(stop, 2, f->c2, n2 * 128, st);
+  SYN_FB_STOP(stop, 1, f->p1, nf * (np1 * 48), st);
+  if (int rc = fb_conv(f, 1, f->p1, nullptr, g.hp1, g.wp1, 48, 0, f->c2, 128, 0, st, frames)) return rc;
+  SYN_FB_STOP(stop, 2, f->c2, nf * (n2 * 128), st);
   fb_maxpool_kernel<<<pool_grid(n3 * 128), 256, 0, st>>>(f->c2, g.h2, g.w2, 128, f->xa, g.h3, g.w3);
   SYN_LAUNCH_CHECK("fb_maxpool_kernel");
   ++f->launches;
-  SYN_FB_STOP(stop, 3, f->xa, n3 * 128, st);
+  SYN_FB_STOP(stop, 3, f->xa, nf * (n3 * 128), st);
   // three inception blocks: every branch writes its 32-channel slice of the next 128-channel tensor     :124-126, :33-47
   float *x = f->xa, *y = f->xb;
   for (int blk = 0; blk < 3; ++blk) {
     const int L0 = 2 + 7 * blk, s0 = 4 + 8 * blk;
-    if (int rc = fb_conv(f, L0 + 0, x, nullptr, g.h3, g.w3, 128, 0, y, 128, 0, st)) return rc;
-    SYN_FB_STOP(stop, s0 + 0, y, n3 * 128, st);
+    if (int rc = fb_conv(f, L0 + 0, x, nullptr, g.h3, g.w3, 128, 0, y, 128, 0, st, frames)) return rc;
+    SYN_FB_STOP(stop, s0 + 0, y, nf * (n3 * 128), st);
     fb_avgpool_kernel<<<pool_grid(n3 * 128), 256, 0, st>>>(x, g.h3, g.w3, 128, f->avg);
     SYN_LAUNCH_CHECK("fb_avgpool_kernel");
     ++f->launches;
-    SYN_FB_STOP(stop, s0 + 1, f->avg, n3 * 128, st);
-    if (int rc = fb_conv(f, L0 + 1, f->avg, nullptr, g.h3, g.w3, 128, 0, y, 128, 32, st)) return rc;
-    SYN_FB_STOP(stop, s0 + 2, y, n3 * 128, st);
-    if (int rc = fb_conv(f, L0 + 2, x, nullptr, g.h3, g.w3, 128, 0, f->r1, 24, 0, st)) return rc;
-    SYN_FB_STOP(stop, s0 + 3, f->r1, n3 * 24, st);
-    if (int rc = fb_conv(f, L0 + 3, f->r1, nullptr, g.h3, g.w3, 24, 0, y, 128, 64, st)) return rc;
-    SYN_FB_STOP(stop, s0 + 4, y, n3 * 128, st);
-    if (int rc = fb_conv(f, L0 + 4, x, nullptr, g.h3, g.w3, 128, 0, f->r2, 24, 0, st)) return rc;
-    SYN_FB_STOP(stop, s0 + 5, f->r2, n3 * 24, st);
-    if (int rc = fb_conv(f, L0 + 5, f->r2, nullptr, g.h3, g.w3, 24, 0, f->t3, 32, 0, st)) return rc;
-    SYN_FB_STOP(stop, s0 + 6, f->t3, n3 * 32, st);
-    if (int rc = fb_conv(f, L0 + 6, f->t3, nullptr, g.h3, g.w3, 32, 0, y, 128, 96, st)) return rc;
-    SYN_FB_STOP(stop, s0 + 7, y, n3 * 128, st);
+    SYN_FB_STOP(stop, s0 + 1, f->avg, nf * (n3 * 128), st);
+    if (int rc = fb_conv(f, L0 + 1, f->avg, nullptr, g.h3, g.w3, 128, 0, y, 128, 32, st, frames)) return rc;
+    SYN_FB_STOP(stop, s0 + 2, y, nf * (n3 * 128), st);
+    if (int rc = fb_conv(f, L0 + 2, x, nullptr, g.h3, g.w3, 128, 0, f->r1, 24, 0, st, frames)) return rc;
+    SYN_FB_STOP(stop, s0 + 3, f->r1, nf * (n3 * 24), st);
+    if (int rc = fb_conv(f, L0 + 3, f->r1, nullptr, g.h3, g.w3, 24, 0, y, 128, 64, st, frames)) return rc;
+    SYN_FB_STOP(stop, s0 + 4, y, nf * (n3 * 128), st);
+    if (int rc = fb_conv(f, L0 + 4, x, nullptr, g.h3, g.w3, 128, 0, f->r2, 24, 0, st, frames)) return rc;
+    SYN_FB_STOP(stop, s0 + 5, f->r2, nf * (n3 * 24), st);
+    if (int rc = fb_conv(f, L0 + 5, f->r2, nullptr, g.h3, g.w3, 24, 0, f->t3, 32, 0, st, frames)) return rc;
+    SYN_FB_STOP(stop, s0 + 6, f->t3, nf * (n3 * 32), st);
+    if (int rc = fb_conv(f, L0 + 6, f->t3, nullptr, g.h3, g.w3, 32, 0, y, 128, 96, st, frames)) return rc;
+    SYN_FB_STOP(stop, s0 + 7, y, nf * (n3 * 128), st);
     float* t = x; x = y; y = t;
   }
   // x = inception3 output (detection source 0); conv3_x, conv4_x give sources 1 and 2                  :127-135
-  if (int rc = fb_conv(f, 23, x, nullptr, g.h3, g.w3, 128, 0, f->c31, 128, 0, st)) return rc;
-  SYN_FB_STOP(stop, 28, f->c31, n3 * 128, st);
-  if (int rc = fb_conv(f, 24, f->c31, nullptr, g.h3, g.w3, 128, 0, f->c32, 256, 0, st)) return rc;
-  SYN_FB_STOP(stop, 29, f->c32, n4 * 256, st);
-  if (int rc = fb_conv(f, 25, f->c32, nullptr, g.h4, g.w4, 256, 0, f->c41, 128, 0, st)) return rc;
-  SYN_FB_STOP(stop, 30, f->c41, n4 * 128, st);
-  if (int rc = fb_conv(f, 26, f->c41, nullptr, g.h4, g.w4, 128, 0, f->c42, 256, 0, st)) return rc;
-  SYN_FB_STOP(stop, 31, f->c42, n5 * 256, st);
+  if (int rc = fb_conv(f, 23, x, nullptr, g.h3, g.w3, 128, 0, f->c31, 128, 0, st, frames)) return rc;
+  SYN_FB_STOP(stop, 28, f->c31, nf * (n3 * 128), st);
+  if (int rc = fb_conv(f, 24, f->c31, nullptr, g.h3, g.w3, 128, 0, f->c32, 256, 0, st, frames)) return rc;
+  SYN_FB_STOP(stop, 29, f->c32, nf * (n4 * 256), st);
+  if (int rc = fb_conv(f, 25, f->c32, nullptr, g.h4, g.w4, 256, 0, f->c41, 128, 0, st, frames)) return rc;
+  SYN_FB_STOP(stop, 30, f->c41, nf * (n4 * 128), st);
+  if (int rc = fb_conv(f, 26, f->c41, nullptr, g.h4, g.w4, 128, 0, f->c42, 256, 0, st, frames)) return rc;
+  SYN_FB_STOP(stop, 31, f->c42, nf * (n5 * 256), st);
   // heads: NHWC output of each source IS permute(0,2,3,1).view(-1) (:137-142); the three sources are concatenated by offset
-  if (int rc = fb_conv(f, 27, x, nullptr, g.h3, g.w3, 128, 0, loc_dev, 84, 0, st)) return rc;
-  SYN_FB_STOP(stop, 32, loc_dev, (size_t)np * 4, st);
-  if (int rc = fb_conv(f, 28, f->c32, nullptr, g.h4, g.w4, 256, 0, loc_dev + n3 * 84, 4, 0, st)) return rc;
-  SYN_FB_STOP(stop, 33, loc_dev, (size_t)np * 4, st);
-  if (int rc = fb_conv(f, 29, f->c42, nullptr, g.h5, g.w5, 256, 0, loc_dev + n3 * 84 + n4 * 4, 4, 0, st)) return rc;
-  SYN_FB_STOP(stop, 34, loc_dev, (size_t)np * 4, st);
-  if (int rc = fb_conv(f, 30, x, nullptr, g.h3, g.w3, 128, 0, conf_dev, 42, 0, st)) return rc;
-  SYN_FB_STOP(stop, 35, conf_dev, (size_t)np * 2, st);
-  if (int rc = fb_conv(f, 31, f->c32, nullptr, g.h4, g.w4, 256, 0, conf_dev + n3 * 42, 2, 0, st)) return rc;
-  SYN_FB_STOP(stop, 36, conf_dev, (size_t)np * 2, st);
-  if (int rc = fb_conv(f, 32, f->c42, nullptr, g.h5, g.w5, 256, 0, conf_dev + n3 * 42 + n4 * 2, 2, 0, st)) return rc;
-  SYN_FB_STOP(stop, 37, conf_dev, (size_t)np * 2, st);
-  fb_softmax2_kernel<<<(np + 255) / 256, 256, 0, st>>>(conf_dev, np);
+  if (int rc = fb_conv(f, 27, x, nullptr, g.h3, g.w3, 128, 0, loc_dev, 84, 0, st, frames, (size_t)np * 4)) return rc;
+  SYN_FB_STOP(stop, 32, loc_dev, nf * ((size_t)np * 4), st);
+  if (int rc = fb_conv(f, 28, f->c32, nullptr, g.h4, g.w4, 256, 0, loc_dev + n3 * 84, 4, 0, st, frames, (size_t)np * 4)) return rc;
+  SYN_FB_STOP(stop, 33, loc_dev, nf * ((size_t)np * 4), st);
+  if (int rc = fb_conv(f, 29, f->c42, nullptr, g.h5, g.w5, 256, 0, loc_dev + n3 * 84 + n4 * 4, 4, 0, st, frames, (size_t)np * 4)) return rc;
+  SYN_FB_STOP(stop, 34, loc_dev, nf * ((size_t)np * 4), st);
+  if (int rc = fb_conv(f, 30, x, nullptr, g.h3, g.w3, 128, 0, conf_dev, 42, 0, st, frames, (size_t)np * 2)) return rc;
+  SYN_FB_STOP(stop, 35, conf_dev, nf * ((size_t)np * 2), st);
+  if (int rc = fb_conv(f, 31, f->c32, nullptr, g.h4, g.w4, 256, 0, conf_dev + n3 * 42, 2, 0, st, frames, (size_t)np * 2)) return rc;
+  SYN_FB_STOP(stop, 36, conf_dev, nf * ((size_t)np * 2), st);
+  if (int rc = fb_conv(f, 32, f->c42, nullptr, g.h5, g.w5, 256, 0, conf_dev + n3 * 42 + n4 * 2, 2, 0, st, frames, (size_t)np * 2)) return rc;
+  SYN_FB_STOP(stop, 37, conf_dev, nf * ((size_t)np * 2), st);
+  fb_softmax2_kernel<<<(nf * np + 255) / 256, 256, 0, st>>>(conf_dev, nf * np);
   SYN_LAUNCH_CHECK("fb_softmax2_kernel");
   ++f->launches;
-  SYN_FB_STOP(stop, 38, conf_dev, (size_t)np * 2, st);
+  SYN_FB_STOP(stop, 38, conf_dev, nf * ((size_t)np * 2), st);
   return SYN_OK;
 }
 
@@ -491,7 +580,13 @@ int syn_fb_commit(syn_fb_t* f) {
 int64_t syn_fb_launch_count(const syn_fb_t* f) { return f ? f->launches : 0; }
 
 int syn_fb_forward(syn_fb_t* f, const uint8_t* image_dev, int height, int width, float* loc_dev, float* conf_dev, void* stream) {
-  return fb_forward_body(f, image_dev, height, width, loc_dev, conf_dev, (cudaStream_t)stream, nullptr, "syn_fb_forward");
+  return fb_forward_body(f, image_dev, 0, height, width, loc_dev, conf_dev, (cudaStream_t)stream, nullptr, "syn_fb_forward");
+}
+
+int syn_fb_forward_batch(syn_fb_t* f, const uint8_t* images_dev, int n_frames, int height, int width, float* loc_dev, float* conf_dev,
+                         void* stream) {
+  if (n_frames <= 0) return fail(SYN_ERR_INVALID, "syn_fb_forward_batch: %d frames", n_frames);
+  return fb_forward_body(f, images_dev, n_frames, height, width, loc_dev, conf_dev, (cudaStream_t)stream, nullptr, "syn_fb_forward_batch");
 }
 
 int syn_fb_debug_forward_until(syn_fb_t* f, const uint8_t* image_dev, int height, int width, int stage, float* out_dev,
@@ -500,7 +595,17 @@ int syn_fb_debug_forward_until(syn_fb_t* f, const uint8_t* image_dev, int height
     return fail(SYN_ERR_INVALID, "syn_fb_debug_forward_until: stage %d outside 0..%d", stage, kFbStages - 1);
   if (!f || !out_dev) return fail(SYN_ERR_INVALID, "syn_fb_debug_forward_until: null handle or output");
   const FbStop stop{stage, out_dev, out_numel};
-  return fb_forward_body(f, image_dev, height, width, loc_dev, conf_dev, (cudaStream_t)stream, &stop, "syn_fb_debug_forward_until");
+  return fb_forward_body(f, image_dev, 0, height, width, loc_dev, conf_dev, (cudaStream_t)stream, &stop, "syn_fb_debug_forward_until");
+}
+
+int syn_fb_debug_forward_batch_until(syn_fb_t* f, const uint8_t* images_dev, int n_frames, int height, int width, int stage,
+                                     float* out_dev, int64_t out_numel, float* loc_dev, float* conf_dev, void* stream) {
+  const char* who = "syn_fb_debug_forward_batch_until";
+  if (stage < 0 || stage >= kFbStages) return fail(SYN_ERR_INVALID, "%s: stage %d outside 0..%d", who, stage, kFbStages - 1);
+  if (!f || !out_dev) return fail(SYN_ERR_INVALID, "%s: null handle or output", who);
+  if (n_frames <= 0) return fail(SYN_ERR_INVALID, "%s: %d frames", who, n_frames);
+  const FbStop stop{stage, out_dev, out_numel};
+  return fb_forward_body(f, images_dev, n_frames, height, width, loc_dev, conf_dev, (cudaStream_t)stream, &stop, who);
 }
 
 }  // extern "C"

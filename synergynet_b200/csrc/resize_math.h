@@ -44,7 +44,8 @@ enum { kInterLinear = 1, kInterLanczos4 = 4 };          // cv::INTER_LINEAR, cv:
 struct RoiHdr {
   int32_t x0, y0, cw, ch;    // crop origin in the image (may be negative) and crop size
   int32_t area;              // 1: exact 2x shrink on both axes in linear mode (resizeAreaFast_); tables unused
-  int32_t pad[3];
+  int32_t frame;             // image of the stack this ROI reads (syn_crop_resize_batch); 0 in a one-image plan
+  int32_t pad[2];
 };
 
 struct PlanView {
@@ -134,8 +135,9 @@ inline bool exact_halving(int n_w, int n_h, int m_w, int m_h) {
 }
 
 // rois: (B,4) int32 x0, y0, x1, y1 already rounded; every ROI non-empty, sizes >= 1, mode linear / Lanczos4 (the caller
-// validated them).  plan: plan_bytes(batch, out_h, out_w, taps_of(mode)) bytes.
-inline void build_plan(const int32_t* rois, int batch, int out_h, int out_w, int mode, void* plan) {
+// validated them).  plan: plan_bytes(batch, out_h, out_w, taps_of(mode)) bytes.  frames: nullptr (one image), or the
+// frame index of every ROI.
+inline void build_plan(const int32_t* rois, int batch, int out_h, int out_w, int mode, void* plan, const int32_t* frames = nullptr) {
   const int k = taps_of(mode);
   const PlanView v = plan_view(plan, batch, out_h, out_w, k);
   RoiHdr* hdr = const_cast<RoiHdr*>(v.hdr);
@@ -146,7 +148,8 @@ inline void build_plan(const int32_t* rois, int batch, int out_h, int out_w, int
     h.cw = rois[4 * b + 2] - rois[4 * b];
     h.ch = rois[4 * b + 3] - rois[4 * b + 1];
     h.area = (mode == kInterLinear && exact_halving(h.cw, h.ch, out_w, out_h)) ? 1 : 0;
-    h.pad[0] = h.pad[1] = h.pad[2] = 0;
+    h.frame = frames ? frames[b] : 0;
+    h.pad[0] = h.pad[1] = 0;
     build_axis(h.cw, out_w, mode, true, const_cast<int32_t*>(v.xofs) + (size_t)b * out_w, const_cast<int16_t*>(v.xcoef) + (size_t)b * out_w * k);
     build_axis(h.ch, out_h, mode, false, const_cast<int32_t*>(v.yofs) + (size_t)b * out_h, const_cast<int16_t*>(v.ycoef) + (size_t)b * out_h * k);
   }

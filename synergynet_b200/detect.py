@@ -97,6 +97,48 @@ def decode_device(loc: torch.Tensor, conf: torch.Tensor, im_height: int, im_widt
     return dets, n
 
 
+def decode_batch_device(loc: torch.Tensor, conf: torch.Tensor, im_height: int, im_width: int, scale: float = 1.0,
+                        conf_thresh: float = confidence_threshold, k: int = top_k):
+    """:func:`decode_device` for N frames of one size in the same two launches: ``loc`` (N,P,4), ``conf`` (N,P,2) ->
+    ``(dets, n)``: (N,k',5) and (N,) device int32, frame i's block and count being what ``decode_device`` gives for
+    ``loc[i]``, ``conf[i]``.  k' = min(k, P): a frame cannot have more candidates than priors."""
+    lib = _lib.load()
+    p = num_priors(im_height, im_width)
+    if loc.dim() != 3 or conf.dim() != 3 or tuple(loc.shape[1:]) != (p, 4) or tuple(conf.shape) != (loc.shape[0], p, 2) or \
+            loc.shape[0] == 0 or loc.dtype != torch.float32 or conf.dtype != torch.float32 or not loc.is_cuda or conf.device != loc.device:
+        raise ValueError(f'loc / conf must be float32 CUDA tensors (N,{p},4) / (N,{p},2) for {im_height}x{im_width} inputs')
+    loc, conf = loc.contiguous(), conf.contiguous()
+    nf, k = int(loc.shape[0]), min(int(k), p)
+    cand = torch.empty((nf, p + 1), dtype=torch.int32, device=loc.device)
+    dets = torch.zeros((nf, k, 5), dtype=torch.float32, device=loc.device)
+    n = torch.zeros((nf,), dtype=torch.int32, device=loc.device)
+    with torch.cuda.device(loc.device):
+        _lib.check(lib.syn_faceboxes_decode_batch(loc.data_ptr(), conf.data_ptr(), nf, int(im_height), int(im_width), float(im_width),
+                                                  float(im_height), float(scale), float(conf_thresh), k, cand.data_ptr(),
+                                                  dets.data_ptr(), n.data_ptr(), torch.cuda.current_stream(loc.device).cuda_stream))
+    return dets, n
+
+
+def nms_batch_device(dets: torch.Tensor, n: torch.Tensor, thresh: float, mode: int = _lib.NMS_CPU_NMS):
+    """:func:`nms_device` per frame without a host round trip: ``dets`` (N,K,5) in descending score order per frame, ``n``
+    (N,) device int32 counts (``decode_batch_device``'s outputs).  Returns ``(keep (N,K) int32, n_keep (N,) int32)``; the
+    first ``n_keep[i]`` entries of ``keep[i]`` are frame i's kept rows, the rest is not written."""
+    lib = _lib.load()
+    if dets.dtype != torch.float32 or dets.dim() != 3 or dets.shape[2] != 5 or dets.shape[0] == 0 or dets.shape[1] == 0 or \
+            not dets.is_cuda or not dets.is_contiguous():
+        raise ValueError('dets must be a contiguous float32 (N,K,5) CUDA tensor')
+    nf, rows = int(dets.shape[0]), int(dets.shape[1])
+    if n.dtype != torch.int32 or tuple(n.shape) != (nf,) or n.device != dets.device or not n.is_contiguous():
+        raise ValueError(f'n must be the ({nf},) int32 counts on the device of dets')
+    mask = torch.empty((nf * rows * ((rows + 63) // 64),), dtype=torch.int64, device=dets.device)
+    keep = torch.empty((nf, rows), dtype=torch.int32, device=dets.device)
+    n_keep = torch.zeros((nf,), dtype=torch.int32, device=dets.device)
+    with torch.cuda.device(dets.device):
+        _lib.check(lib.syn_nms_batch(dets.data_ptr(), n.data_ptr(), nf, rows, float(thresh), int(mode), mask.data_ptr(),
+                                     keep.data_ptr(), n_keep.data_ptr(), torch.cuda.current_stream(dets.device).cuda_stream))
+    return keep, n_keep
+
+
 def detect_postprocess(loc, conf, im_height: int, im_width: int, scale: float = 1.0):
     """``FaceBoxes.__call__`` after the forward pass (``FaceBoxes/FaceBoxes.py:98-143``): list of
     ``[xmin, ymin, xmax, ymax, score]`` with score above ``vis_thres``, at most ``keep_top_k`` after NMS."""

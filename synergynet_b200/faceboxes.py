@@ -4,7 +4,8 @@ Reference-shaped surface: :class:`FaceBoxes` has the constructor and call signat
 (``FaceBoxes(timer_flag=False)``, ``face_boxes(img_bgr_uint8) -> [[xmin, ymin, xmax, ymax, score], ...]``) and loads the
 reference's checkpoint schema (``FaceBoxes/models/faceboxes.py``: ``conv1.conv.weight``, ``inception2.branch3x3.bn.*``,
 ``loc.0.bias`` ..., optional ``module.`` prefix, ``utils/functions.py:19-43``).  The 33 convolutions, the pools and the
-softmax run in ``libsynergy_b200.so`` (``csrc/kernels_detect.cuh``).  An image above 720 x 1080 is uploaded as it is
+softmax run in ``libsynergy_b200.so`` (``csrc/kernels_detect.cuh``); :meth:`FaceBoxes.detect_batch` runs them on a stack of
+equally sized frames in the same launches, with one host synchronisation for the whole stack.  An image above 720 x 1080 is uploaded as it is
 and shrunk on the device (``inference.crop_resize_device``, ``csrc/kernels_resize.cuh``) to the bytes the reference's
 ``cv2.resize`` makes on the host.  No CPU fallback.
 """
@@ -18,7 +19,7 @@ import numpy as np
 import torch
 
 from . import _lib, detect
-from .inference import INTER_LINEAR, crop_resize_device
+from .inference import INTER_LINEAR, crop_resize_device, crop_resize_frames_device, chunk_ranges, stack_frames_device
 
 # FaceBoxes/FaceBoxes.py:24-25
 scale_flag = True
@@ -122,6 +123,41 @@ class FaceBoxesNet:
                                                             torch.cuda.current_stream(self.device).cuda_stream))
         return out
 
+    def _check_stack(self, images: torch.Tensor):
+        if not isinstance(images, torch.Tensor) or images.dtype != torch.uint8 or images.dim() != 4 or images.shape[3] != 3 or \
+                images.shape[0] == 0 or images.device != self.device or not images.is_contiguous():
+            raise ValueError('images must be a contiguous uint8 (N,H,W,3) tensor with N >= 1 on the detector device')
+        if images.shape[0] > _lib.FB_MAX_FRAMES:
+            raise ValueError(f'{images.shape[0]} frames in one call, at most {_lib.FB_MAX_FRAMES} (FaceBoxes.detect_batch splits a stack)')
+        return int(images.shape[0]), int(images.shape[1]), int(images.shape[2])
+
+    def forward_batch(self, images: torch.Tensor):
+        """:meth:`forward` for a stack of frames in the same 39 launches: ``images`` (N,H,W,3) uint8 BGR on the device ->
+        ``(loc (N,P,4), conf (N,P,2))``; ``loc[i]``, ``conf[i]`` have the bits of ``forward(images[i])``."""
+        n, h, w = self._check_stack(images)
+        p = detect.num_priors(h, w)
+        loc = torch.empty((n, p, 4), dtype=torch.float32, device=self.device)
+        conf = torch.empty((n, p, 2), dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.syn_fb_forward_batch(self._h, images.data_ptr(), n, h, w, loc.data_ptr(), conf.data_ptr(),
+                                                      torch.cuda.current_stream(self.device).cuda_stream))
+        return loc, conf
+
+    def debug_forward_batch_until(self, images: torch.Tensor, stage: int) -> torch.Tensor:
+        """:meth:`debug_forward_until` on :meth:`forward_batch`'s launch sequence: the ``(N, h, w, channels)`` stack of the
+        maps launch ``stage`` wrote, or the ``(N, P*4)`` loc / ``(N, P*2)`` conf for stages 32..38 (NaN where no head has
+        written yet).  Per-stage tests only."""
+        n, h, w = self._check_stack(images)
+        p = detect.num_priors(h, w)
+        loc = torch.full((n, p * 4), float('nan'), dtype=torch.float32, device=self.device)
+        conf = torch.full((n, p * 2), float('nan'), dtype=torch.float32, device=self.device)
+        out = torch.empty((n,) + tuple(debug_stage_shape(stage, h, w)), dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.syn_fb_debug_forward_batch_until(self._h, images.data_ptr(), n, h, w, stage, out.data_ptr(),
+                                                                  out.numel(), loc.data_ptr(), conf.data_ptr(),
+                                                                  torch.cuda.current_stream(self.device).cuda_stream))
+        return out
+
 
 def _conv_out(n: int, k: int, s: int, p: int) -> int:
     return (n + 2 * p - k) // s + 1
@@ -180,3 +216,46 @@ class FaceBoxes:
         keep, n_keep = detect.nms_device(dets, detect.nms_threshold, _lib.NMS_CPU_NMS, n=n_host)
         kept = dets[keep[:int(n_keep.item())].long()][:detect.keep_top_k].cpu().numpy()
         return [[b[0], b[1], b[2], b[3], b[4]] for b in kept if b[4] > detect.vis_thres]
+
+    def detect_batch(self, frames):
+        """``__call__`` for N frames of one size: ``frames`` is a list / (N,H,W,3) array of BGR uint8 images, or the uint8
+        (N,H,W,3) CUDA stack a caller already uploaded.  Returns N box lists, ``detect_batch(frames)[i]`` being exactly
+        ``self(frames[i])`` (the > 720 x 1080 shrink, ``keep_top_k`` and ``vis_thres`` included).
+
+        One upload of the stack; network, decode and NMS run over all frames of a chunk (at most ``_lib.FB_MAX_FRAMES``
+        frames) per launch, the counts going from decode to NMS on the device; the kept boxes and their counts of every
+        chunk come back in one host synchronisation at the end, whatever N is."""
+        stack = stack_frames_device(frames, self.net.device)
+        h, w = int(stack.shape[1]), int(stack.shape[2])
+        scale = 1
+        if scale_flag:                                                                        # FaceBoxes.py:62-79
+            if h > HEIGHT:
+                scale = HEIGHT / h
+            if w * scale > WIDTH:
+                scale *= WIDTH / (w * scale)
+        pending = []
+        for a, b in chunk_ranges(int(stack.shape[0]), _lib.FB_MAX_FRAMES):
+            images = stack[a:b]
+            if scale != 1:                                                                    # cv2.resize, INTER_LINEAR
+                images = crop_resize_frames_device(images, list(range(b - a)), [[0, 0, w, h]] * (b - a),
+                                                   (int(scale * w), int(scale * h)), INTER_LINEAR, planar=False)
+            im_h, im_w = int(images.shape[1]), int(images.shape[2])
+            loc, conf = self.net.forward_batch(images)
+            dets, n = detect.decode_batch_device(loc, conf, im_h, im_w, scale=float(scale))
+            keep, n_keep = detect.nms_batch_device(dets, n, detect.nms_threshold, _lib.NMS_CPU_NMS)
+            # the first keep_top_k kept rows of every frame (entries past a frame's count are unwritten: clamped, never read)
+            idx = keep[:, :detect.keep_top_k].long().clamp_(0, dets.shape[1] - 1)
+            kept = torch.gather(dets, 1, idx[:, :, None].expand(-1, -1, 5))
+            kept_host = torch.empty(kept.shape, dtype=kept.dtype, pin_memory=True)
+            n_host = torch.empty(n_keep.shape, dtype=n_keep.dtype, pin_memory=True)
+            kept_host.copy_(kept, non_blocking=True)
+            n_host.copy_(n_keep, non_blocking=True)
+            pending.append((kept_host, n_host))
+        torch.cuda.current_stream(self.net.device).synchronize()
+        out = []
+        for kept_host, n_host in pending:
+            kept_np, n_np = kept_host.numpy(), n_host.numpy()
+            for i in range(kept_np.shape[0]):
+                rows = kept_np[i, :min(int(n_np[i]), detect.keep_top_k)]
+                out.append([[b[0], b[1], b[2], b[3], b[4]] for b in rows if b[4] > detect.vis_thres])
+        return out

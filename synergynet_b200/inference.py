@@ -39,14 +39,22 @@ def crop_img(img: np.ndarray, roi_box: Sequence[float]) -> np.ndarray:
     return out
 
 
-def resize_plan(rois: np.ndarray, out_h: int, out_w: int, interpolation: int) -> np.ndarray:
-    """Host-built tap tables for ``crop_resize_device`` (``syn_crop_resize_plan_host``): ``rois`` (B,4) int32 x0, y0, x1, y1."""
+def resize_plan(rois: np.ndarray, out_h: int, out_w: int, interpolation: int, frame_index=None, n_frames: int = 0) -> np.ndarray:
+    """Host-built tap tables for ``crop_resize_device`` (``syn_crop_resize_plan_host``): ``rois`` (B,4) int32 x0, y0, x1, y1.
+    With ``frame_index`` (B,), the plan of ``crop_resize_frames_device``: ROI b reads frame ``frame_index[b]`` of ``n_frames``."""
     from . import _lib
     lib = _lib.load()
     rois = np.ascontiguousarray(rois, dtype=np.int32).reshape(-1, 4)
     n = int(lib.syn_crop_resize_plan_size(rois.shape[0], out_h, out_w, interpolation))
     plan = np.zeros(max(n, 1), np.uint8)
-    _lib.check(lib.syn_crop_resize_plan_host(rois.ctypes.data, rois.shape[0], out_h, out_w, interpolation, plan.ctypes.data, n))
+    if frame_index is None:
+        _lib.check(lib.syn_crop_resize_plan_host(rois.ctypes.data, rois.shape[0], out_h, out_w, interpolation, plan.ctypes.data, n))
+    else:
+        fi = np.ascontiguousarray(frame_index, dtype=np.int32).reshape(-1)
+        if fi.shape[0] != rois.shape[0]:
+            raise ValueError(f'{fi.shape[0]} frame indices for {rois.shape[0]} ROIs')
+        _lib.check(lib.syn_crop_resize_plan_frames_host(rois.ctypes.data, fi.ctypes.data, int(n_frames), rois.shape[0], out_h, out_w,
+                                                        interpolation, plan.ctypes.data, n))
     return plan
 
 
@@ -75,6 +83,79 @@ def crop_resize_device(image, roi_boxes: Sequence[Sequence[float]], dsize: Tuple
         _lib.check(_lib.load().syn_crop_resize(image.data_ptr(), image.shape[0], image.shape[1], image.shape[2], plan.data_ptr(), B,
                                                out_h, out_w, interpolation, out.data_ptr(), *strides,
                                                torch.cuda.current_stream(image.device).cuda_stream))
+    return out
+
+
+def crop_resize_frames_device(frames, frame_index: Sequence[int], roi_boxes: Sequence[Sequence[float]],
+                              dsize: Tuple[int, int] = (STD_SIZE, STD_SIZE), interpolation: int = INTER_LINEAR, planar: bool = True):
+    """:func:`crop_resize_device` for a stack of frames in one launch: ``frames`` (N,H,W,3) uint8 CUDA tensor, ROI b is
+    ``roi_boxes[b]`` of frame ``frame_index[b]``.  The bytes are those of ``crop_resize_device(frames[i], ...)`` frame
+    by frame; a frame may contribute any number of ROIs, none included."""
+    import torch
+    from . import _lib
+    if frames.dtype != torch.uint8 or frames.dim() != 4 or not frames.is_cuda or not frames.is_contiguous():
+        raise ValueError('frames must be a contiguous (N,H,W,C) uint8 CUDA tensor')
+    out_w, out_h = int(dsize[0]), int(dsize[1])
+    B = len(roi_boxes)
+    plan = torch.from_numpy(resize_plan(np.array([roi_ints(b) for b in roi_boxes], np.int32), out_h, out_w, interpolation,
+                                        frame_index, int(frames.shape[0]))).to(frames.device)
+    if planar:
+        out = torch.empty((B, 3, out_h, out_w), dtype=torch.uint8, device=frames.device)
+        strides = (3 * out_h * out_w, out_w, 1, out_h * out_w)
+    else:
+        out = torch.empty((B, out_h, out_w, 3), dtype=torch.uint8, device=frames.device)
+        strides = (3 * out_h * out_w, 3 * out_w, 3, 1)
+    with torch.cuda.device(frames.device):
+        _lib.check(_lib.load().syn_crop_resize_batch(frames.data_ptr(), frames.shape[0], frames.shape[1], frames.shape[2],
+                                                     frames.shape[3], plan.data_ptr(), B, out_h, out_w, interpolation,
+                                                     out.data_ptr(), *strides, torch.cuda.current_stream(frames.device).cuda_stream))
+    return out
+
+
+def stack_frames_host(frames) -> np.ndarray:
+    """N equally sized (H,W,3) BGR images (a list, or one (N,H,W,3) array) -> one contiguous uint8 (N,H,W,3) array."""
+    if not (isinstance(frames, np.ndarray) and frames.ndim == 4):
+        frames = [np.asarray(f) for f in frames]
+        if not frames:
+            raise ValueError('no frames: a frame batch needs at least one image')
+        shapes = [tuple(f.shape) for f in frames]
+        if any(sh != shapes[0] for sh in shapes):
+            sizes = ', '.join('x'.join(str(d) for d in sh) for sh in sorted(set(shapes)))
+            raise ValueError(f'the frames of one batch must have one size, got {sizes}; group the frames by size')
+        frames = np.stack(frames)
+    if frames.shape[0] == 0 or frames.shape[3] != 3:
+        raise ValueError(f'frames must be (N,H,W,3) with N >= 1, got {tuple(frames.shape)}')
+    return np.ascontiguousarray(frames, dtype=np.uint8)
+
+
+def stack_frames_device(frames, device):
+    """The frame stack on ``device``: one upload of :func:`stack_frames_host`, or the (N,H,W,3) uint8 CUDA tensor the
+    caller already holds (``get_all_outputs_batch`` hands its stack to the detector this way)."""
+    import torch
+    if isinstance(frames, torch.Tensor):
+        if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3 or frames.shape[0] == 0:
+            raise ValueError(f'a frame stack must be a uint8 (N,H,W,3) tensor with N >= 1, got {frames.dtype} {tuple(frames.shape)}')
+        return frames.to(device).contiguous()
+    return torch.from_numpy(stack_frames_host(frames)).to(device)
+
+
+def chunk_ranges(n: int, limit: int) -> list:
+    """``[(start, stop), ...]`` covering items 0..n-1 in order, at most ``limit`` each (frames per detector call, faces
+    per dense reconstruction)."""
+    if limit < 1:
+        raise ValueError(f'chunk limit {limit}')
+    return [(a, min(a + limit, n)) for a in range(0, n, limit)]
+
+
+def split_by_counts(items: Sequence, counts: Sequence[int]) -> list:
+    """Undo the frame -> faces flattening: ``items`` holds the faces of frame 0, then frame 1, ...; ``counts[i]`` faces
+    belong to frame i (0 for a frame without a face).  Returns one list per frame."""
+    if sum(counts) != len(items):
+        raise ValueError(f'{len(items)} items for counts that sum to {sum(counts)}')
+    out, at = [], 0
+    for c in counts:
+        out.append(list(items[at:at + c]))
+        at += c
     return out
 
 

@@ -18,7 +18,8 @@ import torch.nn as nn
 from . import backbone as mobilenetv2_backbone
 from .backbone import MLP_for, MLP_rev
 from .engine import Engine
-from .inference import INTER_LANCZOS4, INTER_LINEAR, crop_resize_device, roi_affine, square_roi
+from .inference import (INTER_LANCZOS4, INTER_LINEAR, crop_resize_device, crop_resize_frames_device, chunk_ranges, roi_affine,
+                        split_by_counts, square_roi, stack_frames_device)
 from .params import ParamsPack, get_param_pack, set_param_pack  # noqa: F401  (re-exported)
 
 _LOSS_KEYS = ('loss_LMK_f0', 'loss_LMK_pointNet', 'loss_Param_In', 'loss_Param_S2', 'loss_Param_S1S2')
@@ -366,6 +367,57 @@ class _SynergyBase(nn.Module):
         ang, t3d = ang.cpu().numpy(), t3d.cpu().numpy()
         eng.raise_if_error()
         return list(lmk), list(mesh), [[ang[i].tolist(), t3d[i]] for i in range(len(boxes))]
+
+    # device memory the dense meshes of one reconstruct_image call may take in get_all_outputs_batch (638 KB per face:
+    # 1682 faces); beyond it the faces are reconstructed and copied back in chunks
+    dense_chunk_bytes = 1 << 30
+
+    def get_all_outputs_batch(self, frames, rects: Optional[Sequence[Sequence[Sequence[float]]]] = None):
+        """:meth:`get_all_outputs` for N equally sized BGR uint8 frames (a list, an (N,H,W,3) array, or a uint8 CUDA
+        stack): a list of N ``(lmks, meshes, poses)`` triples, entry i being what ``get_all_outputs(frames[i], rects[i])``
+        returns, ``([], [], [])`` for a frame without a face.
+
+        The frames are uploaded once.  With ``rects=None`` the detector's ``detect_batch`` gets that device stack (a
+        detector without one is called frame by frame).  Then one crop launch over the faces of all frames, one backbone
+        call, one landmark and one dense reconstruction (the latter in chunks of faces above ``dense_chunk_bytes``), one
+        pose decode.  ROIs are computed on the host in float64 exactly as the one-image call does."""
+        dev = self._compute_device()
+        eng = self._engine(dev)
+        stack = stack_frames_device(frames, dev)
+        n = int(stack.shape[0])
+        if rects is None:
+            if self.face_detector is None:
+                raise RuntimeError('no face detector configured: pass rects (one list of [x0,y0,x1,y1,score] per frame) '
+                                   'or set model.face_detector')
+            if hasattr(self.face_detector, 'detect_batch'):
+                rects = self.face_detector.detect_batch(stack)
+            else:
+                host = stack.cpu().numpy() if isinstance(frames, torch.Tensor) else frames
+                rects = [self.face_detector(host[i]) for i in range(n)]
+        if len(rects) != n:
+            raise ValueError(f'{len(rects)} rect lists for {n} frames')
+        counts = [len(r) for r in rects]
+        boxes = [square_roi(list(r)) for fr in rects for r in fr]
+        if not boxes:
+            return [([], [], []) for _ in range(n)]
+        frame_index = [i for i, c in enumerate(counts) for _ in range(c)]
+        interp = INTER_LANCZOS4 if self.resize_interpolation == 'lanczos4' else INTER_LINEAR
+        batch = crop_resize_frames_device(stack, frame_index, boxes, (120, 120), interp)
+        if self.I2P._adapted:
+            out = eng.forward_mobilenet_v1(batch)[0] if self.I2P._is_mbv1 else eng.forward_resnet(batch)[0]
+            params = out[:, :62].contiguous()
+        else:
+            _, params = eng.forward_landmarks(batch, want_params=True)
+        roi5 = torch.from_numpy(roi_affine(boxes)).to(dev)
+        lmk = eng.reconstruct_image(params, roi5, dense=False).cpu().numpy()
+        per_chunk = max(1, self.dense_chunk_bytes // (3 * 4 * max(eng.n_vert, 1)))
+        mesh = [eng.reconstruct_image(params[a:b], roi5[a:b], dense=True).cpu().numpy() for a, b in chunk_ranges(len(boxes), per_chunk)]
+        mesh = mesh[0] if len(mesh) == 1 else np.concatenate(mesh)
+        ang, t3d = eng.pose_decode(params, roi5)
+        ang, t3d = ang.cpu().numpy(), t3d.cpu().numpy()
+        eng.raise_if_error()
+        poses = [[ang[i].tolist(), t3d[i]] for i in range(len(boxes))]
+        return list(zip(split_by_counts(lmk, counts), split_by_counts(mesh, counts), split_by_counts(poses, counts)))
 
 
 class SynergyNet(_SynergyBase):
