@@ -101,3 +101,41 @@ def test_batch_chooser_covers_every_tile_plan(sms):
     assert {0, 2 * sms - 2, 2 * sms - 1, 2 * sms, batches['mixed_pairs'] - 1} <= set(faces)
     faces = tile_cover.faces_to_check(batches['ragged_quads'], sms)
     assert set(range(4 * sms, 4 * sms + 3)) <= set(faces) and len(faces) < 30
+
+
+@pytest.mark.parametrize('sms', [114, 132])
+def test_pool_placement_reaches_every_slot_and_tile_kind(sms):
+    """The placement of tests/test_gpu_every_face.py: a 64-face pool over B = 1024 and the three tile-cover batches.
+    Together the batches meet every claim; each batch drops only the claims its plans cannot meet."""
+    pool = 64
+    place = tile_cover.placement(1024, pool)
+    assert place[:pool].tolist() == list(range(pool)) and place[pool:2 * pool].tolist() == list(range(1, pool)) + [0]
+    assert torch.bincount(place).tolist() == [1024 // pool] * pool
+    batches = {'bench': 1024, **tile_cover.choose_batches(sms)}
+    met = {kind: tile_cover.check_placement(b, sms, pool) for kind, b in batches.items()}
+    claims = set(met['bench'][0]) | set(met['bench'][1])
+    assert len(claims) == 14
+    for kind, (ok, dropped) in met.items():
+        assert set(ok) | set(dropped) == claims and not set(ok) & set(dropped), kind
+        assert all(dropped.values()), kind
+    assert set().union(*(ok for ok, _ in met.values())) == claims
+    # every pool face sits in both slots of the two-face groups, every slot of the four-face groups and of the tail
+    # kernel's tiles, and at several row offsets of every map size, at B = 1024
+    full = list(range(pool))
+    bench = met['bench'][0]
+    for claim in ['pair_both_slots', 'quad_every_slot', 'tail_every_slot'] + [f'rows{px}' for px in tile_cover.MAP_PIXELS]:
+        assert bench[claim] == full, claim
+    # what each plan cannot hold, on an H100 SXM (132 SMs) and PCIe (114 SMs)
+    expect = {132: {'bench': {'single_face_group', 'quad_ragged_last'},
+                    'mixed_pairs': {'tail_every_slot', 'later_tile_quad'},
+                    'odd_pairs': {'tail_every_slot', 'later_tile_pair', 'later_tile_quad'},
+                    'ragged_quads': set()},
+              114: {'bench': {'quad_ragged_last'},
+                    'mixed_pairs': {'quad_ragged_last', 'tail_every_slot', 'later_tile_quad'},
+                    'odd_pairs': {'quad_every_slot', 'tail_every_slot', 'later_tile_pair', 'later_tile_quad'},
+                    'ragged_quads': set()}}[sms]
+    assert {kind: set(d) for kind, (_, d) in met.items()} == expect
+    assert met['ragged_quads'][0]['quad_ragged_last'] == sorted(place[4 * sms:4 * sms + 3].tolist())
+    # a batch smaller than the pool reaches no slot twice
+    ok, dropped = tile_cover.check_placement(33, sms, pool)
+    assert {'pair_both_slots', 'quad_every_slot', 'tail_every_slot'} <= set(dropped)
