@@ -277,6 +277,36 @@ int syn_rasterize(uint8_t* image_dev, int height, int width, int channels, const
                   int stride_vertex, int stride_coord, int batch, int nver, const int32_t* tri_dev, int ntri,
                   const float* colors_dev, float alpha, int reverse, uint64_t* keys_ws_dev, float* depth_out_dev, void* stream);
 
+/* The overlay stage of utils/render.py:38-47 for a stack of frames (the reference runs it once per image): n_frames
+ * equally sized frames, frame f owning meshes [mesh_start[f], mesh_start[f+1]) of the n_meshes meshes, in draw order.
+ * Each frame's solid overlay is what syn_rasterize draws onto a copy of that frame with that frame's meshes
+ * (Sim3DR/lighting.py:37-72 for the colours, rasterize_kernel.cpp:217-287 for the z-buffer, alpha 1, no reverse, no
+ * depth output).  A mesh keys only its pixel box -- the union of its triangles' boxes clamped to the frame -- so the key
+ * workspace is the sum of the box areas, not n_meshes * height * width.  Two steps:
+ *   syn_render_frames_plan writes boxes_dev (n_meshes,4) int32 (x0, y0, x1, y1; an empty or off-frame mesh: (0,0,-1,-1))
+ *   and key_off_dev (n_meshes+1) int64, the exclusive prefix sum of the box areas: key_off_dev[n_meshes] is the number
+ *   of uint64 key slots syn_rasterize_frames needs.  Reading it back is the one host synchronisation of the stage.
+ *   syn_rasterize_frames reads frames_dev (n_frames,height,width,channels) uint8 and writes the solid overlays to
+ *   solid_dev (same shape; it may be frames_dev, to draw in place -- later meshes of a frame can so be drawn by a later
+ *   call onto what an earlier call drew, with the same bytes as one call).  colors_dev (n_meshes,nver,color_channels)
+ *   as syn_mesh_lighting writes them; mesh_start_dev is mesh_start_host on the device; n_keys = key_off_dev[n_meshes];
+ *   keys_ws_dev holds keys_ws_count >= n_keys uint64.
+ * Both take the vertices through element strides as syn_rasterize does, and check mesh_start_host before any launch:
+ * mesh_start[0] = 0, monotone, mesh_start[n_frames] = n_meshes (SYN_ERR_SHAPE otherwise).  1..65535 frames and meshes
+ * per call.  A channel mismatch or a key workspace smaller than n_keys is SYN_ERR_SHAPE. */
+int syn_render_frames_plan(const float* vertices_dev, int64_t stride_mesh, int stride_vertex, int stride_coord, int n_meshes, int nver,
+                           const int32_t* tri_dev, int ntri, const int32_t* mesh_start_host, int n_frames, int height, int width,
+                           int32_t* boxes_dev, int64_t* key_off_dev, void* stream);
+int syn_rasterize_frames(const uint8_t* frames_dev, uint8_t* solid_dev, int n_frames, int height, int width, int channels,
+                         const float* vertices_dev, int64_t stride_mesh, int stride_vertex, int stride_coord, int n_meshes, int nver,
+                         const int32_t* tri_dev, int ntri, const float* colors_dev, int color_channels, const int32_t* mesh_start_host,
+                         const int32_t* mesh_start_dev, const int32_t* boxes_dev, const int64_t* key_off_dev, int64_t n_keys,
+                         uint64_t* keys_ws_dev, int64_t keys_ws_count, void* stream);
+/* cv2.addWeighted(a, 1 - alpha, b, alpha, 0) on n uint8 values (utils/render.py:45), byte for byte with OpenCV 4.x:
+ * out = saturate(round_half_even(fmaf(a, (float)(1 - alpha), b * (float)alpha))), 1 - alpha in double (csrc/render_math.h
+ * add_weighted_u8).  out_dev may be a_dev or b_dev.  Any finite alpha; otherwise SYN_ERR_INVALID. */
+int syn_add_weighted_u8(const uint8_t* a_dev, const uint8_t* b_dev, double alpha, uint8_t* out_dev, int64_t n, void* stream);
+
 /* ---- FaceBoxes post-processing (SURVEY.md section 8 row f3) -----------------------------------------------------------
  * These entries take the detector network's outputs (syn_fb_forward below, or any other producer). */
 enum {
@@ -384,7 +414,8 @@ int  syn_fb_forward_batch(syn_fb_t* f, const uint8_t* images_dev, int n_frames, 
                           float* conf_dev, void* stream);
 /* Per-stage tests of the detector network.  Runs syn_fb_forward's launch sequence unchanged and returns right after launch
  * `stage` (0..38), having copied (on the stream) the whole tensor that launch wrote to out_dev, which holds out_numel
- * floats (SYN_ERR_SHAPE if that is not the tensor's size).  NHWC maps of an h x w image, n3/n4/n5 = the pixels of the
+ * floats (SYN_ERR_SHAPE if that is not the tensor's size).  The activation workspace is zeroed first, so channel slices
+ * of that tensor which later launches would write read 0.  NHWC maps of an h x w image, n3/n4/n5 = the pixels of the
  * stride-32/64/128 maps, P = syn_faceboxes_num_priors(h, w):
  *   0 conv1 (CReLU, 48 ch)   1 max-pool (48 ch)   2 conv2 (CReLU, 128 ch)   3 max-pool (128 ch: inception1's input)
  *   4 + 8b .. 11 + 8b, inception b = 0..2: branch1x1 -> block output (all 128 ch; it owns 0..31), avg-pool of the

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """scripts/single_image_demo.py for a batch of frames: a seeded stack of synthetic scenes goes through
-``get_all_outputs_batch`` (one detector pass, one crop launch, one backbone call for the faces of all frames) and every
-frame gets its solid-mesh overlay.
+``overlay_batch`` (one detector pass, one crop launch, one backbone call for the faces of all frames, then every face's
+dense mesh lit, drawn and blended onto its frame on the device) and each frame's overlay is written as one image.
 
     python scripts/frames_demo.py [--frames 4] [--out-dir frames_demo]
 
@@ -36,7 +36,8 @@ def main():
     ap.add_argument('--max-faces', type=int, default=8)
     ap.add_argument('--out-dir', default='frames_demo')
     args = ap.parse_args()
-    from synergynet_b200 import Sim3DR, faceboxes, model_building, synthetic
+    import cv2
+    from synergynet_b200 import faceboxes, model_building, synthetic
     from synergynet_b200.params import ParamsPack, set_param_pack
 
     frames = np.stack([synthetic.make_scene_u8(args.height, args.width, seed) for seed in range(args.frames)])
@@ -46,15 +47,13 @@ def main():
     synthetic.randomize_batchnorm_(model, 0)
     model.eval()
     model.face_detector = _TopFaces(faceboxes.FaceBoxes(weights=synthetic.make_faceboxes_state_dict(0)), args.max_faces)
-    results = model.get_all_outputs_batch(frames)
-    tri = np.ascontiguousarray(synthetic.make_render_topology())
+    # one pass for the whole stack: detector, crops, backbone, dense meshes, lighting, z-buffer and blend on the device
+    blended, _solid = model.overlay_batch(frames, alpha=0.6, connectivity=synthetic.make_render_topology().T)
     os.makedirs(args.out_dir, exist_ok=True)
-    for i, (lmks, meshes, poses) in enumerate(results):
+    for i in range(len(frames)):
         out = os.path.join(args.out_dir, f'frame{i:03d}.png')
-        if meshes:
-            Sim3DR.render(frames[i], meshes, tri, alpha=0.6, wfp=out)                 # batched over the frame's meshes
-        print(f'frame {i}: {len(lmks)} faces' + (f', first pose {poses[0][0]}, wrote {out}' if meshes else ''))
-
+        cv2.imwrite(out, blended[i])
+        print(f'frame {i}: {int((blended[i] != frames[i]).any(-1).sum())} pixels overlaid, wrote {out}')
 
 if __name__ == '__main__':
     main()

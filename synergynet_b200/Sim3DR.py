@@ -132,6 +132,88 @@ class MeshRenderer:
         nrm = self.normals(vertices)
         return self.rasterize(image, vertices, self.colors(vertices, nrm, cfg, texture))
 
+    # -- the frame axis ----------------------------------------------------------------------------------------------------
+    @staticmethod
+    def _mesh_start(counts, n_frames: int) -> np.ndarray:
+        counts = [int(c) for c in counts]
+        if len(counts) != n_frames or min(counts, default=0) < 0:
+            raise ValueError(f'counts must give a non-negative mesh count for each of the {n_frames} frames, got {counts}')
+        return np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+
+    def plan_frames(self, vertices: torch.Tensor, counts, height: int, width: int):
+        """Pixel boxes (M,4) int32 ``x0, y0, x1, y1`` of the M meshes on a ``height`` x ``width`` frame and the key offsets
+        (M+1) int64 of :meth:`rasterize_frames` (``syn_render_frames_plan``).  ``counts[f]`` meshes belong to frame f."""
+        v, view = self._view(vertices)
+        m = view[4]
+        start = self._mesh_start(counts, len(counts))
+        boxes = torch.empty((m, 4), dtype=torch.int32, device=self.device)
+        key_off = torch.empty(m + 1, dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.syn_render_frames_plan(*view, self.tri.data_ptr(), self.ntri, start.ctypes.data, len(counts), int(height),
+                                                        int(width), boxes.data_ptr(), key_off.data_ptr(), _stream_ptr(self.device)))
+        self.launches += 2
+        return boxes, key_off
+
+    def rasterize_frames(self, frames: torch.Tensor, vertices: torch.Tensor, colors: torch.Tensor, counts,
+                         out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Solid overlays of a frame stack: ``frames`` (N,H,W,C) uint8, frame f's meshes are the next ``counts[f]`` of the
+        M meshes of ``vertices`` / ``colors`` (M,nver,C), drawn in order as :meth:`rasterize` draws them onto one image.
+        Returns ``out`` (a new stack if None; ``out=frames`` draws in place).  One host synchronisation: the key count."""
+        v, view = self._view(vertices)
+        m = view[4]
+        if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.device != self.device or not frames.is_contiguous():
+            raise ValueError('frames must be a contiguous uint8 (N,H,W,C) tensor on the renderer device')
+        n, h, w, c = (int(s) for s in frames.shape)
+        colors = colors.contiguous()
+        if colors.dim() != 3 or tuple(colors.shape[:2]) != (m, self.nver) or colors.dtype != torch.float32 or colors.device != self.device:
+            raise ValueError(f'colors must be float32 (M,nver,C) on the renderer device; got {tuple(colors.shape)}')
+        if out is None:
+            out = torch.empty_like(frames)
+        elif out.shape != frames.shape or out.dtype != torch.uint8 or out.device != self.device or not out.is_contiguous():
+            raise ValueError('out must be a contiguous uint8 tensor shaped like frames')
+        start = self._mesh_start(counts, n)
+        boxes, key_off = self.plan_frames(v, counts, h, w)
+        n_keys = int(key_off[m].item())                                   # the stage's one host synchronisation
+        keys = torch.empty(max(n_keys, 1), dtype=torch.int64, device=self.device)
+        self.last_key_count = n_keys
+        start_dev = torch.from_numpy(start).to(self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.syn_rasterize_frames(frames.data_ptr(), out.data_ptr(), n, h, w, c, *view, self.tri.data_ptr(),
+                                                      self.ntri, colors.data_ptr(), int(colors.shape[2]), start.ctypes.data,
+                                                      start_dev.data_ptr(), boxes.data_ptr(), key_off.data_ptr(), n_keys,
+                                                      keys.data_ptr(), keys.numel(), _stream_ptr(self.device)))
+        self.launches += 2
+        return out
+
+    def render_frames(self, frames_dev: torch.Tensor, vertices: torch.Tensor, counts, cfg: Optional[_lib.LightCfg] = None,
+                      texture: Optional[torch.Tensor] = None, alpha: float = 0.6):
+        """``utils/render.py:38-45`` for every frame of a stack at once: frame f's ``counts[f]`` meshes (the next ones of
+        ``vertices`` (M,nver,3), any strides: ``reconstruct_image(...).transpose(1, 2)``) are lit and drawn onto a copy of
+        it, which is then blended with it as ``cv2.addWeighted(frame, 1 - alpha, solid, alpha, 0)``.  Returns the device
+        stacks ``(blended, solid)``, each frame's bytes those of :func:`render` on that frame alone."""
+        if sum(int(c) for c in counts) == 0:
+            self._mesh_start(counts, int(frames_dev.shape[0]))
+            solid = frames_dev.clone()
+        else:
+            col = self.colors(vertices, self.normals(vertices), cfg, texture)
+            solid = self.rasterize_frames(frames_dev, vertices, col, counts)
+        return add_weighted(frames_dev, solid, alpha), solid
+
+
+def add_weighted(a: torch.Tensor, b: torch.Tensor, alpha: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``cv2.addWeighted(a, 1 - alpha, b, alpha, 0)`` of two uint8 CUDA tensors of one shape, byte for byte
+    (``syn_add_weighted_u8``).  ``out`` may be ``a`` or ``b``."""
+    if a.dtype != torch.uint8 or b.dtype != torch.uint8 or a.shape != b.shape or not a.is_cuda or a.device != b.device:
+        raise ValueError('add_weighted takes two uint8 CUDA tensors of one shape on one device')
+    a, b = a.contiguous(), b.contiguous()
+    out = torch.empty_like(a) if out is None else out
+    if out.shape != a.shape or out.dtype != torch.uint8 or out.device != a.device or not out.is_contiguous():
+        raise ValueError('out must be a contiguous uint8 tensor shaped like the inputs')
+    with torch.cuda.device(a.device):
+        _lib.check(_lib.load().syn_add_weighted_u8(a.data_ptr(), b.data_ptr(), float(alpha), out.data_ptr(), a.numel(),
+                                                   _stream_ptr(a.device)))
+    return out
+
 
 _renderers = {}
 
@@ -242,3 +324,42 @@ def render(img: np.ndarray, ver_lst, tri, alpha: float = 0.6, wfp=None, tex=None
         cv2.imwrite(wfp[:-4] + '_solid' + '.png', overlap)
         cv2.imwrite(wfp, res)
     return res, overlap
+
+
+def render_batch(frames, ver_lsts, tri, alpha: float = 0.6, wfps=None, tex=None, cfg: Optional[dict] = None):
+    """:func:`render` for N equally sized frames in one pass: entry i of the returned list is the ``(blended, overlap)``
+    pair ``render(frames[i], ver_lsts[i], tri, alpha, wfps[i], tex, cfg)`` returns, bit for bit.  One upload of the frames
+    and of all meshes, one normals / lighting / rasterisation / blend launch sequence for all of them, one download of
+    each result stack.  A frame without a mesh gets ``overlap = frame`` and ``blended = cv2.addWeighted(frame, 1 - alpha,
+    frame, alpha, 0)``, as the reference's ``render(img, [], ...)`` computes.  ``wfps``: None, or one path (or None) per
+    frame, written as :func:`render` writes them."""
+    import cv2
+    from .inference import RENDER_CFG, stack_frames_host
+    stack = stack_frames_host(frames)
+    n = stack.shape[0]
+    if len(ver_lsts) != n or (wfps is not None and len(wfps) != n):
+        raise ValueError(f'{len(ver_lsts)} mesh lists and {"no" if wfps is None else len(wfps)} paths for {n} frames')
+    counts = [len(v) for v in ver_lsts]
+    meshes = [np.asarray(v, dtype=np.float32) for vl in ver_lsts for v in vl]
+    if not torch.cuda.is_available():
+        raise RuntimeError('synergynet_b200.Sim3DR needs a CUDA device (H100, sm_90a); there is no CPU fallback')
+    dev = torch.device('cuda', torch.cuda.current_device())
+    frames_dev = torch.from_numpy(stack).to(dev)
+    if meshes:
+        ver = np.stack(meshes)                                                      # (M,3,N)
+        r = _renderer_for(tri, ver.shape[2])
+        v = torch.from_numpy(ver).to(r.device).transpose(1, 2)
+        texture = None if tex is None else torch.from_numpy(np.ascontiguousarray(tex, dtype=np.float32))
+        blended, solid = r.render_frames(frames_dev, v, counts, _light_cfg(**(cfg or RENDER_CFG)), texture, alpha)
+    else:
+        solid = frames_dev
+        blended = add_weighted(frames_dev, solid, alpha)
+    blended, solid = blended.cpu().numpy(), solid.cpu().numpy()
+    out = []
+    for i in range(n):
+        res, overlap = blended[i], solid[i]
+        if wfps is not None and wfps[i] is not None:
+            cv2.imwrite(wfps[i][:-4] + '_solid' + '.png', overlap)
+            cv2.imwrite(wfps[i], res)
+        out.append((res, overlap))
+    return out

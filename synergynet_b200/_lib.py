@@ -104,6 +104,9 @@ SIGNATURES = {
     'syn_mesh_normals': (_I, [_F, _L, _I, _I, _I, _I, _F, _I, _F, _F, _F, _F, _P]),
     'syn_mesh_lighting': (_I, [_F, _L, _I, _I, _I, _I, _F, C.POINTER(LightCfg), _F, _F, _F, _P]),
     'syn_rasterize': (_I, [_F, _I, _I, _I, _F, _L, _I, _I, _I, _I, _F, _I, _F, C.c_float, _I, _F, _F, _P]),
+    'syn_render_frames_plan': (_I, [_F, _L, _I, _I, _I, _I, _F, _I, _P, _I, _I, _I, _F, _F, _P]),
+    'syn_rasterize_frames': (_I, [_F, _F, _I, _I, _I, _I, _F, _L, _I, _I, _I, _I, _F, _I, _F, _I, _P, _F, _F, _F, _L, _F, _L, _P]),
+    'syn_add_weighted_u8': (_I, [_F, _F, C.c_double, _F, _L, _P]),
     'syn_nms': (_I, [_F, _I, C.c_double, _I, _F, _F, _F, _P]),
     'syn_crop_resize_plan_size': (_L, [_I, _I, _I, _I]),
     'syn_crop_resize_plan_host': (_I, [_P, _I, _I, _I, _I, _P, _L]),
@@ -151,7 +154,8 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_fb_destroy', 'syn_fb_set_layer', 'syn_fb_commit', 'syn_fb_forward', 'syn_fb_launch_count',
                                              'syn_fb_debug_forward_until', 'syn_fb_forward_batch', 'syn_fb_debug_forward_batch_until',
                                              'syn_faceboxes_decode_batch', 'syn_nms_batch', 'syn_crop_resize_plan_frames_host',
-                                             'syn_crop_resize_batch')}
+                                             'syn_crop_resize_batch', 'syn_render_frames_plan', 'syn_rasterize_frames',
+                                             'syn_add_weighted_u8')}
 
 
 def declared_symbols(header: str = HEADER_PATH):

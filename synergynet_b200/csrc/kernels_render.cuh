@@ -11,6 +11,13 @@
 //                                  one after the other onto the same image, utils/render.py:41-45, each with a fresh
 //                                  depth buffer), barycentric weights recomputed from the winning triangle, colours
 //                                  interpolated and written as the reference's (unsigned char) expression.
+// The frame axis (syn_render_frames_plan / syn_rasterize_frames: the meshes of N frames, frame f owning a contiguous
+// range of them) keeps the same per-pixel arithmetic, but a mesh's keys live only in its pixel box -- the union of its
+// triangles' clamped boxes -- so the workspace is the sum of the box areas instead of B x H x W:
+//   pass 0  mesh_box_kernel + mesh_box_scan_kernel   the boxes, and their areas' exclusive prefix sum (key offsets)
+//   pass 1  raster_depth_kernel                      unchanged, each key addressed inside its mesh's box
+//   pass 2  raster_resolve_frames_kernel             one thread per (frame, pixel) over that frame's meshes only
+// and the overlay blend of utils/render.py:45 (cv2.addWeighted) runs as add_weighted_u8_kernel.
 // Vertex normals are the sum of the incident face normals IN TRIANGLE ORDER (:189-199): a per-vertex incidence list,
 // ascending by construction (syn_mesh_incidence_host), replaces the scatter loop, so the float sums associate exactly
 // as the reference's do.  All arithmetic comes from render_math.h (no FMA contraction): normals and rasterisation are
@@ -136,21 +143,32 @@ __device__ __forceinline__ bool load_tri(const MeshView& m, int b, const int32_t
 
 constexpr int kRasterSmallBox = 64;     // bounding boxes up to this many pixels are walked by the owning thread
 
-// keys: (B, h, w) uint64, zero = empty.  One thread per (mesh, triangle).
+// keys: zero = empty.  BOXED = false (syn_rasterize): the (B, h, w) canvas of every mesh; boxes / key_off are not read.
+// BOXED = true (the frame axis): mesh b keys only its pixel box boxes[b] = (x0, y0, x1, y1), in the box-many slots at
+// keys + key_off[b] (mesh_box_kernel / mesh_box_scan_kernel plan them).  The canvas instantiation is the one-image kernel
+// as it was before the frame axis existed, instruction for instruction.  One thread per (mesh, triangle).
+template <bool BOXED>
 __global__ void raster_depth_kernel(MeshView m, const int32_t* __restrict__ tri, int ntri, int w, int h,
-                                    unsigned long long* __restrict__ keys) {
+                                    unsigned long long* __restrict__ keys, const int4* __restrict__ boxes,
+                                    const long long* __restrict__ key_off) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
   const int lane = threadIdx.x & 31;
   rmath::TriSetup t;
   const bool live = (i < ntri) && load_tri(m, b, tri, i, w, h, t);
-  unsigned long long* kb = keys + (size_t)b * w * h;
+  unsigned long long* kb = keys + (size_t)b * w * h;     // key of pixel (x, y): kb[y * ks + x]
+  int ks = w;
+  if constexpr (BOXED) {                                  // the box's row-major slots, addressed from the canvas origin
+    const int4 q = boxes[b];
+    ks = q.z - q.x + 1;
+    kb = keys + key_off[b] - ((long long)q.y * ks + q.x);
+  }
   int bw = 0, area = 0;
   if (live) { bw = t.xmax - t.xmin + 1; area = bw * (t.ymax - t.ymin + 1); }
   if (live && area <= kRasterSmallBox) {
     for (int y = t.ymin; y <= t.ymax; ++y)
       for (int x = t.xmin; x <= t.xmax; ++x) {
         uint64_t key;
-        if (rmath::pixel_key(t, (uint32_t)i, x, y, key)) atomicMax(kb + (size_t)y * w + x, (unsigned long long)key);
+        if (rmath::pixel_key(t, (uint32_t)i, x, y, key)) atomicMax(kb + (size_t)y * ks + x, (unsigned long long)key);
       }
   }
   // large boxes: the warp walks them together, one triangle at a time
@@ -168,8 +186,31 @@ __global__ void raster_depth_kernel(MeshView m, const int32_t* __restrict__ tri,
     for (int q = lane; q < sarea; q += 32) {
       const int y = s.ymin + q / sbw, x = s.xmin + q % sbw;
       uint64_t key;
-      if (rmath::pixel_key(s, (uint32_t)si, x, y, key)) atomicMax(kb + (size_t)y * w + x, (unsigned long long)key);
+      if (rmath::pixel_key(s, (uint32_t)si, x, y, key)) atomicMax(kb + (size_t)y * ks + x, (unsigned long long)key);
     }
+  }
+}
+
+// The winning triangle `key` of mesh b at pixel (x, y): barycentric weights recomputed from its vertices, colours
+// interpolated, written as the reference's (unsigned char) expression over the pixel's bytes (:239-255).  The pixel is
+// row `row`, column x of the (h, w, c) images src and dst (row = y, or h - 1 - y when drawing upside down).
+__device__ __forceinline__ void shade_pixel(const MeshView& m, int b, const int32_t* __restrict__ tri, const float* __restrict__ colors,
+                                            int c, int w, int x, int y, int row, unsigned long long key, float alpha,
+                                            const unsigned char* src, unsigned char* dst) {
+  const int i = (int)rmath::key_tri(key);
+  const int i0 = __ldg(tri + 3 * i), i1 = __ldg(tri + 3 * i + 1), i2 = __ldg(tri + 3 * i + 2);
+  float p0[3], p1[3], p2[3];
+  load_vertex(m, b, i0, p0);
+  load_vertex(m, b, i1, p1);
+  load_vertex(m, b, i2, p2);
+  const rmath::Bary bw = rmath::barycentric((float)x, (float)y, p0[0], p0[1], p1[0], p1[1], p2[0], p2[1]);
+  const float* cb = colors + (size_t)b * m.nver * c;
+  const size_t at = ((size_t)row * w + x) * c;
+  src += at;
+  dst += at;
+  for (int k = 0; k < c; ++k) {
+    const float pc = rmath::interp(bw, __ldg(cb + (size_t)i0 * c + k), __ldg(cb + (size_t)i1 * c + k), __ldg(cb + (size_t)i2 * c + k));
+    dst[k] = rmath::blend_u8(src[k], alpha, pc);
   }
 }
 
@@ -187,20 +228,106 @@ __global__ void raster_resolve_kernel(MeshView m, const int32_t* __restrict__ tr
     if (depth_out) depth_out[(size_t)b * w * h + pix] = key ? rmath::key_depth(key) : rmath::kDepthInit;
     if (key == 0ull || drawn) continue;
     drawn = true;                       // later meshes overwrite earlier ones (alpha == 1)
-    const int i = (int)rmath::key_tri(key);
-    const int i0 = __ldg(tri + 3 * i), i1 = __ldg(tri + 3 * i + 1), i2 = __ldg(tri + 3 * i + 2);
-    float p0[3], p1[3], p2[3];
-    load_vertex(m, b, i0, p0);
-    load_vertex(m, b, i1, p1);
-    load_vertex(m, b, i2, p2);
-    const rmath::Bary bw = rmath::barycentric((float)x, (float)y, p0[0], p0[1], p1[0], p1[1], p2[0], p2[1]);
-    const float* cb = colors + (size_t)b * m.nver * c;
-    unsigned char* dst = image + ((size_t)(reverse ? h - 1 - y : y) * w + x) * c;
-    for (int k = 0; k < c; ++k) {
-      const float pc = rmath::interp(bw, __ldg(cb + (size_t)i0 * c + k), __ldg(cb + (size_t)i1 * c + k), __ldg(cb + (size_t)i2 * c + k));
-      dst[k] = rmath::blend_u8(dst[k], alpha, pc);
-    }
+    shade_pixel(m, b, tri, colors, c, w, x, y, reverse ? h - 1 - y : y, key, alpha, image, image);
     if (!depth_out) break;
+  }
+}
+
+// ---- the frame axis: meshes grouped by frame, keys in per-mesh boxes ---------------------------------------------------------
+// Pass 0a: acc (M,4) int32, set to 0x7F7F7F7F bytes by the caller, receives min x0, min y0, min -x1, min -y1 over the
+// triangles load_tri draws (the same skips: bad indices, boxes empty after clamping).  One thread per (mesh, triangle).
+__global__ void mesh_box_kernel(MeshView m, const int32_t* __restrict__ tri, int ntri, int w, int h, int* __restrict__ acc) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+  rmath::TriSetup t;
+  const bool live = (i < ntri) && load_tri(m, b, tri, i, w, h, t);
+  const int big = 0x7F7F7F7F;
+  const int v[4] = {live ? t.xmin : big, live ? t.ymin : big, live ? -t.xmax : big, live ? -t.ymax : big};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int r = __reduce_min_sync(0xFFFFFFFFu, v[k]);
+    if ((threadIdx.x & 31) == 0 && r != big) atomicMin(acc + 4 * b + k, r);
+  }
+}
+
+// Pass 0b, one CTA: acc -> the boxes (x0, y0, x1, y1) in place (an empty mesh: (0, 0, -1, -1), area 0) and key_off (M+1)
+// = the exclusive prefix sum of the box areas; key_off[M] is the key count of the whole call.
+constexpr int kBoxScanThreads = 1024;
+__global__ void __launch_bounds__(kBoxScanThreads) mesh_box_scan_kernel(int nmesh, int* __restrict__ acc, long long* __restrict__ key_off) {
+  __shared__ long long part[kBoxScanThreads];
+  const int tid = threadIdx.x, per = (nmesh + kBoxScanThreads - 1) / kBoxScanThreads;
+  const int j0 = min(tid * per, nmesh), j1 = min(j0 + per, nmesh);
+  long long s = 0;
+  for (int j = j0; j < j1; ++j) {
+    int* q = acc + 4 * j;
+    rmath::PixBox bx;
+    bx.x0 = q[0]; bx.y0 = q[1]; bx.x1 = -q[2]; bx.y1 = -q[3];
+    if (bx.x1 < bx.x0 || bx.y1 < bx.y0) bx = rmath::pix_box_empty();
+    q[0] = bx.x0; q[1] = bx.y0; q[2] = bx.x1; q[3] = bx.y1;
+    s += rmath::pix_box_area(bx);
+  }
+  part[tid] = s;
+  __syncthreads();
+  for (int d = 1; d < kBoxScanThreads; d <<= 1) {        // inclusive scan of the per-thread sums
+    const long long add = tid >= d ? part[tid - d] : 0ll;
+    __syncthreads();
+    part[tid] += add;
+    __syncthreads();
+  }
+  long long base = part[tid] - s;
+  for (int j = j0; j < j1; ++j) {
+    key_off[j] = base;
+    const int* q = acc + 4 * j;
+    rmath::PixBox bx;
+    bx.x0 = q[0]; bx.y0 = q[1]; bx.x1 = q[2]; bx.y1 = q[3];
+    base += rmath::pix_box_area(bx);
+  }
+  if (tid == kBoxScanThreads - 1) key_off[nmesh] = part[tid];
+}
+
+// Pass 2 of the frame axis: one thread per (frame, pixel), grid.z = frame.  Frame f's meshes [mesh_start[f],
+// mesh_start[f+1]) are walked last to first; the first whose box holds the pixel and whose key there is set is drawn (alpha
+// = 1, so it overwrites whatever the earlier meshes drew), as raster_resolve_kernel draws a one-image batch.  src and dst
+// are (N, h, w, c) stacks and may be the same buffer; an undrawn pixel is copied.
+__global__ void raster_resolve_frames_kernel(MeshView m, const int32_t* __restrict__ tri, const float* __restrict__ colors, int c,
+                                             int w, int h, const int32_t* __restrict__ mesh_start, const int4* __restrict__ boxes,
+                                             const long long* __restrict__ key_off, const unsigned long long* __restrict__ keys,
+                                             const unsigned char* src, unsigned char* dst) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, f = blockIdx.z;
+  if (x >= w || y >= h) return;
+  const size_t pix = (((size_t)f * h + y) * w + x) * c;
+  const int b0 = mesh_start[f];
+  for (int b = mesh_start[f + 1] - 1; b >= b0; --b) {
+    const int4 q = boxes[b];
+    if (x < q.x || x > q.z || y < q.y || y > q.w) continue;
+    rmath::PixBox box;
+    box.x0 = q.x; box.y0 = q.y; box.x1 = q.z; box.y1 = q.w;
+    const unsigned long long key = keys[key_off[b] + rmath::pix_box_slot(box, x, y)];
+    if (key == 0ull) continue;
+    const size_t frame = (size_t)f * h * w * c;
+    shade_pixel(m, b, tri, colors, c, w, x, y, y, key, 1.0f, src + frame, dst + frame);
+    return;
+  }
+  if (src != dst)
+    for (int k = 0; k < c; ++k) dst[pix + k] = src[pix + k];
+}
+
+// out = cv2.addWeighted(a, 1 - alpha, b, alpha, 0) over n bytes (rmath::add_weighted_u8).  vec: n % 16 == 0 and all three
+// pointers 16-byte aligned, sixteen bytes per load.  out may be a or b.
+__global__ void add_weighted_u8_kernel(const unsigned char* a, const unsigned char* b, double alpha, unsigned char* out, long long n,
+                                       int vec) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
+  if (vec) {
+    union V { uint4 v; unsigned char c[16]; };
+    for (long long q = t; q < n / 16; q += stride) {
+      V va, vb, vo;
+      va.v = reinterpret_cast<const uint4*>(a)[q];
+      vb.v = reinterpret_cast<const uint4*>(b)[q];
+#pragma unroll
+      for (int k = 0; k < 16; ++k) vo.c[k] = rmath::add_weighted_u8(va.c[k], vb.c[k], alpha);
+      reinterpret_cast<uint4*>(out)[q] = vo.v;
+    }
+  } else {
+    for (long long i = t; i < n; i += stride) out[i] = rmath::add_weighted_u8(a[i], b[i], alpha);
   }
 }
 

@@ -6,7 +6,9 @@
 #include "kernels_detect.cuh"
 #include "kernels_resize.cuh"
 
+#include <algorithm>
 #include <cmath>
+#include <cstdint>
 #include <new>
 #include <vector>
 
@@ -19,6 +21,25 @@ int check_mesh(const float* v, long long sb, int sv, int sc, int batch, int nver
     return fail(SYN_ERR_INVALID, "mesh view: null pointer, empty batch or non-positive stride");
   m.v = v; m.sb = sb; m.sv = sv; m.sc = sc; m.nver = nver; m.batch = batch;
   return SYN_OK;
+}
+
+// the shared checks of the frame-axis entries: the mesh view, the frame size and mesh_start_host (n_frames + 1 entries,
+// 0 = mesh_start[0] <= ... <= mesh_start[n_frames] = n_meshes); meshes and frames each sit on one grid axis
+int check_frames(const float* v, long long sb, int sv, int sc, int n_meshes, int nver, const int32_t* mesh_start_host, int n_frames,
+                 int height, int width, MeshView& m, const char* who) {
+  if (!v || !mesh_start_host || n_meshes <= 0 || nver <= 0 || sv <= 0 || sc <= 0 || (n_meshes > 1 && sb <= 0))
+    return fail(SYN_ERR_INVALID, "%s: null pointer, no mesh or non-positive stride", who);
+  if (n_frames <= 0 || n_frames > 65535 || n_meshes > 65535)
+    return fail(SYN_ERR_INVALID, "%s: %d frames and %d meshes (1..65535 of each per call)", who, n_frames, n_meshes);
+  if (height <= 0 || width <= 0) return fail(SYN_ERR_INVALID, "%s: frame size %dx%d", who, height, width);
+  if (mesh_start_host[0] != 0 || mesh_start_host[n_frames] != n_meshes)
+    return fail(SYN_ERR_SHAPE, "%s: mesh_start runs from %d to %d, must run from 0 to %d meshes", who, mesh_start_host[0],
+                mesh_start_host[n_frames], n_meshes);
+  for (int f = 0; f < n_frames; ++f)
+    if (mesh_start_host[f + 1] < mesh_start_host[f])
+      return fail(SYN_ERR_SHAPE, "%s: mesh_start is not monotone at frame %d (%d after %d)", who, f, mesh_start_host[f + 1],
+                  mesh_start_host[f]);
+  return check_mesh(v, sb, sv, sc, n_meshes, nver, m);
 }
 
 // the host planner of both crop entries; frames_host == nullptr: one image
@@ -136,14 +157,81 @@ int syn_rasterize(uint8_t* image_dev, int height, int width, int channels, const
   cudaStream_t st = (cudaStream_t)stream;
   SYN_CUDA(cudaMemsetAsync(keys_ws_dev, 0, sizeof(uint64_t) * (size_t)batch * height * width, st));
   if (ntri > 0) {
-    raster_depth_kernel<<<dim3((ntri + 255) / 256, batch), 256, 0, st>>>(m, tri_dev, ntri, width, height,
-                                                                         reinterpret_cast<unsigned long long*>(keys_ws_dev));
+    raster_depth_kernel<false><<<dim3((ntri + 255) / 256, batch), 256, 0, st>>>(m, tri_dev, ntri, width, height,
+                                                                         reinterpret_cast<unsigned long long*>(keys_ws_dev), nullptr,
+                                                                         nullptr);
     SYN_LAUNCH_CHECK("raster_depth_kernel");
   }
   raster_resolve_kernel<<<dim3((width + 31) / 32, (height + 7) / 8), dim3(32, 8), 0, st>>>(
       m, tri_dev, colors_dev, channels, width, height, alpha, reverse, reinterpret_cast<const unsigned long long*>(keys_ws_dev),
       image_dev, depth_out_dev);
   SYN_LAUNCH_CHECK("raster_resolve_kernel");
+  return SYN_OK;
+}
+
+int syn_render_frames_plan(const float* vertices_dev, int64_t stride_mesh, int stride_vertex, int stride_coord, int n_meshes, int nver,
+                           const int32_t* tri_dev, int ntri, const int32_t* mesh_start_host, int n_frames, int height, int width,
+                           int32_t* boxes_dev, int64_t* key_off_dev, void* stream) {
+  const char* who = "syn_render_frames_plan";
+  MeshView m;
+  if (int rc = check_frames(vertices_dev, stride_mesh, stride_vertex, stride_coord, n_meshes, nver, mesh_start_host, n_frames, height,
+                            width, m, who))
+    return rc;
+  if (!tri_dev || ntri < 0 || !boxes_dev || !key_off_dev) return fail(SYN_ERR_INVALID, "%s: null pointer or negative triangle count", who);
+  cudaStream_t st = (cudaStream_t)stream;
+  SYN_CUDA(cudaMemsetAsync(boxes_dev, 0x7F, sizeof(int32_t) * 4 * (size_t)n_meshes, st));
+  if (ntri > 0) {
+    mesh_box_kernel<<<dim3((ntri + 255) / 256, n_meshes), 256, 0, st>>>(m, tri_dev, ntri, width, height, boxes_dev);
+    SYN_LAUNCH_CHECK("mesh_box_kernel");
+  }
+  mesh_box_scan_kernel<<<1, kBoxScanThreads, 0, st>>>(n_meshes, boxes_dev, reinterpret_cast<long long*>(key_off_dev));
+  SYN_LAUNCH_CHECK("mesh_box_scan_kernel");
+  return SYN_OK;
+}
+
+int syn_rasterize_frames(const uint8_t* frames_dev, uint8_t* solid_dev, int n_frames, int height, int width, int channels,
+                         const float* vertices_dev, int64_t stride_mesh, int stride_vertex, int stride_coord, int n_meshes, int nver,
+                         const int32_t* tri_dev, int ntri, const float* colors_dev, int color_channels, const int32_t* mesh_start_host,
+                         const int32_t* mesh_start_dev, const int32_t* boxes_dev, const int64_t* key_off_dev, int64_t n_keys,
+                         uint64_t* keys_ws_dev, int64_t keys_ws_count, void* stream) {
+  const char* who = "syn_rasterize_frames";
+  MeshView m;
+  if (int rc = check_frames(vertices_dev, stride_mesh, stride_vertex, stride_coord, n_meshes, nver, mesh_start_host, n_frames, height,
+                            width, m, who))
+    return rc;
+  if (!frames_dev || !solid_dev || !tri_dev || !colors_dev || !mesh_start_dev || !boxes_dev || !key_off_dev || !keys_ws_dev || ntri < 0)
+    return fail(SYN_ERR_INVALID, "%s: null pointer or negative triangle count", who);
+  if (channels <= 0 || channels != color_channels)
+    return fail(SYN_ERR_SHAPE, "%s: %d image channels, colours of %d channels", who, channels, color_channels);
+  if (n_keys < 0 || keys_ws_count < n_keys)
+    return fail(SYN_ERR_SHAPE, "%s: key workspace of %lld slots, the plan needs %lld", who, (long long)keys_ws_count, (long long)n_keys);
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(keys_ws_dev);
+  const int4* boxes = reinterpret_cast<const int4*>(boxes_dev);
+  const long long* off = reinterpret_cast<const long long*>(key_off_dev);
+  if (n_keys > 0) {
+    SYN_CUDA(cudaMemsetAsync(keys_ws_dev, 0, sizeof(uint64_t) * (size_t)n_keys, st));
+    if (ntri > 0) {
+      raster_depth_kernel<true><<<dim3((ntri + 255) / 256, n_meshes), 256, 0, st>>>(m, tri_dev, ntri, width, height, keys, boxes, off);
+      SYN_LAUNCH_CHECK("raster_depth_kernel");
+    }
+  }
+  raster_resolve_frames_kernel<<<dim3((width + 31) / 32, (height + 7) / 8, n_frames), dim3(32, 8), 0, st>>>(
+      m, tri_dev, colors_dev, channels, width, height, mesh_start_dev, boxes, off, keys, frames_dev, solid_dev);
+  SYN_LAUNCH_CHECK("raster_resolve_frames_kernel");
+  return SYN_OK;
+}
+
+int syn_add_weighted_u8(const uint8_t* a_dev, const uint8_t* b_dev, double alpha, uint8_t* out_dev, int64_t n, void* stream) {
+  if (!a_dev || !b_dev || !out_dev || n < 0) return fail(SYN_ERR_INVALID, "syn_add_weighted_u8: null pointer or negative size");
+  if (!std::isfinite(alpha)) return fail(SYN_ERR_INVALID, "syn_add_weighted_u8: alpha %g is not finite", alpha);
+  if (n == 0) return SYN_OK;
+  const bool vec = n % 16 == 0 && ((reinterpret_cast<uintptr_t>(a_dev) | reinterpret_cast<uintptr_t>(b_dev) |
+                                    reinterpret_cast<uintptr_t>(out_dev)) & 15) == 0;
+  const long long work = vec ? n / 16 : n;
+  const int blocks = (int)std::min<long long>((work + 255) / 256, 1 << 20);
+  add_weighted_u8_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a_dev, b_dev, alpha, out_dev, (long long)n, vec ? 1 : 0);
+  SYN_LAUNCH_CHECK("add_weighted_u8_kernel");
   return SYN_OK;
 }
 
@@ -307,6 +395,7 @@ struct syn_fb {
   int ws_h = 0, ws_w = 0, ws_frames = 0;
   float *c1 = nullptr, *p1 = nullptr, *c2 = nullptr, *xa = nullptr, *xb = nullptr, *avg = nullptr, *r1 = nullptr, *r2 = nullptr,
         *t3 = nullptr, *c31 = nullptr, *c32 = nullptr, *c41 = nullptr, *c42 = nullptr;
+  size_t ws_sizes[13] = {};                 // bytes of c1 ... c42, in that order
   int64_t launches = 0;
 };
 
@@ -315,6 +404,7 @@ namespace {
 void fb_free_ws(syn_fb* f) {
   float** bufs[] = {&f->c1, &f->p1, &f->c2, &f->xa, &f->xb, &f->avg, &f->r1, &f->r2, &f->t3, &f->c31, &f->c32, &f->c41, &f->c42};
   for (float** q : bufs) { cudaFree(*q); *q = nullptr; }
+  for (size_t& b : f->ws_sizes) b = 0;
   f->ws_h = f->ws_w = f->ws_frames = 0;
 }
 
@@ -338,19 +428,13 @@ int fb_workspace(syn_fb* f, int h, int w, int nf) {
   fb_free_ws(f);
   const FbGeom g = fb_geom(h, w);
   const size_t n3 = (size_t)nf * g.h3 * g.w3, n4 = (size_t)nf * g.h4 * g.w4, n5 = (size_t)nf * g.h5 * g.w5;
-  SYN_CUDA(cudaMalloc(&f->c1, sizeof(float) * nf * g.h1 * g.w1 * 48));
-  SYN_CUDA(cudaMalloc(&f->p1, sizeof(float) * nf * g.hp1 * g.wp1 * 48));
-  SYN_CUDA(cudaMalloc(&f->c2, sizeof(float) * nf * g.h2 * g.w2 * 128));
-  SYN_CUDA(cudaMalloc(&f->xa, sizeof(float) * n3 * 128));
-  SYN_CUDA(cudaMalloc(&f->xb, sizeof(float) * n3 * 128));
-  SYN_CUDA(cudaMalloc(&f->avg, sizeof(float) * n3 * 128));
-  SYN_CUDA(cudaMalloc(&f->r1, sizeof(float) * n3 * 24));
-  SYN_CUDA(cudaMalloc(&f->r2, sizeof(float) * n3 * 24));
-  SYN_CUDA(cudaMalloc(&f->t3, sizeof(float) * n3 * 32));
-  SYN_CUDA(cudaMalloc(&f->c31, sizeof(float) * n3 * 128));
-  SYN_CUDA(cudaMalloc(&f->c32, sizeof(float) * n4 * 256));
-  SYN_CUDA(cudaMalloc(&f->c41, sizeof(float) * n4 * 128));
-  SYN_CUDA(cudaMalloc(&f->c42, sizeof(float) * n5 * 256));
+  float** bufs[13] = {&f->c1, &f->p1, &f->c2, &f->xa, &f->xb, &f->avg, &f->r1, &f->r2, &f->t3, &f->c31, &f->c32, &f->c41, &f->c42};
+  const size_t floats[13] = {(size_t)nf * g.h1 * g.w1 * 48, (size_t)nf * g.hp1 * g.wp1 * 48, (size_t)nf * g.h2 * g.w2 * 128,
+                             n3 * 128, n3 * 128, n3 * 128, n3 * 24, n3 * 24, n3 * 32, n3 * 128, n4 * 256, n4 * 128, n5 * 256};
+  for (int k = 0; k < 13; ++k) {
+    f->ws_sizes[k] = sizeof(float) * floats[k];
+    SYN_CUDA(cudaMalloc(bufs[k], f->ws_sizes[k]));
+  }
   f->ws_h = h; f->ws_w = w; f->ws_frames = nf;
   return SYN_OK;
 }
@@ -421,6 +505,12 @@ int fb_forward_body(syn_fb* f, const uint8_t* image_dev, int frames, int height,
   SYN_CUDA(cudaSetDevice(f->device));
   const int nf = frames ? frames : 1;
   if (int rc = fb_workspace(f, height, width, nf)) return rc;
+  if (stop) {
+    // A debug run copies a stage's whole destination, slices that later launches write included: start from a zeroed
+    // workspace so that those slices read 0 instead of whatever an earlier call (another image, another frame count) left.
+    float* bufs[13] = {f->c1, f->p1, f->c2, f->xa, f->xb, f->avg, f->r1, f->r2, f->t3, f->c31, f->c32, f->c41, f->c42};
+    for (int k = 0; k < 13; ++k) SYN_CUDA(cudaMemsetAsync(bufs[k], 0, f->ws_sizes[k], st));
+  }
   const FbGeom g = fb_geom(height, width);
   if (g.h3 != fb_cells(height, 32) || g.w3 != fb_cells(width, 32) || g.h4 != fb_cells(height, 64) || g.w4 != fb_cells(width, 64) ||
       g.h5 != fb_cells(height, 128) || g.w5 != fb_cells(width, 128))

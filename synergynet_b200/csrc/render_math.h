@@ -26,6 +26,7 @@ SYN_HD float sub(float a, float b) { return __fsub_rn(a, b); }
 SYN_HD float dvd(float a, float b) { return __fdiv_rn(a, b); }
 SYN_HD float sqr(float a) { return __fsqrt_rn(a); }
 SYN_HD double dmul(double a, double b) { return __dmul_rn(a, b); }
+SYN_HD float fma_rn(float a, float b, float c) { return __fmaf_rn(a, b, c); }
 #else
 SYN_HD float mul(float a, float b) { return a * b; }
 SYN_HD float add(float a, float b) { return a + b; }
@@ -33,6 +34,7 @@ SYN_HD float sub(float a, float b) { return a - b; }
 SYN_HD float dvd(float a, float b) { return a / b; }
 SYN_HD float sqr(float a) { return sqrtf(a); }
 SYN_HD double dmul(double a, double b) { return a * b; }
+SYN_HD float fma_rn(float a, float b, float c) { return fmaf(a, b, c); }
 #endif
 
 // std::min / std::max as the reference calls them (NaN behaviour of the comparison form, not fminf/fmaxf)
@@ -129,6 +131,40 @@ SYN_HD unsigned char blend_u8(unsigned char img, float alpha, float p_color) {
   const float v = add(mul(sub(1.0f, alpha), (float)(int)img), mul(mul(alpha, 255.0f), p_color));
   return (unsigned char)(int)v;
 }
+
+// ---- the overlay blend (utils/render.py:45, cv2.addWeighted(img, 1 - alpha, overlap, alpha, 0) on uint8) ----------------
+// OpenCV 4.x evaluates every element, in its SIMD body and its scalar tail alike, as
+//   saturate_cast<uchar>(fma(a, w_a, b * w_b))      w_a = (float)(1 - alpha) (the subtraction is Python's, in double),
+//                                                   w_b = (float)alpha, the product b * w_b rounded once, gamma = 0
+// so the fused multiply-add is written out here rather than left to the compiler's contraction: the unfused
+// a * w_a + b * w_b gives other bytes (733 of the 65 536 (a, b) pairs at alpha = 0.1).  saturate_cast rounds half to
+// even (cvRound) and clamps to [0, 255]; a value outside int's range converts to INT_MIN on x86 (cvtss2si / cvtps2dq),
+// which the clamp then sends to 0 -- kept so that every finite alpha gives cv2's byte.
+SYN_HD unsigned char add_weighted_u8(unsigned char a, unsigned char b, double alpha) {
+  const float wa = (float)(1.0 - alpha), wb = (float)alpha;
+  const float v = rintf(fma_rn((float)a, wa, mul((float)b, wb)));
+  if (!(v >= -2147483648.0f && v < 2147483648.0f)) return 0;
+  const int iv = (int)v;
+  return (unsigned char)(iv < 0 ? 0 : (iv > 255 ? 255 : iv));
+}
+
+// ---- per-mesh pixel boxes of the frame-axis rasteriser ---------------------------------------------------------------------
+// A mesh's box is the union of the clamped boxes tri_setup gives its drawable triangles: every pixel its depth pass can
+// key lies inside, so its keys need only box-many slots.  Empty: x1 < x0 (then area 0).
+struct PixBox { int x0, y0, x1, y1; };
+SYN_HD PixBox pix_box_empty() { PixBox b; b.x0 = b.y0 = 0; b.x1 = b.y1 = -1; return b; }
+SYN_HD void pix_box_add(PixBox& b, const TriSetup& t) {
+  if (b.x1 < b.x0 || b.y1 < b.y0) { b.x0 = t.xmin; b.y0 = t.ymin; b.x1 = t.xmax; b.y1 = t.ymax; return; }
+  if (t.xmin < b.x0) b.x0 = t.xmin;
+  if (t.ymin < b.y0) b.y0 = t.ymin;
+  if (t.xmax > b.x1) b.x1 = t.xmax;
+  if (t.ymax > b.y1) b.y1 = t.ymax;
+}
+SYN_HD long long pix_box_area(const PixBox& b) {
+  return (b.x1 < b.x0 || b.y1 < b.y0) ? 0ll : (long long)(b.x1 - b.x0 + 1) * (long long)(b.y1 - b.y0 + 1);
+}
+// slot of pixel (x, y) in the box's keys, row-major
+SYN_HD long long pix_box_slot(const PixBox& b, int x, int y) { return (long long)(y - b.y0) * (b.x1 - b.x0 + 1) + (x - b.x0); }
 
 // ---- normals (Sim3DR/lib/rasterize_kernel.cpp:158-213, _get_normal) ----------------------------------------------------
 // un-normalised face normal (p1 - p0) x (p2 - p0)  (:173-186)

@@ -381,6 +381,27 @@ class _SynergyBase(nn.Module):
         detector without one is called frame by frame).  Then one crop launch over the faces of all frames, one backbone
         call, one landmark and one dense reconstruction (the latter in chunks of faces above ``dense_chunk_bytes``), one
         pose decode.  ROIs are computed on the host in float64 exactly as the one-image call does."""
+        eng, stack, counts, frame_index, params, roi5 = self._frames_front(frames, rects)
+        n_faces = len(frame_index)
+        if not n_faces:
+            return [([], [], []) for _ in range(len(counts))]
+        lmk = eng.reconstruct_image(params, roi5, dense=False).cpu().numpy()
+        mesh = [eng.reconstruct_image(params[a:b], roi5[a:b], dense=True).cpu().numpy() for a, b in self._dense_chunks(eng, n_faces)]
+        mesh = mesh[0] if len(mesh) == 1 else np.concatenate(mesh)
+        ang, t3d = eng.pose_decode(params, roi5)
+        ang, t3d = ang.cpu().numpy(), t3d.cpu().numpy()
+        eng.raise_if_error()
+        poses = [[ang[i].tolist(), t3d[i]] for i in range(n_faces)]
+        return list(zip(split_by_counts(lmk, counts), split_by_counts(mesh, counts), split_by_counts(poses, counts)))
+
+    def _dense_chunks(self, eng: Engine, n_faces: int) -> list:
+        per_chunk = max(1, self.dense_chunk_bytes // (3 * 4 * max(eng.n_vert, 1)))
+        return chunk_ranges(n_faces, per_chunk)
+
+    def _frames_front(self, frames, rects):
+        """The stages of :meth:`get_all_outputs_batch` up to the parameters, on the device: ``(engine, frame stack, faces
+        per frame, frame of each face, whitened params (F,62), crop -> image maps (F,5))``; the last two are None when no
+        frame has a face."""
         dev = self._compute_device()
         eng = self._engine(dev)
         stack = stack_frames_device(frames, dev)
@@ -398,9 +419,9 @@ class _SynergyBase(nn.Module):
             raise ValueError(f'{len(rects)} rect lists for {n} frames')
         counts = [len(r) for r in rects]
         boxes = [square_roi(list(r)) for fr in rects for r in fr]
-        if not boxes:
-            return [([], [], []) for _ in range(n)]
         frame_index = [i for i, c in enumerate(counts) for _ in range(c)]
+        if not boxes:
+            return eng, stack, counts, frame_index, None, None
         interp = INTER_LANCZOS4 if self.resize_interpolation == 'lanczos4' else INTER_LINEAR
         batch = crop_resize_frames_device(stack, frame_index, boxes, (120, 120), interp)
         if self.I2P._adapted:
@@ -409,15 +430,40 @@ class _SynergyBase(nn.Module):
         else:
             _, params = eng.forward_landmarks(batch, want_params=True)
         roi5 = torch.from_numpy(roi_affine(boxes)).to(dev)
-        lmk = eng.reconstruct_image(params, roi5, dense=False).cpu().numpy()
-        per_chunk = max(1, self.dense_chunk_bytes // (3 * 4 * max(eng.n_vert, 1)))
-        mesh = [eng.reconstruct_image(params[a:b], roi5[a:b], dense=True).cpu().numpy() for a, b in chunk_ranges(len(boxes), per_chunk)]
-        mesh = mesh[0] if len(mesh) == 1 else np.concatenate(mesh)
-        ang, t3d = eng.pose_decode(params, roi5)
-        ang, t3d = ang.cpu().numpy(), t3d.cpu().numpy()
-        eng.raise_if_error()
-        poses = [[ang[i].tolist(), t3d[i]] for i in range(len(boxes))]
-        return list(zip(split_by_counts(lmk, counts), split_by_counts(mesh, counts), split_by_counts(poses, counts)))
+        return eng, stack, counts, frame_index, params, roi5
+
+    def overlay_batch(self, frames, rects: Optional[Sequence[Sequence[Sequence[float]]]] = None, alpha: float = 0.6, tex=None,
+                      connectivity=None):
+        """The solid-mesh overlay of every face of N equally sized BGR uint8 frames (``get_all_outputs_batch`` followed by
+        ``utils/render.render`` per frame, singleImage.py's flow) in one pass: ``(blended, solid)`` (N,H,W,3) uint8 stacks,
+        numpy arrays -- or CUDA tensors when ``frames`` is a CUDA stack.  Frame i's bytes are those of
+        ``Sim3DR.render(frames[i], meshes_i, tri, alpha, tex=tex)`` with the dense meshes ``get_all_outputs`` returns for
+        it (a frame without a face: ``solid = frame``, ``blended = cv2.addWeighted(frame, 1 - alpha, frame, alpha, 0)``).
+
+        The dense meshes stay on the device: they are reconstructed, lit and drawn in chunks of faces above
+        ``dense_chunk_bytes`` onto the same canvases (a chunk may end inside a frame), then every frame is blended once.
+        ``connectivity`` (3,ntri) 0-based replaces the model's ``triangles`` as in ``render.render``."""
+        from . import Sim3DR
+        from .inference import RENDER_CFG
+        eng, stack, counts, frame_index, params, roi5 = self._frames_front(frames, rects)
+        solid = stack.clone()
+        if frame_index:
+            tri = np.asarray(connectivity).T if connectivity is not None else self.triangles.T.cpu().numpy()
+            with torch.cuda.device(stack.device):
+                r = Sim3DR._renderer_for(np.ascontiguousarray(tri, dtype=np.int32), eng.n_vert)
+            cfg = Sim3DR._light_cfg(**RENDER_CFG)
+            texture = None if tex is None else torch.from_numpy(np.ascontiguousarray(tex, dtype=np.float32))
+            fi = np.asarray(frame_index)
+            for a, b in self._dense_chunks(eng, len(frame_index)):
+                v = eng.reconstruct_image(params[a:b], roi5[a:b], dense=True).transpose(1, 2)
+                f0, f1 = int(fi[a]), int(fi[b - 1]) + 1                   # the frames this chunk draws on, in place
+                col = r.colors(v, r.normals(v), cfg, texture)
+                r.rasterize_frames(solid[f0:f1], v, col, np.bincount(fi[a:b] - f0, minlength=f1 - f0), out=solid[f0:f1])
+            eng.raise_if_error()
+        blended = Sim3DR.add_weighted(stack, solid, alpha)
+        if isinstance(frames, torch.Tensor) and frames.is_cuda:
+            return blended, solid
+        return blended.cpu().numpy(), solid.cpu().numpy()
 
 
 class SynergyNet(_SynergyBase):

@@ -19,15 +19,27 @@ def _to_ctype(arr):
     return arr if arr.flags.c_contiguous else arr.copy(order='C')
 
 
-def render(img, ver_lst, alpha=0.6, wfp=None, tex=None, connectivity=None):
+def _triangles(connectivity):
     if connectivity is not None:
-        tri = _to_ctype(np.asarray(connectivity).T).astype(np.int32)                  # :37-38
-    else:
-        pack_tri = get_param_pack().tri
-        if pack_tri is None:
-            raise RuntimeError('Missing data: 3dmm_data/tri.mat')                    # the reference's loadmat would raise here
-        tri = _to_ctype((np.asarray(pack_tri) - 1).T).astype(np.int32)               # :32-33
-    res, _overlap = Sim3DR.render(img, ver_lst, tri, alpha=alpha, wfp=wfp, tex=tex, cfg=cfg)
+        return _to_ctype(np.asarray(connectivity).T).astype(np.int32)                 # :35-36
+    pack_tri = get_param_pack().tri
+    if pack_tri is None:
+        raise RuntimeError('Missing data: 3dmm_data/tri.mat')                        # the reference's loadmat would raise here
+    return _to_ctype((np.asarray(pack_tri) - 1).T).astype(np.int32)                  # :32-33
+
+
+def render(img, ver_lst, alpha=0.6, wfp=None, tex=None, connectivity=None):
+    res, _overlap = Sim3DR.render(img, ver_lst, _triangles(connectivity), alpha=alpha, wfp=wfp, tex=tex, cfg=cfg)
     if wfp is not None:
         print(f'Save mesh result to {wfp}')
     return res
+
+
+def render_batch(imgs, ver_lsts, alpha=0.6, wfps=None, tex=None, connectivity=None):
+    """:func:`render` for N equally sized frames in one pass (:func:`synergynet_b200.Sim3DR.render_batch`): returns the
+    list of blended images, entry i being ``render(imgs[i], ver_lsts[i], alpha, wfps[i], tex, connectivity)``."""
+    out = Sim3DR.render_batch(imgs, ver_lsts, _triangles(connectivity), alpha=alpha, wfps=wfps, tex=tex, cfg=cfg)
+    for wfp in wfps or []:
+        if wfp is not None:
+            print(f'Save mesh result to {wfp}')
+    return [res for res, _overlap in out]
