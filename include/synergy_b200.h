@@ -125,7 +125,9 @@ int syn_reconstruct_image(syn_handle_t* h, const float* params62_dev, int batch,
                           float* out_dev, void* stream);
 /* parse_pose + predict_pose (utils/inference.py:33-62,86-92,146-157) for B whitened vectors: angles_dev (B,3) fp64
  * degrees [pitch-like x, yaw-like y, roll-like z in the reference's order], t3d_dev (B,3) fp32 (image coordinates when
- * roi5_dev is given, crop coordinates when NULL). */
+ * roi5_dev is given, crop coordinates when NULL).  One deliberate departure from the reference: the fp32 cross product
+ * gives |R20| = 1 + 2^-23 for some camera rows at yaw +-90 degrees, where the reference's math.asin raises; every
+ * |R20| >= 1 takes the gimbal-lock branch of R20's sign, the reference's own value at R20 = +-1 (x = +90 for -1). */
 int syn_pose_decode(syn_handle_t* h, const float* params62_dev, int batch, const float* roi5_dev, double* angles_dev,
                     float* t3d_dev, void* stream);
 /* CenterCrop(margin, mode='test') of the reference loader (utils/ddfa.py:162-243, benchmark.py:116): the uint8 entry
@@ -313,6 +315,7 @@ enum {
   SYN_NMS_CPU_NMS = 0,     /* FaceBoxes/utils/nms/cpu_nms.pyx:17-68, the path nms_wrapper.py:13-18 takes: suppress on   */
                            /* ovr >= thresh, compared in double                                                       */
   SYN_NMS_PY_CPU_NMS = 1   /* FaceBoxes/utils/nms/py_cpu_nms.py:10-38: keep on ovr <= thresh, compared in float32     */
+                           /* (a NaN overlap, from a box with a NaN coordinate, fails that test: the box is dropped)   */
 };
 /* Greedy NMS of dets_dev (n,5) fp32 rows [x1 y1 x2 y2 score] ALREADY in descending score order (FaceBoxes.py:116-121
  * sorts before it calls nms).  keep_dev (n) int32 receives the kept row indices in order, *n_keep_dev their count:

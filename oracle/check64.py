@@ -34,6 +34,15 @@ def worst(got, want, s) -> Tuple[float, tuple]:
     return float(r.reshape(-1)[i]), tuple(int(v) for v in np.unravel_index(i, r.shape))
 
 
+def f32_dot3(a: np.ndarray, b: np.ndarray) -> np.ndarray:
+    """((a0 b0 + a1 b1) + a2 b2) over the last axis in elementwise float32, one rounding per operation and no fused
+    multiply-add: the order of a kernel's unrolled three-term sum (np.linalg.norm / np.dot go through BLAS, whose order
+    and FMA use depend on the host)."""
+    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
+    with np.errstate(all='ignore'):
+        return (a[..., 0] * b[..., 0] + a[..., 1] * b[..., 1]) + a[..., 2] * b[..., 2]
+
+
 def fold_bn(sd: Dict[str, torch.Tensor], bn_key: str, w: torch.Tensor,
             conv_bias: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """The eval-mode BatchNorm ``bn_key`` folded into the conv weight ``w`` (output channels first) and its bias:

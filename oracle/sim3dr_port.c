@@ -102,7 +102,7 @@ void port_rasterize(unsigned char* image, const float* vertices, const int32_t* 
 
 /* dets (n,5) float32, order (n) = indices by descending score (the caller's argsort, as :27); keep (n) out; returns count.
  * ge != 0: suppress when ovr >= thresh (cpu_nms.pyx:65, thresh a C double); ge == 0: py_cpu_nms.py:35 keeps ovr <= thresh
- * with a float32 comparison */
+ * with a float32 comparison, so a NaN overlap suppresses there */
 int port_nms(const float* dets, const int64_t* order, int n, double thresh, int ge, int64_t* keep) {
   unsigned char* dead = (unsigned char*)calloc((size_t)(n > 0 ? n : 1), 1);
   int cnt = 0;
@@ -124,7 +124,7 @@ int port_nms(const float* dets, const int64_t* order, int n, double thresh, int 
       const float iw = 0.0f >= ww ? 0.0f : ww, ih = 0.0f >= hh ? 0.0f : hh;
       const float inter = iw * ih;
       const float ovr = inter / (area_i + area_j - inter);
-      if (ge ? ((double)ovr >= thresh) : (ovr > thr_f)) dead[j] = 1;
+      if (ge ? ((double)ovr >= thresh) : !(ovr <= thr_f)) dead[j] = 1;
     }
   }
   free(dead);

@@ -62,6 +62,18 @@ TAU = {
     # Negative control (tests/test_recon_oracle.py, numpy emulation): one of the three passes dropped measures >= 3.7e-5,
     # coefficients clamped at 60000 instead of face-scaled 0.998: >= 15x the bar.
 }
+# post64 (the kernels either side of the path: pose decode, box decode, losses).  'pose_seq' holds the kernel's angles
+# to the double-precision angles of the fp32 R it claims to compute (S in double ulps: a few ulps of libm); the rest hold
+# fp32 results to float64 (S without the unit round-off 2^-24 = 6.0e-8, which TAU carries).  At most 4x the worst ratio
+# measured on an H100 80GB HBM3 (132 SMs, 700 W power limit) over tests/test_gpu_post_oracle.py (worst in the comment):
+TAU['post64'] = {'pose_seq': 6.8e-16,   # 1.70e-16: the device's double asin / cos / atan2 against the host's
+                 'pose': 1.6e-7,        # 4.09e-08: the yaw sweep through the lock (the host emulation measures the same)
+                 't3d': 2.2e-7,         # 5.62e-08: t * k + s with the crop box
+                 'decode': 1.2e-7,      # 3.10e-08: expf (torch's CPU decode measures 2.62e-08)
+                 'wing': 1.6e-7,        # 7.45e-09; the reference's own fp32 sums (torch, CPU) measure 3.8e-08
+                 'param_loss': 5.8e-8}  # 1.45e-08
+# Negative controls (tests/test_post_oracle.py): an FMA-contracted norm measures 2.8e-06 on 'pose_seq' (4e9 x the bar),
+# the float32-trigonometry pose and a decode whose exp is 64 ulps off fail 'pose' / 'decode'.
 # mbv1_64.  'gemm' and 'pool' are those of gemm64; 'dw' holds the fp32 CUDA-core stages (stem, K = 27, and the depthwise
 # convs, K = 9), at most 4x the worst ratio measured on an H100 80GB HBM3 (132 SMs, 700 W power limit) over the five
 # widths, the batches and both checkpoints of tests/test_gpu_mbv1.py (worst in the comment):

@@ -39,26 +39,32 @@ __global__ void bits_to_float_kernel(const unsigned* __restrict__ src, float* __
   if (i < n) dst[i] = __uint_as_float(src[i]);
 }
 
-// WingLoss (loss_definition.py:8-27): mean over all B*3*N coordinates of
-//   omega * log(1 + d / eps)  if d < omega   else   d - (omega - omega * log(1 + omega / eps)),   d = |target - pred|.
+// WingLoss (loss_definition.py:8-27): mean over the B*3*N coordinates whose d = |target - pred| passes `d < omega` or
+// `d >= omega` (a NaN delta passes neither and is left out of the sums and the count, as the reference's masks do) of
+//   omega * log(1 + d / eps)  if d < omega   else   d - C,   C = omega - omega * log(1 + omega / eps)
+// with C evaluated in double and rounded to fp32 where it meets the fp32 delta, like the reference's Python float.
 // One CTA; partial sums in double, fixed reduction order (deterministic).
 __global__ void __launch_bounds__(1024) wing_loss_kernel(const float* __restrict__ pred, const float* __restrict__ target,
                                                          size_t n, float omega, float epsilon, float* __restrict__ out) {
   __shared__ double part[1024];
-  const float log_term = logf(1.0f + omega / epsilon);
-  const float C = omega - omega * log_term;
+  __shared__ unsigned long long cnt[1024];
+  const double om = omega;
+  const float C = (float)__dsub_rn(om, __dmul_rn(om, log(1.0 + om / (double)epsilon)));
   double s = 0.0;
+  unsigned long long c = 0;
   for (size_t i = threadIdx.x; i < n; i += blockDim.x) {
     const float d = fabsf(target[i] - pred[i]);
-    s += (d < omega) ? (double)(omega * logf(1.0f + d / epsilon)) : (double)(d - C);
+    if (d < omega) { s += (double)(omega * logf(1.0f + d / epsilon)); ++c; }
+    else if (d >= omega) { s += (double)(d - C); ++c; }
   }
   part[threadIdx.x] = s;
+  cnt[threadIdx.x] = c;
   __syncthreads();
   for (int o = 512; o > 0; o >>= 1) {
-    if ((int)threadIdx.x < o) part[threadIdx.x] += part[threadIdx.x + o];
+    if ((int)threadIdx.x < o) { part[threadIdx.x] += part[threadIdx.x + o]; cnt[threadIdx.x] += cnt[threadIdx.x + o]; }
     __syncthreads();
   }
-  if (threadIdx.x == 0) out[0] = (float)(part[0] / (double)n);
+  if (threadIdx.x == 0) out[0] = (float)(part[0] / (double)cnt[0]);
 }
 
 // ParamLoss (loss_definition.py:29-42), one value per sample:

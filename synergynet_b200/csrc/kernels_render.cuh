@@ -334,7 +334,8 @@ __global__ void add_weighted_u8_kernel(const unsigned char* a, const unsigned ch
 // ---- NMS (SURVEY.md section 8 row f3: FaceBoxes/utils/nms/cpu_nms.pyx:17-68, py_cpu_nms.py:10-38) -----------------------
 // dets (n, 5) fp32 [x1 y1 x2 y2 score], ALREADY in the order the greedy loop visits them (descending score).
 // mask[i][j / 64] bit (j % 64) = box j (> i) is suppressed by box i.  ge != 0: `ovr >= thresh` in double (cpu_nms.pyx:65,
-// thresh is a C double there); ge == 0: py_cpu_nms keeps `ovr <= thresh` in float32, i.e. suppresses on `ovr > thresh`.
+// thresh is a C double there); ge == 0: py_cpu_nms keeps `ovr <= thresh` in float32, i.e. suppresses on `!(ovr <= thresh)`,
+// so a NaN overlap (a box with a NaN or +-inf-minus-inf coordinate) is suppressed there and kept by cpu_nms.
 // Segmented (syn_nms_batch): n_dev != nullptr, grid.z = frame.  Frame f owns rows [f * n, (f + 1) * n) of dets and a mask
 // block sized for n rows, of which its own count n_dev[f] <= n are valid and laid out with ITS OWN word count, so the
 // bits (and the scan below) are those of a one-image call with that count.  The grid is sized for n.
@@ -365,7 +366,7 @@ __global__ void nms_mask_kernel(const float* __restrict__ dets, int n, double th
       if (j <= i || j >= n) continue;
       const float bq[4] = {dets[j * 5], dets[j * 5 + 1], dets[j * 5 + 2], dets[j * 5 + 3]};
       const float ovr = rmath::box_overlap(a, area_a, bq, rmath::box_area(bq[0], bq[1], bq[2], bq[3]));
-      const bool sup = ge ? ((double)ovr >= thresh) : (ovr > thr_f);
+      const bool sup = ge ? ((double)ovr >= thresh) : !(ovr <= thr_f);
       if (sup) bits |= 1ull << jj;
     }
   }

@@ -59,14 +59,15 @@ __global__ void pose_decode_kernel(const float* __restrict__ params, const float
   const double R00 = r1[0], R01 = r1[1], R02 = r1[2], R12 = r2[2], R20 = r3[0], R22 = r3[2];
   const double kPi = 3.14159265358979323846;
   double x, y, z;
-  if (R20 != 1.0 && R20 != -1.0) {                           // matrix2angle_corr, utils/inference.py:45-62
+  // matrix2angle_corr, utils/inference.py:45-62, with one deliberate departure: the fp32 cross product can give
+  // |R20| = 1 + 2^-23 for rows at yaw +-90 degrees, where asin is NaN (the reference's math.asin raises).  Every
+  // |R20| >= 1 takes the gimbal-lock branch of R20's sign, the reference's own value at +-1; NaN takes the general one.
+  if (R20 >= 1.0) { z = 0.0; x = -kPi / 2; y = -z + atan2(-R01, -R02); }
+  else if (R20 <= -1.0) { z = 0.0; x = kPi / 2; y = z + atan2(R01, R02); }
+  else {
     x = asin(R20);
     y = atan2(R12 / cos(x), R22 / cos(x));
     z = atan2(R01 / cos(x), R00 / cos(x));
-  } else {                                                   // gimbal lock
-    z = 0.0;
-    if (R20 == -1.0) { x = kPi / 2; y = z + atan2(R01, R02); }
-    else { x = -kPi / 2; y = -z + atan2(-R01, -R02); }
   }
   angles[(size_t)b * 3 + 0] = x * 180 / kPi;
   angles[(size_t)b * 3 + 1] = y * 180 / kPi;

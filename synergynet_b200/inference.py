@@ -1,7 +1,8 @@
 """Host-side API semantics around the hot path, batched (reference ``utils/inference.py``).
 
-Only tiny per-face affine / pose algebra, the integer ROI crop (the host restatement the tests compare against) and its
-device twin ``crop_resize_device`` live here; vertex reconstruction itself runs on the GPU (``Engine.reconstruct``).
+Only tiny per-face affine algebra, the integer ROI crop (the host restatement the tests compare against) and its
+device twin ``crop_resize_device`` live here; vertex reconstruction and the pose decode run on the GPU
+(``Engine.reconstruct``, ``Engine.pose_decode``).
 """
 from __future__ import annotations
 
@@ -190,50 +191,6 @@ def roi_affine(roi_boxes: Sequence[Sequence[float]]) -> np.ndarray:
         sx, sy, ex, ey = box[:4]
         kx, ky = (ex - sx) / STD_SIZE, (ey - sy) / STD_SIZE
         out[i] = (kx, sx, ky, sy, (kx + ky) / 2)
-    return out
-
-
-def decompose_camera(P: np.ndarray) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
-    """Batched P2sRt (utils/inference.py:33-43): P (B,3,4) -> scale (B,), R (B,3,3), t (B,3)."""
-    r1, r2 = P[:, 0, :3], P[:, 1, :3]
-    n1 = np.linalg.norm(r1, axis=1, keepdims=True)
-    n2 = np.linalg.norm(r2, axis=1, keepdims=True)
-    u1, u2 = r1 / n1, r2 / n2
-    R = np.stack([u1, u2, np.cross(u1, u2)], axis=1)
-    return ((n1 + n2) / 2.0)[:, 0], R, P[:, :, 3]
-
-
-def rotation_to_euler_deg(R: np.ndarray) -> np.ndarray:
-    """Batched matrix2angle_corr (utils/inference.py:45-62) -> (B,3) degrees."""
-    r20 = R[:, 2, 0]
-    lock = (r20 == 1) | (r20 == -1)
-    x = np.arcsin(np.clip(r20, -1, 1))
-    cx = np.where(lock, 1.0, np.cos(x))
-    y = np.arctan2(R[:, 1, 2] / cx, R[:, 2, 2] / cx)
-    z = np.arctan2(R[:, 0, 1] / cx, R[:, 0, 0] / cx)
-    neg = r20 == -1
-    x = np.where(lock, np.where(neg, np.pi / 2, -np.pi / 2), x)
-    y = np.where(lock, np.where(neg, np.arctan2(R[:, 0, 1], R[:, 0, 2]),
-                                np.arctan2(-R[:, 0, 1], -R[:, 0, 2])), y)
-    z = np.where(lock, 0.0, z)
-    return np.stack([x, y, z], 1) * (180.0 / np.pi)
-
-
-def predict_pose_batch(params: np.ndarray, param_mean: np.ndarray, param_std: np.ndarray,
-                       roi_boxes: Sequence[Sequence[float]]):
-    """parse_pose + predict_pose (utils/inference.py:86-92,146-157) for B whitened vectors.
-    Returns a list of ``[angles(list of 3), t3d(ndarray 3)]`` like the reference."""
-    p = params * param_std[:62] + param_mean[:62]
-    cam = p[:, :12].reshape(-1, 3, 4)
-    _, R, t3d = decompose_camera(cam)
-    ang = rotation_to_euler_deg(R)
-    out = []
-    for i, box in enumerate(roi_boxes):
-        sx, sy, ex, ey = box[:4]
-        t = t3d[i].copy()
-        t[0] = t[0] * ((ex - sx) / STD_SIZE) + sx
-        t[1] = t[1] * ((ey - sy) / STD_SIZE) + sy
-        out.append([[float(a) for a in ang[i]], t])
     return out
 
 

@@ -104,7 +104,7 @@ int emul_nms(const float* dets, int n, double thresh, int ge, int32_t* keep) {
     for (int j = i + 1; j < n; ++j) {
       const float* b = dets + 5 * (size_t)j;
       const float ovr = box_overlap(a, area_a, b, box_area(b[0], b[1], b[2], b[3]));
-      if (ge ? ((double)ovr >= thresh) : (ovr > thr_f)) mask[(size_t)i * words + j / 64] |= 1ull << (j % 64);
+      if (ge ? ((double)ovr >= thresh) : !(ovr <= thr_f)) mask[(size_t)i * words + j / 64] |= 1ull << (j % 64);
     }
   }
   // the scan of nms_scan_kernel: one 64-box block at a time -- resolve the block against its diagonal word, then OR the

@@ -105,18 +105,6 @@ def test_crop_img_matches_oracle_on_random_boxes():
     assert np.array_equal(inference.crop_img(gray, [-3.2, 4.4, 50.5, 60.6, 1]), rp.crop_img(gray, [-3.2, 4.4, 50.5, 60.6, 1]))
 
 
-def test_pose_decode_matches_oracle(synth_pack):
-    rng = np.random.default_rng(1)
-    params = rng.standard_normal((16, 62)).astype(np.float32)
-    boxes = [[10.0 + i, 20.0, 150.0 + 2 * i, 170.0, 1.0] for i in range(16)]
-    pack = dict(param_mean=synth_pack.param_mean, param_std=synth_pack.param_std)
-    got = inference.predict_pose_batch(params, synth_pack.param_mean, synth_pack.param_std, boxes)
-    for i in range(16):
-        ang, t3d = rp.predict_pose(params[i], pack, boxes[i])
-        assert np.allclose(got[i][0], ang, atol=1e-3)
-        assert np.allclose(got[i][1], t3d, rtol=1e-5)
-
-
 def test_rescale_and_square_roi_match_oracle():
     v = np.random.default_rng(2).standard_normal((3, 68)).astype(np.float32) * 50
     box = [12.5, 7.25, 190.0, 201.5, 0.9]
