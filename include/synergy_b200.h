@@ -345,6 +345,16 @@ int syn_faceboxes_decode(const float* loc_dev, const float* conf_dev, int im_hei
 int syn_faceboxes_decode_batch(const float* loc_dev, const float* conf_dev, int n_frames, int im_height, int im_width,
                                float box_scale_w, float box_scale_h, float scale, float conf_thresh, int top_k, int32_t* cand_ws_dev,
                                float* dets_dev, int32_t* n_dets_dev, void* stream);
+/* FaceBoxes.py:98-121 (FaceBoxes.__call__ once per image) for n_images network inputs of any sizes in the same two
+ * launches: loc_dev (sum P_i,4), conf_dev (sum P_i,2) as syn_fb_forward_images writes them, P_i =
+ * syn_faceboxes_num_priors(heights_host[i], widths_host[i]) and image i's priors after those of images 0..i-1.  Image i
+ * decodes with box scale (widths_host[i], heights_host[i]) (:101) and shrink factor scale_host[i] (:104) into its own
+ * (top_k,5) block of dets_dev (n_images,top_k,5) and its own count in n_dets_dev (n_images): the rows and count
+ * syn_faceboxes_decode gives for that image alone.  cand_ws_dev: n_images + sum P_i int32.  1 <= n_images <=
+ * SYN_FB_MAX_FRAMES; sizes < 1 or a scale that is not > 0 are SYN_ERR_INVALID before anything is launched. */
+int syn_faceboxes_decode_images(const float* loc_dev, const float* conf_dev, int n_images, const int32_t* heights_host,
+                                const int32_t* widths_host, const float* scale_host, float conf_thresh, int top_k, int32_t* cand_ws_dev,
+                                float* dets_dev, int32_t* n_dets_dev, void* stream);
 
 /* ---- crop + resize of uint8 BGR images (crop_img + cv2.resize) ---------------------------------------------------------
  * The face crops of get_all_outputs (utils/inference.py:95-125 crop_img, then cv2.resize to 120x120: INTER_LANCZOS4 in
@@ -379,12 +389,30 @@ int syn_crop_resize_plan_frames_host(const int32_t* rois_host, const int32_t* fr
 int syn_crop_resize_batch(const uint8_t* images_dev, int n_frames, int height, int width, int channels, const void* plan_dev,
                           int batch, int out_h, int out_w, int mode, uint8_t* out_dev, int64_t stride_roi, int64_t stride_y,
                           int64_t stride_x, int64_t stride_c, void* stream);
+/* The same stage for a list of images of any sizes in ONE launch, every ROI with its own output size: the crops of every
+ * face of every image (synergy3DMM.py:186-188 once per face per image), or the detector's shrink of every oversized image
+ * to its own size (FaceBoxes.py:62-79, a different scale per image).  images_dev: n_images uint8 BGR images packed back to
+ * back, image i (heights_host[i] x widths_host[i] x 3) at byte sum_{j<i} 3 h_j w_j.  ROI b reads image images_host[b] and
+ * is resized to out_h_host[b] x out_w_host[b]; its output follows the outputs of ROIs 0..b-1 (3 out_h out_w bytes each),
+ * planar (3,h,w) when planar = 1, interleaved (h,w,3) when planar = 0.  The plan, syn_crop_resize_images_plan_size bytes
+ * (-1 for a bad argument), is CropImagesRoi[batch] followed by, for every ROI, the bytes syn_crop_resize_plan_host makes
+ * for that ROI alone.  Output bytes are those of syn_crop_resize on each image.  Null pointers, an empty batch, sizes < 1
+ * and an unknown mode fail before anything is written or launched; an image index outside 0..n_images-1 is
+ * SYN_ERR_SHAPE. */
+int64_t syn_crop_resize_images_plan_size(int batch, const int32_t* out_h_host, const int32_t* out_w_host, int mode);
+int syn_crop_resize_plan_images_host(const int32_t* rois_host, const int32_t* images_host, int n_images, const int32_t* heights_host,
+                                     const int32_t* widths_host, int batch, const int32_t* out_h_host, const int32_t* out_w_host,
+                                     int mode, void* plan_out, int64_t plan_bytes);
+int syn_crop_resize_images(const uint8_t* images_dev, const void* plan_dev, int batch, const int32_t* out_h_host, const int32_t* out_w_host,
+                           int mode, int planar, uint8_t* out_dev, void* stream);
 
 /* The detector network (FaceBoxes/models/faceboxes.py:68-150, FaceBoxesNet in 'test' phase) on ONE image of any size
- * (syn_fb_forward), or on a stack of frames of one size (syn_fb_forward_batch).
+ * (syn_fb_forward), on a stack of frames of one size (syn_fb_forward_batch), or on a list of images of any sizes
+ * (syn_fb_forward_images).
  * A separate handle: the detector has its own weights and workspace and does not touch syn_handle_t.  Like syn_handle_t
  * it is bound to one device and is not re-entrant (its activation workspace is shared by consecutive calls, which are
- * ordered by the stream they are enqueued on; a change of image size synchronises the device and reallocates).
+ * ordered by the stream they are enqueued on).  The workspace only grows: a call that needs more bytes than an earlier
+ * one synchronises the device and reallocates, a call that fits runs without any synchronisation.
  * 33 convolutions in execution order (syn_fb_layer_desc names them with the reference's state_dict prefixes:
  * "conv1", "inception2.branch3x3_2", "loc.0" ...): layers with has_bn take the conv weight (OIHW fp32, no bias) and
  * the eval-mode BatchNorm2d of the same block (<name>.conv.weight / <name>.bn.*), the six head layers take weight +
@@ -408,13 +436,23 @@ int  syn_fb_forward(syn_fb_t* f, const uint8_t* image_dev, int height, int width
 int64_t syn_fb_launch_count(const syn_fb_t* f);
 /* FaceBoxes.__call__ lines 88-96 for n_frames images of one size in the SAME 39 launches (syn_fb_launch_count grows by 39
  * whatever n_frames is): images_dev (n_frames,height,width,3) uint8 BGR -> loc_dev (n_frames,P,4), conf_dev
- * (n_frames,P,2).  Rows of every convolution's implicit GEMM run over frame * pixels + pixel; each output element is
- * computed by the one-image kernel's arithmetic in its order, so frame i's outputs are, bit for bit, syn_fb_forward's for
- * image i.  The workspace grows to n_frames times the one-image maps (15.5 MB per 720 x 1080 frame, so about 1 GB at
- * SYN_FB_MAX_FRAMES); more frames per call are SYN_ERR_INVALID, callers split the stack. */
+ * (n_frames,P,2).  This is syn_fb_forward_images with every size equal.  Rows of every convolution's implicit GEMM run
+ * over the packed pixels of all frames; each output element is computed by the one-image kernel's arithmetic in its
+ * order, so frame i's outputs are, bit for bit, syn_fb_forward's for image i.  The workspace grows to n_frames times the
+ * one-image maps (15.5 MB per 720 x 1080 frame, so about 1 GB at SYN_FB_MAX_FRAMES); more frames per call are
+ * SYN_ERR_INVALID, callers split the stack. */
 #define SYN_FB_MAX_FRAMES 64
 int  syn_fb_forward_batch(syn_fb_t* f, const uint8_t* images_dev, int n_frames, int height, int width, float* loc_dev,
                           float* conf_dev, void* stream);
+/* FaceBoxes.__call__ lines 88-96 (FaceBoxes/FaceBoxes.py, once per image) for n_images images of any sizes in the SAME 39
+ * launches: images_dev holds them packed back to back, image i (heights_host[i] x widths_host[i] x 3 uint8 BGR) at byte
+ * sum_{j<i} 3 h_j w_j; loc_dev (sum P_i,4) and conf_dev (sum P_i,2) get image i's priors after those of images 0..i-1.
+ * Every map of the network is packed the same way; each launch takes a per-image geometry table (map sizes and first
+ * pixel of every image at every map size), uploaded with one asynchronous copy per call.  Image i's outputs are, bit for
+ * bit, syn_fb_forward's on image i alone.  1 <= n_images <= SYN_FB_MAX_FRAMES; null pointers and sizes < 1 fail before
+ * anything is launched. */
+int  syn_fb_forward_images(syn_fb_t* f, const uint8_t* images_dev, int n_images, const int32_t* heights_host, const int32_t* widths_host,
+                           float* loc_dev, float* conf_dev, void* stream);
 /* Per-stage tests of the detector network.  Runs syn_fb_forward's launch sequence unchanged and returns right after launch
  * `stage` (0..38), having copied (on the stream) the whole tensor that launch wrote to out_dev, which holds out_numel
  * floats (SYN_ERR_SHAPE if that is not the tensor's size).  The activation workspace is zeroed first, so channel slices
@@ -434,6 +472,12 @@ int  syn_fb_debug_forward_until(syn_fb_t* f, const uint8_t* image_dev, int heigh
  * launch's maps, or the whole (n_frames,P*4) loc / (n_frames,P*2) conf for stages 32..38. */
 int  syn_fb_debug_forward_batch_until(syn_fb_t* f, const uint8_t* images_dev, int n_frames, int height, int width, int stage,
                                       float* out_dev, int64_t out_numel, float* loc_dev, float* conf_dev, void* stream);
+/* syn_fb_forward_images stopped after launch `stage` of the same table: out_dev receives every image's map of that launch
+ * packed back to back (image i's (h_i,w_i,c) map after those of images 0..i-1), or the whole packed (sum P_i * 4) loc /
+ * (sum P_i * 2) conf for stages 32..38. */
+int  syn_fb_debug_forward_images_until(syn_fb_t* f, const uint8_t* images_dev, int n_images, const int32_t* heights_host,
+                                       const int32_t* widths_host, int stage, float* out_dev, int64_t out_numel, float* loc_dev,
+                                       float* conf_dev, void* stream);
 
 /* ---- introspection ---------------------------------------------------------------------------*/
 /* Number of kernels this handle has launched since creation (bench.py "gpu_launches"). */

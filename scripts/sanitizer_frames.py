@@ -1,7 +1,9 @@
 #!/usr/bin/env python
-"""The frame-batch path for `compute-sanitizer --tool memcheck` (needs an H100): one batched detector pass on frames whose
-maps make 64-row tiles straddle frames, one ``detect_batch`` with the device shrink, one ``get_all_outputs_batch`` with
-ROIs over the frame edges and a frame without a face.  scripts/sanitizer_smoke.py covers the one-image kernels."""
+"""The frame-batch and image-list paths for `compute-sanitizer --tool memcheck` / `--tool racecheck` (needs an H100): one
+batched detector pass on frames whose maps make 64-row tiles straddle frames, one ``detect_batch`` with the device
+shrink, one ``get_all_outputs_batch`` with ROIs over the frame edges and a frame without a face; then the same on a list of
+images of different sizes (1 x 1 images sharing a tile, two oversized images shrunk by different scales).
+scripts/sanitizer_smoke.py covers the one-image kernels."""
 import os
 import sys
 import types
@@ -27,9 +29,17 @@ def main():
     m.eval()
     rects = [[[-10.0, -5.0, 50.0, 55.0, 0.9], [150.0, 120.0, 300.0, 230.0, 0.8]], [], [[40.0, 20.0, 100.0, 80.0, 0.7]]]
     out = m.get_all_outputs_batch(frames, rects=rects)
+    sizes = [(193, 258), (1, 1), (1, 333), (1, 1), (750, 1100), (1500, 900), (97, 61)]
+    images = [synthetic.make_scene_u8(h, w, s) for s, (h, w) in enumerate(sizes)]
+    small = [torch.from_numpy(im).cuda() for im in images if im.shape[0] <= 720 and im.shape[1] <= 1080]
+    loc_i, _ = det.net.forward_images(small)
+    boxes_i = det.detect_images(images)
+    rects_i = [rects[0], [], rects[2], [], [[600.0, 650.0, 1200.0, 780.0, 0.9]], [], [[-3.0, -3.0, 80.0, 70.0, 0.9]]]
+    out_i = m.get_all_outputs_images(images, rects=rects_i)
     torch.cuda.synchronize()
     m._engine(torch.device('cuda', 0)).raise_if_error()
     print('sanitizer frames done:', tuple(loc.shape), [len(b) for b in boxes], [len(b) for b in big], [len(t[0]) for t in out])
+    print('sanitizer images done:', [tuple(x.shape) for x in loc_i], [len(b) for b in boxes_i], [len(t[0]) for t in out_i])
 
 
 if __name__ == '__main__':

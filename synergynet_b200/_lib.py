@@ -128,6 +128,12 @@ SIGNATURES = {
     'syn_nms_batch': (_I, [_F, _F, _I, _I, C.c_double, _I, _F, _F, _F, _P]),
     'syn_crop_resize_plan_frames_host': (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _L]),
     'syn_crop_resize_batch': (_I, [_P, _I, _I, _I, _I, _P, _I, _I, _I, _I, _P, _L, _L, _L, _L, _P]),
+    'syn_fb_forward_images': (_I, [_P, _F, _I, _P, _P, _F, _F, _P]),
+    'syn_fb_debug_forward_images_until': (_I, [_P, _F, _I, _P, _P, _I, _F, _L, _F, _F, _P]),
+    'syn_faceboxes_decode_images': (_I, [_F, _F, _I, _P, _P, _P, C.c_float, _I, _F, _F, _F, _P]),
+    'syn_crop_resize_images_plan_size': (_L, [_I, _P, _P, _I]),
+    'syn_crop_resize_plan_images_host': (_I, [_P, _P, _I, _P, _P, _I, _P, _P, _I, _P, _L]),
+    'syn_crop_resize_images': (_I, [_P, _P, _I, _P, _P, _I, _I, _F, _P]),
     'syn_launch_count': (_L, [_P]),
     'syn_set_timing': (_I, [_P, _I]),
     'syn_get_timings': (_I, [_P, C.POINTER(C.c_float), C.POINTER(C.c_char_p), _I, C.POINTER(C.c_int)]),
@@ -155,7 +161,9 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_fb_debug_forward_until', 'syn_fb_forward_batch', 'syn_fb_debug_forward_batch_until',
                                              'syn_faceboxes_decode_batch', 'syn_nms_batch', 'syn_crop_resize_plan_frames_host',
                                              'syn_crop_resize_batch', 'syn_render_frames_plan', 'syn_rasterize_frames',
-                                             'syn_add_weighted_u8')}
+                                             'syn_add_weighted_u8', 'syn_fb_forward_images', 'syn_fb_debug_forward_images_until',
+                                             'syn_faceboxes_decode_images', 'syn_crop_resize_images_plan_size',
+                                             'syn_crop_resize_plan_images_host', 'syn_crop_resize_images')}
 
 
 def declared_symbols(header: str = HEADER_PATH):

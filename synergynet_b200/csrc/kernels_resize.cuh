@@ -33,4 +33,34 @@ __global__ void __launch_bounds__(kResizeBX * kResizeBY) crop_resize_kernel(cons
   o[2 * sc] = px[2];
 }
 
+// The crops of a list of images of any sizes (syn_crop_resize_images): every ROI has its own source image and its own output
+// size.  The plan is CropImagesRoi[B] followed by one one-ROI plan per ROI (resize_math.h's layout and tables, the bytes
+// syn_crop_resize_plan_host makes for that ROI alone).
+struct CropImagesRoi {
+  long long src;           // byte offset of the ROI's image in the packed images (image i at sum_{j<i} 3 h_j w_j)
+  int h, w;                // that image's size
+  int out_h, out_w;        // this ROI's output size
+  long long out;           // byte offset of its output: outputs packed back to back, 3 out_h out_w bytes each
+  long long plan;          // byte offset of its one-ROI plan in the plan buffer
+};
+
+// grid.z = ROI, grid.x / .y cover the largest output; planar: (3,h,w) outputs (the backbone's crops), else (h,w,3) images
+template <int K>
+__global__ void __launch_bounds__(kResizeBX * kResizeBY) crop_resize_images_kernel(const uint8_t* __restrict__ images,
+                                                                                   const void* __restrict__ plan,
+                                                                                   uint8_t* __restrict__ out, int planar) {
+  const CropImagesRoi r = static_cast<const CropImagesRoi*>(plan)[blockIdx.z];
+  const int ox = blockIdx.x * kResizeBX + threadIdx.x, oy = blockIdx.y * kResizeBY + threadIdx.y;
+  if (ox >= r.out_w || oy >= r.out_h) return;
+  const rsz::PlanView v = rsz::plan_view(static_cast<const char*>(plan) + r.plan, 1, r.out_h, r.out_w, K);
+  uint8_t px[3];
+  rsz::resize_pixel<K>(images + r.src, r.h, r.w, v, 0, r.out_h, r.out_w, oy, ox, px);
+  const long long plane = (long long)r.out_h * r.out_w, at = (long long)oy * r.out_w + ox;
+  uint8_t* o = out + r.out + (planar ? at : 3 * at);
+  const long long sc = planar ? plane : 1;
+  o[0] = px[0];
+  o[sc] = px[1];
+  o[2 * sc] = px[2];
+}
+
 }  // namespace syn

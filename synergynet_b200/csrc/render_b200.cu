@@ -85,6 +85,25 @@ int crop_launch(const uint8_t* image_dev, int n_frames, int height, int width, i
   return SYN_OK;
 }
 
+// frame f of a decode launch's table
+FbDecodeFrames decode_frame(FbDecodeFrames t, int f, int h, int w, float box_scale_w, float box_scale_h, float scale, int p0, int c0,
+                            int i0) {
+  t.h[f] = h; t.w[f] = w; t.np[f] = faceboxes_num_priors(h, w); t.p0[f] = p0; t.c0[f] = c0; t.i0[f] = i0;
+  t.box_scale_w[f] = box_scale_w; t.box_scale_h[f] = box_scale_h; t.scale[f] = scale;
+  return t;
+}
+
+// the two decode launches of every decode entry: grid.y = frame, grid.x sized for np_max priors; counts already zeroed
+int decode_launch(const float* loc, const float* conf, const FbDecodeFrames& t, int n_frames, int np_max, float conf_thresh, int top_k,
+                  int32_t* cand, float* dets, int32_t* n_dets, cudaStream_t st) {
+  faceboxes_select_kernel<<<dim3((np_max + 255) / 256, n_frames), 256, 0, st>>>(conf, t, conf_thresh, cand);
+  SYN_LAUNCH_CHECK("faceboxes_select_kernel");
+  faceboxes_rank_decode_kernel<<<dim3((np_max + 127) / 128, n_frames), 128, 0, st>>>(loc, conf, t, top_k, cand,
+                                                                                                        dets, n_dets);
+  SYN_LAUNCH_CHECK("faceboxes_rank_decode_kernel");
+  return SYN_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -309,6 +328,73 @@ int syn_crop_resize_batch(const uint8_t* images_dev, int n_frames, int height, i
                      stride_y, stride_x, stride_c, (cudaStream_t)stream, "syn_crop_resize_batch");
 }
 
+int64_t syn_crop_resize_images_plan_size(int batch, const int32_t* out_h_host, const int32_t* out_w_host, int mode) {
+  if (batch <= 0 || !out_h_host || !out_w_host || (mode != SYN_INTER_LINEAR && mode != SYN_INTER_LANCZOS4)) return -1;
+  int64_t n = (int64_t)sizeof(CropImagesRoi) * batch;
+  for (int b = 0; b < batch; ++b) {
+    if (out_h_host[b] < 1 || out_w_host[b] < 1) return -1;
+    n += rsz::plan_bytes(1, out_h_host[b], out_w_host[b], rsz::taps_of(mode));
+  }
+  return n;
+}
+
+int syn_crop_resize_plan_images_host(const int32_t* rois_host, const int32_t* images_host, int n_images, const int32_t* heights_host,
+                                     const int32_t* widths_host, int batch, const int32_t* out_h_host, const int32_t* out_w_host,
+                                     int mode, void* plan_out, int64_t plan_bytes) {
+  const char* who = "syn_crop_resize_plan_images_host";
+  if (!rois_host || !images_host || !heights_host || !widths_host || !out_h_host || !out_w_host || !plan_out || batch <= 0)
+    return fail(SYN_ERR_INVALID, "%s: null pointer or empty batch", who);
+  if (n_images <= 0) return fail(SYN_ERR_INVALID, "%s: %d images", who, n_images);
+  if (mode != SYN_INTER_LINEAR && mode != SYN_INTER_LANCZOS4)
+    return fail(SYN_ERR_UNSUPPORTED, "%s: interpolation %d (only INTER_LINEAR = 1 and INTER_LANCZOS4 = 4)", who, mode);
+  for (int i = 0; i < n_images; ++i)
+    if (heights_host[i] < 1 || widths_host[i] < 1) return fail(SYN_ERR_INVALID, "%s: image %d is %dx%d", who, i, heights_host[i], widths_host[i]);
+  for (int b = 0; b < batch; ++b) {
+    const int32_t* r = rois_host + 4 * b;
+    if (out_h_host[b] < 1 || out_w_host[b] < 1) return fail(SYN_ERR_INVALID, "%s: ROI %d output %dx%d", who, b, out_h_host[b], out_w_host[b]);
+    if (r[2] <= r[0] || r[3] <= r[1]) return fail(SYN_ERR_SHAPE, "%s: ROI %d (%d,%d,%d,%d) is empty", who, b, r[0], r[1], r[2], r[3]);
+    if (images_host[b] < 0 || images_host[b] >= n_images)
+      return fail(SYN_ERR_SHAPE, "%s: ROI %d names image %d of %d", who, b, images_host[b], n_images);
+  }
+  const int64_t need = syn_crop_resize_images_plan_size(batch, out_h_host, out_w_host, mode);
+  if (plan_bytes < need) return fail(SYN_ERR_SHAPE, "%s: plan buffer of %lld bytes, %lld needed", who, (long long)plan_bytes, (long long)need);
+  std::vector<long long> src(n_images + 1, 0);
+  for (int i = 0; i < n_images; ++i) src[i + 1] = src[i] + 3LL * heights_host[i] * widths_host[i];
+  CropImagesRoi* hdr = static_cast<CropImagesRoi*>(plan_out);
+  long long out = 0, at = (long long)sizeof(CropImagesRoi) * batch;
+  for (int b = 0; b < batch; ++b) {
+    const int im = images_host[b];
+    hdr[b] = CropImagesRoi{src[im], heights_host[im], widths_host[im], out_h_host[b], out_w_host[b], out, at};
+    rsz::build_plan(rois_host + 4 * b, 1, out_h_host[b], out_w_host[b], mode, static_cast<char*>(plan_out) + at);
+    out += 3LL * out_h_host[b] * out_w_host[b];
+    at += rsz::plan_bytes(1, out_h_host[b], out_w_host[b], rsz::taps_of(mode));
+  }
+  return SYN_OK;
+}
+
+int syn_crop_resize_images(const uint8_t* images_dev, const void* plan_dev, int batch, const int32_t* out_h_host, const int32_t* out_w_host,
+                           int mode, int planar, uint8_t* out_dev, void* stream) {
+  const char* who = "syn_crop_resize_images";
+  if (!images_dev || !plan_dev || !out_dev || !out_h_host || !out_w_host || batch <= 0)
+    return fail(SYN_ERR_INVALID, "%s: null pointer or empty batch", who);
+  if (mode != SYN_INTER_LINEAR && mode != SYN_INTER_LANCZOS4)
+    return fail(SYN_ERR_UNSUPPORTED, "%s: interpolation %d (only INTER_LINEAR = 1 and INTER_LANCZOS4 = 4)", who, mode);
+  if (planar != 0 && planar != 1) return fail(SYN_ERR_INVALID, "%s: planar = %d", who, planar);
+  if (batch > 65535) return fail(SYN_ERR_SHAPE, "%s: %d ROIs exceed one launch's grid", who, batch);
+  int mh = 0, mw = 0;
+  for (int b = 0; b < batch; ++b) {
+    if (out_h_host[b] < 1 || out_w_host[b] < 1) return fail(SYN_ERR_INVALID, "%s: ROI %d output %dx%d", who, b, out_h_host[b], out_w_host[b]);
+    mh = std::max(mh, (int)out_h_host[b]);
+    mw = std::max(mw, (int)out_w_host[b]);
+  }
+  const dim3 grid((mw + kResizeBX - 1) / kResizeBX, (mh + kResizeBY - 1) / kResizeBY, batch), block(kResizeBX, kResizeBY);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (mode == SYN_INTER_LANCZOS4) crop_resize_images_kernel<8><<<grid, block, 0, st>>>(images_dev, plan_dev, out_dev, planar);
+  else crop_resize_images_kernel<2><<<grid, block, 0, st>>>(images_dev, plan_dev, out_dev, planar);
+  SYN_LAUNCH_CHECK("crop_resize_images_kernel");
+  return SYN_OK;
+}
+
 int syn_faceboxes_num_priors(int im_height, int im_width) {
   if (im_height <= 0 || im_width <= 0) return -1;
   return faceboxes_num_priors(im_height, im_width);
@@ -323,12 +409,8 @@ int syn_faceboxes_decode(const float* loc_dev, const float* conf_dev, int im_hei
   const int np = faceboxes_num_priors(im_height, im_width);
   SYN_CUDA(cudaMemsetAsync(n_dets_dev, 0, sizeof(int32_t), st));
   SYN_CUDA(cudaMemsetAsync(cand_ws_dev, 0, sizeof(int32_t), st));
-  faceboxes_select_kernel<<<(np + 255) / 256, 256, 0, st>>>(conf_dev, np, conf_thresh, cand_ws_dev);
-  SYN_LAUNCH_CHECK("faceboxes_select_kernel");
-  faceboxes_rank_decode_kernel<<<(np + 127) / 128, 128, 0, st>>>(loc_dev, conf_dev, im_height, im_width, box_scale_w, box_scale_h, scale,
-                                                                top_k, cand_ws_dev, dets_dev, n_dets_dev);
-  SYN_LAUNCH_CHECK("faceboxes_rank_decode_kernel");
-  return SYN_OK;
+  return decode_launch(loc_dev, conf_dev, decode_frame(FbDecodeFrames{}, 0, im_height, im_width, box_scale_w, box_scale_h, scale, 0, 0, 1),
+                       1, np, conf_thresh, top_k, cand_ws_dev, dets_dev, n_dets_dev, st);
 }
 
 int syn_faceboxes_decode_batch(const float* loc_dev, const float* conf_dev, int n_frames, int im_height, int im_width,
@@ -341,15 +423,38 @@ int syn_faceboxes_decode_batch(const float* loc_dev, const float* conf_dev, int 
     return fail(SYN_ERR_INVALID, "syn_faceboxes_decode_batch: %d frames, at most %d per call", n_frames, SYN_FB_MAX_FRAMES);
   cudaStream_t st = (cudaStream_t)stream;
   const int np = faceboxes_num_priors(im_height, im_width);
+  FbDecodeFrames t{};
+  for (int f = 0; f < n_frames; ++f)                     // frame f: rows f * np.., candidates in its (np + 1) block
+    t = decode_frame(t, f, im_height, im_width, box_scale_w, box_scale_h, scale, f * np, f * (np + 1), f * (np + 1) + 1);
   SYN_CUDA(cudaMemsetAsync(n_dets_dev, 0, sizeof(int32_t) * n_frames, st));
   SYN_CUDA(cudaMemset2DAsync(cand_ws_dev, sizeof(int32_t) * (np + 1), 0, sizeof(int32_t), n_frames, st));   // every frame's count
-  faceboxes_select_kernel<<<dim3((np + 255) / 256, n_frames), 256, 0, st>>>(conf_dev, np, conf_thresh, cand_ws_dev);
-  SYN_LAUNCH_CHECK("faceboxes_select_kernel");
-  faceboxes_rank_decode_kernel<<<dim3((np + 127) / 128, n_frames), 128, 0, st>>>(loc_dev, conf_dev, im_height, im_width, box_scale_w,
-                                                                                box_scale_h, scale, top_k, cand_ws_dev, dets_dev,
-                                                                                n_dets_dev);
-  SYN_LAUNCH_CHECK("faceboxes_rank_decode_kernel");
-  return SYN_OK;
+  return decode_launch(loc_dev, conf_dev, t, n_frames, np, conf_thresh, top_k, cand_ws_dev, dets_dev, n_dets_dev, st);
+}
+
+int syn_faceboxes_decode_images(const float* loc_dev, const float* conf_dev, int n_images, const int32_t* heights_host,
+                                const int32_t* widths_host, const float* scale_host, float conf_thresh, int top_k, int32_t* cand_ws_dev,
+                                float* dets_dev, int32_t* n_dets_dev, void* stream) {
+  const char* who = "syn_faceboxes_decode_images";
+  if (!loc_dev || !conf_dev || !heights_host || !widths_host || !scale_host || !cand_ws_dev || !dets_dev || !n_dets_dev || top_k <= 0)
+    return fail(SYN_ERR_INVALID, "%s: null pointer or top_k < 1", who);
+  if (n_images <= 0 || n_images > SYN_FB_MAX_FRAMES)
+    return fail(SYN_ERR_INVALID, "%s: %d images, 1..%d per call", who, n_images, SYN_FB_MAX_FRAMES);
+  FbDecodeFrames t{};
+  int p0 = 0, np_max = 0;
+  for (int f = 0; f < n_images; ++f) {
+    if (heights_host[f] < 1 || widths_host[f] < 1 || !(scale_host[f] > 0.f))
+      return fail(SYN_ERR_INVALID, "%s: image %d is %dx%d at scale %g", who, f, heights_host[f], widths_host[f], (double)scale_host[f]);
+    const int np = faceboxes_num_priors(heights_host[f], widths_host[f]);
+    // priors at p0.. of the packed (sum P) rows; the n_images counts first in cand_ws, then every image's indices
+    t = decode_frame(t, f, heights_host[f], widths_host[f], (float)widths_host[f], (float)heights_host[f], scale_host[f], p0, f,
+                     n_images + p0);
+    p0 += np;
+    np_max = std::max(np_max, np);
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  SYN_CUDA(cudaMemsetAsync(n_dets_dev, 0, sizeof(int32_t) * n_images, st));
+  SYN_CUDA(cudaMemsetAsync(cand_ws_dev, 0, sizeof(int32_t) * n_images, st));
+  return decode_launch(loc_dev, conf_dev, t, n_images, np_max, conf_thresh, top_k, cand_ws_dev, dets_dev, n_dets_dev, st);
 }
 
 }  // extern "C"
@@ -384,6 +489,10 @@ inline int conv_out(int n, int k, int s, int p) { return (n + 2 * p - k) / s + 1
 
 }  // namespace
 
+// map sizes of the network on the frame axis: 0 image, 1 conv1, 2 pool1, 3 conv2, 4 / 5 / 6 detection sources 0 / 1 / 2,
+// 7 / 8 / 9 the heads' view of sources 0 / 1 / 2 (their frames' slices of the packed prior axis)
+constexpr int kFbLevels = 10;
+
 struct syn_fb {
   int device = 0;
   std::vector<float> w[33], b[33];          // folded [K][cout] weights and bias, host
@@ -391,11 +500,13 @@ struct syn_fb {
   float* d_w[33] = {};
   float* d_b[33] = {};
   bool committed = false;
-  // workspace for the current image size, ws_frames frames of it
-  int ws_h = 0, ws_w = 0, ws_frames = 0;
+  // activation workspace, grown (never shrunk) to the bytes a call needs
   float *c1 = nullptr, *p1 = nullptr, *c2 = nullptr, *xa = nullptr, *xb = nullptr, *avg = nullptr, *r1 = nullptr, *r2 = nullptr,
         *t3 = nullptr, *c31 = nullptr, *c32 = nullptr, *c41 = nullptr, *c42 = nullptr;
   size_t ws_sizes[13] = {};                 // bytes of c1 ... c42, in that order
+  // frame-axis geometry, FbLevel[kFbLevels][frames]: built on the host per call, one copy to the device
+  FbLevel geo_host[kFbLevels * SYN_FB_MAX_FRAMES] = {};
+  FbLevel* geo_dev = nullptr;
   int64_t launches = 0;
 };
 
@@ -405,7 +516,8 @@ void fb_free_ws(syn_fb* f) {
   float** bufs[] = {&f->c1, &f->p1, &f->c2, &f->xa, &f->xb, &f->avg, &f->r1, &f->r2, &f->t3, &f->c31, &f->c32, &f->c41, &f->c42};
   for (float** q : bufs) { cudaFree(*q); *q = nullptr; }
   for (size_t& b : f->ws_sizes) b = 0;
-  f->ws_h = f->ws_w = f->ws_frames = 0;
+  cudaFree(f->geo_dev);
+  f->geo_dev = nullptr;
 }
 
 struct FbGeom { int h1, w1, hp1, wp1, h2, w2, h3, w3, h4, w4, h5, w5; };
@@ -420,29 +532,40 @@ inline FbGeom fb_geom(int h, int w) {
   return g;
 }
 
-// nf frames of an h x w input: every buffer is the (nf, h', w', c) stack of its one-image map.  Grown (never shrunk for the
-// same size) with the device idle, like Workspace::ensure of the backbones.
-int fb_workspace(syn_fb* f, int h, int w, int nf) {
-  if (h == f->ws_h && w == f->ws_w && nf <= f->ws_frames) return SYN_OK;
+// Pixels of every level summed over the frames of a call -> every buffer is the packed map of its level.  A buffer that
+// is too small for the call is reallocated with the device idle (like Workspace::ensure of the backbones); one that is
+// large enough is kept, so a stream of calls of different sizes stops allocating once it has met its largest.
+int fb_workspace(syn_fb* f, const size_t* pix) {
+  const size_t floats[13] = {pix[1] * 48, pix[2] * 48, pix[3] * 128, pix[4] * 128, pix[4] * 128, pix[4] * 128, pix[4] * 24,
+                             pix[4] * 24, pix[4] * 32, pix[4] * 128, pix[5] * 256, pix[5] * 128, pix[6] * 256};
+  bool fits = f->geo_dev != nullptr;
+  for (int k = 0; k < 13; ++k) fits = fits && sizeof(float) * floats[k] <= f->ws_sizes[k];
+  if (fits) return SYN_OK;
   SYN_CUDA(cudaDeviceSynchronize());
+  size_t keep[13];
+  for (int k = 0; k < 13; ++k) keep[k] = std::max(f->ws_sizes[k], sizeof(float) * floats[k]);
   fb_free_ws(f);
-  const FbGeom g = fb_geom(h, w);
-  const size_t n3 = (size_t)nf * g.h3 * g.w3, n4 = (size_t)nf * g.h4 * g.w4, n5 = (size_t)nf * g.h5 * g.w5;
   float** bufs[13] = {&f->c1, &f->p1, &f->c2, &f->xa, &f->xb, &f->avg, &f->r1, &f->r2, &f->t3, &f->c31, &f->c32, &f->c41, &f->c42};
-  const size_t floats[13] = {(size_t)nf * g.h1 * g.w1 * 48, (size_t)nf * g.hp1 * g.wp1 * 48, (size_t)nf * g.h2 * g.w2 * 128,
-                             n3 * 128, n3 * 128, n3 * 128, n3 * 24, n3 * 24, n3 * 32, n3 * 128, n4 * 256, n4 * 128, n5 * 256};
   for (int k = 0; k < 13; ++k) {
-    f->ws_sizes[k] = sizeof(float) * floats[k];
+    f->ws_sizes[k] = keep[k];
     SYN_CUDA(cudaMalloc(bufs[k], f->ws_sizes[k]));
   }
-  f->ws_h = h; f->ws_w = w; f->ws_frames = nf;
+  SYN_CUDA(cudaMalloc(&f->geo_dev, sizeof(f->geo_host)));
   return SYN_OK;
 }
 
-// frames == 0: the one-image kernels.  frames >= 1: their FRAMES instantiations on stacks of `frames` maps; y_fs = floats
-// from one frame's output to the next (0: the dense (frames, ho, wo, cout_stride) stack).
+// The frame axis of one call: its frame count and, per level, the device geometry and the packed pixel count
+struct FbFrames {
+  int n;
+  const FbLevel* geo;      // device FbLevel[kFbLevels][n]
+  size_t pix[kFbLevels];
+  const FbLevel* level(int l) const { return geo + (size_t)l * n; }
+};
+
+// R == nullptr: the one-image kernels on an h x w input.  Otherwise their FRAMES instantiations on the packed maps of
+// R->n frames: lin / lout = input / output level.
 int fb_conv(syn_fb* f, int idx, const float* x, const uint8_t* x_u8, int h, int w, int cin_stride, int cin_off, float* y,
-            int cout_stride, int cout_off, cudaStream_t st, int frames = 0, size_t y_fs = 0) {
+            int cout_stride, int cout_off, cudaStream_t st, const FbFrames* R = nullptr, int lin = 0, int lout = 0) {
   const FbLayer& L = kFbLayers[idx];
   FbConvArgs a;
   a.x = x; a.x_u8 = x_u8; a.wk = f->d_w[idx]; a.bias = f->d_b[idx]; a.y = y;
@@ -451,15 +574,15 @@ int fb_conv(syn_fb* f, int idx, const float* x, const uint8_t* x_u8, int h, int 
   a.cout = L.cout; a.cout_stride = cout_stride; a.cout_off = cout_off;
   a.k = L.k; a.stride = L.stride; a.pad = L.pad; a.act = L.act;
   a.mean[0] = 104.f; a.mean[1] = 117.f; a.mean[2] = 123.f;          // FaceBoxes.py:92
-  const int M1 = a.ho * a.wo, M = M1 * (frames ? frames : 1);
-  a.frames = frames;
-  a.x_fs = (long long)h * w * (x_u8 ? 3 : cin_stride);
-  a.y_fs = y_fs ? (long long)y_fs : (long long)M1 * cout_stride;
+  a.frames = R ? R->n : 0;
+  a.gin = R ? R->level(lin) : nullptr;
+  a.gout = R ? R->level(lout) : nullptr;
+  const int M = R ? (int)R->pix[lout] : a.ho * a.wo;
   const dim3 grid((M + FB_BM - 1) / FB_BM, (L.cout + FB_BN - 1) / FB_BN);
   const bool vec = x_u8 == nullptr && L.cin % 4 == 0 && cin_stride % 4 == 0 && cin_off % 4 == 0 && L.cout % 4 == 0 &&
                    (reinterpret_cast<uintptr_t>(x) & 15) == 0;
   const bool smalln = L.cout <= FB_SMALLN && L.k * L.k * L.cin >= 512;
-  if (frames) {
+  if (R) {
     if (smalln) fb_conv_smalln_kernel<true><<<M, 128, 0, st>>>(a);
     else if (vec) fb_conv_kernel<true, true><<<grid, 256, 0, st>>>(a);
     else fb_conv_kernel<false, true><<<grid, 256, 0, st>>>(a);
@@ -494,94 +617,135 @@ int fb_stop_copy(const FbStop* d, const float* src, size_t n, cudaStream_t st) {
 #define SYN_FB_STOP(d, s, src, n, st) \
   do { if ((d) != nullptr && (d)->stage == (s)) return fb_stop_copy((d), (src), (n), (st)); } while (0)
 
-// syn_fb_forward's launch sequence; `stop` (nullable) ends it early.  Stages are the launches in order, see the table
-// at syn_fb_debug_forward_until in include/synergy_b200.h.  frames == 0: one image.  frames >= 1 (syn_fb_forward_batch): the
-// same 39 launches, each over the stack of `frames` maps; loc / conf are (frames, P, 4) / (frames, P, 2).
-int fb_forward_body(syn_fb* f, const uint8_t* image_dev, int frames, int height, int width, float* loc_dev, float* conf_dev,
-                    cudaStream_t st, const FbStop* stop, const char* who) {
-  if (!f || !image_dev || !loc_dev || !conf_dev || height <= 0 || width <= 0) return fail(SYN_ERR_INVALID, "%s: bad argument", who);
+// The argument checks of every detector entry, before anything is read or launched: `frames` == 0 is one image of
+// heights[0] x widths[0], else `frames` images of any sizes packed back to back.
+int fb_check(const syn_fb* f, const uint8_t* image_dev, int frames, const int32_t* heights, const int32_t* widths, const float* loc_dev,
+             const float* conf_dev, const char* who) {
   if (frames < 0 || frames > SYN_FB_MAX_FRAMES) return fail(SYN_ERR_INVALID, "%s: %d frames, 1..%d per call", who, frames, SYN_FB_MAX_FRAMES);
+  if (!f || !image_dev || !loc_dev || !conf_dev || !heights || !widths) return fail(SYN_ERR_INVALID, "%s: bad argument", who);
+  for (int i = 0; i < std::max(frames, 1); ++i) {
+    if (heights[i] <= 0 || widths[i] <= 0) return fail(SYN_ERR_INVALID, "%s: bad argument: image %d is %dx%d", who, i, heights[i], widths[i]);
+    const FbGeom g = fb_geom(heights[i], widths[i]);
+    if (g.h3 != fb_cells(heights[i], 32) || g.w3 != fb_cells(widths[i], 32) || g.h4 != fb_cells(heights[i], 64) ||
+        g.w4 != fb_cells(widths[i], 64) || g.h5 != fb_cells(heights[i], 128) || g.w5 != fb_cells(widths[i], 128))
+      return fail(SYN_ERR_SHAPE, "%s: feature maps of a %dx%d input do not match the prior grid", who, heights[i], widths[i]);
+  }
   if (!f->committed) return fail(SYN_ERR_STATE, "%s before syn_fb_commit", who);
+  return SYN_OK;
+}
+
+// syn_fb_forward's launch sequence; `stop` (nullable) ends it early.  Stages are the launches in order, see the table
+// at syn_fb_debug_forward_until in include/synergy_b200.h.  frames == 0: one image (heights[0] x widths[0]).  frames >= 1
+// (syn_fb_forward_images, and syn_fb_forward_batch with one size): the same 39 launches over the packed maps of every
+// frame; loc / conf are the packed (sum P, 4) / (sum P, 2), frame i's priors after those of frames 0 .. i-1.
+int fb_forward_body(syn_fb* f, const uint8_t* image_dev, int frames, const int32_t* heights, const int32_t* widths, float* loc_dev,
+                    float* conf_dev, cudaStream_t st, const FbStop* stop, const char* who) {
+  if (int rc = fb_check(f, image_dev, frames, heights, widths, loc_dev, conf_dev, who)) return rc;
   SYN_CUDA(cudaSetDevice(f->device));
-  const int nf = frames ? frames : 1;
-  if (int rc = fb_workspace(f, height, width, nf)) return rc;
+  const int nf = std::max(frames, 1), height = heights[0], width = widths[0];
+  // every level of every frame: size, first packed pixel, and for the detection sources the first prior
+  FbFrames R{nf, nullptr, {}};
+  size_t np_all = 0;
+  for (int i = 0; i < nf; ++i) {
+    const FbGeom g = fb_geom(heights[i], widths[i]);
+    const int hw[kFbLevels][2] = {{heights[i], widths[i]}, {g.h1, g.w1}, {g.hp1, g.wp1}, {g.h2, g.w2}, {g.h3, g.w3}, {g.h4, g.w4},
+                                  {g.h5, g.w5}, {g.h3, g.w3}, {g.h4, g.w4}, {g.h5, g.w5}};
+    const int s1 = (int)np_all + 21 * g.h3 * g.w3, s2 = s1 + g.h4 * g.w4;
+    const int prior[kFbLevels] = {0, 0, 0, 0, 0, 0, 0, (int)np_all, s1, s2}, ppp[kFbLevels] = {0, 0, 0, 0, 0, 0, 0, 21, 1, 1};
+    for (int l = 0; l < kFbLevels; ++l) {
+      f->geo_host[l * nf + i] = FbLevel{(int)R.pix[l], hw[l][0], hw[l][1], prior[l], ppp[l]};
+      R.pix[l] += (size_t)hw[l][0] * hw[l][1];
+    }
+    np_all += (size_t)faceboxes_num_priors(heights[i], widths[i]);
+  }
+  if (frames && (R.pix[0] * 3 > (size_t)INT32_MAX || np_all * 4 > (size_t)INT32_MAX))
+    return fail(SYN_ERR_SHAPE, "%s: %zu pixels in one call exceed the packed maps' int32 indices", who, R.pix[0]);
+  if (int rc = fb_workspace(f, R.pix)) return rc;
+  R.geo = f->geo_dev;
+  if (frames) SYN_CUDA(cudaMemcpyAsync(f->geo_dev, f->geo_host, sizeof(FbLevel) * kFbLevels * nf, cudaMemcpyHostToDevice, st));
   if (stop) {
     // A debug run copies a stage's whole destination, slices that later launches write included: start from a zeroed
     // workspace so that those slices read 0 instead of whatever an earlier call (another image, another frame count) left.
     float* bufs[13] = {f->c1, f->p1, f->c2, f->xa, f->xb, f->avg, f->r1, f->r2, f->t3, f->c31, f->c32, f->c41, f->c42};
     for (int k = 0; k < 13; ++k) SYN_CUDA(cudaMemsetAsync(bufs[k], 0, f->ws_sizes[k], st));
   }
-  const FbGeom g = fb_geom(height, width);
-  if (g.h3 != fb_cells(height, 32) || g.w3 != fb_cells(width, 32) || g.h4 != fb_cells(height, 64) || g.w4 != fb_cells(width, 64) ||
-      g.h5 != fb_cells(height, 128) || g.w5 != fb_cells(width, 128))
-    return fail(SYN_ERR_SHAPE, "%s: feature maps of a %dx%d input do not match the prior grid", who, height, width);
-  auto pool_grid = [nf](size_t n) { return dim3((unsigned)((n + 255) / 256), nf); };
-  const size_t n1 = (size_t)g.h1 * g.w1, np1 = (size_t)g.hp1 * g.wp1, n2 = (size_t)g.h2 * g.w2;
-  const size_t n3 = (size_t)g.h3 * g.w3, n4 = (size_t)g.h4 * g.w4, n5 = (size_t)g.h5 * g.w5;
-  const int np = (int)(n3 * 21 + n4 + n5);
+  const FbFrames* Rp = frames ? &R : nullptr;
+  const FbGeom g = fb_geom(height, width);            // the one-image launches' sizes
+  auto pool_frames = [&](int lin, int lout) { return FbPoolFrames{R.level(lin), R.level(lout), nf, (int)R.pix[lout]}; };
+  auto pool_grid = [](size_t n) { return dim3((unsigned)((n + 255) / 256)); };
+  const size_t n1 = R.pix[1], np1 = R.pix[2], n2 = R.pix[3], n3 = R.pix[4], n4 = R.pix[5], n5 = R.pix[6];
+  const size_t np = np_all;
   // conv1 (CReLU) -> max-pool -> conv2 (CReLU) -> max-pool                                          faceboxes.py:120-123
-  if (int rc = fb_conv(f, 0, nullptr, image_dev, height, width, 3, 0, f->c1, 48, 0, st, frames)) return rc;
-  SYN_FB_STOP(stop, 0, f->c1, nf * (n1 * 48), st);
-  fb_maxpool_kernel<<<pool_grid(np1 * 48), 256, 0, st>>>(f->c1, g.h1, g.w1, 48, f->p1, g.hp1, g.wp1);
+  if (int rc = fb_conv(f, 0, nullptr, image_dev, height, width, 3, 0, f->c1, 48, 0, st, Rp, 0, 1)) return rc;
+  SYN_FB_STOP(stop, 0, f->c1, n1 * 48, st);
+  if (frames) fb_maxpool_kernel<true><<<pool_grid(np1 * 48), 256, 0, st>>>(f->c1, 0, 0, 48, f->p1, 0, 0, pool_frames(1, 2));
+  else fb_maxpool_kernel<false><<<pool_grid(np1 * 48), 256, 0, st>>>(f->c1, g.h1, g.w1, 48, f->p1, g.hp1, g.wp1, FbPoolFrames{});
   SYN_LAUNCH_CHECK("fb_maxpool_kernel");
   ++f->launches;
-  SYN_FB_STOP(stop, 1, f->p1, nf * (np1 * 48), st);
-  if (int rc = fb_conv(f, 1, f->p1, nullptr, g.hp1, g.wp1, 48, 0, f->c2, 128, 0, st, frames)) return rc;
-  SYN_FB_STOP(stop, 2, f->c2, nf * (n2 * 128), st);
-  fb_maxpool_kernel<<<pool_grid(n3 * 128), 256, 0, st>>>(f->c2, g.h2, g.w2, 128, f->xa, g.h3, g.w3);
+  SYN_FB_STOP(stop, 1, f->p1, np1 * 48, st);
+  if (int rc = fb_conv(f, 1, f->p1, nullptr, g.hp1, g.wp1, 48, 0, f->c2, 128, 0, st, Rp, 2, 3)) return rc;
+  SYN_FB_STOP(stop, 2, f->c2, n2 * 128, st);
+  if (frames) fb_maxpool_kernel<true><<<pool_grid(n3 * 128), 256, 0, st>>>(f->c2, 0, 0, 128, f->xa, 0, 0, pool_frames(3, 4));
+  else fb_maxpool_kernel<false><<<pool_grid(n3 * 128), 256, 0, st>>>(f->c2, g.h2, g.w2, 128, f->xa, g.h3, g.w3, FbPoolFrames{});
   SYN_LAUNCH_CHECK("fb_maxpool_kernel");
   ++f->launches;
-  SYN_FB_STOP(stop, 3, f->xa, nf * (n3 * 128), st);
+  SYN_FB_STOP(stop, 3, f->xa, n3 * 128, st);
   // three inception blocks: every branch writes its 32-channel slice of the next 128-channel tensor     :124-126, :33-47
   float *x = f->xa, *y = f->xb;
   for (int blk = 0; blk < 3; ++blk) {
     const int L0 = 2 + 7 * blk, s0 = 4 + 8 * blk;
-    if (int rc = fb_conv(f, L0 + 0, x, nullptr, g.h3, g.w3, 128, 0, y, 128, 0, st, frames)) return rc;
-    SYN_FB_STOP(stop, s0 + 0, y, nf * (n3 * 128), st);
-    fb_avgpool_kernel<<<pool_grid(n3 * 128), 256, 0, st>>>(x, g.h3, g.w3, 128, f->avg);
+    if (int rc = fb_conv(f, L0 + 0, x, nullptr, g.h3, g.w3, 128, 0, y, 128, 0, st, Rp, 4, 4)) return rc;
+    SYN_FB_STOP(stop, s0 + 0, y, n3 * 128, st);
+    if (frames) fb_avgpool_kernel<true><<<pool_grid(n3 * 128), 256, 0, st>>>(x, 0, 0, 128, f->avg, pool_frames(4, 4));
+    else fb_avgpool_kernel<false><<<pool_grid(n3 * 128), 256, 0, st>>>(x, g.h3, g.w3, 128, f->avg, FbPoolFrames{});
     SYN_LAUNCH_CHECK("fb_avgpool_kernel");
     ++f->launches;
-    SYN_FB_STOP(stop, s0 + 1, f->avg, nf * (n3 * 128), st);
-    if (int rc = fb_conv(f, L0 + 1, f->avg, nullptr, g.h3, g.w3, 128, 0, y, 128, 32, st, frames)) return rc;
-    SYN_FB_STOP(stop, s0 + 2, y, nf * (n3 * 128), st);
-    if (int rc = fb_conv(f, L0 + 2, x, nullptr, g.h3, g.w3, 128, 0, f->r1, 24, 0, st, frames)) return rc;
-    SYN_FB_STOP(stop, s0 + 3, f->r1, nf * (n3 * 24), st);
-    if (int rc = fb_conv(f, L0 + 3, f->r1, nullptr, g.h3, g.w3, 24, 0, y, 128, 64, st, frames)) return rc;
-    SYN_FB_STOP(stop, s0 + 4, y, nf * (n3 * 128), st);
-    if (int rc = fb_conv(f, L0 + 4, x, nullptr, g.h3, g.w3, 128, 0, f->r2, 24, 0, st, frames)) return rc;
-    SYN_FB_STOP(stop, s0 + 5, f->r2, nf * (n3 * 24), st);
-    if (int rc = fb_conv(f, L0 + 5, f->r2, nullptr, g.h3, g.w3, 24, 0, f->t3, 32, 0, st, frames)) return rc;
-    SYN_FB_STOP(stop, s0 + 6, f->t3, nf * (n3 * 32), st);
-    if (int rc = fb_conv(f, L0 + 6, f->t3, nullptr, g.h3, g.w3, 32, 0, y, 128, 96, st, frames)) return rc;
-    SYN_FB_STOP(stop, s0 + 7, y, nf * (n3 * 128), st);
+    SYN_FB_STOP(stop, s0 + 1, f->avg, n3 * 128, st);
+    if (int rc = fb_conv(f, L0 + 1, f->avg, nullptr, g.h3, g.w3, 128, 0, y, 128, 32, st, Rp, 4, 4)) return rc;
+    SYN_FB_STOP(stop, s0 + 2, y, n3 * 128, st);
+    if (int rc = fb_conv(f, L0 + 2, x, nullptr, g.h3, g.w3, 128, 0, f->r1, 24, 0, st, Rp, 4, 4)) return rc;
+    SYN_FB_STOP(stop, s0 + 3, f->r1, n3 * 24, st);
+    if (int rc = fb_conv(f, L0 + 3, f->r1, nullptr, g.h3, g.w3, 24, 0, y, 128, 64, st, Rp, 4, 4)) return rc;
+    SYN_FB_STOP(stop, s0 + 4, y, n3 * 128, st);
+    if (int rc = fb_conv(f, L0 + 4, x, nullptr, g.h3, g.w3, 128, 0, f->r2, 24, 0, st, Rp, 4, 4)) return rc;
+    SYN_FB_STOP(stop, s0 + 5, f->r2, n3 * 24, st);
+    if (int rc = fb_conv(f, L0 + 5, f->r2, nullptr, g.h3, g.w3, 24, 0, f->t3, 32, 0, st, Rp, 4, 4)) return rc;
+    SYN_FB_STOP(stop, s0 + 6, f->t3, n3 * 32, st);
+    if (int rc = fb_conv(f, L0 + 6, f->t3, nullptr, g.h3, g.w3, 32, 0, y, 128, 96, st, Rp, 4, 4)) return rc;
+    SYN_FB_STOP(stop, s0 + 7, y, n3 * 128, st);
     float* t = x; x = y; y = t;
   }
   // x = inception3 output (detection source 0); conv3_x, conv4_x give sources 1 and 2                  :127-135
-  if (int rc = fb_conv(f, 23, x, nullptr, g.h3, g.w3, 128, 0, f->c31, 128, 0, st, frames)) return rc;
-  SYN_FB_STOP(stop, 28, f->c31, nf * (n3 * 128), st);
-  if (int rc = fb_conv(f, 24, f->c31, nullptr, g.h3, g.w3, 128, 0, f->c32, 256, 0, st, frames)) return rc;
-  SYN_FB_STOP(stop, 29, f->c32, nf * (n4 * 256), st);
-  if (int rc = fb_conv(f, 25, f->c32, nullptr, g.h4, g.w4, 256, 0, f->c41, 128, 0, st, frames)) return rc;
-  SYN_FB_STOP(stop, 30, f->c41, nf * (n4 * 128), st);
-  if (int rc = fb_conv(f, 26, f->c41, nullptr, g.h4, g.w4, 128, 0, f->c42, 256, 0, st, frames)) return rc;
-  SYN_FB_STOP(stop, 31, f->c42, nf * (n5 * 256), st);
-  // heads: NHWC output of each source IS permute(0,2,3,1).view(-1) (:137-142); the three sources are concatenated by offset
-  if (int rc = fb_conv(f, 27, x, nullptr, g.h3, g.w3, 128, 0, loc_dev, 84, 0, st, frames, (size_t)np * 4)) return rc;
-  SYN_FB_STOP(stop, 32, loc_dev, nf * ((size_t)np * 4), st);
-  if (int rc = fb_conv(f, 28, f->c32, nullptr, g.h4, g.w4, 256, 0, loc_dev + n3 * 84, 4, 0, st, frames, (size_t)np * 4)) return rc;
-  SYN_FB_STOP(stop, 33, loc_dev, nf * ((size_t)np * 4), st);
-  if (int rc = fb_conv(f, 29, f->c42, nullptr, g.h5, g.w5, 256, 0, loc_dev + n3 * 84 + n4 * 4, 4, 0, st, frames, (size_t)np * 4)) return rc;
-  SYN_FB_STOP(stop, 34, loc_dev, nf * ((size_t)np * 4), st);
-  if (int rc = fb_conv(f, 30, x, nullptr, g.h3, g.w3, 128, 0, conf_dev, 42, 0, st, frames, (size_t)np * 2)) return rc;
-  SYN_FB_STOP(stop, 35, conf_dev, nf * ((size_t)np * 2), st);
-  if (int rc = fb_conv(f, 31, f->c32, nullptr, g.h4, g.w4, 256, 0, conf_dev + n3 * 42, 2, 0, st, frames, (size_t)np * 2)) return rc;
-  SYN_FB_STOP(stop, 36, conf_dev, nf * ((size_t)np * 2), st);
-  if (int rc = fb_conv(f, 32, f->c42, nullptr, g.h5, g.w5, 256, 0, conf_dev + n3 * 42 + n4 * 2, 2, 0, st, frames, (size_t)np * 2)) return rc;
-  SYN_FB_STOP(stop, 37, conf_dev, nf * ((size_t)np * 2), st);
-  fb_softmax2_kernel<<<(nf * np + 255) / 256, 256, 0, st>>>(conf_dev, nf * np);
+  if (int rc = fb_conv(f, 23, x, nullptr, g.h3, g.w3, 128, 0, f->c31, 128, 0, st, Rp, 4, 4)) return rc;
+  SYN_FB_STOP(stop, 28, f->c31, n3 * 128, st);
+  if (int rc = fb_conv(f, 24, f->c31, nullptr, g.h3, g.w3, 128, 0, f->c32, 256, 0, st, Rp, 4, 5)) return rc;
+  SYN_FB_STOP(stop, 29, f->c32, n4 * 256, st);
+  if (int rc = fb_conv(f, 25, f->c32, nullptr, g.h4, g.w4, 256, 0, f->c41, 128, 0, st, Rp, 5, 5)) return rc;
+  SYN_FB_STOP(stop, 30, f->c41, n4 * 128, st);
+  if (int rc = fb_conv(f, 26, f->c41, nullptr, g.h4, g.w4, 128, 0, f->c42, 256, 0, st, Rp, 5, 6)) return rc;
+  SYN_FB_STOP(stop, 31, f->c42, n5 * 256, st);
+  // heads: NHWC output of each source IS permute(0,2,3,1).view(-1) (:137-142); the three sources are concatenated by
+  // offset (one image), or by each frame's prior offsets (the frame axis: the head levels 7..9)
+  float* loc1 = frames ? loc_dev : loc_dev + n3 * 84;
+  float* loc2 = frames ? loc_dev : loc_dev + n3 * 84 + n4 * 4;
+  float* conf1 = frames ? conf_dev : conf_dev + n3 * 42;
+  float* conf2 = frames ? conf_dev : conf_dev + n3 * 42 + n4 * 2;
+  if (int rc = fb_conv(f, 27, x, nullptr, g.h3, g.w3, 128, 0, loc_dev, 84, 0, st, Rp, 4, 7)) return rc;
+  SYN_FB_STOP(stop, 32, loc_dev, np * 4, st);
+  if (int rc = fb_conv(f, 28, f->c32, nullptr, g.h4, g.w4, 256, 0, loc1, 4, 0, st, Rp, 5, 8)) return rc;
+  SYN_FB_STOP(stop, 33, loc_dev, np * 4, st);
+  if (int rc = fb_conv(f, 29, f->c42, nullptr, g.h5, g.w5, 256, 0, loc2, 4, 0, st, Rp, 6, 9)) return rc;
+  SYN_FB_STOP(stop, 34, loc_dev, np * 4, st);
+  if (int rc = fb_conv(f, 30, x, nullptr, g.h3, g.w3, 128, 0, conf_dev, 42, 0, st, Rp, 4, 7)) return rc;
+  SYN_FB_STOP(stop, 35, conf_dev, np * 2, st);
+  if (int rc = fb_conv(f, 31, f->c32, nullptr, g.h4, g.w4, 256, 0, conf1, 2, 0, st, Rp, 5, 8)) return rc;
+  SYN_FB_STOP(stop, 36, conf_dev, np * 2, st);
+  if (int rc = fb_conv(f, 32, f->c42, nullptr, g.h5, g.w5, 256, 0, conf2, 2, 0, st, Rp, 6, 9)) return rc;
+  SYN_FB_STOP(stop, 37, conf_dev, np * 2, st);
+  fb_softmax2_kernel<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(conf_dev, (int)np);
   SYN_LAUNCH_CHECK("fb_softmax2_kernel");
   ++f->launches;
-  SYN_FB_STOP(stop, 38, conf_dev, nf * ((size_t)np * 2), st);
+  SYN_FB_STOP(stop, 38, conf_dev, np * 2, st);
   return SYN_OK;
 }
 
@@ -670,13 +834,22 @@ int syn_fb_commit(syn_fb_t* f) {
 int64_t syn_fb_launch_count(const syn_fb_t* f) { return f ? f->launches : 0; }
 
 int syn_fb_forward(syn_fb_t* f, const uint8_t* image_dev, int height, int width, float* loc_dev, float* conf_dev, void* stream) {
-  return fb_forward_body(f, image_dev, 0, height, width, loc_dev, conf_dev, (cudaStream_t)stream, nullptr, "syn_fb_forward");
+  return fb_forward_body(f, image_dev, 0, &height, &width, loc_dev, conf_dev, (cudaStream_t)stream, nullptr, "syn_fb_forward");
 }
 
 int syn_fb_forward_batch(syn_fb_t* f, const uint8_t* images_dev, int n_frames, int height, int width, float* loc_dev, float* conf_dev,
                          void* stream) {
   if (n_frames <= 0) return fail(SYN_ERR_INVALID, "syn_fb_forward_batch: %d frames", n_frames);
-  return fb_forward_body(f, images_dev, n_frames, height, width, loc_dev, conf_dev, (cudaStream_t)stream, nullptr, "syn_fb_forward_batch");
+  const std::vector<int32_t> hs(std::min(n_frames, SYN_FB_MAX_FRAMES + 1), height), ws(hs.size(), width);   // one size, every frame
+  return fb_forward_body(f, images_dev, n_frames, hs.data(), ws.data(), loc_dev, conf_dev, (cudaStream_t)stream, nullptr,
+                         "syn_fb_forward_batch");
+}
+
+int syn_fb_forward_images(syn_fb_t* f, const uint8_t* images_dev, int n_images, const int32_t* heights_host, const int32_t* widths_host,
+                          float* loc_dev, float* conf_dev, void* stream) {
+  if (n_images <= 0) return fail(SYN_ERR_INVALID, "syn_fb_forward_images: %d images", n_images);
+  return fb_forward_body(f, images_dev, n_images, heights_host, widths_host, loc_dev, conf_dev, (cudaStream_t)stream, nullptr,
+                         "syn_fb_forward_images");
 }
 
 int syn_fb_debug_forward_until(syn_fb_t* f, const uint8_t* image_dev, int height, int width, int stage, float* out_dev,
@@ -685,7 +858,7 @@ int syn_fb_debug_forward_until(syn_fb_t* f, const uint8_t* image_dev, int height
     return fail(SYN_ERR_INVALID, "syn_fb_debug_forward_until: stage %d outside 0..%d", stage, kFbStages - 1);
   if (!f || !out_dev) return fail(SYN_ERR_INVALID, "syn_fb_debug_forward_until: null handle or output");
   const FbStop stop{stage, out_dev, out_numel};
-  return fb_forward_body(f, image_dev, 0, height, width, loc_dev, conf_dev, (cudaStream_t)stream, &stop, "syn_fb_debug_forward_until");
+  return fb_forward_body(f, image_dev, 0, &height, &width, loc_dev, conf_dev, (cudaStream_t)stream, &stop, "syn_fb_debug_forward_until");
 }
 
 int syn_fb_debug_forward_batch_until(syn_fb_t* f, const uint8_t* images_dev, int n_frames, int height, int width, int stage,
@@ -694,8 +867,20 @@ int syn_fb_debug_forward_batch_until(syn_fb_t* f, const uint8_t* images_dev, int
   if (stage < 0 || stage >= kFbStages) return fail(SYN_ERR_INVALID, "%s: stage %d outside 0..%d", who, stage, kFbStages - 1);
   if (!f || !out_dev) return fail(SYN_ERR_INVALID, "%s: null handle or output", who);
   if (n_frames <= 0) return fail(SYN_ERR_INVALID, "%s: %d frames", who, n_frames);
+  const std::vector<int32_t> hs(std::min(n_frames, SYN_FB_MAX_FRAMES + 1), height), ws(hs.size(), width);
   const FbStop stop{stage, out_dev, out_numel};
-  return fb_forward_body(f, images_dev, n_frames, height, width, loc_dev, conf_dev, (cudaStream_t)stream, &stop, who);
+  return fb_forward_body(f, images_dev, n_frames, hs.data(), ws.data(), loc_dev, conf_dev, (cudaStream_t)stream, &stop, who);
+}
+
+int syn_fb_debug_forward_images_until(syn_fb_t* f, const uint8_t* images_dev, int n_images, const int32_t* heights_host,
+                                      const int32_t* widths_host, int stage, float* out_dev, int64_t out_numel, float* loc_dev,
+                                      float* conf_dev, void* stream) {
+  const char* who = "syn_fb_debug_forward_images_until";
+  if (stage < 0 || stage >= kFbStages) return fail(SYN_ERR_INVALID, "%s: stage %d outside 0..%d", who, stage, kFbStages - 1);
+  if (!f || !out_dev) return fail(SYN_ERR_INVALID, "%s: null handle or output", who);
+  if (n_images <= 0) return fail(SYN_ERR_INVALID, "%s: %d images", who, n_images);
+  const FbStop stop{stage, out_dev, out_numel};
+  return fb_forward_body(f, images_dev, n_images, heights_host, widths_host, loc_dev, conf_dev, (cudaStream_t)stream, &stop, who);
 }
 
 }  // extern "C"

@@ -119,6 +119,35 @@ def decode_batch_device(loc: torch.Tensor, conf: torch.Tensor, im_height: int, i
     return dets, n
 
 
+def decode_images_device(loc: torch.Tensor, conf: torch.Tensor, sizes, scales, conf_thresh: float = confidence_threshold,
+                         k: int = top_k):
+    """:func:`decode_device` for N network inputs of any sizes in the same two launches: ``loc`` (sum P_i,4), ``conf``
+    (sum P_i,2) as ``FaceBoxesNet`` packs them, ``sizes`` the N (h, w) inputs, ``scales`` their shrink factors ->
+    ``(dets, n)``: (N,k',5) and (N,) device int32, image i's block and count being what ``decode_device`` gives for its
+    priors alone.  k' = min(k, max P_i)."""
+    lib = _lib.load()
+    hw = np.ascontiguousarray(np.array(sizes, np.int32).reshape(-1, 2))
+    hs, ws = np.ascontiguousarray(hw[:, 0]), np.ascontiguousarray(hw[:, 1])
+    sc = np.ascontiguousarray(scales, dtype=np.float32).reshape(-1)
+    nf = int(hw.shape[0])
+    if nf == 0 or sc.shape[0] != nf or (hw < 1).any():
+        raise ValueError(f'{nf} image sizes (each >= 1) and {sc.shape[0]} scales: one of each per image, at least one image')
+    ps = [num_priors(h, w) for h, w in hw.tolist()]
+    if loc.dim() != 2 or conf.dim() != 2 or tuple(loc.shape) != (sum(ps), 4) or tuple(conf.shape) != (sum(ps), 2) or \
+            loc.dtype != torch.float32 or conf.dtype != torch.float32 or not loc.is_cuda or conf.device != loc.device:
+        raise ValueError(f'loc / conf must be float32 CUDA tensors ({sum(ps)},4) / ({sum(ps)},2) for these {nf} inputs')
+    loc, conf = loc.contiguous(), conf.contiguous()
+    k = min(int(k), max(ps))
+    cand = torch.empty((nf + sum(ps),), dtype=torch.int32, device=loc.device)
+    dets = torch.zeros((nf, k, 5), dtype=torch.float32, device=loc.device)
+    n = torch.zeros((nf,), dtype=torch.int32, device=loc.device)
+    with torch.cuda.device(loc.device):
+        _lib.check(lib.syn_faceboxes_decode_images(loc.data_ptr(), conf.data_ptr(), nf, hs.ctypes.data, ws.ctypes.data, sc.ctypes.data,
+                                                   float(conf_thresh), k, cand.data_ptr(), dets.data_ptr(), n.data_ptr(),
+                                                   torch.cuda.current_stream(loc.device).cuda_stream))
+    return dets, n
+
+
 def nms_batch_device(dets: torch.Tensor, n: torch.Tensor, thresh: float, mode: int = _lib.NMS_CPU_NMS):
     """:func:`nms_device` per frame without a host round trip: ``dets`` (N,K,5) in descending score order per frame, ``n``
     (N,) device int32 counts (``decode_batch_device``'s outputs).  Returns ``(keep (N,K) int32, n_keep (N,) int32)``; the

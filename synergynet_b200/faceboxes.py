@@ -19,11 +19,24 @@ import numpy as np
 import torch
 
 from . import _lib, detect
-from .inference import INTER_LINEAR, crop_resize_device, crop_resize_frames_device, chunk_ranges, stack_frames_device
+from .inference import (INTER_LINEAR, ImagePack, chunk_ranges, crop_resize_device, crop_resize_frames_device, crop_resize_images_device,
+                        pack_images, stack_frames_device)
 
 # FaceBoxes/FaceBoxes.py:24-25
 scale_flag = True
 HEIGHT, WIDTH = 720, 1080
+
+
+def shrink_size(h: int, w: int):
+    """``(scale, (out_w, out_h))`` of the detector's shrink of an h x w image (FaceBoxes/FaceBoxes.py:62-79): the
+    image's own size at scale 1 when it fits in HEIGHT x WIDTH (or ``scale_flag`` is off), else cv2.resize's dsize."""
+    scale = 1
+    if scale_flag:
+        if h > HEIGHT:
+            scale = HEIGHT / h
+        if w * scale > WIDTH:
+            scale *= WIDTH / (w * scale)
+    return scale, ((int(scale * w), int(scale * h)) if scale != 1 else (w, h))
 
 
 def layer_plan() -> List[dict]:
@@ -158,6 +171,61 @@ class FaceBoxesNet:
                                                                   torch.cuda.current_stream(self.device).cuda_stream))
         return out
 
+    def _check_images(self, images):
+        """A list of contiguous (h,w,3) uint8 CUDA tensors on the detector device, or an ImagePack there -> ImagePack."""
+        if isinstance(images, ImagePack):
+            if images.data.device != self.device or images.data.dtype != torch.uint8 or not images.data.is_contiguous():
+                raise ValueError(f'packed images must be contiguous uint8 on the detector device {self.device}, got '
+                                 f'{images.data.dtype} on {images.data.device}')
+        else:
+            images = list(images)
+            for im in images:
+                if not isinstance(im, torch.Tensor) or im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3 or \
+                        im.device != self.device or not im.is_contiguous():
+                    raise ValueError('images must be contiguous uint8 (H,W,3) tensors on the detector device')
+            images = pack_images(images, self.device)
+        if not 1 <= len(images) <= _lib.FB_MAX_FRAMES:
+            raise ValueError(f'{len(images)} images in one call, 1..{_lib.FB_MAX_FRAMES} (FaceBoxes.detect_images splits a list)')
+        return images
+
+    def forward_packed(self, images):
+        """:meth:`forward` for N images of any sizes in the same 39 launches: ``images`` a list of (h_i,w_i,3) uint8 CUDA
+        tensors or an :class:`ImagePack` -> ``(loc (sum P_i,4), conf (sum P_i,2), p)``, image i's priors being rows
+        ``p[i]:p[i+1]``."""
+        pack = self._check_images(images)
+        p = np.concatenate([[0], np.cumsum([detect.num_priors(h, w) for h, w in pack.sizes])]).astype(int).tolist()
+        loc = torch.empty((p[-1], 4), dtype=torch.float32, device=self.device)
+        conf = torch.empty((p[-1], 2), dtype=torch.float32, device=self.device)
+        hs, ws = pack.arrays()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.syn_fb_forward_images(self._h, pack.data.data_ptr(), len(pack), hs.ctypes.data, ws.ctypes.data,
+                                                       loc.data_ptr(), conf.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream))
+        return loc, conf, p
+
+    def forward_images(self, images):
+        """:meth:`forward` for N images of any sizes in the same 39 launches: a list of contiguous (h_i,w_i,3) uint8 CUDA
+        tensors -> lists of ``(P_i,4)`` loc and ``(P_i,2)`` conf views, entry i having the bits of ``forward(images[i])``."""
+        loc, conf, p = self.forward_packed(images)
+        return [loc[a:b] for a, b in zip(p[:-1], p[1:])], [conf[a:b] for a, b in zip(p[:-1], p[1:])]
+
+    def debug_forward_images_until(self, images, stage: int) -> list:
+        """:meth:`debug_forward_until` on :meth:`forward_images`'s launch sequence: one tensor per image, shaped as
+        ``debug_forward_until`` returns it for that image alone.  Per-stage tests only."""
+        pack = self._check_images(images)
+        shapes = [debug_stage_shape(stage, h, w) for h, w in pack.sizes]
+        p = sum(detect.num_priors(h, w) for h, w in pack.sizes)
+        loc = torch.full((p * 4,), float('nan'), dtype=torch.float32, device=self.device)
+        conf = torch.full((p * 2,), float('nan'), dtype=torch.float32, device=self.device)
+        numel = [int(np.prod(sh)) for sh in shapes]
+        out = torch.empty((sum(numel),), dtype=torch.float32, device=self.device)
+        hs, ws = pack.arrays()
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.syn_fb_debug_forward_images_until(self._h, pack.data.data_ptr(), len(pack), hs.ctypes.data, ws.ctypes.data,
+                                                                   stage, out.data_ptr(), out.numel(), loc.data_ptr(), conf.data_ptr(),
+                                                                   torch.cuda.current_stream(self.device).cuda_stream))
+        at = np.concatenate([[0], np.cumsum(numel)]).astype(int).tolist()
+        return [out[a:b].view(sh) for a, b, sh in zip(at[:-1], at[1:], shapes)]
+
 
 def _conv_out(n: int, k: int, s: int, p: int) -> int:
     return (n + 2 * p - k) // s + 1
@@ -198,15 +266,10 @@ class FaceBoxes:
 
     def __call__(self, img_: np.ndarray):
         image = torch.from_numpy(np.ascontiguousarray(img_, dtype=np.uint8)).to(self.net.device)
-        scale = 1
-        if scale_flag:                                                                        # FaceBoxes.py:62-79
-            h, w = img_.shape[:2]
-            if h > HEIGHT:
-                scale = HEIGHT / h
-            if w * scale > WIDTH:
-                scale *= WIDTH / (w * scale)
-            if scale != 1:                                                                    # cv2.resize, INTER_LINEAR
-                image = crop_resize_device(image, [[0, 0, w, h]], (int(scale * w), int(scale * h)), INTER_LINEAR, planar=False)[0]
+        h, w = img_.shape[:2]
+        scale, dsize = shrink_size(h, w)                                                      # FaceBoxes.py:62-79
+        if scale != 1:                                                                        # cv2.resize, INTER_LINEAR
+            image = crop_resize_device(image, [[0, 0, w, h]], dsize, INTER_LINEAR, planar=False)[0]
         im_h, im_w = int(image.shape[0]), int(image.shape[1])
         loc, conf = self.net.forward(image)
         dets, n = detect.decode_device(loc, conf, im_h, im_w, scale=float(scale))
@@ -216,6 +279,61 @@ class FaceBoxes:
         keep, n_keep = detect.nms_device(dets, detect.nms_threshold, _lib.NMS_CPU_NMS, n=n_host)
         kept = dets[keep[:int(n_keep.item())].long()][:detect.keep_top_k].cpu().numpy()
         return [[b[0], b[1], b[2], b[3], b[4]] for b in kept if b[4] > detect.vis_thres]
+
+    def detect_images(self, images):
+        """``[self(img) for img in images]`` for images of any sizes: ``images`` is a list of BGR uint8 (H,W,3) host arrays or
+        CUDA tensors (or an :class:`~synergynet_b200.inference.ImagePack` a caller already uploaded).
+
+        One upload of the packed bytes; per chunk of at most ``_lib.FB_MAX_FRAMES`` images one crop launch shrinks every
+        image above 720 x 1080 to its own size on the device, then network, decode and NMS run over the whole chunk; the
+        kept boxes and counts of every chunk come back in one host synchronisation at the end."""
+        pack = pack_images(images, self.net.device)
+        pending = []
+        for a, b in chunk_ranges(len(pack), _lib.FB_MAX_FRAMES):
+            sub = pack.slice(a, b)
+            shrink = [shrink_size(h, w) for h, w in sub.sizes]
+            big = [i for i, (scale, _) in enumerate(shrink) if scale != 1]
+            net_in = sub
+            if big:                                                                            # FaceBoxes.py:62-79
+                shrunk = crop_resize_images_device(sub, big, [[0, 0, sub.sizes[i][1], sub.sizes[i][0]] for i in big],
+                                                   [shrink[i][1] for i in big], INTER_LINEAR, planar=False)
+                parts, at = [], 0
+                for i in range(len(sub)):
+                    if shrink[i][0] != 1:
+                        ow, oh = shrink[i][1]
+                        parts.append(shrunk[at:at + 3 * oh * ow])
+                        at += 3 * oh * ow
+                    else:
+                        parts.append(sub.image(i).reshape(-1))
+                net_in = ImagePack(torch.cat(parts), [(d[1], d[0]) for _, d in shrink])
+            scales = [float(sc) for sc, _ in shrink]
+            loc, conf, _ = self.net.forward_packed(net_in)
+            dets, n = detect.decode_images_device(loc, conf, net_in.sizes, scales)
+            pending.append(self._nms_to_host(dets, n))
+        return self._boxes_of(pending)
+
+    def _nms_to_host(self, dets, n):
+        """NMS of every frame of a decoded chunk and the asynchronous copy of its first keep_top_k kept rows and counts."""
+        keep, n_keep = detect.nms_batch_device(dets, n, detect.nms_threshold, _lib.NMS_CPU_NMS)
+        # the first keep_top_k kept rows of every frame (entries past a frame's count are unwritten: clamped, never read)
+        idx = keep[:, :detect.keep_top_k].long().clamp_(0, dets.shape[1] - 1)
+        kept = torch.gather(dets, 1, idx[:, :, None].expand(-1, -1, 5))
+        kept_host = torch.empty(kept.shape, dtype=kept.dtype, pin_memory=True)
+        n_host = torch.empty(n_keep.shape, dtype=n_keep.dtype, pin_memory=True)
+        kept_host.copy_(kept, non_blocking=True)
+        n_host.copy_(n_keep, non_blocking=True)
+        return kept_host, n_host
+
+    def _boxes_of(self, pending):
+        """One host synchronisation, then every frame's box list from the chunks' copies."""
+        torch.cuda.current_stream(self.net.device).synchronize()
+        out = []
+        for kept_host, n_host in pending:
+            kept_np, n_np = kept_host.numpy(), n_host.numpy()
+            for i in range(kept_np.shape[0]):
+                rows = kept_np[i, :min(int(n_np[i]), detect.keep_top_k)]
+                out.append([[b[0], b[1], b[2], b[3], b[4]] for b in rows if b[4] > detect.vis_thres])
+        return out
 
     def detect_batch(self, frames):
         """``__call__`` for N frames of one size: ``frames`` is a list / (N,H,W,3) array of BGR uint8 images, or the uint8
@@ -227,35 +345,15 @@ class FaceBoxes:
         chunk come back in one host synchronisation at the end, whatever N is."""
         stack = stack_frames_device(frames, self.net.device)
         h, w = int(stack.shape[1]), int(stack.shape[2])
-        scale = 1
-        if scale_flag:                                                                        # FaceBoxes.py:62-79
-            if h > HEIGHT:
-                scale = HEIGHT / h
-            if w * scale > WIDTH:
-                scale *= WIDTH / (w * scale)
+        scale, dsize = shrink_size(h, w)                                                      # FaceBoxes.py:62-79
         pending = []
         for a, b in chunk_ranges(int(stack.shape[0]), _lib.FB_MAX_FRAMES):
             images = stack[a:b]
             if scale != 1:                                                                    # cv2.resize, INTER_LINEAR
-                images = crop_resize_frames_device(images, list(range(b - a)), [[0, 0, w, h]] * (b - a),
-                                                   (int(scale * w), int(scale * h)), INTER_LINEAR, planar=False)
+                images = crop_resize_frames_device(images, list(range(b - a)), [[0, 0, w, h]] * (b - a), dsize, INTER_LINEAR,
+                                                   planar=False)
             im_h, im_w = int(images.shape[1]), int(images.shape[2])
             loc, conf = self.net.forward_batch(images)
             dets, n = detect.decode_batch_device(loc, conf, im_h, im_w, scale=float(scale))
-            keep, n_keep = detect.nms_batch_device(dets, n, detect.nms_threshold, _lib.NMS_CPU_NMS)
-            # the first keep_top_k kept rows of every frame (entries past a frame's count are unwritten: clamped, never read)
-            idx = keep[:, :detect.keep_top_k].long().clamp_(0, dets.shape[1] - 1)
-            kept = torch.gather(dets, 1, idx[:, :, None].expand(-1, -1, 5))
-            kept_host = torch.empty(kept.shape, dtype=kept.dtype, pin_memory=True)
-            n_host = torch.empty(n_keep.shape, dtype=n_keep.dtype, pin_memory=True)
-            kept_host.copy_(kept, non_blocking=True)
-            n_host.copy_(n_keep, non_blocking=True)
-            pending.append((kept_host, n_host))
-        torch.cuda.current_stream(self.net.device).synchronize()
-        out = []
-        for kept_host, n_host in pending:
-            kept_np, n_np = kept_host.numpy(), n_host.numpy()
-            for i in range(kept_np.shape[0]):
-                rows = kept_np[i, :min(int(n_np[i]), detect.keep_top_k)]
-                out.append([[b[0], b[1], b[2], b[3], b[4]] for b in rows if b[4] > detect.vis_thres])
-        return out
+            pending.append(self._nms_to_host(dets, n))
+        return self._boxes_of(pending)

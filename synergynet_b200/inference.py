@@ -113,6 +113,99 @@ def crop_resize_frames_device(frames, frame_index: Sequence[int], roi_boxes: Seq
     return out
 
 
+class ImagePack:
+    """N uint8 BGR images of any sizes packed back to back on one device: ``data`` is a flat uint8 CUDA tensor, image i
+    ((h_i, w_i, 3), ``sizes[i] = (h_i, w_i)``) starting at byte ``offsets[i]`` = sum of 3 h_j w_j over j < i -- the layout
+    the ``*_images`` entries of the library take."""
+
+    def __init__(self, data, sizes):
+        self.data = data
+        self.sizes = [(int(h), int(w)) for h, w in sizes]
+        self.offsets = np.concatenate([[0], np.cumsum([3 * h * w for h, w in self.sizes])]).astype(np.int64).tolist()
+        if int(data.numel()) != self.offsets[-1]:
+            raise ValueError(f'{int(data.numel())} bytes for images of {self.offsets[-1]} bytes')
+
+    def __len__(self):
+        return len(self.sizes)
+
+    def image(self, i: int):
+        """Image i as a (h, w, 3) view."""
+        h, w = self.sizes[i]
+        return self.data[self.offsets[i]:self.offsets[i + 1]].view(h, w, 3)
+
+    def slice(self, a: int, b: int) -> 'ImagePack':
+        """Images a..b-1 (a view of the same bytes)."""
+        return ImagePack(self.data[self.offsets[a]:self.offsets[b]], self.sizes[a:b])
+
+    def arrays(self):
+        """(heights, widths) as int32 arrays, for the C entries."""
+        hw = np.array(self.sizes, np.int32).reshape(-1, 2)
+        return np.ascontiguousarray(hw[:, 0]), np.ascontiguousarray(hw[:, 1])
+
+
+def pack_images(images, device) -> ImagePack:
+    """A list of (h_i, w_i, 3) BGR uint8 images of any sizes -> one :class:`ImagePack` on ``device``: host arrays are
+    packed on the host and uploaded in one copy, CUDA tensors are packed on the device.  An ImagePack on ``device``
+    passes through; one elsewhere is copied there."""
+    import torch
+    if isinstance(images, ImagePack):
+        if images.data.device == torch.device(device):
+            return images
+        return ImagePack(images.data.to(device), images.sizes)                         # bytes on another device: moved
+    images = list(images)
+    if not images:
+        raise ValueError('no images: an image list needs at least one image')
+    for im in images:
+        if im.ndim != 3 or im.shape[2] != 3 or im.shape[0] < 1 or im.shape[1] < 1:
+            raise ValueError(f'every image must be (H,W,3) with H, W >= 1, got {tuple(im.shape)}')
+        if isinstance(im, torch.Tensor) and im.dtype != torch.uint8:
+            raise ValueError(f'image tensors must be uint8, got {im.dtype}')
+    sizes = [(int(im.shape[0]), int(im.shape[1])) for im in images]
+    if all(isinstance(im, torch.Tensor) and im.is_cuda for im in images):
+        return ImagePack(torch.cat([im.to(device).reshape(-1) for im in images]), sizes)
+    host = [im.cpu().numpy() if isinstance(im, torch.Tensor) else np.asarray(im) for im in images]
+    flat = [np.ascontiguousarray(im, dtype=np.uint8).reshape(-1) for im in host]
+    # one image is already packed: no host copy of its bytes (6 MB at 1080 x 1920) before the upload
+    flat = flat[0] if len(flat) == 1 else np.concatenate(flat)
+    return ImagePack(torch.from_numpy(flat).to(device), sizes)
+
+
+def crop_resize_images_device(images: ImagePack, image_index: Sequence[int], roi_boxes: Sequence[Sequence[float]],
+                              dsize=(STD_SIZE, STD_SIZE), interpolation: int = INTER_LINEAR, planar: bool = True):
+    """:func:`crop_resize_device` for a list of images of any sizes in one launch: ROI b is ``roi_boxes[b]`` of image
+    ``image_index[b]`` of the :class:`ImagePack` ``images``.  ``dsize``: one (width, height) for every ROI -- the result is
+    then a (B,3,h,w) (``planar``) or (B,h,w,3) tensor -- or a list of one (width, height) per ROI, and the result is the
+    flat uint8 tensor of the outputs packed back to back.  The bytes of ROI b are those of
+    ``crop_resize_device(image, [roi_boxes[b]], ...)`` on its image alone."""
+    import torch
+    from . import _lib
+    lib = _lib.load()
+    B = len(roi_boxes)
+    one = len(dsize) == 2 and not hasattr(dsize[0], '__len__')
+    dsizes = [tuple(dsize)] * B if one else [tuple(d) for d in dsize]
+    if len(dsizes) != B or len(image_index) != B:
+        raise ValueError(f'{len(dsizes)} output sizes and {len(image_index)} image indices for {B} ROIs')
+    out_w = np.ascontiguousarray([int(d[0]) for d in dsizes], np.int32)
+    out_h = np.ascontiguousarray([int(d[1]) for d in dsizes], np.int32)
+    rois = np.ascontiguousarray(np.array([roi_ints(b) for b in roi_boxes], np.int32).reshape(-1, 4))
+    idx = np.ascontiguousarray(image_index, dtype=np.int32)
+    hs, ws = images.arrays()
+    n = int(lib.syn_crop_resize_images_plan_size(B, out_h.ctypes.data, out_w.ctypes.data, interpolation))
+    plan = np.zeros(max(n, 1), np.uint8)
+    _lib.check(lib.syn_crop_resize_plan_images_host(rois.ctypes.data, idx.ctypes.data, len(images), hs.ctypes.data, ws.ctypes.data, B,
+                                                    out_h.ctypes.data, out_w.ctypes.data, interpolation, plan.ctypes.data, n))
+    dev = images.data.device
+    plan = torch.from_numpy(plan).to(dev)
+    out = torch.empty((int((3 * out_h.astype(np.int64) * out_w).sum()),), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.syn_crop_resize_images(images.data.data_ptr(), plan.data_ptr(), B, out_h.ctypes.data, out_w.ctypes.data,
+                                              interpolation, int(bool(planar)), out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+    if not one:
+        return out
+    w, h = dsizes[0]
+    return out.view(B, 3, h, w) if planar else out.view(B, h, w, 3)
+
+
 def stack_frames_host(frames) -> np.ndarray:
     """N equally sized (H,W,3) BGR images (a list, or one (N,H,W,3) array) -> one contiguous uint8 (N,H,W,3) array."""
     if not (isinstance(frames, np.ndarray) and frames.ndim == 4):
@@ -122,7 +215,8 @@ def stack_frames_host(frames) -> np.ndarray:
         shapes = [tuple(f.shape) for f in frames]
         if any(sh != shapes[0] for sh in shapes):
             sizes = ', '.join('x'.join(str(d) for d in sh) for sh in sorted(set(shapes)))
-            raise ValueError(f'the frames of one batch must have one size, got {sizes}; group the frames by size')
+            raise ValueError(f'the frames of one batch must have one size, got {sizes}; group the frames by size, or use the '
+                             '*_images methods (FaceBoxes.detect_images, get_all_outputs_images), which take images of any sizes')
         frames = np.stack(frames)
     if frames.shape[0] == 0 or frames.shape[3] != 3:
         raise ValueError(f'frames must be (N,H,W,3) with N >= 1, got {tuple(frames.shape)}')

@@ -18,8 +18,8 @@ import torch.nn as nn
 from . import backbone as mobilenetv2_backbone
 from .backbone import MLP_for, MLP_rev
 from .engine import Engine
-from .inference import (INTER_LANCZOS4, INTER_LINEAR, crop_resize_device, crop_resize_frames_device, chunk_ranges, roi_affine,
-                        split_by_counts, square_roi, stack_frames_device)
+from .inference import (INTER_LANCZOS4, INTER_LINEAR, crop_resize_device, crop_resize_frames_device, crop_resize_images_device,
+                        chunk_ranges, pack_images, roi_affine, split_by_counts, square_roi, stack_frames_device)
 from .params import ParamsPack, get_param_pack, set_param_pack  # noqa: F401  (re-exported)
 
 _LOSS_KEYS = ('loss_LMK_f0', 'loss_LMK_pointNet', 'loss_Param_In', 'loss_Param_S2', 'loss_Param_S1S2')
@@ -381,7 +381,18 @@ class _SynergyBase(nn.Module):
         detector without one is called frame by frame).  Then one crop launch over the faces of all frames, one backbone
         call, one landmark and one dense reconstruction (the latter in chunks of faces above ``dense_chunk_bytes``), one
         pose decode.  ROIs are computed on the host in float64 exactly as the one-image call does."""
-        eng, stack, counts, frame_index, params, roi5 = self._frames_front(frames, rects)
+        return self._outputs(*self._frames_front(frames, rects))
+
+    def get_all_outputs_images(self, images, rects: Optional[Sequence[Sequence[Sequence[float]]]] = None):
+        """:meth:`get_all_outputs_batch` for N BGR uint8 images of any sizes (a list of host arrays or CUDA tensors): entry
+        i is what ``get_all_outputs(images[i], rects[i])`` returns, ``([], [], [])`` for an image without a face.
+
+        The images are uploaded once, packed back to back.  With ``rects=None`` the detector's ``detect_images`` gets
+        that upload (a detector without one is called image by image).  Then the same single crop launch, backbone call,
+        reconstructions and pose decode as :meth:`get_all_outputs_batch`."""
+        return self._outputs(*self._frames_front(images, rects, ragged=True))
+
+    def _outputs(self, eng, stack, counts, frame_index, params, roi5):
         n_faces = len(frame_index)
         if not n_faces:
             return [([], [], []) for _ in range(len(counts))]
@@ -398,20 +409,24 @@ class _SynergyBase(nn.Module):
         per_chunk = max(1, self.dense_chunk_bytes // (3 * 4 * max(eng.n_vert, 1)))
         return chunk_ranges(n_faces, per_chunk)
 
-    def _frames_front(self, frames, rects):
+    def _frames_front(self, frames, rects, ragged: bool = False):
         """The stages of :meth:`get_all_outputs_batch` up to the parameters, on the device: ``(engine, frame stack, faces
         per frame, frame of each face, whitened params (F,62), crop -> image maps (F,5))``; the last two are None when no
-        frame has a face."""
+        frame has a face.  ``ragged``: ``frames`` is a list of images of any sizes (:meth:`get_all_outputs_images`) and
+        the "stack" is their :class:`~synergynet_b200.inference.ImagePack`."""
         dev = self._compute_device()
         eng = self._engine(dev)
-        stack = stack_frames_device(frames, dev)
-        n = int(stack.shape[0])
+        stack = pack_images(frames, dev) if ragged else stack_frames_device(frames, dev)
+        n = len(stack) if ragged else int(stack.shape[0])
         if rects is None:
             if self.face_detector is None:
                 raise RuntimeError('no face detector configured: pass rects (one list of [x0,y0,x1,y1,score] per frame) '
                                    'or set model.face_detector')
-            if hasattr(self.face_detector, 'detect_batch'):
-                rects = self.face_detector.detect_batch(stack)
+            batched = getattr(self.face_detector, 'detect_images' if ragged else 'detect_batch', None)
+            if batched is not None:
+                rects = batched(stack)
+            elif ragged:
+                rects = [self.face_detector(stack.image(i).cpu().numpy()) for i in range(n)]
             else:
                 host = stack.cpu().numpy() if isinstance(frames, torch.Tensor) else frames
                 rects = [self.face_detector(host[i]) for i in range(n)]
@@ -423,7 +438,10 @@ class _SynergyBase(nn.Module):
         if not boxes:
             return eng, stack, counts, frame_index, None, None
         interp = INTER_LANCZOS4 if self.resize_interpolation == 'lanczos4' else INTER_LINEAR
-        batch = crop_resize_frames_device(stack, frame_index, boxes, (120, 120), interp)
+        if ragged:
+            batch = crop_resize_images_device(stack, frame_index, boxes, (120, 120), interp)
+        else:
+            batch = crop_resize_frames_device(stack, frame_index, boxes, (120, 120), interp)
         if self.I2P._adapted:
             out = eng.forward_mobilenet_v1(batch)[0] if self.I2P._is_mbv1 else eng.forward_resnet(batch)[0]
             params = out[:, :62].contiguous()
