@@ -41,6 +41,13 @@ SYN_HD float fma_rn(float a, float b, float c) { return fmaf(a, b, c); }
 SYN_HD float min_std(float a, float b) { return (b < a) ? b : a; }
 SYN_HD float max_std(float a, float b) { return (a < b) ? b : a; }
 
+// (int)v as the reference's x86-64 build computes it (cvttss2si): truncation inside [-2^31, 2^31), INT_MIN for
+// everything else, NaN included.  C leaves the out-of-range conversion undefined and nvcc resolves it differently
+// (cvt.rzi.s32.f32 saturates to INT_MAX, NaN -> 0), so the range is tested here rather than left to either compiler.
+SYN_HD int to_int_x86(float v) {
+  return (v >= -2147483648.0f && v < 2147483648.0f) ? (int)v : (int)0x80000000u;
+}
+
 // ---- barycentric coordinates -------------------------------------------------------------------------------------
 // Sim3DR/lib/rasterize_kernel.cpp:26-51 (is_point_in_tri) and :53-80 (get_point_weight) evaluate the same
 // expressions; one evaluation serves both.  v0 = p2 - p0, v1 = p1 - p0, v2 = p - p0.
@@ -81,11 +88,12 @@ struct TriSetup {
   int xmin, xmax, ymin, ymax;   // pixel bounding box, clamped to the image (:226-234); empty if xmax < xmin || ymax < ymin
 };
 
+// A maximum at or beyond 2^31 (or NaN) converts to INT_MIN, so the reference skips the triangle (its box is empty).
 SYN_HD bool tri_setup(TriSetup& t, int w, int h) {
-  t.xmin = (int)floorf(min_std(t.x0, min_std(t.x1, t.x2)));
-  t.xmax = (int)ceilf(max_std(t.x0, max_std(t.x1, t.x2)));
-  t.ymin = (int)floorf(min_std(t.y0, min_std(t.y1, t.y2)));
-  t.ymax = (int)ceilf(max_std(t.y0, max_std(t.y1, t.y2)));
+  t.xmin = to_int_x86(floorf(min_std(t.x0, min_std(t.x1, t.x2))));
+  t.xmax = to_int_x86(ceilf(max_std(t.x0, max_std(t.x1, t.x2))));
+  t.ymin = to_int_x86(floorf(min_std(t.y0, min_std(t.y1, t.y2))));
+  t.ymax = to_int_x86(ceilf(max_std(t.y0, max_std(t.y1, t.y2))));
   if (t.xmin < 0) t.xmin = 0;
   if (t.xmax > w - 1) t.xmax = w - 1;
   if (t.ymin < 0) t.ymin = 0;
@@ -126,10 +134,11 @@ SYN_HD bool pixel_key(const TriSetup& t, uint32_t tri, int x, int y, uint64_t& k
   return true;
 }
 
-// (unsigned char)((1 - alpha) * image + alpha * 255 * p_color)  (:249-255); in-range values truncate toward zero
+// (unsigned char)((1 - alpha) * image + alpha * 255 * p_color)  (:249-255): x86 truncates to int32 and keeps the low
+// byte, so a value in [256, 2^31) wraps, a negative one wraps from below, and one at or beyond 2^31 (or NaN) gives 0
 SYN_HD unsigned char blend_u8(unsigned char img, float alpha, float p_color) {
   const float v = add(mul(sub(1.0f, alpha), (float)(int)img), mul(mul(alpha, 255.0f), p_color));
-  return (unsigned char)(int)v;
+  return (unsigned char)to_int_x86(v);
 }
 
 // ---- the overlay blend (utils/render.py:45, cv2.addWeighted(img, 1 - alpha, overlap, alpha, 0) on uint8) ----------------
@@ -139,12 +148,10 @@ SYN_HD unsigned char blend_u8(unsigned char img, float alpha, float p_color) {
 // so the fused multiply-add is written out here rather than left to the compiler's contraction: the unfused
 // a * w_a + b * w_b gives other bytes (733 of the 65 536 (a, b) pairs at alpha = 0.1).  saturate_cast rounds half to
 // even (cvRound) and clamps to [0, 255]; a value outside int's range converts to INT_MIN on x86 (cvtss2si / cvtps2dq),
-// which the clamp then sends to 0 -- kept so that every finite alpha gives cv2's byte.
+// which the clamp then sends to 0 (to_int_x86) -- kept so that every finite alpha gives cv2's byte.
 SYN_HD unsigned char add_weighted_u8(unsigned char a, unsigned char b, double alpha) {
   const float wa = (float)(1.0 - alpha), wb = (float)alpha;
-  const float v = rintf(fma_rn((float)a, wa, mul((float)b, wb)));
-  if (!(v >= -2147483648.0f && v < 2147483648.0f)) return 0;
-  const int iv = (int)v;
+  const int iv = to_int_x86(rintf(fma_rn((float)a, wa, mul((float)b, wb))));
   return (unsigned char)(iv < 0 ? 0 : (iv > 255 ? 255 : iv));
 }
 

@@ -10,6 +10,7 @@ import tempfile
 import numpy as np
 import pytest
 
+from oracle import render_cases as rc
 from oracle import render_port as rp
 from synergynet_b200 import _lib, synthetic
 
@@ -146,6 +147,52 @@ def test_rasterize_signed_zero_depth_tie(emul):
         depth = np.zeros((1, 32, 32), np.float32)
         emul.emul_rasterize(P(img), 32, 32, 3, P(ver), C.c_longlong(0), 3, 1, 1, 6, P(tri), 2, P(col), C.c_float(1.0), 0, P(depth), shuffle)
         assert np.array_equal(img, want) and np.array_equal(depth[0], dwant)
+
+
+OOR = rc.out_of_range_cases()
+
+
+@pytest.mark.parametrize('case', OOR, ids=[c[0] for c in OOR])
+def test_rasterize_out_of_range_values(emul, case):
+    """Coordinates at and beyond 2^31, infinities and NaN, depths at the buffer's initial -1e8, colours whose byte wraps
+    or overflows int, degenerate triangles: render_math.h's conversions must give the reference's x86 results (a far
+    vertex skips its triangle, an overflowing colour writes 0), bit for bit with the port and the reference itself."""
+    _, ver, tri, col = case
+    h, w = rc.CANVAS
+    bg = np.random.default_rng(len(case[0])).integers(0, 256, (h, w, 3), dtype=np.uint8)
+    for reverse in (False, True):
+        want, dwant = rp.rasterize(ver, tri, col, bg.copy(), reverse=reverse, return_depth=True)
+        if rp.have_ref():
+            ref, dref = rp.rasterize(ver, tri, col, bg.copy(), reverse=reverse, return_depth=True, kind='ref')
+            assert np.array_equal(ref, want) and np.array_equal(dref, dwant)
+        for shuffle in (0, 1):
+            img = bg.copy()
+            depth = np.zeros((1, h, w), np.float32)
+            emul.emul_rasterize(P(img), h, w, 3, P(ver), C.c_longlong(0), 3, 1, 1, ver.shape[0], P(tri), tri.shape[0], P(col),
+                                C.c_float(1.0), int(reverse), P(depth), shuffle)
+            assert np.array_equal(img, want) and np.array_equal(depth[0], dwant)
+        assert (want != bg).any()                                   # the ordinary triangle of every case is drawn
+
+
+def test_out_of_range_cases_separate_x86_from_saturation():
+    """The cases hold the values where x86's conversion and a saturating one part: a far vertex skips its triangle, an
+    overflowing colour is written as 0."""
+    h, w = rc.CANVAS
+    names = {c[0]: c for c in OOR}
+    bg = np.zeros((h, w, 3), np.uint8)
+    _, ver, tri, col = names['vertex_x=3e+09']
+    assert not rc.tri_boxes(ver, tri, h, w)[1][0]
+    alone = rp.rasterize(ver, tri[:1], col, bg.copy())
+    assert not alone.any()                                          # a saturating conversion would draw 640 pixels
+    for tag in ('8421505', '1e10', 'inf'):
+        _, ver, tri, col = names[f'colour={tag}']
+        img, d = rp.rasterize(ver, tri[:1], col, bg.copy(), return_depth=True)
+        assert (d > -1e8).sum() > 100 and (img[..., 0][d > -1e8] == 0).mean() > 0.5, tag
+    _, ver, tri, col = names['colour=8421504']
+    img, d = rp.rasterize(ver, tri[:1], col, bg.copy(), return_depth=True)
+    assert (img[..., 0][d > -1e8] == 128).any()                     # 255 * 8421504 = 2^31 - 128: converts, low byte 0x80
+    assert np.array_equal(rc.x86_int(np.array([rc.F_BELOW_2_31, 2.0 ** 31, -2.0 ** 31, np.nan, -np.inf, -1.5], np.float32)),
+                          [2 ** 31 - 128, rc.INT_MIN, rc.INT_MIN, rc.INT_MIN, rc.INT_MIN, -1])
 
 
 def test_nms_bitmatrix_equals_greedy(emul, gold):
