@@ -17,6 +17,17 @@
  *   - one handle per device; a handle is not re-entrant (one call at a time per handle), but
  *     different handles may be driven from different host threads (nn.DataParallel replicas,
  *     main_train.py:176).
+ *   - CUDA graphs: an entry that takes a `stream` may be captured on it once an eager call of the
+ *     same size has run on that handle (workspaces grow, never shrink, and only eagerly).  A replay
+ *     runs with the arguments fixed at capture: the workspace pointers, the tile plans and the
+ *     syn_set_center_crop margin of that moment.  Replays are valid while no call grows that
+ *     handle's workspace and no syn_*commit, syn_resnet_select or syn_mbv1_set_widen runs; the
+ *     caller orders replays against eager calls of the same handle (they share its workspace).
+ *     A call that would grow a workspace while its stream is capturing, and the detector's frame
+ *     paths (syn_fb_forward_batch / _images: their per-call geometry comes from host memory),
+ *     return SYN_ERR_STATE before they launch anything, leaving the capture valid.  The host
+ *     pipelines (syn_forward_landmarks_host*, _submit) run on the library's own streams and wait on
+ *     the host: never call them during a capture (the Python Engine refuses).
  *   - tensors are fp32 and contiguous in the layouts the reference uses.
  */
 #ifndef SYNERGY_H100_H_
@@ -412,7 +423,8 @@ int syn_crop_resize_images(const uint8_t* images_dev, const void* plan_dev, int 
  * A separate handle: the detector has its own weights and workspace and does not touch syn_handle_t.  Like syn_handle_t
  * it is bound to one device and is not re-entrant (its activation workspace is shared by consecutive calls, which are
  * ordered by the stream they are enqueued on).  The workspace only grows: a call that needs more bytes than an earlier
- * one synchronises the device and reallocates, a call that fits runs without any synchronisation.
+ * one synchronises the device and reallocates (SYN_ERR_STATE under capture), a call that fits runs without any
+ * synchronisation.  Only syn_fb_forward can be captured in a CUDA graph (see the conventions at the top).
  * 33 convolutions in execution order (syn_fb_layer_desc names them with the reference's state_dict prefixes:
  * "conv1", "inception2.branch3x3_2", "loc.0" ...): layers with has_bn take the conv weight (OIHW fp32, no bias) and
  * the eval-mode BatchNorm2d of the same block (<name>.conv.weight / <name>.bn.*), the six head layers take weight +

@@ -14,6 +14,7 @@ LIB_PATH = os.environ.get('SYN_LIB_PATH') or os.path.join(_PKG, 'libsynergy_b200
 HEADER_PATH = os.path.join(_PKG, '..', 'include', 'synergy_b200.h')
 
 SYN_OK = 0
+SYN_ERR_STATE = 3
 ERR_NAMES = {1: 'SYN_ERR_INVALID', 2: 'SYN_ERR_CUDA', 3: 'SYN_ERR_STATE', 4: 'SYN_ERR_SHAPE',
              5: 'SYN_ERR_NOMEM', 6: 'SYN_ERR_UNSUPPORTED'}
 ENGINE_SIMT_FP32, ENGINE_TC_BF16X3, ENGINE_TC_FUSED, ENGINE_TC_FUSED_1PASS = 0, 1, 2, 3

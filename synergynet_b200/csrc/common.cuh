@@ -37,6 +37,24 @@ inline int fail(int code, const char* fmt, ...) {
       return ::syn::fail(SYN_ERR_CUDA, "launch %s -> %s", name, cudaGetErrorString(e__)); \
   } while (0)
 
+// SYN_ERR_STATE with the formatted message when `st` is capturing a CUDA graph (or holds an invalidated capture).  Called
+// before a step that a graph cannot record: a workspace growth (its cudaDeviceSynchronize is illegal under capture and
+// would invalidate it, and its cudaFree would leave earlier replays reading freed memory) or a copy from a host buffer
+// the next call rewrites.  Every call site comes before the entry's first launch, so a refused call records nothing
+// and the caller can end the capture cleanly.
+inline int refuse_capture(cudaStream_t st, const char* fmt, ...) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  SYN_CUDA(cudaStreamIsCapturing(st, &cs));
+  if (cs == cudaStreamCaptureStatusNone) return SYN_OK;
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(last_error_buf(), 512, fmt, ap);
+  va_end(ap);
+  return SYN_ERR_STATE;
+}
+// the end of a growth refusal's message
+#define SYN_EAGER_FIRST " cannot grow while the stream is capturing a CUDA graph: make an eager call before capture at this size or larger"
+
 // ---- network geometry (reference backbone_nets/mobilenetv2_backbone.py:108-138) ---------------
 constexpr int kImg = 120;
 constexpr int kNumConv = 52;

@@ -535,12 +535,13 @@ inline FbGeom fb_geom(int h, int w) {
 // Pixels of every level summed over the frames of a call -> every buffer is the packed map of its level.  A buffer that
 // is too small for the call is reallocated with the device idle (like Workspace::ensure of the backbones); one that is
 // large enough is kept, so a stream of calls of different sizes stops allocating once it has met its largest.
-int fb_workspace(syn_fb* f, const size_t* pix) {
+int fb_workspace(syn_fb* f, const size_t* pix, cudaStream_t st, const char* who, int height, int width) {
   const size_t floats[13] = {pix[1] * 48, pix[2] * 48, pix[3] * 128, pix[4] * 128, pix[4] * 128, pix[4] * 128, pix[4] * 24,
                              pix[4] * 24, pix[4] * 32, pix[4] * 128, pix[5] * 256, pix[5] * 128, pix[6] * 256};
   bool fits = f->geo_dev != nullptr;
   for (int k = 0; k < 13; ++k) fits = fits && sizeof(float) * floats[k] <= f->ws_sizes[k];
   if (fits) return SYN_OK;
+  if (int rc = refuse_capture(st, "%s: a %dx%d input: the detector workspace" SYN_EAGER_FIRST, who, height, width)) return rc;
   SYN_CUDA(cudaDeviceSynchronize());
   size_t keep[13];
   for (int k = 0; k < 13; ++k) keep[k] = std::max(f->ws_sizes[k], sizeof(float) * floats[k]);
@@ -660,7 +661,13 @@ int fb_forward_body(syn_fb* f, const uint8_t* image_dev, int frames, const int32
   }
   if (frames && (R.pix[0] * 3 > (size_t)INT32_MAX || np_all * 4 > (size_t)INT32_MAX))
     return fail(SYN_ERR_SHAPE, "%s: %zu pixels in one call exceed the packed maps' int32 indices", who, R.pix[0]);
-  if (int rc = fb_workspace(f, R.pix)) return rc;
+  // the frame paths copy this call's geometry from geo_host, which the next call rewrites: a graph would replay the
+  // copy from whatever the host buffer then holds.  Only the one-image path (frames == 0) can be captured.
+  if (frames)
+    if (int rc = refuse_capture(st, "%s: %d frames: the frame paths cannot be captured in a CUDA graph (their per-call geometry "
+                                    "is copied from host memory); capture syn_fb_forward, one image per call", who, frames))
+      return rc;
+  if (int rc = fb_workspace(f, R.pix, st, who, height, width)) return rc;
   R.geo = f->geo_dev;
   if (frames) SYN_CUDA(cudaMemcpyAsync(f->geo_dev, f->geo_host, sizeof(FbLevel) * kFbLevels * nf, cudaMemcpyHostToDevice, st));
   if (stop) {

@@ -156,8 +156,9 @@ void mark(syn_handle* h, cudaStream_t st, const char* name) {
   cudaEventRecord(h->tev[h->tn++], st);
 }
 
-int ensure_workspace(syn_handle* h, int batch) {
+int ensure_workspace(syn_handle* h, int batch, cudaStream_t st) {
   if (batch <= h->ws_batch) return SYN_OK;
+  if (int rc = refuse_capture(st, "batch %d: the activation workspace (%d faces)" SYN_EAGER_FIRST, batch, h->ws_batch)) return rc;
   SYN_CUDA(cudaDeviceSynchronize());
   cudaFree(h->buf_io[0]); cudaFree(h->buf_io[1]); cudaFree(h->buf_hid); cudaFree(h->buf_dw);
   cudaFree(h->d_params_tmp); cudaFree(h->d_pool_tmp);
@@ -233,11 +234,12 @@ int launch_fused(syn_handle* h, const float* x, int block, float* y, int batch, 
 int run_backbone(syn_handle* h, const float* x, int batch, float* params, float* pool,
                  int stop_layer, float* dbg_out, cudaStream_t st, const uint8_t* x_u8 = nullptr) {
   const Plan& P = plan();
-  int rc = ensure_workspace(h, batch);
+  int rc = ensure_workspace(h, batch, st);
   if (rc != SYN_OK) return rc;
   if (x_u8 != nullptr && !h->fused()) {
     // engines whose stem reads fp32: normalise into a scratch buffer first
     if (batch > h->x_f32_batch) {
+      if ((rc = refuse_capture(st, "batch %d: the uint8 crops' fp32 scratch (%d faces)" SYN_EAGER_FIRST, batch, h->x_f32_batch))) return rc;
       SYN_CUDA(cudaDeviceSynchronize());
       cudaFree(h->d_x_f32);
       h->d_x_f32 = nullptr;
@@ -365,17 +367,25 @@ static cudaError_t launch_after_prepass(void (*kernel)(DenseArgs), int grid, int
   return cudaLaunchKernelEx(&cfg, kernel, a);
 }
 
+// The tensor-core reconstruction's per-call tiles (alpha images and pose rows) for `batch` faces.
+int ensure_recon_tiles(syn_handle* h, int batch, cudaStream_t st) {
+  const int n_ftiles = (batch + kDnFaces - 1) / kDnFaces;
+  if (n_ftiles <= h->recon_ftiles) return SYN_OK;
+  if (int rc = refuse_capture(st, "batch %d: the reconstruction tiles (%d faces)" SYN_EAGER_FIRST, batch, h->recon_ftiles * kDnFaces))
+    return rc;
+  SYN_CUDA(cudaDeviceSynchronize());
+  cudaFree(h->d_alpha_img); cudaFree(h->d_pose);
+  h->d_alpha_img = nullptr; h->d_pose = nullptr; h->recon_ftiles = 0;
+  SYN_CUDA(cudaMalloc(&h->d_alpha_img, (size_t)n_ftiles * kDnBTile));
+  SYN_CUDA(cudaMalloc(&h->d_pose, (size_t)n_ftiles * kDnPoseTile));
+  h->recon_ftiles = n_ftiles;
+  return SYN_OK;
+}
+
 int run_reconstruct_tc(syn_handle* h, const float* params, int batch, int dense, int whitening, int transform,
                        float* out, cudaStream_t st, const float* roi5 = nullptr) {
   const int n_ftiles = (batch + kDnFaces - 1) / kDnFaces;
-  if (n_ftiles > h->recon_ftiles) {
-    SYN_CUDA(cudaDeviceSynchronize());
-    cudaFree(h->d_alpha_img); cudaFree(h->d_pose);
-    h->d_alpha_img = nullptr; h->d_pose = nullptr; h->recon_ftiles = 0;
-    SYN_CUDA(cudaMalloc(&h->d_alpha_img, (size_t)n_ftiles * kDnBTile));
-    SYN_CUDA(cudaMalloc(&h->d_pose, (size_t)n_ftiles * kDnPoseTile));
-    h->recon_ftiles = n_ftiles;
-  }
+  if (int rc = ensure_recon_tiles(h, batch, st)) return rc;
   dense_alpha_kernel<<<n_ftiles, kDnAlphaThreads, 0, st>>>(params, h->d_mean, h->d_std, h->d_ascale, h->d_alpha_img, h->d_pose, batch,
                                              whitening, roi5);
   SYN_LAUNCH_CHECK("dense_alpha_kernel");
@@ -1004,7 +1014,9 @@ int syn_forward_landmarks(syn_handle_t* h, const float* x, int batch, float* par
   SYN_CHECK_READY(h, "syn_forward_landmarks");
   if (x == nullptr || lmk == nullptr || batch <= 0) return fail(SYN_ERR_INVALID, "syn_forward_landmarks: bad argument");
   DeviceGuard g(h->device);
-  int rc = ensure_workspace(h, batch);
+  // every buffer the call needs grows before its first launch (a refused capture then records nothing)
+  int rc = ensure_workspace(h, batch, (cudaStream_t)stream);
+  if (rc == SYN_OK) rc = ensure_recon_tiles(h, batch, (cudaStream_t)stream);
   if (rc != SYN_OK) return rc;
   float* p = params ? params : h->d_params_tmp;
   if (h->timing) { mark(h, (cudaStream_t)stream, "start"); h->launches--; }
@@ -1035,7 +1047,9 @@ int syn_forward_landmarks_u8(syn_handle_t* h, const uint8_t* x_u8, int batch, fl
   SYN_CHECK_READY(h, "syn_forward_landmarks_u8");
   if (x_u8 == nullptr || lmk == nullptr || batch <= 0) return fail(SYN_ERR_INVALID, "syn_forward_landmarks_u8: bad argument");
   DeviceGuard g(h->device);
-  int rc = ensure_workspace(h, batch);
+  // every buffer the call needs grows before its first launch (a refused capture then records nothing)
+  int rc = ensure_workspace(h, batch, (cudaStream_t)stream);
+  if (rc == SYN_OK) rc = ensure_recon_tiles(h, batch, (cudaStream_t)stream);
   if (rc != SYN_OK) return rc;
   float* p = params ? params : h->d_params_tmp;
   rc = run_backbone(h, nullptr, batch, p, nullptr, -1, nullptr, (cudaStream_t)stream, x_u8);
@@ -1096,7 +1110,7 @@ static int host_submit_impl(syn_handle_t* h, const void* x_host, int is_u8, int 
     }
     stage[0] = h->d_stage_x[0]; stage[1] = h->d_stage_x[1];
   }
-  int rc = ensure_workspace(h, chunk);
+  int rc = ensure_workspace(h, chunk, h->s_compute);
   if (rc != SYN_OK) return rc;
   int issued = 0;
   for (int b0 = 0, nb = 0; b0 < batch; b0 += nb, h->host_slot ^= 1, ++h->host_chunks, ++issued) {

@@ -25,6 +25,52 @@ def _host_f32(t) -> torch.Tensor:
     return t.detach().to(device='cpu', dtype=torch.float32).contiguous()
 
 
+class StreamOrder:
+    """Orders the calls of one library handle that arrive on different CUDA streams.  The handle's calls share one
+    device workspace, so a call waits (on its own stream, through an event) for the device work of the previous call
+    when that ran on another stream.  The caller holds the handle's lock around ``begin`` .. the C call .. ``end``.
+
+    Under CUDA-graph capture neither records an event (it would join the graph): the caller orders replays against
+    eager calls of the same handle, e.g. ``s2.wait_stream(s1)`` after a replay on ``s1``."""
+
+    def __init__(self, device: torch.device):
+        self.device = device
+        self._last_stream = None
+        self._last_event = None
+
+    def begin(self) -> int:
+        """The current stream of the device, ordered after the previous call; returns its handle for the C call."""
+        st = torch.cuda.current_stream(self.device)
+        if torch.cuda.is_current_stream_capturing():
+            return st.cuda_stream
+        if self._last_stream is not None and self._last_stream != st.cuda_stream:
+            st.wait_event(self._last_event)
+        return st.cuda_stream
+
+    def end(self) -> None:
+        """Mark the device work of the call just enqueued on the current stream."""
+        if torch.cuda.is_current_stream_capturing():
+            return
+        st = torch.cuda.current_stream(self.device)
+        if self._last_event is None:
+            self._last_event = torch.cuda.Event()
+        self._last_event.record(st)
+        self._last_stream = st.cuda_stream
+
+    def synchronize(self) -> None:
+        """Block the host until the device work of the last call has finished."""
+        if self._last_event is not None:
+            self._last_event.synchronize()
+
+
+def refuse_under_capture(what: str) -> None:
+    """Raise SYN_ERR_STATE if the current stream is capturing a CUDA graph: for calls that run on the library's own
+    streams and synchronise the host, which a graph cannot hold."""
+    if torch.cuda.is_current_stream_capturing():
+        raise _lib.SynergyLibError(_lib.SYN_ERR_STATE, f"{what}: runs on the library's own streams and waits on the host, "
+                                                       "so it cannot be captured in a CUDA graph; call it outside the capture")
+
+
 class Engine:
     """Owns one ``syn_handle_t`` bound to ``cuda:<device>``."""
 
@@ -48,8 +94,7 @@ class Engine:
         # consecutive calls that arrive on different CUDA streams with an event.
         self._lock = threading.RLock()
         self._host_inflight: Dict[int, tuple] = {}     # ticket -> tensors of a submitted host call (kept alive)
-        self._last_stream = None
-        self._last_event = None
+        self._order = StreamOrder(self.device)
 
     def close(self):
         if getattr(self, '_h', None):
@@ -130,25 +175,15 @@ class Engine:
         return x.to(torch.float32).contiguous()
 
     def _stream(self) -> int:
-        """Current torch stream of the engine's device; if the previous call ran on another stream, that
-        stream's work is ordered before this call (the workspace buffers are shared)."""
-        st = torch.cuda.current_stream(self.device)
-        if torch.cuda.is_current_stream_capturing():
-            return st.cuda_stream            # CUDA-graph capture: no cross-stream events (they would join the graph)
-        for ticket in list(self._host_inflight):     # submitted host calls run on the library's own streams and use the
-            _lib.check(self._lib.syn_host_wait(self._h, ticket))   # same workspace: let them finish (tickets stay valid)
-        if self._last_stream is not None and self._last_stream != st.cuda_stream and self._last_event is not None:
-            st.wait_event(self._last_event)
-        return st.cuda_stream
+        """Current torch stream of the engine's device, ordered after the previous call (``StreamOrder``) and after
+        any submitted host call."""
+        if not torch.cuda.is_current_stream_capturing():
+            for ticket in list(self._host_inflight):     # submitted host calls run on the library's own streams and use
+                _lib.check(self._lib.syn_host_wait(self._h, ticket))   # the same workspace: let them finish (tickets stay valid)
+        return self._order.begin()
 
     def _done(self) -> None:
-        if torch.cuda.is_current_stream_capturing():
-            return
-        st = torch.cuda.current_stream(self.device)
-        if self._last_event is None:
-            self._last_event = torch.cuda.Event()
-        self._last_event.record(st)
-        self._last_stream = st.cuda_stream
+        self._order.end()
 
     def raise_if_error(self) -> None:
         """Cheap (no device sync) look at the sticky time-out flag of the bounded in-kernel waits; call it after a
@@ -289,6 +324,7 @@ class Engine:
         if x_host.dim() != 4 or tuple(x_host.shape[1:]) != (3, 120, 120):
             raise RuntimeError(f'expected (B,3,120,120) crops, got {tuple(x_host.shape)}')
         b = x_host.shape[0]
+        refuse_under_capture(f'forward_landmarks_host: batch {b}')
         if lmk_host is None:
             lmk_host = torch.empty((b, 3, self.n_pts), dtype=torch.float32)
         # the C side writes B*3*n_pts and B*62 floats through these pointers: refuse anything it could overrun
@@ -299,8 +335,7 @@ class Engine:
                 raise RuntimeError(f'{name} must be a contiguous CPU float32 tensor with at least {need} elements')
         ticket = C.c_int(0)
         with self._lock:
-            if self._last_event is not None:         # stream-ordered calls share the workspace with the host pipeline
-                self._last_event.synchronize()
+            self._order.synchronize()                # stream-ordered calls share the workspace with the host pipeline
             _lib.check(self._lib.syn_forward_landmarks_host_submit(
                 self._h, x_host.data_ptr(), 1 if x_host.dtype == torch.uint8 else 0, b,
                 params_host.data_ptr() if params_host is not None else None, lmk_host.data_ptr(), C.byref(ticket)))

@@ -13,12 +13,14 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import threading
 from typing import Dict, List, Optional
 
 import numpy as np
 import torch
 
 from . import _lib, detect
+from .engine import StreamOrder
 from .inference import (INTER_LINEAR, ImagePack, chunk_ranges, crop_resize_device, crop_resize_frames_device, crop_resize_images_device,
                         pack_images, stack_frames_device)
 
@@ -74,6 +76,10 @@ class FaceBoxesNet:
         h = C.c_void_p()
         _lib.check(self._lib.syn_fb_create(self.device.index or 0, C.byref(h)))
         self._h = h
+        # the handle is not re-entrant and its calls share one activation workspace: serialise the host threads and order
+        # calls that arrive on different streams, as Engine does
+        self._lock = threading.RLock()
+        self._order = StreamOrder(self.device)
         sd = {(k[7:] if k.startswith('module.') else k): v for k, v in state_dict.items()}       # utils/functions.py:19-24
         f32 = lambda t: torch.as_tensor(t).detach().to(device='cpu', dtype=torch.float32).contiguous()
         for L in layer_plan():
@@ -112,9 +118,10 @@ class FaceBoxesNet:
         p = detect.num_priors(h, w)
         loc = torch.empty((p, 4), dtype=torch.float32, device=self.device)
         conf = torch.empty((p, 2), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
+        with torch.cuda.device(self.device), self._lock:
             _lib.check(self._lib.syn_fb_forward(self._h, image.data_ptr(), h, w, loc.data_ptr(), conf.data_ptr(),
-                                                torch.cuda.current_stream(self.device).cuda_stream))
+                                                self._order.begin()))
+            self._order.end()
         return loc, conf
 
     def debug_forward_until(self, image: torch.Tensor, stage: int) -> torch.Tensor:
@@ -130,10 +137,11 @@ class FaceBoxesNet:
         conf = torch.full((p * 2,), float('nan'), dtype=torch.float32, device=self.device)
         shape = debug_stage_shape(stage, h, w)
         out = torch.empty(shape, dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
+        with torch.cuda.device(self.device), self._lock:
             _lib.check(self._lib.syn_fb_debug_forward_until(self._h, image.data_ptr(), h, w, stage, out.data_ptr(), out.numel(),
                                                             loc.data_ptr(), conf.data_ptr(),
-                                                            torch.cuda.current_stream(self.device).cuda_stream))
+                                                            self._order.begin()))
+            self._order.end()
         return out
 
     def _check_stack(self, images: torch.Tensor):
@@ -151,9 +159,10 @@ class FaceBoxesNet:
         p = detect.num_priors(h, w)
         loc = torch.empty((n, p, 4), dtype=torch.float32, device=self.device)
         conf = torch.empty((n, p, 2), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
+        with torch.cuda.device(self.device), self._lock:
             _lib.check(self._lib.syn_fb_forward_batch(self._h, images.data_ptr(), n, h, w, loc.data_ptr(), conf.data_ptr(),
-                                                      torch.cuda.current_stream(self.device).cuda_stream))
+                                                      self._order.begin()))
+            self._order.end()
         return loc, conf
 
     def debug_forward_batch_until(self, images: torch.Tensor, stage: int) -> torch.Tensor:
@@ -165,10 +174,11 @@ class FaceBoxesNet:
         loc = torch.full((n, p * 4), float('nan'), dtype=torch.float32, device=self.device)
         conf = torch.full((n, p * 2), float('nan'), dtype=torch.float32, device=self.device)
         out = torch.empty((n,) + tuple(debug_stage_shape(stage, h, w)), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
+        with torch.cuda.device(self.device), self._lock:
             _lib.check(self._lib.syn_fb_debug_forward_batch_until(self._h, images.data_ptr(), n, h, w, stage, out.data_ptr(),
                                                                   out.numel(), loc.data_ptr(), conf.data_ptr(),
-                                                                  torch.cuda.current_stream(self.device).cuda_stream))
+                                                                  self._order.begin()))
+            self._order.end()
         return out
 
     def _check_images(self, images):
@@ -197,9 +207,10 @@ class FaceBoxesNet:
         loc = torch.empty((p[-1], 4), dtype=torch.float32, device=self.device)
         conf = torch.empty((p[-1], 2), dtype=torch.float32, device=self.device)
         hs, ws = pack.arrays()
-        with torch.cuda.device(self.device):
+        with torch.cuda.device(self.device), self._lock:
             _lib.check(self._lib.syn_fb_forward_images(self._h, pack.data.data_ptr(), len(pack), hs.ctypes.data, ws.ctypes.data,
-                                                       loc.data_ptr(), conf.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream))
+                                                       loc.data_ptr(), conf.data_ptr(), self._order.begin()))
+            self._order.end()
         return loc, conf, p
 
     def forward_images(self, images):
@@ -219,10 +230,11 @@ class FaceBoxesNet:
         numel = [int(np.prod(sh)) for sh in shapes]
         out = torch.empty((sum(numel),), dtype=torch.float32, device=self.device)
         hs, ws = pack.arrays()
-        with torch.cuda.device(self.device):
+        with torch.cuda.device(self.device), self._lock:
             _lib.check(self._lib.syn_fb_debug_forward_images_until(self._h, pack.data.data_ptr(), len(pack), hs.ctypes.data, ws.ctypes.data,
                                                                    stage, out.data_ptr(), out.numel(), loc.data_ptr(), conf.data_ptr(),
-                                                                   torch.cuda.current_stream(self.device).cuda_stream))
+                                                                   self._order.begin()))
+            self._order.end()
         at = np.concatenate([[0], np.cumsum(numel)]).astype(int).tolist()
         return [out[a:b].view(sh) for a, b, sh in zip(at[:-1], at[1:], shapes)]
 
