@@ -319,6 +319,23 @@ int syn_rasterize_frames(const uint8_t* frames_dev, uint8_t* solid_dev, int n_fr
  * out = saturate(round_half_even(fmaf(a, (float)(1 - alpha), b * (float)alpha))), 1 - alpha in double (csrc/render_math.h
  * add_weighted_u8).  out_dev may be a_dev or b_dev.  Any finite alpha; otherwise SYN_ERR_INVALID. */
 int syn_add_weighted_u8(const uint8_t* a_dev, const uint8_t* b_dev, double alpha, uint8_t* out_dev, int64_t n, void* stream);
+/* The pose axes of draw_axis (utils/inference.py:199-244, three cv2.line calls of thickness 4 per face, called once per
+ * face in rect order by singleImage.py:112-117) for many images at once: cv2.line(img, p0, p1, colour, 4) with LINE_8
+ * and shift 0, byte for byte with OpenCV 4.x (csrc/draw_math.h), for every segment, drawn IN PLACE.
+ *   images_dev: image_bytes uint8; image f is (h, w, 3) BGR at byte offset off of the frame table (n_frames,3) int64
+ *     (off, h, w), given as frames_host (checked here) and frames_dev (its device copy, which the kernel reads); the
+ *     images lie in memory order, disjoint, inside the image bytes (an equal-size stack, or an ImagePack).
+ *   segs_dev (n_segs,5) int32: x0, y0, x1, y1 and the colour b | g << 8 | r << 16; image f owns segments
+ *     [seg_start[f], seg_start[f+1]), in draw order: where segments overlap, the later one's colour is left.  seg_start
+ *     comes as seg_start_host (checked here) and seg_start_dev (read by the kernel).
+ * A segment that leaves its image is clipped to it; nothing outside an image's own bytes is written.  thickness other
+ * than 4 or line_type other than 8 is SYN_ERR_UNSUPPORTED, a null pointer or a negative count SYN_ERR_INVALID, a
+ * seg_start that does not run monotonically from 0 to n_segs or a frame table that does not fit SYN_ERR_SHAPE, all
+ * before any launch.  No allocation and no synchronisation (graph capture is fine); host arrays are read during the
+ * call only. */
+int syn_draw_lines(uint8_t* images_dev, int64_t image_bytes, const int64_t* frames_host, const int64_t* frames_dev, int n_frames,
+                   const int32_t* seg_start_host, const int32_t* seg_start_dev, const int32_t* segs_dev, int n_segs, int thickness,
+                   int line_type, void* stream);
 
 /* ---- FaceBoxes post-processing (SURVEY.md section 8 row f3) -----------------------------------------------------------
  * These entries take the detector network's outputs (syn_fb_forward below, or any other producer). */

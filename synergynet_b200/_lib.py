@@ -108,6 +108,7 @@ SIGNATURES = {
     'syn_render_frames_plan': (_I, [_F, _L, _I, _I, _I, _I, _F, _I, _P, _I, _I, _I, _F, _F, _P]),
     'syn_rasterize_frames': (_I, [_F, _F, _I, _I, _I, _I, _F, _L, _I, _I, _I, _I, _F, _I, _F, _I, _P, _F, _F, _F, _L, _F, _L, _P]),
     'syn_add_weighted_u8': (_I, [_F, _F, C.c_double, _F, _L, _P]),
+    'syn_draw_lines': (_I, [_F, _L, _P, _F, _I, _P, _F, _F, _I, _I, _I, _P]),
     'syn_nms': (_I, [_F, _I, C.c_double, _I, _F, _F, _F, _P]),
     'syn_crop_resize_plan_size': (_L, [_I, _I, _I, _I]),
     'syn_crop_resize_plan_host': (_I, [_P, _I, _I, _I, _I, _P, _L]),
@@ -164,7 +165,7 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_crop_resize_batch', 'syn_render_frames_plan', 'syn_rasterize_frames',
                                              'syn_add_weighted_u8', 'syn_fb_forward_images', 'syn_fb_debug_forward_images_until',
                                              'syn_faceboxes_decode_images', 'syn_crop_resize_images_plan_size',
-                                             'syn_crop_resize_plan_images_host', 'syn_crop_resize_images')}
+                                             'syn_crop_resize_plan_images_host', 'syn_crop_resize_images', 'syn_draw_lines')}
 
 
 def declared_symbols(header: str = HEADER_PATH):

@@ -1,10 +1,11 @@
 // C ABI of the stages either side of the 3DMM path (SURVEY.md section 8 rows f2, f3): Sim3DR normals / lighting /
-// rasterisation of the dense meshes, the FaceBoxes box decode + greedy NMS that produces the crops, and the crop + resize
-// that turns boxes (or an oversized detector input) into network inputs.
+// rasterisation of the dense meshes, the FaceBoxes box decode + greedy NMS that produces the crops, the crop + resize
+// that turns boxes (or an oversized detector input) into network inputs, and the pose axes drawn over the frames.
 // Handle-free: device pointers and workspaces belong to the caller (include/synergy_b200.h states the sizes).
 #include "kernels_render.cuh"
 #include "kernels_detect.cuh"
 #include "kernels_resize.cuh"
+#include "kernels_draw.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -251,6 +252,42 @@ int syn_add_weighted_u8(const uint8_t* a_dev, const uint8_t* b_dev, double alpha
   const int blocks = (int)std::min<long long>((work + 255) / 256, 1 << 20);
   add_weighted_u8_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a_dev, b_dev, alpha, out_dev, (long long)n, vec ? 1 : 0);
   SYN_LAUNCH_CHECK("add_weighted_u8_kernel");
+  return SYN_OK;
+}
+
+int syn_draw_lines(uint8_t* images_dev, int64_t image_bytes, const int64_t* frames_host, const int64_t* frames_dev, int n_frames,
+                   const int32_t* seg_start_host, const int32_t* seg_start_dev, const int32_t* segs_dev, int n_segs, int thickness,
+                   int line_type, void* stream) {
+  const char* who = "syn_draw_lines";
+  if (!images_dev || !frames_host || !frames_dev || !seg_start_host || !seg_start_dev || (n_segs > 0 && !segs_dev))
+    return fail(SYN_ERR_INVALID, "%s: null pointer", who);
+  if (n_frames <= 0 || n_segs < 0 || image_bytes < 0)
+    return fail(SYN_ERR_INVALID, "%s: %d frames, %d segments, %lld image bytes", who, n_frames, n_segs, (long long)image_bytes);
+  if (thickness != dmath::kThickness)
+    return fail(SYN_ERR_UNSUPPORTED, "%s: thickness %d (only %d, the thickness of draw_axis, is restated)", who, thickness,
+                dmath::kThickness);
+  if (line_type != 8) return fail(SYN_ERR_UNSUPPORTED, "%s: line type %d (only LINE_8 = 8)", who, line_type);
+  if (seg_start_host[0] != 0 || seg_start_host[n_frames] != n_segs)
+    return fail(SYN_ERR_SHAPE, "%s: seg_start runs from %d to %d, must run from 0 to %d segments", who, seg_start_host[0],
+                seg_start_host[n_frames], n_segs);
+  for (int f = 0; f < n_frames; ++f)
+    if (seg_start_host[f + 1] < seg_start_host[f])
+      return fail(SYN_ERR_SHAPE, "%s: seg_start is not monotone at frame %d (%d after %d)", who, f, seg_start_host[f + 1],
+                  seg_start_host[f]);
+  int64_t end = 0;                                   // the frames in memory order, disjoint, inside the image bytes
+  for (int f = 0; f < n_frames; ++f) {
+    const int64_t off = frames_host[3 * f], h = frames_host[3 * f + 1], w = frames_host[3 * f + 2];
+    if (h < 1 || w < 1 || h > INT32_MAX || w > INT32_MAX)
+      return fail(SYN_ERR_SHAPE, "%s: frame %d is %lldx%lld", who, f, (long long)h, (long long)w);
+    if (off < end || off > image_bytes || h > (image_bytes - off) / 3 / w)
+      return fail(SYN_ERR_SHAPE, "%s: frame %d (%lldx%lld at byte %lld) does not fit the %lld image bytes after the frame before it", who,
+                  f, (long long)h, (long long)w, (long long)off, (long long)image_bytes);
+    end = off + 3 * h * w;
+  }
+  if (n_segs == 0) return SYN_OK;
+  draw_lines_kernel<<<n_frames, kDrawThreads, 0, (cudaStream_t)stream>>>(images_dev, reinterpret_cast<const long long*>(frames_dev),
+                                                                       seg_start_dev, segs_dev);
+  SYN_LAUNCH_CHECK("draw_lines_kernel");
   return SYN_OK;
 }
 

@@ -6,6 +6,8 @@ device twin ``crop_resize_device`` live here; vertex reconstruction and the pose
 """
 from __future__ import annotations
 
+import math
+from math import cos, sin
 from typing import Sequence, Tuple
 
 import numpy as np
@@ -295,3 +297,124 @@ RENDER_CFG = {
     'intensity_specular': 0.2, 'specular_exp': 5,
     'light_pos': (0, 0, 5), 'view_pos': (0, 0, 5),
 }
+
+
+# ---- the pose axes (utils/inference.py:199-244, draw_axis; singleImage.py:112-117 calls it once per face) ----------------
+AXIS_COLOURS = ((0, 0, 255), (0, 255, 0), (255, 0, 0))        # BGR of the x (red), y (green) and z (blue) axes
+AXIS_THICKNESS = 4
+_INT32 = (-2 ** 31, 2 ** 31 - 1)
+
+
+def plan_axis(yaw, pitch, roll, pts68):
+    """The three ``cv2.line`` segments ``draw_axis`` draws for one face: ``(segments, error)``.  ``segments`` is a list of
+    ``(x0, y0, x1, y1, (b, g, r))`` integer segments, in draw order; ``error`` is None, or the exception the reference
+    raises after drawing those segments (``ValueError`` for a NaN point, ``OverflowError`` for an infinite one, and
+    for a point outside int32 -- where the reference's ``cv2.line`` raises ``cv2.error`` -- an ``OverflowError`` naming
+    it).
+
+    The expressions are the reference's, in its scalar types: with Python float angles and float32 ``pts68`` (what
+    ``get_all_outputs`` returns), the extents' product is float32, ``size`` a Python float, and every end point
+    ``size * (...) + tdx`` a NumPy float32 (NEP 50: the Python float term is cast to float32, then added), truncated
+    toward zero by ``int()``.  ``math.cos`` / ``math.sin`` are libm's, as the reference's are.  ``tdx``, ``tdy`` and
+    ``size`` of the reference's signature are overwritten by it, so they are not taken here."""
+    try:
+        pitch = pitch * np.pi / 180
+        yaw = -(yaw * np.pi / 180)
+        roll = roll * np.pi / 180
+        tdx = pts68[0, 30]
+        tdy = pts68[1, 30]
+        minx, maxx = np.min(pts68[0, :]), np.max(pts68[0, :])
+        miny, maxy = np.min(pts68[1, :]), np.max(pts68[1, :])
+        size = math.sqrt((maxx - minx) * (maxy - miny)) * 0.5
+        ends = ((size * (cos(yaw) * cos(roll)) + tdx, size * (cos(pitch) * sin(roll) + cos(roll) * sin(pitch) * sin(yaw)) + tdy),
+                (size * (-cos(yaw) * sin(roll)) + tdx, size * (cos(pitch) * cos(roll) - sin(pitch) * sin(yaw) * sin(roll)) + tdy),
+                (size * (sin(yaw)) + tdx, size * (-cos(yaw) * sin(pitch)) + tdy))
+    except (ValueError, OverflowError) as e:             # math.cos of an infinite angle: before any line, as there
+        return [], e
+    segments = []
+    for (x, y), colour in zip(ends, AXIS_COLOURS):
+        try:
+            p0, p1 = (int(tdx), int(tdy)), (int(x), int(y))
+        except (ValueError, OverflowError) as e:
+            return segments, e
+        for p in (p0, p1):
+            if not all(_INT32[0] <= v <= _INT32[1] for v in p):
+                return segments, OverflowError(f'draw_axis: point {p} lies outside int32, which cv2.line cannot draw')
+        segments.append((*p0, *p1, colour))
+    return segments, None
+
+
+def _segment_table(seg_lists, frames):
+    """One int64 buffer for syn_draw_lines: frames (n,3) | seg_start (n+1) int32 | segments (S,5) int32, 8-byte aligned.
+    ``frames``: (n,3) int64 byte offset, height, width.  Returns (buffer, n_segs, seg_start view, frames view)."""
+    counts = [len(s) for s in seg_lists]
+    n, n_segs = len(counts), sum(counts)
+    start = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+    segs = np.array([[x0, y0, x1, y1, b | (g << 8) | (r << 16)] for sl in seg_lists for x0, y0, x1, y1, (b, g, r) in sl],
+                    np.int64).reshape(-1, 5).astype(np.int32)
+    a = 3 * n
+    b = a + (n + 2) // 2
+    buf = np.zeros(b + (5 * n_segs + 1) // 2, np.int64)
+    buf[:a] = np.asarray(frames, np.int64).reshape(-1)
+    buf[a:b].view(np.int32)[:n + 1] = start
+    buf[b:].view(np.int32)[:5 * n_segs] = segs.reshape(-1)
+    return buf, (a, b), n_segs, start
+
+
+def draw_lines_device(images, seg_lists, thickness: int = AXIS_THICKNESS):
+    """``cv2.line(image, (x0, y0), (x1, y1), (b, g, r), thickness)`` for every segment of ``seg_lists[i]`` onto image i,
+    in order, IN PLACE, in one launch (``syn_draw_lines``; only thickness 4 -- draw_axis's -- is restated).  ``images``:
+    a contiguous uint8 (N,H,W,3) CUDA stack, or an :class:`ImagePack`.  One upload of the segments; no synchronisation."""
+    import torch
+    from . import _lib
+    if isinstance(images, ImagePack):
+        data, sizes = images.data, images.sizes
+        offsets = images.offsets[:-1]
+    else:
+        if images.dtype != torch.uint8 or images.dim() != 4 or images.shape[3] != 3 or not images.is_cuda or not images.is_contiguous():
+            raise ValueError('images must be a contiguous uint8 (N,H,W,3) CUDA tensor or an ImagePack')
+        n, h, w = (int(v) for v in images.shape[:3])
+        data, sizes, offsets = images, [(h, w)] * n, [3 * h * w * i for i in range(n)]
+    if len(seg_lists) != len(sizes):
+        raise ValueError(f'{len(seg_lists)} segment lists for {len(sizes)} images')
+    frames = np.array([[o, h, w] for o, (h, w) in zip(offsets, sizes)], np.int64)
+    buf, (a, b), n_segs, start = _segment_table(seg_lists, frames)
+    if n_segs == 0:
+        return images
+    dev = data.device
+    table = torch.from_numpy(buf).to(dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().syn_draw_lines(data.data_ptr(), data.numel(), frames.ctypes.data, table.data_ptr(), len(sizes),
+                                              start.ctypes.data, table[a:b].data_ptr(), table[b:].data_ptr(), n_segs, int(thickness),
+                                              8, torch.cuda.current_stream(dev).cuda_stream))
+    return images
+
+
+def draw_axis(img, yaw, pitch, roll, tdx=None, tdy=None, size=100, pts68=None):
+    """``utils/inference.py:199-244`` on the GPU, byte for byte: the x, y and z axes of one face as three ``cv2.line``
+    segments of thickness 4 from landmark 30 of ``pts68`` (3,68), scaled by the landmarks' extent; ``tdx``, ``tdy`` and
+    ``size`` are ignored, as the reference overwrites them.  ``img``: a (H,W,3) uint8 BGR numpy array -- drawn on the
+    device and copied back into the same array -- or a contiguous CUDA tensor, drawn in place.  Returns ``img``.
+
+    Where the reference raises, this raises too, after drawing the axes the reference draws before the failing one: a
+    NaN end point is ``ValueError``, a point outside int32 an ``OverflowError`` naming it (``cv2.error`` there)."""
+    import torch
+    segments, error = plan_axis(yaw, pitch, roll, pts68)
+    if isinstance(img, torch.Tensor):
+        if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[2] != 3 or not img.is_cuda or not img.is_contiguous():
+            raise ValueError('draw_axis draws on a contiguous uint8 (H,W,3) CUDA tensor or a uint8 (H,W,3) numpy array')
+        if segments:
+            draw_lines_device(img.unsqueeze(0), [segments])
+    else:
+        if not isinstance(img, np.ndarray) or img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
+            raise ValueError('draw_axis draws on a contiguous uint8 (H,W,3) CUDA tensor or a uint8 (H,W,3) numpy array')
+        if segments:
+            if not torch.cuda.is_available():
+                raise RuntimeError('draw_axis needs a CUDA device (H100, sm_90a); there is no CPU fallback')
+            dev = torch.device('cuda', torch.cuda.current_device())
+            canvas = torch.from_numpy(np.ascontiguousarray(img)).to(dev)
+            draw_lines_device(canvas.unsqueeze(0), [segments])
+            img[...] = canvas.cpu().numpy()
+    if error is not None:
+        raise error
+    return img

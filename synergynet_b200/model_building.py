@@ -18,8 +18,9 @@ import torch.nn as nn
 from . import backbone as mobilenetv2_backbone
 from .backbone import MLP_for, MLP_rev
 from .engine import Engine
-from .inference import (INTER_LANCZOS4, INTER_LINEAR, crop_resize_device, crop_resize_frames_device, crop_resize_images_device,
-                        chunk_ranges, pack_images, roi_affine, split_by_counts, square_roi, stack_frames_device)
+from .inference import (INTER_LANCZOS4, INTER_LINEAR, ImagePack, crop_resize_device, crop_resize_frames_device, crop_resize_images_device,
+                        chunk_ranges, draw_lines_device, pack_images, plan_axis, roi_affine, split_by_counts, square_roi,
+                        stack_frames_device)
 from .params import ParamsPack, get_param_pack, set_param_pack  # noqa: F401  (re-exported)
 
 _LOSS_KEYS = ('loss_LMK_f0', 'loss_LMK_pointNet', 'loss_Param_In', 'loss_Param_S2', 'loss_Param_S1S2')
@@ -482,6 +483,60 @@ class _SynergyBase(nn.Module):
         if isinstance(frames, torch.Tensor) and frames.is_cuda:
             return blended, solid
         return blended.cpu().numpy(), solid.cpu().numpy()
+
+    def pose_overlay_batch(self, frames, rects: Optional[Sequence[Sequence[Sequence[float]]]] = None):
+        """The pose image of singleImage.py:112-118 for N equally sized BGR uint8 frames in one pass: every face's axes
+        drawn by ``draw_axis`` onto a copy of its frame.  Frame i's bytes are those of a loop of
+        ``draw_axis(frame_i_copy, *angles, *t3d[:2], size=50, pts68=lmk)`` over the faces ``get_all_outputs_batch``
+        returns for it; a frame without a face comes back unchanged.  Returns an (N,H,W,3) uint8 numpy array, or a CUDA
+        tensor when ``frames`` is a CUDA stack.
+
+        The frames are uploaded once (and detected on the device when ``rects`` is None); crops, backbone, landmarks and
+        pose decode run as in ``get_all_outputs_batch``; one small copy brings back the landmarks and angles for the
+        host's end-point plan (:func:`~synergynet_b200.inference.plan_axis`), one upload takes the segments, and one
+        launch draws them onto a clone of the frames.  A face whose plan fails -- where the reference's draw_axis would
+        raise -- raises before anything is drawn, naming the frame and the face."""
+        eng, stack, counts, frame_index, params, roi5 = self._frames_front(frames, rects)
+        out = self._pose_overlay(eng, stack.clone(), counts, params, roi5)
+        if isinstance(frames, torch.Tensor) and frames.is_cuda:
+            return out
+        return out.cpu().numpy()
+
+    def pose_overlay_images(self, images, rects: Optional[Sequence[Sequence[Sequence[float]]]] = None):
+        """:meth:`pose_overlay_batch` for N BGR uint8 images of any sizes: a list of N (h_i,w_i,3) images, numpy arrays --
+        or CUDA tensors when every input image is a CUDA tensor -- each with the bytes of the ``draw_axis`` loop over
+        the faces ``get_all_outputs_images`` returns for it."""
+        eng, pack, counts, frame_index, params, roi5 = self._frames_front(images, rects, ragged=True)
+        out = self._pose_overlay(eng, ImagePack(pack.data.clone(), pack.sizes), counts, params, roi5)
+        views = [out.image(i) for i in range(len(out))]
+        if all(isinstance(im, torch.Tensor) and im.is_cuda for im in images):
+            return views
+        host = out.data.cpu().numpy()
+        return [host[out.offsets[i]:out.offsets[i + 1]].reshape(h, w, 3) for i, (h, w) in enumerate(out.sizes)]
+
+    def _pose_overlay(self, eng, canvas, counts, params, roi5):
+        """Plan every face's axes on the host and draw them onto ``canvas`` (a stack or an ImagePack), in place."""
+        n_faces = sum(counts)
+        if not n_faces:
+            return canvas
+        lmk = eng.reconstruct_image(params, roi5, dense=False)                    # (F,3,68) float32
+        ang, _ = eng.pose_decode(params, roi5)                                    # (F,3) float64
+        host = torch.cat([lmk.reshape(-1).view(torch.uint8), ang.reshape(-1).view(torch.uint8)]).cpu().numpy()
+        eng.raise_if_error()
+        nl = lmk.numel() * 4
+        lmk = host[:nl].view(np.float32).reshape(tuple(lmk.shape))
+        ang = host[nl:].view(np.float64).reshape(n_faces, 3)
+        seg_lists, face = [], 0
+        for f, c in enumerate(counts):
+            segs = []
+            for j in range(c):
+                s, err = plan_axis(*ang[face].tolist(), lmk[face])
+                if err is not None:
+                    raise type(err)(f'frame {f}, face {j}: {err}') from err
+                segs += s
+                face += 1
+            seg_lists.append(segs)
+        return draw_lines_device(canvas, seg_lists)
 
 
 class SynergyNet(_SynergyBase):
