@@ -34,6 +34,7 @@
 #define SYNERGY_H100_H_
 
 #include <stdint.h>
+#include <stddef.h>
 
 #ifdef __cplusplus
 extern "C" {
@@ -578,6 +579,22 @@ int syn_debug_gemm(syn_handle_t* h, const float* w_host, const float* bias_host,
  * (the partial last wave is split so that more SMs share it), otherwise the last group may be
  * partial.  Lets the host logic be tested without a GPU. */
 int syn_debug_tile_plan(int batch, int sms, int faces_per_tile, int* split, int* face_groups);
+
+/* Poisoned-workspace tests only; no product path calls these.  A handle's workspaces only grow and are never cleared, so
+ * a call smaller than an earlier one runs on that call's bytes past its own extent.  syn_debug_fill_workspaces sets every
+ * byte of every device buffer the handle has grown -- at its allocated size, not the last call's -- to `byte` (0..255)
+ * with stream-ordered memsets on `stream`, and reports the total in *bytes_filled (nullable): the MobileNetV2 activations,
+ * d_params_tmp and d_pool_tmp, the uint8 crops' fp32 scratch, the reconstruction tiles, the host pipelines' staging
+ * buffers (their streams wait for the fill), the PointNet workspace and the conv+BN backbone workspaces.  Weights, packed
+ * bases, plans and the error and saturation flags are not touched.  syn_fb_debug_fill_workspaces does the same for the
+ * detector's 13 activation buffers; its geometry table (pixel offsets) is cleared to 0 and counted, never filled with
+ * `byte`.  Both refuse a capturing stream with SYN_ERR_STATE, so a fill is never recorded into a graph.
+ * syn_debug_fill_on_grow / syn_fb_debug_fill_on_grow: every later workspace growth of the handle sets its new buffers
+ * to `byte` right after allocating them (the detector's geometry table to 0); -1 (the default) turns this off. */
+int syn_debug_fill_workspaces(syn_handle_t* h, int byte, size_t* bytes_filled, void* stream);
+int syn_debug_fill_on_grow(syn_handle_t* h, int byte);
+int syn_fb_debug_fill_workspaces(syn_fb_t* f, int byte, size_t* bytes_filled, void* stream);
+int syn_fb_debug_fill_on_grow(syn_fb_t* f, int byte);
 
 #ifdef __cplusplus
 }

@@ -144,6 +144,10 @@ SIGNATURES = {
     'syn_poll_saturation': (_I, [_P, C.POINTER(C.c_int)]),
     'syn_debug_forward_until': (_I, [_P, _F, _I, _I, _F, _P]),
     'syn_debug_tile_plan': (_I, [_I, _I, _I, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    'syn_debug_fill_workspaces': (_I, [_P, _I, C.POINTER(C.c_size_t), _P]),
+    'syn_debug_fill_on_grow': (_I, [_P, _I]),
+    'syn_fb_debug_fill_workspaces': (_I, [_P, _I, C.POINTER(C.c_size_t), _P]),
+    'syn_fb_debug_fill_on_grow': (_I, [_P, _I]),
 }
 
 
@@ -165,7 +169,9 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_crop_resize_batch', 'syn_render_frames_plan', 'syn_rasterize_frames',
                                              'syn_add_weighted_u8', 'syn_fb_forward_images', 'syn_fb_debug_forward_images_until',
                                              'syn_faceboxes_decode_images', 'syn_crop_resize_images_plan_size',
-                                             'syn_crop_resize_plan_images_host', 'syn_crop_resize_images', 'syn_draw_lines')}
+                                             'syn_crop_resize_plan_images_host', 'syn_crop_resize_images', 'syn_draw_lines',
+                                             'syn_debug_fill_workspaces', 'syn_debug_fill_on_grow',
+                                             'syn_fb_debug_fill_workspaces', 'syn_fb_debug_fill_on_grow')}
 
 
 def declared_symbols(header: str = HEADER_PATH):

@@ -55,6 +55,25 @@ inline int refuse_capture(cudaStream_t st, const char* fmt, ...) {
 // the end of a growth refusal's message
 #define SYN_EAGER_FIRST " cannot grow while the stream is capturing a CUDA graph: make an eager call before capture at this size or larger"
 
+// The cudaMalloc of every workspace growth site.  fill >= 0 (syn_debug_fill_on_grow / syn_fb_debug_fill_on_grow) sets
+// every byte of the new buffer to `fill` before the growing call launches anything, so that a call which grows its own
+// workspace runs on poison, not on the zeroed pages a fresh allocation usually returns.  Growth sites run with the
+// device idle and never under capture, so the blocking memset orders before every stream of the handle.
+template <class T>
+inline cudaError_t grow_alloc(T** p, size_t bytes, int fill) {
+  cudaError_t e = cudaMalloc(reinterpret_cast<void**>(p), bytes);
+  if (e == cudaSuccess && fill >= 0) e = cudaMemset(*p, fill, bytes);
+  if (e == cudaSuccess && fill >= 0) e = cudaDeviceSynchronize();
+  return e;
+}
+
+// One buffer of a debug fill (syn_debug_fill_workspaces): `bytes` bytes at p set to `byte` on stream st, counted in *total.
+inline cudaError_t fill_buffer(void* p, size_t bytes, int byte, cudaStream_t st, size_t* total) {
+  if (p == nullptr || bytes == 0) return cudaSuccess;
+  *total += bytes;
+  return cudaMemsetAsync(p, byte, bytes, st);
+}
+
 // ---- network geometry (reference backbone_nets/mobilenetv2_backbone.py:108-138) ---------------
 constexpr int kImg = 120;
 constexpr int kNumConv = 52;

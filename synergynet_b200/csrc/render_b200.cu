@@ -544,6 +544,7 @@ struct syn_fb {
   // frame-axis geometry, FbLevel[kFbLevels][frames]: built on the host per call, one copy to the device
   FbLevel geo_host[kFbLevels * SYN_FB_MAX_FRAMES] = {};
   FbLevel* geo_dev = nullptr;
+  int fill_on_grow = -1;                    // debug: byte every workspace growth fills its new buffers with (-1: off)
   int64_t launches = 0;
 };
 
@@ -586,9 +587,9 @@ int fb_workspace(syn_fb* f, const size_t* pix, cudaStream_t st, const char* who,
   float** bufs[13] = {&f->c1, &f->p1, &f->c2, &f->xa, &f->xb, &f->avg, &f->r1, &f->r2, &f->t3, &f->c31, &f->c32, &f->c41, &f->c42};
   for (int k = 0; k < 13; ++k) {
     f->ws_sizes[k] = keep[k];
-    SYN_CUDA(cudaMalloc(bufs[k], f->ws_sizes[k]));
+    SYN_CUDA(grow_alloc(bufs[k], f->ws_sizes[k], f->fill_on_grow));
   }
-  SYN_CUDA(cudaMalloc(&f->geo_dev, sizeof(f->geo_host)));
+  SYN_CUDA(grow_alloc(&f->geo_dev, sizeof(f->geo_host), f->fill_on_grow < 0 ? -1 : 0));
   return SYN_OK;
 }
 
@@ -876,6 +877,27 @@ int syn_fb_commit(syn_fb_t* f) {
 }
 
 int64_t syn_fb_launch_count(const syn_fb_t* f) { return f ? f->launches : 0; }
+
+int syn_fb_debug_fill_workspaces(syn_fb_t* f, int byte, size_t* bytes_filled, void* stream) {
+  const char* who = "syn_fb_debug_fill_workspaces";
+  if (!f || byte < 0 || byte > 255) return fail(SYN_ERR_INVALID, "%s: null handle or byte %d", who, byte);
+  cudaStream_t st = (cudaStream_t)stream;
+  SYN_CUDA(cudaSetDevice(f->device));
+  if (int rc = refuse_capture(st, "%s: a fill is never recorded into a CUDA graph", who)) return rc;
+  float* bufs[13] = {f->c1, f->p1, f->c2, f->xa, f->xb, f->avg, f->r1, f->r2, f->t3, f->c31, f->c32, f->c41, f->c42};
+  size_t total = 0;
+  for (int k = 0; k < 13; ++k) SYN_CUDA(fill_buffer(bufs[k], f->ws_sizes[k], byte, st, &total));
+  // the geometry table holds pixel offsets: cleared, never filled with a byte pattern that could turn into an address
+  SYN_CUDA(fill_buffer(f->geo_dev, sizeof(f->geo_host), 0, st, &total));
+  if (bytes_filled) *bytes_filled = total;
+  return SYN_OK;
+}
+
+int syn_fb_debug_fill_on_grow(syn_fb_t* f, int byte) {
+  if (!f || byte < -1 || byte > 255) return fail(SYN_ERR_INVALID, "syn_fb_debug_fill_on_grow: null handle or byte %d", byte);
+  f->fill_on_grow = byte;
+  return SYN_OK;
+}
 
 int syn_fb_forward(syn_fb_t* f, const uint8_t* image_dev, int height, int width, float* loc_dev, float* conf_dev, void* stream) {
   return fb_forward_body(f, image_dev, 0, &height, &width, loc_dev, conf_dev, (cudaStream_t)stream, nullptr, "syn_fb_forward");

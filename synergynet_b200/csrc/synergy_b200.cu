@@ -51,6 +51,7 @@ struct syn_handle {
   int sm_count = 0;
   int engine = SYN_ENGINE_TC_FUSED;            // default: fused tensor-core engine; 0/1 remain for cross-checks
   int center_crop = 0;                         // CenterCrop margin applied by the uint8 entry points (syn_set_center_crop)
+  int fill_on_grow = -1;                       // debug: byte every workspace growth fills its new buffers with (-1: off)
   int npass() const { return engine == SYN_ENGINE_TC_FUSED_1PASS ? 1 : 3; }
   bool fused() const { return engine == SYN_ENGINE_TC_FUSED || engine == SYN_ENGINE_TC_FUSED_1PASS; }
   bool committed = false;
@@ -116,6 +117,7 @@ struct syn_handle {
   float* d_stage_lmk = nullptr;
   float* d_stage_par = nullptr;
   int stage_chunk = 0, stage_batch = 0;
+  size_t stage_lmk_bytes = 0;
   int host_slot = 0;                             // staging buffer of the next chunk (persists across calls)
   unsigned long long host_chunks = 0;            // chunks issued so far
   unsigned long long host_calls = 0;             // submitted host calls = next ticket
@@ -165,12 +167,12 @@ int ensure_workspace(syn_handle* h, int batch, cudaStream_t st) {
   h->buf_io[0] = h->buf_io[1] = h->buf_hid = h->buf_dw = h->d_params_tmp = h->d_pool_tmp = nullptr;
   h->ws_batch = 0;
   const size_t b = (size_t)batch;
-  SYN_CUDA(cudaMalloc(&h->buf_io[0], b * kIoPerFace * sizeof(float)));
-  SYN_CUDA(cudaMalloc(&h->buf_io[1], b * kIoPerFace * sizeof(float)));
-  SYN_CUDA(cudaMalloc(&h->buf_hid, b * kHidPerFace * sizeof(float)));
-  SYN_CUDA(cudaMalloc(&h->buf_dw, b * kDwPerFace * sizeof(float)));
-  SYN_CUDA(cudaMalloc(&h->d_params_tmp, b * kNumParams * sizeof(float)));
-  SYN_CUDA(cudaMalloc(&h->d_pool_tmp, b * kLastCh * sizeof(float)));
+  SYN_CUDA(grow_alloc(&h->buf_io[0], b * kIoPerFace * sizeof(float), h->fill_on_grow));
+  SYN_CUDA(grow_alloc(&h->buf_io[1], b * kIoPerFace * sizeof(float), h->fill_on_grow));
+  SYN_CUDA(grow_alloc(&h->buf_hid, b * kHidPerFace * sizeof(float), h->fill_on_grow));
+  SYN_CUDA(grow_alloc(&h->buf_dw, b * kDwPerFace * sizeof(float), h->fill_on_grow));
+  SYN_CUDA(grow_alloc(&h->d_params_tmp, b * kNumParams * sizeof(float), h->fill_on_grow));
+  SYN_CUDA(grow_alloc(&h->d_pool_tmp, b * kLastCh * sizeof(float), h->fill_on_grow));
   h->ws_batch = batch;
   return SYN_OK;
 }
@@ -244,7 +246,7 @@ int run_backbone(syn_handle* h, const float* x, int batch, float* params, float*
       cudaFree(h->d_x_f32);
       h->d_x_f32 = nullptr;
       h->x_f32_batch = 0;
-      SYN_CUDA(cudaMalloc(&h->d_x_f32, (size_t)batch * 3 * kImg * kImg * sizeof(float)));
+      SYN_CUDA(grow_alloc(&h->d_x_f32, (size_t)batch * 3 * kImg * kImg * sizeof(float), h->fill_on_grow));
       h->x_f32_batch = batch;
     }
     const size_t n4 = (size_t)batch * 3 * kImg * kImg / 4;
@@ -376,8 +378,8 @@ int ensure_recon_tiles(syn_handle* h, int batch, cudaStream_t st) {
   SYN_CUDA(cudaDeviceSynchronize());
   cudaFree(h->d_alpha_img); cudaFree(h->d_pose);
   h->d_alpha_img = nullptr; h->d_pose = nullptr; h->recon_ftiles = 0;
-  SYN_CUDA(cudaMalloc(&h->d_alpha_img, (size_t)n_ftiles * kDnBTile));
-  SYN_CUDA(cudaMalloc(&h->d_pose, (size_t)n_ftiles * kDnPoseTile));
+  SYN_CUDA(grow_alloc(&h->d_alpha_img, (size_t)n_ftiles * kDnBTile, h->fill_on_grow));
+  SYN_CUDA(grow_alloc(&h->d_pose, (size_t)n_ftiles * kDnPoseTile, h->fill_on_grow));
   h->recon_ftiles = n_ftiles;
   return SYN_OK;
 }
@@ -1082,8 +1084,10 @@ static int host_submit_impl(syn_handle_t* h, const void* x_host, int is_u8, int 
     cudaFree(h->d_stage_lmk); cudaFree(h->d_stage_par);
     h->d_stage_lmk = h->d_stage_par = nullptr;
     h->stage_batch = 0;
-    SYN_CUDA(cudaMalloc(&h->d_stage_lmk, batch * lmk_face * sizeof(float)));
-    SYN_CUDA(cudaMalloc(&h->d_stage_par, (size_t)batch * kNumParams * sizeof(float)));
+    h->stage_lmk_bytes = 0;
+    SYN_CUDA(grow_alloc(&h->d_stage_lmk, batch * lmk_face * sizeof(float), h->fill_on_grow));
+    h->stage_lmk_bytes = batch * lmk_face * sizeof(float);
+    SYN_CUDA(grow_alloc(&h->d_stage_par, (size_t)batch * kNumParams * sizeof(float), h->fill_on_grow));
     h->stage_batch = batch;
   }
   void* stage[2];
@@ -1093,8 +1097,8 @@ static int host_submit_impl(syn_handle_t* h, const void* x_host, int is_u8, int 
       cudaFree(h->d_stage_u8[0]); cudaFree(h->d_stage_u8[1]);
       h->d_stage_u8[0] = h->d_stage_u8[1] = nullptr;
       h->stage_u8_chunk = 0;
-      SYN_CUDA(cudaMalloc(&h->d_stage_u8[0], chunk * x_face));
-      SYN_CUDA(cudaMalloc(&h->d_stage_u8[1], chunk * x_face));
+      SYN_CUDA(grow_alloc(&h->d_stage_u8[0], chunk * x_face, h->fill_on_grow));
+      SYN_CUDA(grow_alloc(&h->d_stage_u8[1], chunk * x_face, h->fill_on_grow));
       h->stage_u8_chunk = chunk;
     }
     stage[0] = h->d_stage_u8[0]; stage[1] = h->d_stage_u8[1];
@@ -1104,8 +1108,8 @@ static int host_submit_impl(syn_handle_t* h, const void* x_host, int is_u8, int 
       cudaFree(h->d_stage_x[0]); cudaFree(h->d_stage_x[1]);
       h->d_stage_x[0] = h->d_stage_x[1] = nullptr;
       h->stage_chunk = 0;
-      SYN_CUDA(cudaMalloc(&h->d_stage_x[0], chunk * x_face * sizeof(float)));
-      SYN_CUDA(cudaMalloc(&h->d_stage_x[1], chunk * x_face * sizeof(float)));
+      SYN_CUDA(grow_alloc(&h->d_stage_x[0], chunk * x_face * sizeof(float), h->fill_on_grow));
+      SYN_CUDA(grow_alloc(&h->d_stage_x[1], chunk * x_face * sizeof(float), h->fill_on_grow));
       h->stage_chunk = chunk;
     }
     stage[0] = h->d_stage_x[0]; stage[1] = h->d_stage_x[1];
@@ -1278,3 +1282,49 @@ int syn_debug_forward_until(syn_handle_t* h, const float* x, int batch, int laye
 #include "convbn_host.inl"
 #include "resnet_host.inl"
 #include "mbv1_host.inl"
+
+// ---- debug: poisoned workspaces (include/synergy_b200.h) ------------------------------------------------------------------
+extern "C" {
+
+int syn_debug_fill_workspaces(syn_handle_t* h, int byte, size_t* bytes_filled, void* stream) {
+  if (h == nullptr || byte < 0 || byte > 255) return fail(SYN_ERR_INVALID, "syn_debug_fill_workspaces: null handle or byte %d", byte);
+  cudaStream_t st = (cudaStream_t)stream;
+  DeviceGuard g(h->device);
+  if (int rc = refuse_capture(st, "syn_debug_fill_workspaces: a fill is never recorded into a CUDA graph")) return rc;
+  const size_t B = (size_t)h->ws_batch, x_face = (size_t)3 * kImg * kImg;
+  const struct { void* p; size_t bytes; } bufs[] = {
+      {h->buf_io[0], B * kIoPerFace * sizeof(float)}, {h->buf_io[1], B * kIoPerFace * sizeof(float)},
+      {h->buf_hid, B * kHidPerFace * sizeof(float)}, {h->buf_dw, B * kDwPerFace * sizeof(float)},
+      {h->d_params_tmp, B * kNumParams * sizeof(float)}, {h->d_pool_tmp, B * kLastCh * sizeof(float)},
+      {h->d_x_f32, (size_t)h->x_f32_batch * x_face * sizeof(float)},
+      {h->d_alpha_img, (size_t)h->recon_ftiles * kDnBTile}, {h->d_pose, (size_t)h->recon_ftiles * kDnPoseTile},
+      {h->d_stage_u8[0], (size_t)h->stage_u8_chunk * x_face}, {h->d_stage_u8[1], (size_t)h->stage_u8_chunk * x_face},
+      {h->d_stage_x[0], (size_t)h->stage_chunk * x_face * sizeof(float)},
+      {h->d_stage_x[1], (size_t)h->stage_chunk * x_face * sizeof(float)},
+      {h->d_stage_lmk, h->stage_lmk_bytes}, {h->d_stage_par, (size_t)h->stage_batch * kNumParams * sizeof(float)}};
+  size_t total = 0;
+  for (const auto& b : bufs) SYN_CUDA(fill_buffer(b.p, b.bytes, byte, st, &total));
+  SYN_CUDA(heads_fill(h->heads, byte, st, &total));
+  if (h->resnet != nullptr) SYN_CUDA(h->resnet->ws.fill(byte, st, &total));
+  if (h->mbv1 != nullptr) SYN_CUDA(h->mbv1->ws.fill(byte, st, &total));
+  // the host pipelines run on the handle's own streams: they start after the fill
+  if (h->s_compute != nullptr && h->s_compute != st) {
+    cudaEvent_t e;
+    SYN_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    cudaError_t err = cudaEventRecord(e, st);
+    if (err == cudaSuccess) err = cudaStreamWaitEvent(h->s_copy, e, 0);
+    if (err == cudaSuccess) err = cudaStreamWaitEvent(h->s_compute, e, 0);
+    cudaEventDestroy(e);
+    SYN_CUDA(err);
+  }
+  if (bytes_filled != nullptr) *bytes_filled = total;
+  return SYN_OK;
+}
+
+int syn_debug_fill_on_grow(syn_handle_t* h, int byte) {
+  if (h == nullptr || byte < -1 || byte > 255) return fail(SYN_ERR_INVALID, "syn_debug_fill_on_grow: null handle or byte %d", byte);
+  h->fill_on_grow = byte;
+  return SYN_OK;
+}
+
+}  // extern "C"

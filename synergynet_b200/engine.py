@@ -625,6 +625,21 @@ class Engine:
             self._done()
         return out, rmo, cm
 
+    # ---- poisoned workspaces (tests only, include/synergy_b200.h syn_debug_fill_workspaces) ------------------------
+    def debug_fill_workspaces(self, byte: int) -> int:
+        """Set every byte of every device workspace the handle has grown, at its allocated size, to ``byte``, ordered
+        on the current stream after the previous call; returns the number of bytes filled."""
+        n = C.c_size_t(0)
+        with self._lock:
+            _lib.check(self._lib.syn_debug_fill_workspaces(self._h, int(byte), C.byref(n), self._stream()))
+            self._done()
+        return int(n.value)
+
+    def debug_fill_on_grow(self, byte: int) -> None:
+        """Every later workspace growth sets its new buffers to ``byte`` (-1: off)."""
+        with self._lock:
+            _lib.check(self._lib.syn_debug_fill_on_grow(self._h, int(byte)))
+
     def debug_forward_until(self, x: torch.Tensor, layer: int) -> torch.Tensor:
         x = self._check_x(x)
         spec = conv_plan()[layer]

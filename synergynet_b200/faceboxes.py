@@ -124,6 +124,21 @@ class FaceBoxesNet:
             self._order.end()
         return loc, conf
 
+    def debug_fill_workspaces(self, byte: int) -> int:
+        """Set every byte of the detector's activation workspace, at its allocated size, to ``byte`` and clear its
+        geometry table, ordered on the current stream after the previous call; returns the number of bytes written.
+        Poisoned-workspace tests only."""
+        n = C.c_size_t(0)
+        with torch.cuda.device(self.device), self._lock:
+            _lib.check(self._lib.syn_fb_debug_fill_workspaces(self._h, int(byte), C.byref(n), self._order.begin()))
+            self._order.end()
+        return int(n.value)
+
+    def debug_fill_on_grow(self, byte: int) -> None:
+        """Every later workspace growth sets its new buffers to ``byte`` (-1: off).  Poisoned-workspace tests only."""
+        with self._lock:
+            _lib.check(self._lib.syn_fb_debug_fill_on_grow(self._h, int(byte)))
+
     def debug_forward_until(self, image: torch.Tensor, stage: int) -> torch.Tensor:
         """Run :meth:`forward`'s launch sequence up to launch ``stage`` (0..38, table at ``syn_fb_debug_forward_until`` in
         include/synergy_b200.h) and return the whole tensor that launch wrote: an NHWC ``(h, w, channels)`` map, or the
