@@ -316,6 +316,33 @@ int syn_rasterize_frames(const uint8_t* frames_dev, uint8_t* solid_dev, int n_fr
                          const int32_t* tri_dev, int ntri, const float* colors_dev, int color_channels, const int32_t* mesh_start_host,
                          const int32_t* mesh_start_dev, const int32_t* boxes_dev, const int64_t* key_off_dev, int64_t n_keys,
                          uint64_t* keys_ws_dev, int64_t keys_ws_count, void* stream);
+/* The same overlay stage (utils/render.py:31-53, per image; rasterize_kernel.cpp:217-287 for the z-buffer) for a list of
+ * images of different sizes, drawn in one pass.  Image f is (h, w, channels) uint8 at byte offset off of the image table
+ * (n_images,3) int64 (off, h, w).  The table comes as images_host (checked here) and images_dev (its device copy, which
+ * the kernels read).  The images lie in memory order, disjoint, inside the image_bytes of the pack, and every off is a
+ * multiple of channels: a packed image list, an equal-size stack, or a slice of either.  Image f owns meshes
+ * [mesh_start[f], mesh_start[f+1]) of the n_meshes meshes, in draw order; mesh_start comes as mesh_start_host (checked)
+ * and mesh_start_dev (read by the kernels).  Each mesh's pixel box is clamped to its OWN image, so a mesh off its image
+ * draws nothing, even where a larger image of the list would hold it.  Nothing outside an image's own bytes is written.
+ *   syn_render_images_plan writes boxes_dev and key_off_dev as syn_render_frames_plan does.
+ *   syn_rasterize_images reads images_dev and writes the solid overlays to solid_dev (the same layout; it may be
+ *   images_dev, to draw in place).  Image f's bytes are what syn_rasterize_frames draws onto a one-frame stack of that
+ *   image with its meshes.  colors_dev (n_meshes,nver,color_channels); n_keys = key_off_dev[n_meshes]; keys_ws_dev holds
+ *   keys_ws_count >= n_keys uint64.
+ * All checks run before any launch.  SYN_ERR_INVALID: a null pointer, or not 1..65535 images and meshes.  SYN_ERR_SHAPE:
+ * a table that is out of order, overlaps, does not fit the image bytes or has an offset that is not a multiple of
+ * channels; a mesh_start that does not run monotonically from 0 to n_meshes; image and colour channels that differ; a
+ * key workspace smaller than n_keys.  Host arrays are read during the call only. */
+int syn_render_images_plan(const float* vertices_dev, int64_t stride_mesh, int stride_vertex, int stride_coord, int n_meshes, int nver,
+                           const int32_t* tri_dev, int ntri, const int32_t* mesh_start_host, const int32_t* mesh_start_dev,
+                           const int64_t* images_host, const int64_t* images_dev, int n_images, int64_t image_bytes, int channels,
+                           int32_t* boxes_dev, int64_t* key_off_dev, void* stream);
+int syn_rasterize_images(const uint8_t* images_dev, uint8_t* solid_dev, int64_t image_bytes, const int64_t* table_host,
+                         const int64_t* table_dev, int n_images, int channels, const float* vertices_dev, int64_t stride_mesh,
+                         int stride_vertex, int stride_coord, int n_meshes, int nver, const int32_t* tri_dev, int ntri,
+                         const float* colors_dev, int color_channels, const int32_t* mesh_start_host, const int32_t* mesh_start_dev,
+                         const int32_t* boxes_dev, const int64_t* key_off_dev, int64_t n_keys, uint64_t* keys_ws_dev,
+                         int64_t keys_ws_count, void* stream);
 /* cv2.addWeighted(a, 1 - alpha, b, alpha, 0) on n uint8 values (utils/render.py:45), byte for byte with OpenCV 4.x:
  * out = saturate(round_half_even(fmaf(a, (float)(1 - alpha), b * (float)alpha))), 1 - alpha in double (csrc/render_math.h
  * add_weighted_u8).  out_dev may be a_dev or b_dev.  Any finite alpha; otherwise SYN_ERR_INVALID. */

@@ -2,7 +2,8 @@
 """The frame-batch and image-list paths for `compute-sanitizer --tool memcheck` / `--tool racecheck` (needs an H100): one
 batched detector pass on frames whose maps make 64-row tiles straddle frames, one ``detect_batch`` with the device
 shrink, one ``get_all_outputs_batch`` with ROIs over the frame edges and a frame without a face; then the same on a list of
-images of different sizes (1 x 1 images sharing a tile, two oversized images shrunk by different scales).
+images of different sizes (1 x 1 images sharing a tile, two oversized images shrunk by different scales), and one
+``overlay_images`` over a 1 x 1 image, faces across their own image's edges and a dense chunk that ends inside an image.
 scripts/sanitizer_smoke.py covers the one-image kernels."""
 import os
 import sys
@@ -36,10 +37,18 @@ def main():
     boxes_i = det.detect_images(images)
     rects_i = [rects[0], [], rects[2], [], [[600.0, 650.0, 1200.0, 780.0, 0.9]], [], [[-3.0, -3.0, 80.0, 70.0, 0.9]]]
     out_i = m.get_all_outputs_images(images, rects=rects_i)
+    # overlay_images: a 1 x 1 image with a face, faces across their own image's edges, and dense chunks of two faces, so
+    # that a chunk ends inside image 0 and the next spans images 0 and 1
+    ov_images = [images[0], images[1], images[2], images[6]]
+    ov_rects = [rects[0] + [[180.0, 150.0, 280.0, 260.0, 0.8]], [[-2.0, -2.0, 3.0, 3.0, 0.9]], [],
+                [[-30.0, 20.0, 40.0, 90.0, 0.9], [30.0, -25.0, 90.0, 50.0, 0.8]]]
+    m.dense_chunk_bytes = 2 * 3 * 4 * synthetic.NVER
+    ov_b, ov_s = m.overlay_images(ov_images, rects=ov_rects, connectivity=synthetic.make_render_topology().T)
     torch.cuda.synchronize()
     m._engine(torch.device('cuda', 0)).raise_if_error()
     print('sanitizer frames done:', tuple(loc.shape), [len(b) for b in boxes], [len(b) for b in big], [len(t[0]) for t in out])
     print('sanitizer images done:', [tuple(x.shape) for x in loc_i], [len(b) for b in boxes_i], [len(t[0]) for t in out_i])
+    print('sanitizer overlay images done:', [x.shape for x in ov_s])
 
 
 if __name__ == '__main__':

@@ -199,6 +199,87 @@ class MeshRenderer:
             solid = self.rasterize_frames(frames_dev, vertices, col, counts)
         return add_weighted(frames_dev, solid, alpha), solid
 
+    # -- the image list: images of any sizes -----------------------------------------------------------------------------
+    def _image_axis(self, pack, counts):
+        """Host and device copies of the image table (n,3) int64 (offset, h, w) and of mesh_start (n+1) int32 of an
+        :class:`~synergynet_b200.inference.ImagePack`: ``(table, start, device buffer, table_dev ptr, start_dev ptr)``.
+        One upload carries both device copies."""
+        from .inference import ImagePack
+        if not isinstance(pack, ImagePack) or pack.data.device != self.device or pack.data.dtype != torch.uint8 \
+                or not pack.data.is_contiguous():
+            raise ValueError('images must be an ImagePack of uint8 bytes on the renderer device')
+        n = len(pack)
+        start = self._mesh_start(counts, n)
+        table = np.array([[o, h, w] for o, (h, w) in zip(pack.offsets[:-1], pack.sizes)], np.int64).reshape(n, 3)
+        buf = np.zeros(3 * n + (n + 2) // 2, np.int64)
+        buf[:3 * n] = table.reshape(-1)
+        buf[3 * n:].view(np.int32)[:n + 1] = start
+        dev = torch.from_numpy(buf).to(self.device)
+        return table, start, dev, dev.data_ptr(), dev[3 * n:].data_ptr()
+
+    def plan_images(self, pack, vertices: torch.Tensor, counts):
+        """:meth:`plan_frames` for the images of an ImagePack (``syn_render_images_plan``): each mesh's box is clamped to
+        its own image.  ``counts[i]`` meshes belong to image i."""
+        return self._plan_images(pack, vertices, self._image_axis(pack, counts))
+
+    def _plan_images(self, pack, vertices, axis):
+        v, view = self._view(vertices)
+        m = view[4]
+        table, start, _keep, table_dev, start_dev = axis
+        boxes = torch.empty((m, 4), dtype=torch.int32, device=self.device)
+        key_off = torch.empty(m + 1, dtype=torch.int64, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.syn_render_images_plan(*view, self.tri.data_ptr(), self.ntri, start.ctypes.data, start_dev,
+                                                        table.ctypes.data, table_dev, len(pack), pack.data.numel(), 3,
+                                                        boxes.data_ptr(), key_off.data_ptr(), _stream_ptr(self.device)))
+        self.launches += 2
+        return boxes, key_off
+
+    def rasterize_images(self, pack, vertices: torch.Tensor, colors: torch.Tensor, counts, out=None):
+        """:meth:`rasterize_frames` for the images of an :class:`~synergynet_b200.inference.ImagePack`: image i's meshes
+        are the next ``counts[i]`` of ``vertices`` / ``colors`` (M,nver,3), drawn in order, each clamped to its own image.
+        Returns ``out``, an ImagePack of the same sizes (a new one if None; ``out=pack`` draws in place).  One host
+        synchronisation: the key count."""
+        from .inference import ImagePack
+        v, view = self._view(vertices)
+        m = view[4]
+        colors = colors.contiguous()
+        if colors.dim() != 3 or tuple(colors.shape[:2]) != (m, self.nver) or colors.dtype != torch.float32 or colors.device != self.device:
+            raise ValueError(f'colors must be float32 (M,nver,C) on the renderer device; got {tuple(colors.shape)}')
+        if not isinstance(pack, ImagePack):
+            raise ValueError('images must be an ImagePack')
+        if out is None:
+            out = ImagePack(torch.empty_like(pack.data), pack.sizes)
+        elif not isinstance(out, ImagePack) or out.sizes != pack.sizes or out.data.dtype != torch.uint8 \
+                or out.data.device != self.device or not out.data.is_contiguous():
+            raise ValueError('out must be an ImagePack of the sizes of the images, on the renderer device')
+        axis = self._image_axis(pack, counts)
+        table, start, _keep, table_dev, start_dev = axis
+        boxes, key_off = self._plan_images(pack, v, axis)
+        n_keys = int(key_off[m].item())                                   # the stage's one host synchronisation
+        keys = torch.empty(max(n_keys, 1), dtype=torch.int64, device=self.device)
+        self.last_key_count = n_keys
+        with torch.cuda.device(self.device):
+            _lib.check(self._lib.syn_rasterize_images(pack.data.data_ptr(), out.data.data_ptr(), pack.data.numel(), table.ctypes.data,
+                                                      table_dev, len(pack), 3, *view, self.tri.data_ptr(), self.ntri, colors.data_ptr(),
+                                                      int(colors.shape[2]), start.ctypes.data, start_dev, boxes.data_ptr(),
+                                                      key_off.data_ptr(), n_keys, keys.data_ptr(), keys.numel(), _stream_ptr(self.device)))
+        self.launches += 2
+        return out
+
+    def render_images(self, pack, vertices: torch.Tensor, counts, cfg: Optional[_lib.LightCfg] = None,
+                      texture: Optional[torch.Tensor] = None, alpha: float = 0.6):
+        """:meth:`render_frames` for the images of an ImagePack: ``(blended, solid)`` ImagePacks, image i's bytes those
+        of :func:`render` on that image alone with its ``counts[i]`` meshes."""
+        from .inference import ImagePack
+        if sum(int(c) for c in counts) == 0:
+            self._mesh_start(counts, len(pack))
+            solid = ImagePack(pack.data.clone(), pack.sizes)
+        else:
+            col = self.colors(vertices, self.normals(vertices), cfg, texture)
+            solid = self.rasterize_images(pack, vertices, col, counts)
+        return ImagePack(add_weighted(pack.data, solid.data, alpha), pack.sizes), solid
+
 
 def add_weighted(a: torch.Tensor, b: torch.Tensor, alpha: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``cv2.addWeighted(a, 1 - alpha, b, alpha, 0)`` of two uint8 CUDA tensors of one shape, byte for byte
@@ -358,6 +439,51 @@ def render_batch(frames, ver_lsts, tri, alpha: float = 0.6, wfps=None, tex=None,
     out = []
     for i in range(n):
         res, overlap = blended[i], solid[i]
+        if wfps is not None and wfps[i] is not None:
+            cv2.imwrite(wfps[i][:-4] + '_solid' + '.png', overlap)
+            cv2.imwrite(wfps[i], res)
+        out.append((res, overlap))
+    return out
+
+
+def render_images(images, ver_lsts, tri, alpha: float = 0.6, wfps=None, tex=None, cfg: Optional[dict] = None):
+    """:func:`render_batch` for N images of any sizes (a list of (h_i,w_i,3) uint8 arrays): entry i of the returned list is
+    the ``(blended, overlap)`` pair ``render(images[i], ver_lsts[i], tri, alpha, wfps[i], tex, cfg)`` returns, bit for
+    bit.  One upload of the packed images and of all meshes, one normals / lighting / rasterisation / blend launch
+    sequence for all of them, one download of each result pack.  An image without a mesh gets ``overlap = image`` and
+    ``blended = cv2.addWeighted(image, 1 - alpha, image, alpha, 0)``, as :func:`render_batch` gives a frame without one."""
+    import cv2
+    from .inference import RENDER_CFG, pack_images
+    images = [np.asarray(im) for im in images]
+    n = len(images)
+    if not n:
+        raise ValueError('no images: an image list needs at least one image')
+    if len(ver_lsts) != n or (wfps is not None and len(wfps) != n):
+        raise ValueError(f'{len(ver_lsts)} mesh lists and {"no" if wfps is None else len(wfps)} paths for {n} images')
+    for im in images:
+        if im.ndim != 3 or im.shape[2] != 3 or im.shape[0] < 1 or im.shape[1] < 1:
+            raise ValueError(f'every image must be (H,W,3) with H, W >= 1, got {tuple(im.shape)}')
+    counts = [len(v) for v in ver_lsts]
+    meshes = [np.asarray(v, dtype=np.float32) for vl in ver_lsts for v in vl]
+    if not torch.cuda.is_available():
+        raise RuntimeError('synergynet_b200.Sim3DR needs a CUDA device (H100, sm_90a); there is no CPU fallback')
+    dev = torch.device('cuda', torch.cuda.current_device())
+    pack = pack_images(images, dev)
+    if meshes:
+        ver = np.stack(meshes)                                                      # (M,3,N)
+        r = _renderer_for(tri, ver.shape[2])
+        v = torch.from_numpy(ver).to(r.device).transpose(1, 2)
+        texture = None if tex is None else torch.from_numpy(np.ascontiguousarray(tex, dtype=np.float32))
+        blended, solid = r.render_images(pack, v, counts, _light_cfg(**(cfg or RENDER_CFG)), texture, alpha)
+        blended, solid = blended.data, solid.data
+    else:
+        solid = pack.data
+        blended = add_weighted(pack.data, solid, alpha)
+    blended, solid = blended.cpu().numpy(), solid.cpu().numpy()
+    out = []
+    for i, (h, w) in enumerate(pack.sizes):
+        a, b = pack.offsets[i], pack.offsets[i + 1]
+        res, overlap = blended[a:b].reshape(h, w, 3), solid[a:b].reshape(h, w, 3)
         if wfps is not None and wfps[i] is not None:
             cv2.imwrite(wfps[i][:-4] + '_solid' + '.png', overlap)
             cv2.imwrite(wfps[i], res)

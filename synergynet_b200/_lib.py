@@ -107,6 +107,8 @@ SIGNATURES = {
     'syn_rasterize': (_I, [_F, _I, _I, _I, _F, _L, _I, _I, _I, _I, _F, _I, _F, C.c_float, _I, _F, _F, _P]),
     'syn_render_frames_plan': (_I, [_F, _L, _I, _I, _I, _I, _F, _I, _P, _I, _I, _I, _F, _F, _P]),
     'syn_rasterize_frames': (_I, [_F, _F, _I, _I, _I, _I, _F, _L, _I, _I, _I, _I, _F, _I, _F, _I, _P, _F, _F, _F, _L, _F, _L, _P]),
+    'syn_render_images_plan': (_I, [_F, _L, _I, _I, _I, _I, _F, _I, _P, _F, _P, _F, _I, _L, _I, _F, _F, _P]),
+    'syn_rasterize_images': (_I, [_F, _F, _L, _P, _F, _I, _I, _F, _L, _I, _I, _I, _I, _F, _I, _F, _I, _P, _F, _F, _F, _L, _F, _L, _P]),
     'syn_add_weighted_u8': (_I, [_F, _F, C.c_double, _F, _L, _P]),
     'syn_draw_lines': (_I, [_F, _L, _P, _F, _I, _P, _F, _F, _I, _I, _I, _P]),
     'syn_nms': (_I, [_F, _I, C.c_double, _I, _F, _F, _F, _P]),
@@ -167,6 +169,7 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_fb_debug_forward_until', 'syn_fb_forward_batch', 'syn_fb_debug_forward_batch_until',
                                              'syn_faceboxes_decode_batch', 'syn_nms_batch', 'syn_crop_resize_plan_frames_host',
                                              'syn_crop_resize_batch', 'syn_render_frames_plan', 'syn_rasterize_frames',
+                                             'syn_render_images_plan', 'syn_rasterize_images',
                                              'syn_add_weighted_u8', 'syn_fb_forward_images', 'syn_fb_debug_forward_images_until',
                                              'syn_faceboxes_decode_images', 'syn_crop_resize_images_plan_size',
                                              'syn_crop_resize_plan_images_host', 'syn_crop_resize_images', 'syn_draw_lines',

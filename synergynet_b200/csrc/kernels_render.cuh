@@ -17,7 +17,9 @@
 //   pass 0  mesh_box_kernel + mesh_box_scan_kernel   the boxes, and their areas' exclusive prefix sum (key offsets)
 //   pass 1  raster_depth_kernel                      unchanged, each key addressed inside its mesh's box
 //   pass 2  raster_resolve_frames_kernel             one thread per (frame, pixel) over that frame's meshes only
-// and the overlay blend of utils/render.py:45 (cv2.addWeighted) runs as add_weighted_u8_kernel.
+// and the overlay blend of utils/render.py:45 (cv2.addWeighted) runs as add_weighted_u8_kernel.  The image list
+// (syn_render_images_plan / syn_rasterize_images: images of different sizes packed back to back) runs the same three
+// passes in their IMAGES instantiations, each mesh clamped to its own image (ImageAxis).
 // Vertex normals are the sum of the incident face normals IN TRIANGLE ORDER (:189-199): a per-vertex incidence list,
 // ascending by construction (syn_mesh_incidence_host), replaces the scatter loop, so the float sums associate exactly
 // as the reference's do.  All arithmetic comes from render_math.h (no FMA contraction): normals and rasterisation are
@@ -143,16 +145,40 @@ __device__ __forceinline__ bool load_tri(const MeshView& m, int b, const int32_t
 
 constexpr int kRasterSmallBox = 64;     // bounding boxes up to this many pixels are walked by the owning thread
 
+// The image list of syn_rasterize_images: image f is (h, w, c) at byte table[3f] of the pack, table = (n, 3) int64
+// (offset, h, w), every offset a multiple of c; image f owns meshes [mesh_start[f], mesh_start[f+1]).  The frame-axis
+// kernels take it as their last argument and read it only in their IMAGES instantiation.
+struct ImageAxis {
+  const int32_t* mesh_start;
+  const long long* table;
+  int n;
+};
+
+// the image of mesh b (the last f with mesh_start[f] <= b: a non-empty one) and its size
+__device__ __forceinline__ int mesh_image(const ImageAxis& ax, int b, int& w, int& h) {
+  int lo = 0, hi = ax.n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(ax.mesh_start + mid) <= b) lo = mid; else hi = mid;
+  }
+  h = (int)__ldg(ax.table + 3 * lo + 1);
+  w = (int)__ldg(ax.table + 3 * lo + 2);
+  return lo;
+}
+
 // keys: zero = empty.  BOXED = false (syn_rasterize): the (B, h, w) canvas of every mesh; boxes / key_off are not read.
 // BOXED = true (the frame axis): mesh b keys only its pixel box boxes[b] = (x0, y0, x1, y1), in the box-many slots at
-// keys + key_off[b] (mesh_box_kernel / mesh_box_scan_kernel plan them).  The canvas instantiation is the one-image kernel
-// as it was before the frame axis existed, instruction for instruction.  One thread per (mesh, triangle).
-template <bool BOXED>
+// keys + key_off[b] (mesh_box_kernel / mesh_box_scan_kernel plan them).  IMAGES (with BOXED): w, h are not read; each
+// mesh clamps to the size of its own image of `ax`.  The canvas instantiation is the one-image kernel as it was before
+// the frame axis existed, instruction for instruction.  One thread per (mesh, triangle).
+template <bool BOXED, bool IMAGES = false>
 __global__ void raster_depth_kernel(MeshView m, const int32_t* __restrict__ tri, int ntri, int w, int h,
                                     unsigned long long* __restrict__ keys, const int4* __restrict__ boxes,
-                                    const long long* __restrict__ key_off) {
+                                    const long long* __restrict__ key_off, ImageAxis ax) {
+  static_assert(BOXED || !IMAGES, "the image list keys boxes");
   const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
   const int lane = threadIdx.x & 31;
+  if constexpr (IMAGES) mesh_image(ax, b, w, h);
   rmath::TriSetup t;
   const bool live = (i < ntri) && load_tri(m, b, tri, i, w, h, t);
   unsigned long long* kb = keys + (size_t)b * w * h;     // key of pixel (x, y): kb[y * ks + x]
@@ -236,8 +262,12 @@ __global__ void raster_resolve_kernel(MeshView m, const int32_t* __restrict__ tr
 // ---- the frame axis: meshes grouped by frame, keys in per-mesh boxes ---------------------------------------------------------
 // Pass 0a: acc (M,4) int32, set to 0x7F7F7F7F bytes by the caller, receives min x0, min y0, min -x1, min -y1 over the
 // triangles load_tri draws (the same skips: bad indices, boxes empty after clamping).  One thread per (mesh, triangle).
-__global__ void mesh_box_kernel(MeshView m, const int32_t* __restrict__ tri, int ntri, int w, int h, int* __restrict__ acc) {
+// IMAGES: w, h are not read; each mesh clamps to its own image of `ax`.
+template <bool IMAGES = false>
+__global__ void mesh_box_kernel(MeshView m, const int32_t* __restrict__ tri, int ntri, int w, int h, int* __restrict__ acc,
+                                ImageAxis ax) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+  if constexpr (IMAGES) mesh_image(ax, b, w, h);
   rmath::TriSetup t;
   const bool live = (i < ntri) && load_tri(m, b, tri, i, w, h, t);
   const int big = 0x7F7F7F7F;
@@ -288,10 +318,41 @@ __global__ void __launch_bounds__(kBoxScanThreads) mesh_box_scan_kernel(int nmes
 // mesh_start[f+1]) are walked last to first; the first whose box holds the pixel and whose key there is set is drawn (alpha
 // = 1, so it overwrites whatever the earlier meshes drew), as raster_resolve_kernel draws a one-image batch.  src and dst
 // are (N, h, w, c) stacks and may be the same buffer; an undrawn pixel is copied.
+// IMAGES: the images of `ax` instead, w, h not read.  One thread per pixel slot of the pack (byte q * c, from the first
+// image's offset to the last image's end, 1-D grid); the slot's image is found by a binary search over the image
+// offsets, as fb_frame_of finds a detector pixel's frame.  A slot between two images (a gap in the table) writes nothing.
+template <bool IMAGES = false>
 __global__ void raster_resolve_frames_kernel(MeshView m, const int32_t* __restrict__ tri, const float* __restrict__ colors, int c,
                                              int w, int h, const int32_t* __restrict__ mesh_start, const int4* __restrict__ boxes,
                                              const long long* __restrict__ key_off, const unsigned long long* __restrict__ keys,
-                                             const unsigned char* src, unsigned char* dst) {
+                                             const unsigned char* src, unsigned char* dst, ImageAxis ax) {
+  if constexpr (IMAGES) {
+    const long long at = __ldg(ax.table) + ((long long)blockIdx.x * blockDim.x + threadIdx.x) * c;    // the slot's first byte
+    int lo = 0, hi = ax.n;
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (__ldg(ax.table + 3 * mid) <= at) lo = mid; else hi = mid;
+    }
+    const long long image = __ldg(ax.table + 3 * lo);
+    const int ih = (int)__ldg(ax.table + 3 * lo + 1), iw = (int)__ldg(ax.table + 3 * lo + 2);
+    const long long p = (at - image) / c;
+    if (p >= (long long)ih * iw) return;
+    const int y = (int)(p / iw), x = (int)(p - (long long)y * iw);
+    const int b0 = __ldg(ax.mesh_start + lo);
+    for (int b = __ldg(ax.mesh_start + lo + 1) - 1; b >= b0; --b) {
+      const int4 q = boxes[b];
+      if (x < q.x || x > q.z || y < q.y || y > q.w) continue;
+      rmath::PixBox box;
+      box.x0 = q.x; box.y0 = q.y; box.x1 = q.z; box.y1 = q.w;
+      const unsigned long long key = keys[key_off[b] + rmath::pix_box_slot(box, x, y)];
+      if (key == 0ull) continue;
+      shade_pixel(m, b, tri, colors, c, iw, x, y, y, key, 1.0f, src + image, dst + image);
+      return;
+    }
+    if (src != dst)
+      for (int k = 0; k < c; ++k) dst[at + k] = src[at + k];
+    return;
+  }
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y, f = blockIdx.z;
   if (x >= w || y >= h) return;
   const size_t pix = (((size_t)f * h + y) * w + x) * c;

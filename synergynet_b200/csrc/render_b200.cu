@@ -27,20 +27,48 @@ int check_mesh(const float* v, long long sb, int sv, int sc, int batch, int nver
 // the shared checks of the frame-axis entries: the mesh view, the frame size and mesh_start_host (n_frames + 1 entries,
 // 0 = mesh_start[0] <= ... <= mesh_start[n_frames] = n_meshes); meshes and frames each sit on one grid axis
 int check_frames(const float* v, long long sb, int sv, int sc, int n_meshes, int nver, const int32_t* mesh_start_host, int n_frames,
-                 int height, int width, MeshView& m, const char* who) {
+                 int height, int width, MeshView& m, const char* who, const char* unit = "frame") {
   if (!v || !mesh_start_host || n_meshes <= 0 || nver <= 0 || sv <= 0 || sc <= 0 || (n_meshes > 1 && sb <= 0))
     return fail(SYN_ERR_INVALID, "%s: null pointer, no mesh or non-positive stride", who);
   if (n_frames <= 0 || n_frames > 65535 || n_meshes > 65535)
-    return fail(SYN_ERR_INVALID, "%s: %d frames and %d meshes (1..65535 of each per call)", who, n_frames, n_meshes);
+    return fail(SYN_ERR_INVALID, "%s: %d %ss and %d meshes (1..65535 of each per call)", who, n_frames, unit, n_meshes);
   if (height <= 0 || width <= 0) return fail(SYN_ERR_INVALID, "%s: frame size %dx%d", who, height, width);
   if (mesh_start_host[0] != 0 || mesh_start_host[n_frames] != n_meshes)
     return fail(SYN_ERR_SHAPE, "%s: mesh_start runs from %d to %d, must run from 0 to %d meshes", who, mesh_start_host[0],
                 mesh_start_host[n_frames], n_meshes);
   for (int f = 0; f < n_frames; ++f)
     if (mesh_start_host[f + 1] < mesh_start_host[f])
-      return fail(SYN_ERR_SHAPE, "%s: mesh_start is not monotone at frame %d (%d after %d)", who, f, mesh_start_host[f + 1],
+      return fail(SYN_ERR_SHAPE, "%s: mesh_start is not monotone at %s %d (%d after %d)", who, unit, f, mesh_start_host[f + 1],
                   mesh_start_host[f]);
   return check_mesh(v, sb, sv, sc, n_meshes, nver, m);
+}
+
+// the shared checks of the image-list entries: check_frames, then the image table (n_images,3) int64 (offset, h, w) --
+// the images in memory order, disjoint, inside the image bytes, each offset a multiple of the channel count -- and the
+// device copies.  Fills the kernels' ImageAxis.
+int check_images(const float* v, long long sb, int sv, int sc, int n_meshes, int nver, const int32_t* mesh_start_host,
+                 const int32_t* mesh_start_dev, const int64_t* table_host, const int64_t* table_dev, int n_images, int64_t image_bytes,
+                 int channels, MeshView& m, ImageAxis& ax, const char* who) {
+  if (!table_host || !table_dev || !mesh_start_dev) return fail(SYN_ERR_INVALID, "%s: null pointer", who);
+  if (int rc = check_frames(v, sb, sv, sc, n_meshes, nver, mesh_start_host, n_images, 1, 1, m, who, "image")) return rc;
+  if (channels <= 0 || image_bytes < 0)
+    return fail(SYN_ERR_SHAPE, "%s: %d image channels, %lld image bytes", who, channels, (long long)image_bytes);
+  int64_t end = 0;
+  for (int f = 0; f < n_images; ++f) {
+    const int64_t off = table_host[3 * f], h = table_host[3 * f + 1], w = table_host[3 * f + 2];
+    if (h < 1 || w < 1 || h > INT32_MAX || w > INT32_MAX)
+      return fail(SYN_ERR_SHAPE, "%s: image %d is %lldx%lld", who, f, (long long)h, (long long)w);
+    if (off < end || off > image_bytes || h > (image_bytes - off) / channels / w)
+      return fail(SYN_ERR_SHAPE, "%s: image %d (%lldx%lld at byte %lld) does not fit the %lld image bytes after the image before it",
+                  who, f, (long long)h, (long long)w, (long long)off, (long long)image_bytes);
+    if (off % channels)
+      return fail(SYN_ERR_SHAPE, "%s: image %d starts at byte %lld, not a multiple of its %d channels", who, f, (long long)off, channels);
+    end = off + channels * h * w;
+  }
+  ax.mesh_start = mesh_start_dev;
+  ax.table = reinterpret_cast<const long long*>(table_dev);
+  ax.n = n_images;
+  return SYN_OK;
 }
 
 // the host planner of both crop entries; frames_host == nullptr: one image
@@ -179,7 +207,7 @@ int syn_rasterize(uint8_t* image_dev, int height, int width, int channels, const
   if (ntri > 0) {
     raster_depth_kernel<false><<<dim3((ntri + 255) / 256, batch), 256, 0, st>>>(m, tri_dev, ntri, width, height,
                                                                          reinterpret_cast<unsigned long long*>(keys_ws_dev), nullptr,
-                                                                         nullptr);
+                                                                         nullptr, ImageAxis{});
     SYN_LAUNCH_CHECK("raster_depth_kernel");
   }
   raster_resolve_kernel<<<dim3((width + 31) / 32, (height + 7) / 8), dim3(32, 8), 0, st>>>(
@@ -201,7 +229,7 @@ int syn_render_frames_plan(const float* vertices_dev, int64_t stride_mesh, int s
   cudaStream_t st = (cudaStream_t)stream;
   SYN_CUDA(cudaMemsetAsync(boxes_dev, 0x7F, sizeof(int32_t) * 4 * (size_t)n_meshes, st));
   if (ntri > 0) {
-    mesh_box_kernel<<<dim3((ntri + 255) / 256, n_meshes), 256, 0, st>>>(m, tri_dev, ntri, width, height, boxes_dev);
+    mesh_box_kernel<false><<<dim3((ntri + 255) / 256, n_meshes), 256, 0, st>>>(m, tri_dev, ntri, width, height, boxes_dev, ImageAxis{});
     SYN_LAUNCH_CHECK("mesh_box_kernel");
   }
   mesh_box_scan_kernel<<<1, kBoxScanThreads, 0, st>>>(n_meshes, boxes_dev, reinterpret_cast<long long*>(key_off_dev));
@@ -232,12 +260,74 @@ int syn_rasterize_frames(const uint8_t* frames_dev, uint8_t* solid_dev, int n_fr
   if (n_keys > 0) {
     SYN_CUDA(cudaMemsetAsync(keys_ws_dev, 0, sizeof(uint64_t) * (size_t)n_keys, st));
     if (ntri > 0) {
-      raster_depth_kernel<true><<<dim3((ntri + 255) / 256, n_meshes), 256, 0, st>>>(m, tri_dev, ntri, width, height, keys, boxes, off);
+      raster_depth_kernel<true><<<dim3((ntri + 255) / 256, n_meshes), 256, 0, st>>>(m, tri_dev, ntri, width, height, keys, boxes, off,
+                                                                                    ImageAxis{});
       SYN_LAUNCH_CHECK("raster_depth_kernel");
     }
   }
-  raster_resolve_frames_kernel<<<dim3((width + 31) / 32, (height + 7) / 8, n_frames), dim3(32, 8), 0, st>>>(
-      m, tri_dev, colors_dev, channels, width, height, mesh_start_dev, boxes, off, keys, frames_dev, solid_dev);
+  raster_resolve_frames_kernel<false><<<dim3((width + 31) / 32, (height + 7) / 8, n_frames), dim3(32, 8), 0, st>>>(
+      m, tri_dev, colors_dev, channels, width, height, mesh_start_dev, boxes, off, keys, frames_dev, solid_dev, ImageAxis{});
+  SYN_LAUNCH_CHECK("raster_resolve_frames_kernel");
+  return SYN_OK;
+}
+
+int syn_render_images_plan(const float* vertices_dev, int64_t stride_mesh, int stride_vertex, int stride_coord, int n_meshes, int nver,
+                           const int32_t* tri_dev, int ntri, const int32_t* mesh_start_host, const int32_t* mesh_start_dev,
+                           const int64_t* images_host, const int64_t* images_dev, int n_images, int64_t image_bytes, int channels,
+                           int32_t* boxes_dev, int64_t* key_off_dev, void* stream) {
+  const char* who = "syn_render_images_plan";
+  MeshView m;
+  ImageAxis ax;
+  if (int rc = check_images(vertices_dev, stride_mesh, stride_vertex, stride_coord, n_meshes, nver, mesh_start_host, mesh_start_dev,
+                            images_host, images_dev, n_images, image_bytes, channels, m, ax, who))
+    return rc;
+  if (!tri_dev || ntri < 0 || !boxes_dev || !key_off_dev) return fail(SYN_ERR_INVALID, "%s: null pointer or negative triangle count", who);
+  cudaStream_t st = (cudaStream_t)stream;
+  SYN_CUDA(cudaMemsetAsync(boxes_dev, 0x7F, sizeof(int32_t) * 4 * (size_t)n_meshes, st));
+  if (ntri > 0) {
+    mesh_box_kernel<true><<<dim3((ntri + 255) / 256, n_meshes), 256, 0, st>>>(m, tri_dev, ntri, 0, 0, boxes_dev, ax);
+    SYN_LAUNCH_CHECK("mesh_box_kernel");
+  }
+  mesh_box_scan_kernel<<<1, kBoxScanThreads, 0, st>>>(n_meshes, boxes_dev, reinterpret_cast<long long*>(key_off_dev));
+  SYN_LAUNCH_CHECK("mesh_box_scan_kernel");
+  return SYN_OK;
+}
+
+int syn_rasterize_images(const uint8_t* images_dev, uint8_t* solid_dev, int64_t image_bytes, const int64_t* table_host,
+                         const int64_t* table_dev, int n_images, int channels, const float* vertices_dev, int64_t stride_mesh,
+                         int stride_vertex, int stride_coord, int n_meshes, int nver, const int32_t* tri_dev, int ntri,
+                         const float* colors_dev, int color_channels, const int32_t* mesh_start_host, const int32_t* mesh_start_dev,
+                         const int32_t* boxes_dev, const int64_t* key_off_dev, int64_t n_keys, uint64_t* keys_ws_dev,
+                         int64_t keys_ws_count, void* stream) {
+  const char* who = "syn_rasterize_images";
+  MeshView m;
+  ImageAxis ax;
+  if (int rc = check_images(vertices_dev, stride_mesh, stride_vertex, stride_coord, n_meshes, nver, mesh_start_host, mesh_start_dev,
+                            table_host, table_dev, n_images, image_bytes, channels, m, ax, who))
+    return rc;
+  if (!images_dev || !solid_dev || !tri_dev || !colors_dev || !boxes_dev || !key_off_dev || !keys_ws_dev || ntri < 0)
+    return fail(SYN_ERR_INVALID, "%s: null pointer or negative triangle count", who);
+  if (channels != color_channels)
+    return fail(SYN_ERR_SHAPE, "%s: %d image channels, colours of %d channels", who, channels, color_channels);
+  if (n_keys < 0 || keys_ws_count < n_keys)
+    return fail(SYN_ERR_SHAPE, "%s: key workspace of %lld slots, the plan needs %lld", who, (long long)keys_ws_count, (long long)n_keys);
+  // pixel slots from the first image's first byte to the last image's end
+  const int64_t first = table_host[0], last = table_host[3 * (n_images - 1)];
+  const int64_t slots = (last - first) / channels + table_host[3 * (n_images - 1) + 1] * table_host[3 * (n_images - 1) + 2];
+  if ((slots + 255) / 256 > INT32_MAX) return fail(SYN_ERR_SHAPE, "%s: %lld pixel slots exceed one launch's grid", who, (long long)slots);
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(keys_ws_dev);
+  const int4* boxes = reinterpret_cast<const int4*>(boxes_dev);
+  const long long* off = reinterpret_cast<const long long*>(key_off_dev);
+  if (n_keys > 0) {
+    SYN_CUDA(cudaMemsetAsync(keys_ws_dev, 0, sizeof(uint64_t) * (size_t)n_keys, st));
+    if (ntri > 0) {
+      raster_depth_kernel<true, true><<<dim3((ntri + 255) / 256, n_meshes), 256, 0, st>>>(m, tri_dev, ntri, 0, 0, keys, boxes, off, ax);
+      SYN_LAUNCH_CHECK("raster_depth_kernel");
+    }
+  }
+  raster_resolve_frames_kernel<true><<<(unsigned)((slots + 255) / 256), 256, 0, st>>>(m, tri_dev, colors_dev, channels, 0, 0, mesh_start_dev,
+                                                                                     boxes, off, keys, images_dev, solid_dev, ax);
   SYN_LAUNCH_CHECK("raster_resolve_frames_kernel");
   return SYN_OK;
 }

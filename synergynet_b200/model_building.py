@@ -463,26 +463,60 @@ class _SynergyBase(nn.Module):
         ``dense_chunk_bytes`` onto the same canvases (a chunk may end inside a frame), then every frame is blended once.
         ``connectivity`` (3,ntri) 0-based replaces the model's ``triangles`` as in ``render.render``."""
         from . import Sim3DR
-        from .inference import RENDER_CFG
         eng, stack, counts, frame_index, params, roi5 = self._frames_front(frames, rects)
         solid = stack.clone()
-        if frame_index:
-            tri = np.asarray(connectivity).T if connectivity is not None else self.triangles.T.cpu().numpy()
-            with torch.cuda.device(stack.device):
-                r = Sim3DR._renderer_for(np.ascontiguousarray(tri, dtype=np.int32), eng.n_vert)
-            cfg = Sim3DR._light_cfg(**RENDER_CFG)
-            texture = None if tex is None else torch.from_numpy(np.ascontiguousarray(tex, dtype=np.float32))
-            fi = np.asarray(frame_index)
-            for a, b in self._dense_chunks(eng, len(frame_index)):
-                v = eng.reconstruct_image(params[a:b], roi5[a:b], dense=True).transpose(1, 2)
-                f0, f1 = int(fi[a]), int(fi[b - 1]) + 1                   # the frames this chunk draws on, in place
-                col = r.colors(v, r.normals(v), cfg, texture)
-                r.rasterize_frames(solid[f0:f1], v, col, np.bincount(fi[a:b] - f0, minlength=f1 - f0), out=solid[f0:f1])
-            eng.raise_if_error()
+        for r, v, col, f0, f1, chunk_counts in self._overlay_chunks(eng, stack.device, frame_index, params, roi5, tex, connectivity):
+            r.rasterize_frames(solid[f0:f1], v, col, chunk_counts, out=solid[f0:f1])
         blended = Sim3DR.add_weighted(stack, solid, alpha)
         if isinstance(frames, torch.Tensor) and frames.is_cuda:
             return blended, solid
         return blended.cpu().numpy(), solid.cpu().numpy()
+
+    def overlay_images(self, images, rects: Optional[Sequence[Sequence[Sequence[float]]]] = None, alpha: float = 0.6, tex=None,
+                       connectivity=None):
+        """:meth:`overlay_batch` for N BGR uint8 images of any sizes: ``(blended, solid)``, two lists of N (h_i,w_i,3)
+        images, numpy arrays -- or CUDA views when every input image is a CUDA tensor.  Image i's bytes are those of
+        ``Sim3DR.render(images[i], meshes_i, tri, alpha, tex=tex)`` with the dense meshes ``get_all_outputs`` returns
+        for it (an image without a face: ``solid = image``, ``blended = cv2.addWeighted(image, 1 - alpha, image, alpha,
+        0)``).
+
+        The images are uploaded once, packed back to back (and detected on the device by ``detect_images`` when
+        ``rects`` is None).  The dense meshes are reconstructed, lit and drawn in chunks of faces above
+        ``dense_chunk_bytes`` onto the packed canvases, each chunk in place on the images it touches (a chunk may end
+        inside an image); then the whole pack is blended once."""
+        from . import Sim3DR
+        eng, pack, counts, frame_index, params, roi5 = self._frames_front(images, rects, ragged=True)
+        solid = ImagePack(pack.data.clone(), pack.sizes)
+        for r, v, col, f0, f1, chunk_counts in self._overlay_chunks(eng, pack.data.device, frame_index, params, roi5, tex, connectivity):
+            part = solid.slice(f0, f1)
+            r.rasterize_images(part, v, col, chunk_counts, out=part)
+        blended = ImagePack(Sim3DR.add_weighted(pack.data, solid.data, alpha), pack.sizes)
+        if all(isinstance(im, torch.Tensor) and im.is_cuda for im in images):
+            return [blended.image(i) for i in range(len(pack))], [solid.image(i) for i in range(len(pack))]
+        hb, hs = blended.data.cpu().numpy(), solid.data.cpu().numpy()
+        split = lambda host: [host[pack.offsets[i]:pack.offsets[i + 1]].reshape(h, w, 3) for i, (h, w) in enumerate(pack.sizes)]
+        return split(hb), split(hs)
+
+    def _overlay_chunks(self, eng, device, frame_index, params, roi5, tex, connectivity):
+        """The dense meshes of the overlay, chunk by chunk of ``dense_chunk_bytes``: yields ``(renderer, vertices (F,nver,3)
+        view, colours, f0, f1, meshes per frame f0..f1-1)`` for the frames f0..f1-1 the chunk draws on.  Raises the
+        engine's error flag after the last chunk."""
+        from . import Sim3DR
+        from .inference import RENDER_CFG
+        if not frame_index:
+            return
+        tri = np.asarray(connectivity).T if connectivity is not None else self.triangles.T.cpu().numpy()
+        with torch.cuda.device(device):
+            r = Sim3DR._renderer_for(np.ascontiguousarray(tri, dtype=np.int32), eng.n_vert)
+        cfg = Sim3DR._light_cfg(**RENDER_CFG)
+        texture = None if tex is None else torch.from_numpy(np.ascontiguousarray(tex, dtype=np.float32))
+        fi = np.asarray(frame_index)
+        for a, b in self._dense_chunks(eng, len(frame_index)):
+            v = eng.reconstruct_image(params[a:b], roi5[a:b], dense=True).transpose(1, 2)
+            f0, f1 = int(fi[a]), int(fi[b - 1]) + 1                   # the frames this chunk draws on, in place
+            col = r.colors(v, r.normals(v), cfg, texture)
+            yield r, v, col, f0, f1, np.bincount(fi[a:b] - f0, minlength=f1 - f0)
+        eng.raise_if_error()
 
     def pose_overlay_batch(self, frames, rects: Optional[Sequence[Sequence[Sequence[float]]]] = None):
         """The pose image of singleImage.py:112-118 for N equally sized BGR uint8 frames in one pass: every face's axes

@@ -43,3 +43,13 @@ def render_batch(imgs, ver_lsts, alpha=0.6, wfps=None, tex=None, connectivity=No
         if wfp is not None:
             print(f'Save mesh result to {wfp}')
     return [res for res, _overlap in out]
+
+
+def render_images(imgs, ver_lsts, alpha=0.6, wfps=None, tex=None, connectivity=None):
+    """:func:`render` for N images of any sizes in one pass (:func:`synergynet_b200.Sim3DR.render_images`): returns the
+    list of blended images, entry i being ``render(imgs[i], ver_lsts[i], alpha, wfps[i], tex, connectivity)``."""
+    out = Sim3DR.render_images(imgs, ver_lsts, _triangles(connectivity), alpha=alpha, wfps=wfps, tex=tex, cfg=cfg)
+    for wfp in wfps or []:
+        if wfp is not None:
+            print(f'Save mesh result to {wfp}')
+    return [res for res, _overlap in out]
