@@ -557,8 +557,11 @@ int syn_peek_error(const syn_handle_t* h, int* flag_out);
  * an input with |x| > 937.5, +-Inf or NaN is changed (NaN is read as -937.5).  The flag is raised
  * wherever that happens: the fused block kernel's input (the fp32 crop at the stem and the inputs of
  * blocks 2-17; engines 2, 3), the tail kernel's input (the block-17 output; engines 2, 3) and the input
- * of every expand conv and of conv 51 on the unfused tensor-core engine (engine 1).  The fp32 engine
- * (SYN_ENGINE_SIMT_FP32) has no such limit.  *flag_out != 0: results of engines 1-3 are suspect. */
+ * of every expand conv and of conv 51 on the unfused tensor-core engine (engine 1).  The GEMM layers
+ * (ResNets, MobileNetV1, PointNet heads) scale every finite input into range and raise it for a +-Inf
+ * or NaN input value (or a value about twice the row maximum they were given or more); the dense reconstruction raises it for a +-Inf or NaN coefficient.  The fp32
+ * engine (SYN_ENGINE_SIMT_FP32) has no such limit.  *flag_out != 0: results of engines 1-3 (or of the
+ * GEMM layers and the dense mesh) are suspect. */
 int syn_poll_saturation(syn_handle_t* h, int* flag_out);
 /* Run the backbone on x_dev but stop after convolution `layer` (0..51) and copy its NHWC
  * activation (batch*h_out*h_out*cout floats, residual already added for project convs) to

@@ -16,14 +16,27 @@ BN_EPS = 1e-5
 Pair = Tuple[torch.Tensor, torch.Tensor]          # (value, error scale S), both float64
 
 
+ABS_ALLOW = 2.0 ** -149        # one fp32 subnormal spacing: what an fp32 result cannot resolve at any scale
+F32_OVERFLOW = 2.0 ** 128 - 2.0 ** 103   # round to nearest takes every |x| from here up to +-Inf
+
+
 def ratio(got, want, s):
-    """|got - want| / S per element (0 where they are equal, inf where S = 0 and they differ), as torch tensors, or as
+    """(|got - want| - 2^-149)+ / S per element, so that ratio <= tau means |got - want| <= tau * S + 2^-149 (0 where
+    they are that close, inf where S = 0 and they differ by more).  An infinite ``got`` with the sign of ``want`` is as
+    far from it as ``want`` is from the fp32 overflow threshold: Inf passes exactly where |want| >= F32_OVERFLOW - tau * S
+    (and a finite ``got`` fails wherever |want| - tau * S is past it by more than FLT_MAX).  As torch tensors, or as
     numpy arrays when ``want`` is one."""
     if isinstance(want, np.ndarray):
-        d = np.abs(np.asarray(got, np.float64) - want)
+        g = np.asarray(got, np.float64)
         with np.errstate(divide='ignore', invalid='ignore'):
+            d = np.abs(g - want)
+            inf_ok = np.isinf(g) & (np.sign(g) == np.sign(want))
+            d = np.where(inf_ok, np.maximum(F32_OVERFLOW - np.abs(want), 0.0), np.maximum(d - ABS_ALLOW, 0.0))
             return np.where(d == 0, 0.0, d / s)
-    d = (got.double() - want).abs()
+    g = got.double()
+    d = (g - want).abs()
+    inf_ok = torch.isinf(g) & (torch.sign(g) == torch.sign(want))
+    d = torch.where(inf_ok, (F32_OVERFLOW - want.abs()).clamp_min(0.0), (d - ABS_ALLOW).clamp_min(0.0))
     return torch.where(d == 0, torch.zeros_like(d), d / s)
 
 

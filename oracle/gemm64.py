@@ -48,20 +48,21 @@ FACE_VEC_LD = 2360                      # kFaceVecLd (csrc/heads_host.inl): 1024
 # ---- floors and the two forms of S ----------------------------------------------------------------------------------
 
 def _floor_exp(m: torch.Tensor) -> torch.Tensor:
-    """floor(log2 m) of fp32 magnitudes m > 0 (the biased exponent the kernel reads)."""
-    _, e = torch.frexp(m.float())                        # m = f * 2^e, f in [0.5, 1)
+    """floor(log2 m) of magnitudes m > 0, exact for every finite fp32 value, subnormals included (frexp in float64)."""
+    _, e = torch.frexp(m.double())                       # m = f * 2^e, f in [0.5, 1)
     return (e - 1).double()
 
 
 def row_floor(rowmax: torch.Tensor) -> torch.Tensor:
     """eps_row per row from the true max |a| of the row."""
-    return torch.where(rowmax > 0, torch.exp2(_floor_exp(rowmax.clamp_min(1e-38)) - 15), torch.zeros_like(rowmax.double()))
+    rm = rowmax.double()
+    return torch.where(rm > 0, torch.exp2(_floor_exp(rm) - 15), torch.zeros_like(rm))
 
 
 def chan_floor(w: torch.Tensor) -> torch.Tensor:
     """eps_n per output channel of an (N, K) weight, from its fp32 values (what the library packs)."""
-    m = w.float().abs().amax(dim=1)
-    return torch.where(m > 0, torch.exp2(_floor_exp(m.clamp_min(1e-38)) - 10), torch.zeros_like(m.double()))
+    m = w.float().abs().amax(dim=1).double()
+    return torch.where(m > 0, torch.exp2(_floor_exp(m) - 10), torch.zeros_like(m))
 
 
 def gemm(a: torch.Tensor, w: torch.Tensor, b: Optional[torch.Tensor], relu: bool, addend: Optional[torch.Tensor] = None,

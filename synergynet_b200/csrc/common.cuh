@@ -1,6 +1,7 @@
 // Shared helpers for the sm_90a SynergyNet hot-path library.
 #pragma once
 #include <cuda_runtime.h>
+#include <float.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>

@@ -47,7 +47,8 @@ constexpr int kDnAlphaThreads = kDnFaces * (kDnK / 8);
 __global__ void __launch_bounds__(kDnAlphaThreads) dense_alpha_kernel(const float* __restrict__ params, const float* __restrict__ mean,
                                                                       const float* __restrict__ stdv, const float* __restrict__ ascale,
                                                                       uint8_t* __restrict__ aimg, float* __restrict__ pose, int batch,
-                                                                      int whitening, const float* __restrict__ roi5) {
+                                                                      int whitening, const float* __restrict__ roi5,
+                                                                      int* __restrict__ sat) {
   // the reconstruction kernel may start its prologue (barriers, basis planes) now; it waits for this grid
   // (griddepcontrol.wait) before it touches the alpha image or the pose rows
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -63,12 +64,15 @@ __global__ void __launch_bounds__(kDnAlphaThreads) dense_alpha_kernel(const floa
     return v;
   };
   float a[8], amax = 0.f;
+  bool nonfinite = false;                                    // NaN / +-Inf: the split clamps it (fmaxf drops a NaN)
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const int k = kg * 8 + j;
     a[j] = (k < kNumAlpha) ? param(12 + k) * ascale[k] : 0.f;
     amax = fmaxf(amax, fabsf(a[j]));
+    nonfinite = nonfinite || !(fabsf(a[j]) <= FLT_MAX);
   }
+  if (nonfinite) *sat = 1;                                   // sticky, cleared by syn_poll_saturation
   // Face scale: ascale bounds |alpha_k * ascale_k| by 2^10 within 8 sigma of the mean, but a face further out (or raw
   // coefficients with whitening off) would hit split2_f16's clamp at 60000.  Such a face is divided by a power of two
   // fs that brings its largest scaled coefficient into [2^14, 2^15); the epilogues multiply the accumulator by fs

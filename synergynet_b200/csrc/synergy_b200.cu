@@ -389,7 +389,7 @@ int run_reconstruct_tc(syn_handle* h, const float* params, int batch, int dense,
   const int n_ftiles = (batch + kDnFaces - 1) / kDnFaces;
   if (int rc = ensure_recon_tiles(h, batch, st)) return rc;
   dense_alpha_kernel<<<n_ftiles, kDnAlphaThreads, 0, st>>>(params, h->d_mean, h->d_std, h->d_ascale, h->d_alpha_img, h->d_pose, batch,
-                                             whitening, roi5);
+                                             whitening, roi5, h->d_sat);
   SYN_LAUNCH_CHECK("dense_alpha_kernel");
   mark(h, st, "dense_alpha_kernel");
   DenseArgs a;
@@ -469,14 +469,22 @@ inline void split_f16_host(float x, uint16_t& hi, uint16_t& lo) {
   hi = __half_as_ushort(h);
   lo = __half_as_ushort(l);
 }
-// power-of-two scale that brings max|w| of one output channel into [256, 512) (tc_common.cuh)
-inline float channel_scale(const float* w, size_t stride, int count) {
+// exponent f of the power-of-two scale 2^f that brings max|w| of one output channel into [256, 512) (tc_common.cuh):
+// f in [-119, 157] for every finite max > 0, subnormal included; 0 for an all-zero or non-finite channel
+inline int channel_exp(const float* w, size_t stride, int count) {
   float m = 0.f;
   for (int i = 0; i < count; ++i) m = std::max(m, fabsf(w[(size_t)i * stride]));
-  if (!(m > 0.f) || !std::isfinite(m)) return 1.f;
+  if (!(m > 0.f) || !std::isfinite(m)) return 0;
   int ex;
   frexpf(m, &ex);                       // m = f * 2^ex, f in [0.5, 1)
-  return ldexpf(1.f, 9 - ex);
+  return 9 - ex;
+}
+// the same scale as a float for the fixed-scale packers, capped at 2^117 so that it stays finite and every epilogue
+// factor the packers derive from it stays a normal fp32 number (1 / (64 scale) >= 2^-123, and the fused expand's
+// 1 / (6 * 64 * scale) > 2^-126), as precise as in range.  A channel whose max is below 2^-108 then packs below
+// [256, 512): finite, with fewer bits.
+inline float channel_scale(const float* w, size_t stride, int count) {
+  return ldexpf(1.f, std::min(channel_exp(w, stride, count), 117));
 }
 constexpr float kActScaleHost = 64.0f;   // == tc::kActScale
 
@@ -645,10 +653,11 @@ void pack_basis(std::vector<float>& dst, const float* u, const float* ws, const 
     }
 }
 
-int upload(float** dptr, const std::vector<float>& src) {
+template <class T>
+int upload(T** dptr, const std::vector<T>& src) {
   if (*dptr != nullptr) { cudaFree(*dptr); *dptr = nullptr; }
-  SYN_CUDA(cudaMalloc(dptr, src.size() * sizeof(float)));
-  SYN_CUDA(cudaMemcpy(*dptr, src.data(), src.size() * sizeof(float), cudaMemcpyHostToDevice));
+  SYN_CUDA(cudaMalloc(dptr, src.size() * sizeof(T)));
+  SYN_CUDA(cudaMemcpy(*dptr, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice));
   return SYN_OK;
 }
 

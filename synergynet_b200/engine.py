@@ -201,7 +201,9 @@ class Engine:
         """Device sync + sticky "an activation was clamped to the fp16 range" flag of the split-fp16 engines, then
         clear it.  Raised when |x| > 937.5, +-Inf or NaN reaches a clamp: the fused kernel's input (fp32 crop and
         block inputs, engines 2 and 3), the tail kernel's input (engines 2 and 3) or an expand / conv 51 input (engine
-        1).  Non-zero: use ``set_engine(0)`` (fp32) for this checkpoint, or check the input for Inf / NaN."""
+        1); and when +-Inf or NaN reaches the input of a GEMM layer (ResNets, MobileNetV1, PointNet heads) or a 3DMM
+        coefficient of the dense reconstruction.  Non-zero: use ``set_engine(0)`` (fp32) for this checkpoint, or check
+        the input for Inf / NaN."""
         fn = getattr(self._lib, 'syn_poll_saturation', None)
         if fn is None:
             return 0

@@ -143,6 +143,30 @@ def test_floors_match_the_kernel_scales():
                                                           dtype=torch.float64))
     w = torch.tensor([[0.5, -1.0], [0.0, 0.0], [300.0, 1.0]])
     assert torch.equal(gemm64.chan_floor(w), torch.tensor([2.0 ** -10, 0.0, 2.0 ** -2], dtype=torch.float64))
+    # the floors are exact over the whole fp32 range, subnormal maxima included
+    rm = torch.tensor([2.0 ** -149, 3.0 * 2.0 ** -140, 2.0 ** -126, 1.5 * 2.0 ** 127])
+    assert torch.equal(gemm64.row_floor(rm), torch.exp2(torch.tensor([-164.0, -154.0, -141.0, 112.0], dtype=torch.float64)))
+    w = torch.tensor([[2.0 ** -149, 0.0], [-(2.0 ** -130), 2.0 ** -131]])
+    assert torch.equal(gemm64.chan_floor(w), torch.exp2(torch.tensor([-159.0, -140.0], dtype=torch.float64)))
+
+
+def test_check_allows_one_subnormal_spacing_and_infinity_past_the_overflow():
+    """|got - want| <= tau * S + 2^-149 at every element, and an infinite result exactly where |want| is within tau * S
+    of the fp32 overflow threshold or past it."""
+    from oracle.check64 import F32_OVERFLOW, ratio
+    tau = TAU['gemm64']['gemm']
+    want = torch.tensor([0.0, 2.0 ** -150, 1.0, 2.0 ** 129, -(2.0 ** 129), F32_OVERFLOW - 2.0 ** 100, 2.0 ** 127],
+                        dtype=torch.float64)
+    s = torch.tensor([0.0, 0.0, 1.0, 2.0 ** 100, 2.0 ** 100, 2.0 ** 100 / tau, 1.0], dtype=torch.float64)
+    got = torch.tensor([2.0 ** -149, 0.0, 1.0 + 2 * tau, float('inf'), -float('inf'), float('inf'), float('inf')])
+    r = ratio(got, want, s)
+    assert r[0] == 0 and r[1] == 0                       # one subnormal spacing off, with S = 0
+    assert r[2] > tau                                     # 2 tau * S off
+    assert r[3] == 0 and r[4] == 0                        # past the threshold: Inf with the sign of want
+    assert r[5] <= tau                                    # within tau * S of it
+    assert r[6] > 1e30                                    # 2^127 is finite in fp32: Inf is far off
+    assert ratio(-got[3:4], want[3:4], s[3:4])[0] == float('inf')   # the wrong infinity
+    assert ratio(torch.tensor([3e38]), want[3:4], s[3:4])[0] > 1e6  # a finite result past the overflow
 
 
 def test_checker_flags_a_small_channel_that_max_rel_err_misses(sd, heads_in):

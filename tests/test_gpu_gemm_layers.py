@@ -338,9 +338,13 @@ def test_wrong_row_scale_fails_the_bar(eng):
     a = _rows(m, k, seed=23)
     w, bias = _layer(n, k, seed=29)
     true_max = a.abs().amax(dim=1)
+    eng.poll_saturation(warn=False)
     r_ok, _ = _kernel_case(eng, a, w, bias, 0, name='true rowmax')
+    assert eng.poll_saturation(warn=False) == 0
     r_lo, _ = _kernel_case(eng, a, w, bias, 0, rowmax_in=true_max / 8, name='rowmax / 8')
+    assert eng.poll_saturation(warn=False) == 1                    # the split clamped: the flag says so
     r_hi, _ = _kernel_case(eng, a, w, bias, 0, rowmax_in=true_max * 2.0 ** 24, name='rowmax * 2^24')
+    assert eng.poll_saturation(warn=False) == 0
     print(f'\n[negative control] true {r_ok:.3e}  rowmax/8 {r_lo:.3e}  rowmax*2^24 {r_hi:.3e}')
     assert r_ok <= BARS['gemm']
     assert r_lo >= 10 * BARS['gemm'] and r_hi >= 10 * BARS['gemm'], (r_lo, r_hi)

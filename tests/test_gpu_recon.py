@@ -266,6 +266,23 @@ def test_coefficients_beyond_fp16_range(eng, packs, model, engine):
     _magnitude_case(eng, packs[model], True, engine, f'beyond {model}')
 
 
+@pytest.mark.parametrize('bad', [float('nan'), float('inf'), -float('inf')], ids=['nan', 'inf', '-inf'])
+def test_nonfinite_coefficient_raises_the_flag(eng, prod, bad):
+    """A NaN or +-Inf shape coefficient of one face reaches the fp16 split of dense_alpha_kernel: the call raises the
+    saturation flag, and every other face of the batch (two face tiles) keeps the clean call's bits."""
+    use(eng, prod)
+    p = random_params(70, 91)
+    clean = recon(eng, p, True).cpu()
+    assert eng.poll_saturation(warn=False) == 0
+    q = p.copy()
+    q[65, 12 + 7] = bad
+    got = recon(eng, q, True).cpu()
+    assert eng.poll_saturation(warn=False) == 1
+    assert eng.poll_saturation(warn=False) == 0
+    keep = torch.arange(70) != 65
+    assert torch.equal(got[keep].view(torch.int32), clean[keep].view(torch.int32))
+
+
 # ---- state changes ----------------------------------------------------------------------------------------------------
 
 def test_state_changes_are_picked_up(eng, base3dmm, prod):
