@@ -365,6 +365,53 @@ int syn_draw_lines(uint8_t* images_dev, int64_t image_bytes, const int64_t* fram
                    const int32_t* seg_start_host, const int32_t* seg_start_dev, const int32_t* segs_dev, int n_segs, int thickness,
                    int line_type, void* stream);
 
+/* ---- OBJ text of dense meshes (utils/inference.py:8-23 write_obj; artistic.py:19-31 and uv_texture_realFaces.py:21-33
+ * write_obj_with_colors) -------------------------------------------------------------------------------------------
+ * The bytes those functions write for B meshes, each mesh's text its vertex lines then its triangle lines:
+ *   vertex line   'v {:.4f} {:.4f} {:.4f}\n' of the float32 coordinates 0, 1, 2 (the exact binary value rounded to 4
+ *                 decimals, ties to even; "nan", "inf", "-inf"; the sign bit always prints), with colours followed by
+ *                 ' {} {} {}' of colours[i, 2], [i, 1], [i, 0] before the newline;
+ *   triangle line 'f {} {} {}\n' of triangles[i, 2], [i, 1], [i, 0] (tri_order 0, write_obj) or [i, 0], [i, 1], [i, 2]
+ *                 (tri_order 1, write_obj_with_colors), the indices as given.
+ * A '{}' field is the int64's digits, or with its dot0 flag the repr of an integral float below 1e16 ("233.0"; the
+ * value INT64_MIN stands for -0.0 and prints "-0.0").  Coordinate k of vertex i of mesh b is
+ * vertices[b * stride_mesh + i * stride_vertex + k * stride_coord] (the (B,3,N) output of syn_reconstruct_image and
+ * (N,3) arrays alike).  keep_host / keep_dev: NULL (vertex line i prints vertex i, nver lines), or n_keep vertex
+ * indices (line i prints vertex keep[i]: vertices[:, keep] without a gather copy).  colors: NULL, or int64 (n, 3) rows
+ * of line i at colors[b * colors_stride_mesh + 3 i]; stride 0 shares one colour table between the meshes.
+ * triangles: int64 (ntri, 3), the same text for every mesh. */
+typedef struct {
+  const float* vertices;
+  int64_t stride_mesh;
+  int32_t stride_vertex, stride_coord, batch, nver;
+  const int32_t* keep_host;
+  const int32_t* keep_dev;
+  int32_t n_keep;
+  const int64_t* colors;
+  int64_t colors_stride_mesh;
+  int32_t colors_dot0;
+  const int64_t* triangles;
+  int32_t ntri, tri_order, tri_dot0;
+} syn_obj_desc_t;
+/* Bytes of the workspace syn_obj_plan fills and syn_obj_write reads for batch meshes of n_lines vertex lines and ntri
+ * triangles; -1 for a negative count, a batch outside 1..65535, or more than INT32_MAX blocks of 256 lines
+ * (batch * ceil(n_lines / 256) + ceil(ntri / 256)), the sizes both entries refuse. */
+int64_t syn_obj_workspace_size(int batch, int n_lines, int ntri);
+/* The byte offset of every mesh's text: offsets_dev (batch + 1) int64, mesh b's text at [offsets[b], offsets[b+1]),
+ * offsets[batch] the total the caller allocates for syn_obj_write (the one value it needs on the host).  Two launches.
+ * SYN_ERR_INVALID before any launch for a null pointer, keep_dev without keep_host, batch outside 1..65535, nver < 1,
+ * n_keep or ntri < 0, more than INT32_MAX blocks of 256 lines, a keep index outside [0, nver), a non-positive vertex
+ * stride (stride_mesh too when batch > 1), a negative colour stride, a flag other than 0 or 1; SYN_ERR_SHAPE for a
+ * workspace below syn_obj_workspace_size.  No allocation and no
+ * synchronisation (graph capture is fine); keep_host is read during the call only. */
+int syn_obj_plan(const syn_obj_desc_t* desc, void* ws_dev, int64_t ws_bytes, int64_t* offsets_dev, void* stream);
+/* The text itself into out_dev (out_bytes, offsets[batch] of the plan of the same desc, workspace and offsets): one
+ * launch, and one more that copies mesh 0's triangle text to the others when batch > 1 and ntri > 0.  Every byte of
+ * [0, offsets[batch]) is written; a store past out_bytes is dropped.  The refusals of syn_obj_plan, and SYN_ERR_INVALID
+ * for a null out_dev or offsets_dev or a negative out_bytes. */
+int syn_obj_write(const syn_obj_desc_t* desc, const void* ws_dev, int64_t ws_bytes, const int64_t* offsets_dev, uint8_t* out_dev,
+                  int64_t out_bytes, void* stream);
+
 /* ---- FaceBoxes post-processing (SURVEY.md section 8 row f3) -----------------------------------------------------------
  * These entries take the detector network's outputs (syn_fb_forward below, or any other producer). */
 enum {

@@ -43,6 +43,14 @@ class FbLayerDesc(C.Structure):
     _fields_ = [('name', C.c_char_p)] + [(n, C.c_int32) for n in ('cin', 'cout', 'ksize', 'stride', 'pad', 'has_bn', 'activation')]
 
 
+class ObjDesc(C.Structure):
+    """``syn_obj_desc_t``: B meshes, their optional kept-vertex list and colours, and one triangle list."""
+    _fields_ = [('vertices', C.c_void_p), ('stride_mesh', C.c_int64), ('stride_vertex', C.c_int32), ('stride_coord', C.c_int32),
+                ('batch', C.c_int32), ('nver', C.c_int32), ('keep_host', C.c_void_p), ('keep_dev', C.c_void_p), ('n_keep', C.c_int32),
+                ('colors', C.c_void_p), ('colors_stride_mesh', C.c_int64), ('colors_dot0', C.c_int32), ('triangles', C.c_void_p),
+                ('ntri', C.c_int32), ('tri_order', C.c_int32), ('tri_dot0', C.c_int32)]
+
+
 NMS_CPU_NMS, NMS_PY_CPU_NMS = 0, 1
 FB_MAX_FRAMES = 64            # SYN_FB_MAX_FRAMES: frames per batched detector call
 
@@ -111,6 +119,9 @@ SIGNATURES = {
     'syn_rasterize_images': (_I, [_F, _F, _L, _P, _F, _I, _I, _F, _L, _I, _I, _I, _I, _F, _I, _F, _I, _P, _F, _F, _F, _L, _F, _L, _P]),
     'syn_add_weighted_u8': (_I, [_F, _F, C.c_double, _F, _L, _P]),
     'syn_draw_lines': (_I, [_F, _L, _P, _F, _I, _P, _F, _F, _I, _I, _I, _P]),
+    'syn_obj_workspace_size': (_L, [_I, _I, _I]),
+    'syn_obj_plan': (_I, [C.POINTER(ObjDesc), _F, _L, _F, _P]),
+    'syn_obj_write': (_I, [C.POINTER(ObjDesc), _F, _L, _F, _F, _L, _P]),
     'syn_nms': (_I, [_F, _I, C.c_double, _I, _F, _F, _F, _P]),
     'syn_crop_resize_plan_size': (_L, [_I, _I, _I, _I]),
     'syn_crop_resize_plan_host': (_I, [_P, _I, _I, _I, _I, _P, _L]),
@@ -173,6 +184,7 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_add_weighted_u8', 'syn_fb_forward_images', 'syn_fb_debug_forward_images_until',
                                              'syn_faceboxes_decode_images', 'syn_crop_resize_images_plan_size',
                                              'syn_crop_resize_plan_images_host', 'syn_crop_resize_images', 'syn_draw_lines',
+                                             'syn_obj_workspace_size', 'syn_obj_plan', 'syn_obj_write',
                                              'syn_debug_fill_workspaces', 'syn_debug_fill_on_grow',
                                              'syn_fb_debug_fill_workspaces', 'syn_fb_debug_fill_on_grow')}
 

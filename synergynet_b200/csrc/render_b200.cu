@@ -6,6 +6,7 @@
 #include "kernels_detect.cuh"
 #include "kernels_resize.cuh"
 #include "kernels_draw.cuh"
+#include "kernels_obj.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -130,6 +131,42 @@ int decode_launch(const float* loc, const float* conf, const FbDecodeFrames& t, 
   faceboxes_rank_decode_kernel<<<dim3((np_max + 127) / 128, n_frames), 128, 0, st>>>(loc, conf, t, top_k, cand,
                                                                                                         dets, n_dets);
   SYN_LAUNCH_CHECK("faceboxes_rank_decode_kernel");
+  return SYN_OK;
+}
+
+int64_t obj_blocks(int n) { return ((int64_t)n + kObjThreads - 1) / kObjThreads; }
+
+// the shared checks of the two OBJ entries; fills the kernels' arguments
+int check_obj(const syn_obj_desc_t* d, const void* ws, int64_t ws_bytes, ObjArgs& a, const char* who) {
+  if (!d || !d->vertices || !ws || (d->keep_host && !d->keep_dev) || (d->ntri > 0 && !d->triangles))
+    return fail(SYN_ERR_INVALID, "%s: null pointer", who);
+  if (d->keep_dev && !d->keep_host)
+    return fail(SYN_ERR_INVALID, "%s: keep_dev without keep_host (the kept indices are checked on the host)", who);
+  if (d->batch < 1 || d->batch > 65535 || d->nver < 1 || d->ntri < 0 || (d->keep_host && d->n_keep < 0))
+    return fail(SYN_ERR_INVALID, "%s: %d meshes (1..65535), %d vertices, %d kept, %d triangles", who, d->batch, d->nver,
+                d->keep_host ? d->n_keep : d->nver, d->ntri);
+  if (d->stride_vertex < 1 || d->stride_coord < 1 || (d->batch > 1 && d->stride_mesh < 1) || d->colors_stride_mesh < 0)
+    return fail(SYN_ERR_INVALID, "%s: strides mesh %lld, vertex %d, coordinate %d, colour mesh %lld", who, (long long)d->stride_mesh,
+                d->stride_vertex, d->stride_coord, (long long)d->colors_stride_mesh);
+  if ((d->tri_order | d->tri_dot0 | d->colors_dot0) & ~1)
+    return fail(SYN_ERR_INVALID, "%s: flags tri_order %d, tri_dot0 %d, colors_dot0 %d (each 0 or 1)", who, d->tri_order, d->tri_dot0,
+                d->colors_dot0);
+  const int n = d->keep_host ? d->n_keep : d->nver;
+  if (d->keep_host)
+    for (int i = 0; i < n; ++i)
+      if (d->keep_host[i] < 0 || d->keep_host[i] >= d->nver)
+        return fail(SYN_ERR_INVALID, "%s: keep[%d] = %d lies outside [0, %d)", who, i, d->keep_host[i], d->nver);
+  if ((int64_t)d->batch * obj_blocks(n) + obj_blocks(d->ntri) > INT32_MAX)
+    return fail(SYN_ERR_INVALID, "%s: %d meshes of %d vertex lines and %d triangles exceed one launch's %d blocks of %d lines", who,
+                d->batch, n, d->ntri, INT32_MAX, kObjThreads);
+  if (ws_bytes < syn_obj_workspace_size(d->batch, n, d->ntri))
+    return fail(SYN_ERR_SHAPE, "%s: workspace of %lld bytes, %lld needed", who, (long long)ws_bytes,
+                (long long)syn_obj_workspace_size(d->batch, n, d->ntri));
+  a.v = d->vertices; a.sb = d->batch > 1 ? d->stride_mesh : 0; a.sv = d->stride_vertex; a.sc = d->stride_coord;
+  a.keep = d->keep_host ? d->keep_dev : nullptr; a.n = n;
+  a.colors = d->colors; a.cb = d->colors_stride_mesh; a.color_dot0 = d->colors_dot0;
+  a.tri = d->triangles; a.ntri = d->ntri; a.tri_order = d->tri_order; a.tri_dot0 = d->tri_dot0;
+  a.batch = d->batch; a.vblocks = (int)obj_blocks(n); a.tblocks = (int)obj_blocks(d->ntri);
   return SYN_OK;
 }
 
@@ -378,6 +415,52 @@ int syn_draw_lines(uint8_t* images_dev, int64_t image_bytes, const int64_t* fram
   draw_lines_kernel<<<n_frames, kDrawThreads, 0, (cudaStream_t)stream>>>(images_dev, reinterpret_cast<const long long*>(frames_dev),
                                                                        seg_start_dev, segs_dev);
   SYN_LAUNCH_CHECK("draw_lines_kernel");
+  return SYN_OK;
+}
+
+int64_t syn_obj_workspace_size(int batch, int n_lines, int ntri) {
+  if (batch < 1 || batch > 65535 || n_lines < 0 || ntri < 0 || (int64_t)batch * obj_blocks(n_lines) + obj_blocks(ntri) > INT32_MAX)
+    return -1;
+  return (int64_t)sizeof(long long) * (1 + batch * obj_blocks(n_lines) + obj_blocks(ntri));
+}
+
+int syn_obj_plan(const syn_obj_desc_t* desc, void* ws_dev, int64_t ws_bytes, int64_t* offsets_dev, void* stream) {
+  const char* who = "syn_obj_plan";
+  ObjArgs a;
+  if (int rc = check_obj(desc, ws_dev, ws_bytes, a, who)) return rc;
+  if (!offsets_dev) return fail(SYN_ERR_INVALID, "%s: null pointer", who);
+  cudaStream_t st = (cudaStream_t)stream;
+  long long* ws = static_cast<long long*>(ws_dev);
+  const long long blocks = (long long)a.batch * a.vblocks + a.tblocks;
+  if (blocks > 0) {
+    obj_len_kernel<<<(unsigned)blocks, kObjThreads, 0, st>>>(a, ws + 1);
+    SYN_LAUNCH_CHECK("obj_len_kernel");
+  }
+  obj_scan_kernel<<<1, kObjScanThreads, 0, st>>>(a.batch, a.vblocks, a.tblocks, ws, reinterpret_cast<long long*>(offsets_dev));
+  SYN_LAUNCH_CHECK("obj_scan_kernel");
+  return SYN_OK;
+}
+
+int syn_obj_write(const syn_obj_desc_t* desc, const void* ws_dev, int64_t ws_bytes, const int64_t* offsets_dev, uint8_t* out_dev,
+                  int64_t out_bytes, void* stream) {
+  const char* who = "syn_obj_write";
+  ObjArgs a;
+  if (int rc = check_obj(desc, ws_dev, ws_bytes, a, who)) return rc;
+  if (!offsets_dev || !out_dev || out_bytes < 0)
+    return fail(SYN_ERR_INVALID, "%s: null pointer or %lld output bytes", who, (long long)out_bytes);
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long* ws = static_cast<const long long*>(ws_dev);
+  const long long* off = reinterpret_cast<const long long*>(offsets_dev);
+  char* out = reinterpret_cast<char*>(out_dev);
+  const long long blocks = (long long)a.batch * a.vblocks + a.tblocks;
+  if (blocks > 0) {
+    obj_write_kernel<<<(unsigned)blocks, kObjThreads, 0, st>>>(a, ws, off, out, (long long)out_bytes);
+    SYN_LAUNCH_CHECK("obj_write_kernel");
+  }
+  if (a.batch > 1 && a.ntri > 0) {
+    obj_copy_kernel<<<dim3(128, a.batch - 1), kObjThreads, 0, st>>>(ws, off, out, (long long)out_bytes);
+    SYN_LAUNCH_CHECK("obj_copy_kernel");
+  }
   return SYN_OK;
 }
 

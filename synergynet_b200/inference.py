@@ -6,9 +6,11 @@ device twin ``crop_resize_device`` live here; vertex reconstruction and the pose
 """
 from __future__ import annotations
 
+import ctypes as C
 import math
+import threading
 from math import cos, sin
-from typing import Sequence, Tuple
+from typing import Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -418,3 +420,239 @@ def draw_axis(img, yaw, pitch, roll, tdx=None, tdy=None, size=100, pts68=None):
     if error is not None:
         raise error
     return img
+
+
+# ---- OBJ text of the dense meshes (utils/inference.py:8-23 write_obj; artistic.py:19-31 write_obj_with_colors) ----------
+OBJ_NEG_ZERO = -2 ** 63                 # how the C entries carry -0.0 in a '{}' field of integral floats
+OBJ_CHUNK_BYTES = 1 << 30               # output text per device pass of obj_bytes (about 3.6 MB per dense face)
+OBJ_MAX_MESHES = 65535                  # meshes per syn_obj_plan / syn_obj_write call
+
+
+def obj_file_name(obj_name: str) -> str:
+    """The file the reference writers open: ``.obj`` appended unless the last dot-separated part is ``obj``."""
+    return obj_name if obj_name.split('.')[-1] == 'obj' else obj_name + '.obj'
+
+
+def obj_field_values(a, what: str):
+    """``(int64 array, dot0)`` of the values the reference writes with ``'{}'``: integer arrays as they are (dot0 = 0),
+    float arrays whose every value is integral and below 1e16 in magnitude as their integers (dot0 = 1: printed as
+    ``N.0``, -0.0 as ``-0.0``).  Any other float would need shortest-round-trip printing, which is not restated: a
+    ValueError names the first one."""
+    a = np.asarray(a)
+    if a.dtype.kind in 'iu':
+        if a.dtype.kind == 'u' and a.size and int(a.max()) > 2 ** 63 - 1:
+            raise ValueError(f'{what}: {int(a.max())} does not fit int64')
+        return np.ascontiguousarray(a, dtype=np.int64), 0
+    if a.dtype.kind != 'f':
+        raise TypeError(f'{what} must be integers or integral floats, got {a.dtype}')
+    f = a.astype(np.float64)
+    with np.errstate(invalid='ignore'):
+        bad = ~(np.isfinite(f) & (np.floor(f) == f) & (np.abs(f) < 1e16))
+    if bad.any():
+        at = tuple(int(i) for i in np.argwhere(bad)[0])
+        raise ValueError(f'{what}{list(at)} = {f[at]!r}: only integral floats below 1e16 are written as the reference '
+                         'writes them (any other float needs shortest round-trip printing)')
+    out = f.astype(np.int64)
+    out[(f == 0) & np.signbit(f)] = OBJ_NEG_ZERO
+    return np.ascontiguousarray(out), 1
+
+
+def _obj_vertices(vertices):
+    """``vertices`` ((3,N) or (B,3,N) float32, numpy or CUDA) checked and seen as (B,3,N), not yet uploaded."""
+    import torch
+    if isinstance(vertices, torch.Tensor):
+        if vertices.dtype != torch.float32:
+            raise TypeError(f'vertices must be float32 (what predict_denseVert and get_all_outputs return), got {vertices.dtype}')
+        if not vertices.is_cuda:
+            vertices = vertices.numpy()
+    if not isinstance(vertices, torch.Tensor):
+        vertices = np.asarray(vertices)
+        if vertices.dtype != np.float32:
+            raise TypeError(f'vertices must be float32 (what predict_denseVert and get_all_outputs return), got {vertices.dtype}')
+    if vertices.ndim == 2:
+        vertices = vertices[None]
+    if vertices.ndim != 3 or vertices.shape[1] != 3 or vertices.shape[0] < 1 or vertices.shape[2] < 1:
+        raise ValueError(f'vertices must be (3,N) or (B,3,N) with B, N >= 1, got {tuple(vertices.shape)}')
+    return vertices
+
+
+def _obj_upload(vertices):
+    """The (B,3,N) meshes of :func:`_obj_vertices` as a CUDA tensor with positive strides (host arrays: one upload)."""
+    import torch
+    if not isinstance(vertices, torch.Tensor):
+        if not torch.cuda.is_available():
+            raise RuntimeError('the OBJ encoder needs a CUDA device (H100, sm_90a); there is no CPU fallback')
+        vertices = torch.from_numpy(np.ascontiguousarray(vertices)).to(torch.device('cuda', torch.cuda.current_device()))
+    if min(vertices.stride()) <= 0:
+        vertices = vertices.contiguous()
+    return vertices
+
+
+class ObjEncoder:
+    """The device side of the OBJ writers on one GPU (``syn_obj_plan`` / ``syn_obj_write``) and ``launches``, the
+    kernels it has launched.  It holds no device memory: every call brings its own workspace (:meth:`workspace`, 8 bytes
+    per 256 lines), so calls from several host threads and streams never share one."""
+
+    def __init__(self, device):
+        import torch
+        self.device = torch.device(device)
+        self.launches = 0
+        self._count = threading.Lock()
+
+    def workspace(self, batch: int, n_lines: int, ntri: int):
+        """A new workspace for one plan and the write that follows it."""
+        import torch
+        from . import _lib
+        need = int(_lib.load().syn_obj_workspace_size(batch, n_lines, ntri))
+        if need < 0:
+            raise ValueError(f'{batch} meshes of {n_lines} vertex lines and {ntri} triangles (1..65535 meshes per call)')
+        return torch.empty((need + 7) // 8, dtype=torch.int64, device=self.device)
+
+    def _launched(self, n: int) -> None:
+        with self._count:
+            self.launches += n
+
+    def plan(self, desc, ws, offsets) -> None:
+        import torch
+        from . import _lib
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().syn_obj_plan(C.byref(desc), ws.data_ptr(), ws.numel() * 8, offsets.data_ptr(),
+                                                torch.cuda.current_stream(self.device).cuda_stream))
+        n_lines = desc.n_keep if desc.keep_host else desc.nver
+        self._launched(2 if n_lines or desc.ntri else 1)
+
+    def write(self, desc, ws, offsets, out) -> None:
+        import torch
+        from . import _lib
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().syn_obj_write(C.byref(desc), ws.data_ptr(), ws.numel() * 8, offsets.data_ptr(), out.data_ptr(),
+                                                 out.numel(), torch.cuda.current_stream(self.device).cuda_stream))
+        n_lines = desc.n_keep if desc.keep_host else desc.nver
+        self._launched((1 if n_lines or desc.ntri else 0) + (1 if desc.batch > 1 and desc.ntri else 0))
+
+
+_obj_encoders = {}
+_obj_encoders_lock = threading.Lock()
+
+
+def obj_encoder(device) -> ObjEncoder:
+    import torch
+    device = torch.device(device)
+    with _obj_encoders_lock:
+        if device not in _obj_encoders:
+            _obj_encoders[device] = ObjEncoder(device)
+        return _obj_encoders[device]
+
+
+class ObjTables:
+    """The parts of an OBJ text every mesh of a call shares, checked on the host and uploaded once: the triangles (3,ntri)
+    as the reference takes them, the colours -- None (write_obj's format), one (n,3) table for every mesh or (M,n,3),
+    one per mesh (write_obj_with_colors' format) -- and the kept-vertex list (None: every vertex).  Every refusal
+    happens here, before any CUDA call."""
+
+    def __init__(self, triangles, nver: int, colors=None, keep=None, n_meshes: Optional[int] = None):
+        tri = np.asarray(triangles)
+        if tri.ndim != 2 or tri.shape[0] != 3:
+            raise ValueError(f'triangles must be (3, ntri) as the reference writers take them, got {tri.shape}')
+        self.tri, self.tri_dot0 = obj_field_values(tri.T, 'triangles.T')
+        self.nver = int(nver)
+        self.keep = None
+        if keep is not None:
+            k = np.asarray(keep)
+            if k.ndim != 1 or k.dtype.kind not in 'iu':
+                raise ValueError(f'keep must be a 1-d integer index array, got {k.dtype} {k.shape}')
+            out = np.argwhere((k < 0) | (k >= self.nver))
+            if out.size:
+                raise ValueError(f'keep[{int(out[0, 0])}] = {int(k[out[0, 0]])} lies outside [0, {self.nver})')
+            self.keep = np.ascontiguousarray(k, dtype=np.int32)
+        self.n_lines = self.nver if self.keep is None else len(self.keep)
+        self.colors, self.colors_dot0 = None, 0
+        if colors is not None:
+            col = colors.cpu().numpy() if hasattr(colors, 'cpu') else np.asarray(colors)
+            if col.ndim == 2:
+                col = col[None]
+            if col.ndim != 3 or col.shape[1:] != (self.n_lines, 3) or (col.shape[0] != 1 and col.shape[0] != n_meshes):
+                raise ValueError(f'colors must be ({self.n_lines}, 3), one row per written vertex, or one such table per mesh; got '
+                                 f'{tuple(np.asarray(colors).shape)}')
+            self.colors, self.colors_dot0 = obj_field_values(col, 'colors')
+        self._dev = None
+
+    def upload(self, device):
+        """(triangles, keep, colours) on ``device``, one upload each, kept for the next call."""
+        import torch
+        if self._dev is None or self._dev[0] != device:
+            up = lambda a: None if a is None else torch.from_numpy(a).to(device)
+            self._dev = (device, up(self.tri), up(self.keep), up(self.colors))
+        return self._dev[1:]
+
+    def desc(self, vertices, m0: int, device):
+        """The syn_obj_desc_t of the (B,3,N) device meshes ``vertices``, meshes m0.. of the call."""
+        from . import _lib
+        tri, keep, col = self.upload(device)
+        b, _, n = (int(s) for s in vertices.shape)
+        if n != self.nver:
+            raise ValueError(f'{n} vertices per mesh, the tables were built for {self.nver}')
+        sb, sc, sv = (int(s) for s in vertices.stride())
+        d = _lib.ObjDesc()
+        d.vertices, d.stride_mesh, d.stride_vertex, d.stride_coord, d.batch, d.nver = vertices.data_ptr(), max(sb, 1), sv, sc, b, n
+        if self.keep is not None:
+            d.keep_host, d.keep_dev, d.n_keep = self.keep.ctypes.data, keep.data_ptr(), len(self.keep)
+        if col is not None:
+            shared = col.shape[0] == 1
+            d.colors = col.data_ptr() if shared else col[m0].data_ptr()
+            d.colors_stride_mesh, d.colors_dot0 = 0 if shared else 3 * self.n_lines, self.colors_dot0
+        d.triangles, d.ntri, d.tri_dot0 = tri.data_ptr() if tri.numel() else None, int(self.tri.shape[0]), self.tri_dot0
+        d.tri_order = 0 if self.colors is None else 1
+        return d
+
+    def encode(self, vertices, m0: int = 0, chunk_bytes: int = OBJ_CHUNK_BYTES) -> list:
+        """The OBJ texts of the (B,3,N) CUDA meshes ``vertices`` (meshes m0.. of the call), as a list of B ``bytes``:
+        plan, one read of the offsets, write and one download per chunk of about ``chunk_bytes`` of text."""
+        import torch
+        dev = vertices.device
+        enc = obj_encoder(dev)
+        per_mesh = 40 * self.n_lines + (32 if self.colors is not None else 0) * self.n_lines + 24 * int(self.tri.shape[0]) + 1
+        out = []
+        for a, b in chunk_ranges(int(vertices.shape[0]), min(OBJ_MAX_MESHES, max(1, chunk_bytes // per_mesh))):
+            d = self.desc(vertices[a:b], m0 + a, dev)
+            ws = enc.workspace(b - a, self.n_lines, d.ntri)
+            offsets = torch.empty(b - a + 1, dtype=torch.int64, device=dev)
+            enc.plan(d, ws, offsets)
+            off = offsets.cpu().numpy()                                   # the one host read: the size to allocate
+            text = torch.empty(int(off[-1]), dtype=torch.uint8, device=dev)
+            enc.write(d, ws, offsets, text)
+            host = text.cpu().numpy()
+            out += [host[off[i]:off[i + 1]].tobytes() for i in range(b - a)]
+        return out
+
+
+def obj_bytes(vertices, triangles, colors=None, keep=None) -> list:
+    """The file bytes of ``write_obj(name, vertices[b], triangles)`` -- or, with ``colors``, of
+    ``write_obj_with_colors(name, vertices[b][:, keep], triangles, colors)`` -- for every mesh b, encoded on the GPU: a
+    list of B ``bytes``.  ``vertices``: float32 (B,3,N) or (3,N), a CUDA tensor of any strides (the dense output of
+    ``reconstruct_image`` as it is) or a numpy array (uploaded once).  ``triangles`` (3,ntri), integers or integral
+    floats, written as given.  ``colors``: (n,3) for every mesh or (B,n,3), BGR as stored, n the written vertex count.
+    ``keep``: the kept vertex indices (``vertices[:, keep]`` without a gather copy)."""
+    v = _obj_vertices(vertices)
+    tables = ObjTables(triangles, int(v.shape[2]), colors, keep, int(v.shape[0]))       # every refusal before CUDA
+    return tables.encode(_obj_upload(v))
+
+
+def write_obj(obj_name, vertices, triangles):
+    """``utils/inference.py:8-23``, the same file bytes, encoded on the GPU: one ``'v {:.4f} {:.4f} {:.4f}'`` line per
+    vertex of the float32 (3,N) ``vertices`` (numpy or CUDA), one ``'f {} {} {}'`` line per triangle of (3,ntri)
+    ``triangles`` in the order 2, 1, 0, to ``obj_name`` (``.obj`` appended unless it ends so)."""
+    triangles = triangles.copy()
+    text = obj_bytes(vertices, triangles)[0]
+    with open(obj_file_name(obj_name), 'wb') as f:
+        f.write(text)
+
+
+def write_obj_with_colors(obj_name, vertices, triangles, colors):
+    """``artistic.py:19-31`` (= ``uv_texture_realFaces.py:21-33``), the same file bytes, encoded on the GPU: each vertex
+    line continues with ``colors[i, 2], [i, 1], [i, 0]`` (uint8 colours as digits, float colours from uint8 as
+    ``233.0``); the triangle lines are in the order 0, 1, 2."""
+    triangles = triangles.copy()
+    text = obj_bytes(vertices, triangles, colors)[0]
+    with open(obj_file_name(obj_name), 'wb') as f:
+        f.write(text)

@@ -548,6 +548,33 @@ class _SynergyBase(nn.Module):
         host = out.data.cpu().numpy()
         return [host[out.offsets[i]:out.offsets[i + 1]].reshape(h, w, 3) for i, (h, w) in enumerate(out.sizes)]
 
+    def obj_batch(self, frames, rects: Optional[Sequence[Sequence[Sequence[float]]]] = None, keep=None, colors=None, triangles=None):
+        """The OBJ file bytes of every face of N equally sized BGR uint8 frames: one list of ``bytes`` per frame, one entry
+        per face.  Face j of frame i is ``write_obj(name, get_all_outputs_batch(frames)[i][1][j], tri)`` byte for byte,
+        with ``tri = model.triangles + 1`` (the (3,ntri) layout of tri.mat, 1-based as meshlab reads it) unless
+        ``triangles`` is given.  With ``colors`` ((n,3) for every face, or one table per face) it is
+        ``write_obj_with_colors(name, mesh[:, keep], triangles, colors)`` instead -- ``keep`` alone writes
+        ``write_obj`` of the kept vertices.  The dense meshes never leave the device: they are reconstructed and encoded
+        in chunks of faces of ``dense_chunk_bytes``, and only the text comes back."""
+        return self._obj(*self._frames_front(frames, rects), keep, colors, triangles)
+
+    def obj_images(self, images, rects: Optional[Sequence[Sequence[Sequence[float]]]] = None, keep=None, colors=None, triangles=None):
+        """:meth:`obj_batch` for N BGR uint8 images of any sizes: face j of image i is what ``write_obj`` writes for
+        ``get_all_outputs_images(images)[i][1][j]``."""
+        return self._obj(*self._frames_front(images, rects, ragged=True), keep, colors, triangles)
+
+    def _obj(self, eng, stack, counts, frame_index, params, roi5, keep, colors, triangles):
+        from .inference import ObjTables
+        if not frame_index:
+            return [[] for _ in counts]
+        tri = self.triangles.cpu().numpy() + 1 if triangles is None else triangles
+        tables = ObjTables(tri, eng.n_vert, colors, keep, len(frame_index))
+        texts = []
+        for a, b in self._dense_chunks(eng, len(frame_index)):
+            texts += tables.encode(eng.reconstruct_image(params[a:b], roi5[a:b], dense=True), a)
+        eng.raise_if_error()
+        return split_by_counts(texts, counts)
+
     def _pose_overlay(self, eng, canvas, counts, params, roi5):
         """Plan every face's axes on the host and draw them onto ``canvas`` (a stack or an ImagePack), in place."""
         n_faces = sum(counts)
