@@ -18,10 +18,6 @@ import torch
 from . import _lib
 
 
-def _stream_ptr(device) -> int:
-    return torch.cuda.current_stream(device).cuda_stream
-
-
 def _light_cfg(**kw) -> _lib.LightCfg:
     """Defaults of ``RenderPipeline.__init__`` (Sim3DR/lighting.py:24-32)."""
     v3 = lambda x: (C.c_float * 3)(*[float(t) for t in x])
@@ -77,9 +73,8 @@ class MeshRenderer:
         b = view[4]
         ws = torch.empty((b, self.ntri, 3), dtype=torch.float32, device=self.device)
         out = torch.empty((b, self.nver, 3), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.syn_mesh_normals(*view, self.tri.data_ptr(), self.ntri, self._inc_start.data_ptr(),
-                                                  self._inc_tri.data_ptr(), ws.data_ptr(), out.data_ptr(), _stream_ptr(self.device)))
+        _lib.launch(self.device, 'syn_mesh_normals', *view, self.tri.data_ptr(), self.ntri, self._inc_start.data_ptr(),
+                    self._inc_tri.data_ptr(), ws.data_ptr(), out.data_ptr())
         self.launches += 2
         return out
 
@@ -100,9 +95,8 @@ class MeshRenderer:
             tex_ptr = texture.data_ptr()
         stats = torch.empty((b, 6), dtype=torch.int32, device=self.device)
         out = torch.empty((b, self.nver, 3), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.syn_mesh_lighting(*view, normals.data_ptr(), C.byref(cfg), tex_ptr, stats.data_ptr(),
-                                                   out.data_ptr(), _stream_ptr(self.device)))
+        _lib.launch(self.device, 'syn_mesh_lighting', *view, normals.data_ptr(), C.byref(cfg), tex_ptr, stats.data_ptr(),
+                    out.data_ptr())
         self.launches += 2
         return out
 
@@ -119,10 +113,8 @@ class MeshRenderer:
             raise ValueError(f'colors must be float32 (B,nver,{c}) on the renderer device')
         keys = torch.empty((b, h, w), dtype=torch.int64, device=self.device)
         depth = torch.empty((b, h, w), dtype=torch.float32, device=self.device) if return_depth else None
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.syn_rasterize(image.data_ptr(), h, w, c, *view, self.tri.data_ptr(), self.ntri, colors.data_ptr(),
-                                               1.0, 1 if reverse else 0, keys.data_ptr(),
-                                               depth.data_ptr() if depth is not None else None, _stream_ptr(self.device)))
+        _lib.launch(self.device, 'syn_rasterize', image.data_ptr(), h, w, c, *view, self.tri.data_ptr(), self.ntri, colors.data_ptr(),
+                    1.0, 1 if reverse else 0, keys.data_ptr(), depth.data_ptr() if depth is not None else None)
         self.launches += 2
         return (image, depth) if return_depth else image
 
@@ -148,9 +140,8 @@ class MeshRenderer:
         start = self._mesh_start(counts, len(counts))
         boxes = torch.empty((m, 4), dtype=torch.int32, device=self.device)
         key_off = torch.empty(m + 1, dtype=torch.int64, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.syn_render_frames_plan(*view, self.tri.data_ptr(), self.ntri, start.ctypes.data, len(counts), int(height),
-                                                        int(width), boxes.data_ptr(), key_off.data_ptr(), _stream_ptr(self.device)))
+        _lib.launch(self.device, 'syn_render_frames_plan', *view, self.tri.data_ptr(), self.ntri, start.ctypes.data, len(counts),
+                    int(height), int(width), boxes.data_ptr(), key_off.data_ptr())
         self.launches += 2
         return boxes, key_off
 
@@ -177,11 +168,9 @@ class MeshRenderer:
         keys = torch.empty(max(n_keys, 1), dtype=torch.int64, device=self.device)
         self.last_key_count = n_keys
         start_dev = torch.from_numpy(start).to(self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.syn_rasterize_frames(frames.data_ptr(), out.data_ptr(), n, h, w, c, *view, self.tri.data_ptr(),
-                                                      self.ntri, colors.data_ptr(), int(colors.shape[2]), start.ctypes.data,
-                                                      start_dev.data_ptr(), boxes.data_ptr(), key_off.data_ptr(), n_keys,
-                                                      keys.data_ptr(), keys.numel(), _stream_ptr(self.device)))
+        _lib.launch(self.device, 'syn_rasterize_frames', frames.data_ptr(), out.data_ptr(), n, h, w, c, *view, self.tri.data_ptr(),
+                    self.ntri, colors.data_ptr(), int(colors.shape[2]), start.ctypes.data, start_dev.data_ptr(), boxes.data_ptr(),
+                    key_off.data_ptr(), n_keys, keys.data_ptr(), keys.numel())
         self.launches += 2
         return out
 
@@ -228,10 +217,8 @@ class MeshRenderer:
         table, start, _keep, table_dev, start_dev = axis
         boxes = torch.empty((m, 4), dtype=torch.int32, device=self.device)
         key_off = torch.empty(m + 1, dtype=torch.int64, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.syn_render_images_plan(*view, self.tri.data_ptr(), self.ntri, start.ctypes.data, start_dev,
-                                                        table.ctypes.data, table_dev, len(pack), pack.data.numel(), 3,
-                                                        boxes.data_ptr(), key_off.data_ptr(), _stream_ptr(self.device)))
+        _lib.launch(self.device, 'syn_render_images_plan', *view, self.tri.data_ptr(), self.ntri, start.ctypes.data, start_dev,
+                    table.ctypes.data, table_dev, len(pack), pack.data.numel(), 3, boxes.data_ptr(), key_off.data_ptr())
         self.launches += 2
         return boxes, key_off
 
@@ -259,11 +246,9 @@ class MeshRenderer:
         n_keys = int(key_off[m].item())                                   # the stage's one host synchronisation
         keys = torch.empty(max(n_keys, 1), dtype=torch.int64, device=self.device)
         self.last_key_count = n_keys
-        with torch.cuda.device(self.device):
-            _lib.check(self._lib.syn_rasterize_images(pack.data.data_ptr(), out.data.data_ptr(), pack.data.numel(), table.ctypes.data,
-                                                      table_dev, len(pack), 3, *view, self.tri.data_ptr(), self.ntri, colors.data_ptr(),
-                                                      int(colors.shape[2]), start.ctypes.data, start_dev, boxes.data_ptr(),
-                                                      key_off.data_ptr(), n_keys, keys.data_ptr(), keys.numel(), _stream_ptr(self.device)))
+        _lib.launch(self.device, 'syn_rasterize_images', pack.data.data_ptr(), out.data.data_ptr(), pack.data.numel(), table.ctypes.data,
+                    table_dev, len(pack), 3, *view, self.tri.data_ptr(), self.ntri, colors.data_ptr(), int(colors.shape[2]),
+                    start.ctypes.data, start_dev, boxes.data_ptr(), key_off.data_ptr(), n_keys, keys.data_ptr(), keys.numel())
         self.launches += 2
         return out
 
@@ -290,9 +275,7 @@ def add_weighted(a: torch.Tensor, b: torch.Tensor, alpha: float, out: Optional[t
     out = torch.empty_like(a) if out is None else out
     if out.shape != a.shape or out.dtype != torch.uint8 or out.device != a.device or not out.is_contiguous():
         raise ValueError('out must be a contiguous uint8 tensor shaped like the inputs')
-    with torch.cuda.device(a.device):
-        _lib.check(_lib.load().syn_add_weighted_u8(a.data_ptr(), b.data_ptr(), float(alpha), out.data_ptr(), a.numel(),
-                                                   _stream_ptr(a.device)))
+    _lib.launch(a.device, 'syn_add_weighted_u8', a.data_ptr(), b.data_ptr(), float(alpha), out.data_ptr(), a.numel())
     return out
 
 

@@ -228,3 +228,12 @@ def load() -> C.CDLL:
 def check(code: int) -> None:
     if code != SYN_OK:
         raise SynergyLibError(code, load().syn_last_error().decode(errors='replace'))
+
+
+def launch(device, name: str, *args) -> None:
+    """Call the handle-free entry ``name`` with ``args`` on the current stream of ``device`` (every streamed entry takes its
+    ``void* stream`` last) and raise :class:`SynergyLibError` if it fails.  The device is made current first, so the call
+    and its stream belong to it whatever device the caller has current."""
+    import torch
+    with torch.cuda.device(device):
+        check(getattr(load(), name)(*args, torch.cuda.current_stream(device).cuda_stream))

@@ -31,7 +31,6 @@ def _device():
 def nms_device(dets: torch.Tensor, thresh: float, mode: int = _lib.NMS_CPU_NMS, n: int = None):
     """Greedy NMS of ``dets`` (N,5) float32 CUDA rows ``[x1 y1 x2 y2 score]`` already in descending score order (only the
     first ``n`` rows if given).  Returns ``(keep, n_keep)`` device tensors: kept row indices in order, and their count."""
-    lib = _lib.load()
     if dets.dtype != torch.float32 or dets.dim() != 2 or dets.shape[1] != 5 or not dets.is_cuda or not dets.is_contiguous():
         raise ValueError('dets must be a contiguous float32 (N,5) CUDA tensor')
     n = int(dets.shape[0]) if n is None else int(n)
@@ -39,9 +38,8 @@ def nms_device(dets: torch.Tensor, thresh: float, mode: int = _lib.NMS_CPU_NMS, 
     mask = torch.empty((max(n * words, 1),), dtype=torch.int64, device=dets.device)
     keep = torch.empty((max(n, 1),), dtype=torch.int32, device=dets.device)
     n_keep = torch.zeros((1,), dtype=torch.int32, device=dets.device)
-    with torch.cuda.device(dets.device):
-        _lib.check(lib.syn_nms(dets.data_ptr(), n, float(thresh), int(mode), mask.data_ptr(), keep.data_ptr(), n_keep.data_ptr(),
-                               torch.cuda.current_stream(dets.device).cuda_stream))
+    _lib.launch(dets.device, 'syn_nms', dets.data_ptr(), n, float(thresh), int(mode), mask.data_ptr(), keep.data_ptr(),
+                n_keep.data_ptr())
     return keep, n_keep
 
 
@@ -82,7 +80,6 @@ def decode_device(loc: torch.Tensor, conf: torch.Tensor, im_height: int, im_widt
     """``FaceBoxes.py:98-121`` on the device: ``loc`` (P,4), ``conf`` (P,2) float32 CUDA tensors (network outputs for an
     ``im_height`` x ``im_width`` input) -> ``(dets, n)``: (k,5) rows ``[x1 y1 x2 y2 score]`` in descending score order in
     original-image pixels, of which the first ``n`` (device int32) are valid."""
-    lib = _lib.load()
     p = num_priors(im_height, im_width)
     loc, conf = loc.reshape(-1, 4).contiguous(), conf.reshape(-1, 2).contiguous()
     if loc.shape[0] != p or conf.shape[0] != p or loc.dtype != torch.float32 or conf.dtype != torch.float32 or not loc.is_cuda:
@@ -90,10 +87,8 @@ def decode_device(loc: torch.Tensor, conf: torch.Tensor, im_height: int, im_widt
     cand = torch.empty((p + 1,), dtype=torch.int32, device=loc.device)
     dets = torch.zeros((k, 5), dtype=torch.float32, device=loc.device)
     n = torch.zeros((1,), dtype=torch.int32, device=loc.device)
-    with torch.cuda.device(loc.device):
-        _lib.check(lib.syn_faceboxes_decode(loc.data_ptr(), conf.data_ptr(), int(im_height), int(im_width), float(im_width),
-                                            float(im_height), float(scale), float(conf_thresh), int(k), cand.data_ptr(),
-                                            dets.data_ptr(), n.data_ptr(), torch.cuda.current_stream(loc.device).cuda_stream))
+    _lib.launch(loc.device, 'syn_faceboxes_decode', loc.data_ptr(), conf.data_ptr(), int(im_height), int(im_width), float(im_width),
+                float(im_height), float(scale), float(conf_thresh), int(k), cand.data_ptr(), dets.data_ptr(), n.data_ptr())
     return dets, n
 
 
@@ -102,7 +97,6 @@ def decode_batch_device(loc: torch.Tensor, conf: torch.Tensor, im_height: int, i
     """:func:`decode_device` for N frames of one size in the same two launches: ``loc`` (N,P,4), ``conf`` (N,P,2) ->
     ``(dets, n)``: (N,k',5) and (N,) device int32, frame i's block and count being what ``decode_device`` gives for
     ``loc[i]``, ``conf[i]``.  k' = min(k, P): a frame cannot have more candidates than priors."""
-    lib = _lib.load()
     p = num_priors(im_height, im_width)
     if loc.dim() != 3 or conf.dim() != 3 or tuple(loc.shape[1:]) != (p, 4) or tuple(conf.shape) != (loc.shape[0], p, 2) or \
             loc.shape[0] == 0 or loc.dtype != torch.float32 or conf.dtype != torch.float32 or not loc.is_cuda or conf.device != loc.device:
@@ -112,10 +106,8 @@ def decode_batch_device(loc: torch.Tensor, conf: torch.Tensor, im_height: int, i
     cand = torch.empty((nf, p + 1), dtype=torch.int32, device=loc.device)
     dets = torch.zeros((nf, k, 5), dtype=torch.float32, device=loc.device)
     n = torch.zeros((nf,), dtype=torch.int32, device=loc.device)
-    with torch.cuda.device(loc.device):
-        _lib.check(lib.syn_faceboxes_decode_batch(loc.data_ptr(), conf.data_ptr(), nf, int(im_height), int(im_width), float(im_width),
-                                                  float(im_height), float(scale), float(conf_thresh), k, cand.data_ptr(),
-                                                  dets.data_ptr(), n.data_ptr(), torch.cuda.current_stream(loc.device).cuda_stream))
+    _lib.launch(loc.device, 'syn_faceboxes_decode_batch', loc.data_ptr(), conf.data_ptr(), nf, int(im_height), int(im_width),
+                float(im_width), float(im_height), float(scale), float(conf_thresh), k, cand.data_ptr(), dets.data_ptr(), n.data_ptr())
     return dets, n
 
 
@@ -125,7 +117,6 @@ def decode_images_device(loc: torch.Tensor, conf: torch.Tensor, sizes, scales, c
     (sum P_i,2) as ``FaceBoxesNet`` packs them, ``sizes`` the N (h, w) inputs, ``scales`` their shrink factors ->
     ``(dets, n)``: (N,k',5) and (N,) device int32, image i's block and count being what ``decode_device`` gives for its
     priors alone.  k' = min(k, max P_i)."""
-    lib = _lib.load()
     hw = np.ascontiguousarray(np.array(sizes, np.int32).reshape(-1, 2))
     hs, ws = np.ascontiguousarray(hw[:, 0]), np.ascontiguousarray(hw[:, 1])
     sc = np.ascontiguousarray(scales, dtype=np.float32).reshape(-1)
@@ -141,10 +132,8 @@ def decode_images_device(loc: torch.Tensor, conf: torch.Tensor, sizes, scales, c
     cand = torch.empty((nf + sum(ps),), dtype=torch.int32, device=loc.device)
     dets = torch.zeros((nf, k, 5), dtype=torch.float32, device=loc.device)
     n = torch.zeros((nf,), dtype=torch.int32, device=loc.device)
-    with torch.cuda.device(loc.device):
-        _lib.check(lib.syn_faceboxes_decode_images(loc.data_ptr(), conf.data_ptr(), nf, hs.ctypes.data, ws.ctypes.data, sc.ctypes.data,
-                                                   float(conf_thresh), k, cand.data_ptr(), dets.data_ptr(), n.data_ptr(),
-                                                   torch.cuda.current_stream(loc.device).cuda_stream))
+    _lib.launch(loc.device, 'syn_faceboxes_decode_images', loc.data_ptr(), conf.data_ptr(), nf, hs.ctypes.data, ws.ctypes.data,
+                sc.ctypes.data, float(conf_thresh), k, cand.data_ptr(), dets.data_ptr(), n.data_ptr())
     return dets, n
 
 
@@ -152,7 +141,6 @@ def nms_batch_device(dets: torch.Tensor, n: torch.Tensor, thresh: float, mode: i
     """:func:`nms_device` per frame without a host round trip: ``dets`` (N,K,5) in descending score order per frame, ``n``
     (N,) device int32 counts (``decode_batch_device``'s outputs).  Returns ``(keep (N,K) int32, n_keep (N,) int32)``; the
     first ``n_keep[i]`` entries of ``keep[i]`` are frame i's kept rows, the rest is not written."""
-    lib = _lib.load()
     if dets.dtype != torch.float32 or dets.dim() != 3 or dets.shape[2] != 5 or dets.shape[0] == 0 or dets.shape[1] == 0 or \
             not dets.is_cuda or not dets.is_contiguous():
         raise ValueError('dets must be a contiguous float32 (N,K,5) CUDA tensor')
@@ -162,9 +150,8 @@ def nms_batch_device(dets: torch.Tensor, n: torch.Tensor, thresh: float, mode: i
     mask = torch.empty((nf * rows * ((rows + 63) // 64),), dtype=torch.int64, device=dets.device)
     keep = torch.empty((nf, rows), dtype=torch.int32, device=dets.device)
     n_keep = torch.zeros((nf,), dtype=torch.int32, device=dets.device)
-    with torch.cuda.device(dets.device):
-        _lib.check(lib.syn_nms_batch(dets.data_ptr(), n.data_ptr(), nf, rows, float(thresh), int(mode), mask.data_ptr(),
-                                     keep.data_ptr(), n_keep.data_ptr(), torch.cuda.current_stream(dets.device).cuda_stream))
+    _lib.launch(dets.device, 'syn_nms_batch', dets.data_ptr(), n.data_ptr(), nf, rows, float(thresh), int(mode), mask.data_ptr(),
+                keep.data_ptr(), n_keep.data_ptr())
     return keep, n_keep
 
 

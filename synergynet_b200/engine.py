@@ -63,6 +63,49 @@ class StreamOrder:
             self._last_event.synchronize()
 
 
+class Handle:
+    """One library handle bound to ``device``, created by the entry ``_CREATE`` and freed by ``_DESTROY``.  The C handle is
+    not re-entrant and all its calls share one device workspace: :meth:`_call` serialises the host threads with the
+    handle's lock and orders calls that arrive on different CUDA streams with a ``StreamOrder``.  A subclass sets
+    ``self._lib`` before it calls this constructor."""
+    _CREATE = _DESTROY = None
+
+    def __init__(self, device: torch.device):
+        self.device = device
+        h = C.c_void_p()
+        _lib.check(getattr(self._lib, self._CREATE)(device.index or 0, C.byref(h)))
+        self._h = h
+        self._lock = threading.RLock()
+        self._order = StreamOrder(device)
+
+    def close(self):
+        if getattr(self, '_h', None):
+            getattr(self._lib, self._DESTROY)(self._h)
+            self._h = None
+
+    def __del__(self):  # pragma: no cover
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _before_stream(self) -> None:
+        """Runs under the lock, on the handle's device, before :meth:`_call` takes the stream."""
+
+    def _call(self, name: str, *args) -> None:
+        """``name(handle, *args, stream)`` on the current stream of the handle's device, ordered after the handle's
+        previous call; raises SynergyLibError if it fails."""
+        with torch.cuda.device(self.device), self._lock:
+            self._before_stream()
+            _lib.check(getattr(self._lib, name)(self._h, *args, self._order.begin()))
+            self._order.end()
+
+    def _call_host(self, name: str, *args) -> None:
+        """``name(handle, *args)`` for an entry that takes no stream, under the handle's lock."""
+        with self._lock:
+            _lib.check(getattr(self._lib, name)(self._h, *args))
+
+
 def refuse_under_capture(what: str) -> None:
     """Raise SYN_ERR_STATE if the current stream is capturing a CUDA graph: for calls that run on the library's own
     streams and synchronise the host, which a graph cannot hold."""
@@ -71,41 +114,24 @@ def refuse_under_capture(what: str) -> None:
                                                        "so it cannot be captured in a CUDA graph; call it outside the capture")
 
 
-class Engine:
-    """Owns one ``syn_handle_t`` bound to ``cuda:<device>``."""
+class Engine(Handle):
+    """Owns one ``syn_handle_t`` bound to ``cuda:<device>``.  nn.DataParallel replicas use one engine per device, but user
+    threads may share a model, hence the handle's lock."""
+    _CREATE, _DESTROY = 'syn_create', 'syn_destroy'
 
     def __init__(self, device: int = 0):
         self._lib = _lib.load()
         if not torch.cuda.is_available():
             raise RuntimeError('synergynet_b200 needs a CUDA device (H100, sm_90a); there is no '
                                'CPU fallback for the inference hot path')
-        self.device = torch.device('cuda', int(device))
-        h = C.c_void_p()
-        _lib.check(self._lib.syn_create(int(device), C.byref(h)))
-        self._h = h
+        super().__init__(torch.device('cuda', int(device)))
         self.n_pts = 0
         self.n_vert = 0
         # the conv+BN backbone each family's part of the handle holds: family -> (arch, pooled feature width); the ResNet
         # part holds resnet50 until syn_resnet_select
         self._backbones: Dict[str, Tuple[str, int]] = {'resnet': ('resnet50', 2048)}
         self._keep = []
-        # The C handle is not re-entrant and all calls share one activation workspace: serialise the host threads
-        # (nn.DataParallel replicas use one engine per device, but user threads may share a model) and order
-        # consecutive calls that arrive on different CUDA streams with an event.
-        self._lock = threading.RLock()
         self._host_inflight: Dict[int, tuple] = {}     # ticket -> tensors of a submitted host call (kept alive)
-        self._order = StreamOrder(self.device)
-
-    def close(self):
-        if getattr(self, '_h', None):
-            self._lib.syn_destroy(self._h)
-            self._h = None
-
-    def __del__(self):  # pragma: no cover
-        try:
-            self.close()
-        except Exception:
-            pass
 
     # ---- weights --------------------------------------------------------------------------------
     def load_backbone(self, sd: Dict[str, torch.Tensor], prefix: str = 'I2P.backbone.') -> None:
@@ -174,16 +200,11 @@ class Engine:
             raise RuntimeError(f'input on {x.device}, engine on {self.device}')
         return x.to(torch.float32).contiguous()
 
-    def _stream(self) -> int:
-        """Current torch stream of the engine's device, ordered after the previous call (``StreamOrder``) and after
-        any submitted host call."""
+    def _before_stream(self) -> None:
+        """Stream-ordered calls also wait for every submitted host call."""
         if not torch.cuda.is_current_stream_capturing():
             for ticket in list(self._host_inflight):     # submitted host calls run on the library's own streams and use
                 _lib.check(self._lib.syn_host_wait(self._h, ticket))   # the same workspace: let them finish (tickets stay valid)
-        return self._order.begin()
-
-    def _done(self) -> None:
-        self._order.end()
 
     def raise_if_error(self) -> None:
         """Cheap (no device sync) look at the sticky time-out flag of the bounded in-kernel waits; call it after a
@@ -219,10 +240,7 @@ class Engine:
         b = x.shape[0]
         params = torch.empty((b, N_PARAMS), device=self.device, dtype=torch.float32)
         pool = torch.empty((b, 1280), device=self.device, dtype=torch.float32) if want_pool else None
-        with self._lock:
-            _lib.check(self._lib.syn_forward(self._h, x.data_ptr(), b, params.data_ptr(),
-                                             pool.data_ptr() if want_pool else None, self._stream()))
-            self._done()
+        self._call('syn_forward', x.data_ptr(), b, params.data_ptr(), pool.data_ptr() if want_pool else None)
         return (params, pool) if want_pool else params
 
     def reconstruct(self, params: torch.Tensor, dense: bool = False, whitening: bool = True,
@@ -235,10 +253,7 @@ class Engine:
         if n == 0:
             raise RuntimeError('dense basis not loaded' if dense else 'sparse basis not loaded')
         out = torch.empty((b, 3, n), device=self.device, dtype=torch.float32)
-        with self._lock:
-            _lib.check(self._lib.syn_reconstruct(self._h, params.data_ptr(), b, int(dense), int(whitening),
-                                                 int(transform), out.data_ptr(), self._stream()))
-            self._done()
+        self._call('syn_reconstruct', params.data_ptr(), b, int(dense), int(whitening), int(transform), out.data_ptr())
         return out
 
     def reconstruct_image(self, params: torch.Tensor, roi5: torch.Tensor, dense: bool = False) -> torch.Tensor:
@@ -255,10 +270,7 @@ class Engine:
         if n == 0:
             raise RuntimeError('dense basis not loaded' if dense else 'sparse basis not loaded')
         out = torch.empty((b, 3, n), device=self.device, dtype=torch.float32)
-        with self._lock:
-            _lib.check(self._lib.syn_reconstruct_image(self._h, params.data_ptr(), b, int(dense), roi5.data_ptr(), out.data_ptr(),
-                                                       self._stream()))
-            self._done()
+        self._call('syn_reconstruct_image', params.data_ptr(), b, int(dense), roi5.data_ptr(), out.data_ptr())
         return out
 
     def pose_decode(self, params: torch.Tensor, roi5: Optional[torch.Tensor] = None):
@@ -272,10 +284,8 @@ class Engine:
                 raise RuntimeError(f'roi5 must be (B,5), got {tuple(roi5.shape)}')
         ang = torch.empty((b, 3), device=self.device, dtype=torch.float64)
         t3d = torch.empty((b, 3), device=self.device, dtype=torch.float32)
-        with self._lock:
-            _lib.check(self._lib.syn_pose_decode(self._h, params.data_ptr(), b, roi5.data_ptr() if roi5 is not None else None,
-                                                 ang.data_ptr(), t3d.data_ptr(), self._stream()))
-            self._done()
+        self._call('syn_pose_decode', params.data_ptr(), b, roi5.data_ptr() if roi5 is not None else None, ang.data_ptr(),
+                   t3d.data_ptr())
         return ang, t3d
 
     def set_center_crop(self, margin: int) -> None:
@@ -290,11 +300,7 @@ class Engine:
         b = x.shape[0]
         lmk = torch.empty((b, 3, self.n_pts), device=self.device, dtype=torch.float32)
         params = torch.empty((b, N_PARAMS), device=self.device, dtype=torch.float32) if want_params else None
-        with self._lock:
-            _lib.check(self._lib.syn_forward_landmarks(self._h, x.data_ptr(), b,
-                                                       params.data_ptr() if want_params else None,
-                                                       lmk.data_ptr(), self._stream()))
-            self._done()
+        self._call('syn_forward_landmarks', x.data_ptr(), b, params.data_ptr() if want_params else None, lmk.data_ptr())
         return (lmk, params) if want_params else lmk
 
     def _forward_landmarks_u8(self, x: torch.Tensor, want_params: bool):
@@ -304,11 +310,7 @@ class Engine:
         b = x.shape[0]
         lmk = torch.empty((b, 3, self.n_pts), device=self.device, dtype=torch.float32)
         params = torch.empty((b, N_PARAMS), device=self.device, dtype=torch.float32) if want_params else None
-        with self._lock:
-            _lib.check(self._lib.syn_forward_landmarks_u8(self._h, x.data_ptr(), b,
-                                                          params.data_ptr() if want_params else None,
-                                                          lmk.data_ptr(), self._stream()))
-            self._done()
+        self._call('syn_forward_landmarks_u8', x.data_ptr(), b, params.data_ptr() if want_params else None, lmk.data_ptr())
         return (lmk, params) if want_params else lmk
 
     def forward_landmarks_host(self, x_host: torch.Tensor, lmk_host: Optional[torch.Tensor] = None,
@@ -363,15 +365,15 @@ class Engine:
         """net 0: MLP_for state dict (conv1..conv9 + bn1..bn9), net 1: MLP_rev (conv1..5, conv6_1/2/3 + their BN);
         keys without prefix, as ``module.state_dict()`` returns them (pointnet_backbone.py:7-29,67-88)."""
         names = self._FOR_LAYERS if net == 0 else self._REV_LAYERS
-        with self._lock:
+        with self._lock:                 # held across the hand-over: another thread's layers never mix with these
             for i, cname in enumerate(names):
                 bname = 'bn' + cname[4:]
                 w = _host_f32(sd[f'{cname}.weight'])
                 cb = _host_f32(sd[f'{cname}.bias'])
                 bn = [_host_f32(sd[f'{bname}.{k}']) for k in ('weight', 'bias', 'running_mean', 'running_var')]
-                _lib.check(self._lib.syn_pointnet_set_layer(self._h, net, i, w.data_ptr(), w.shape[0], w.shape[1], cb.data_ptr(),
-                                                            *[t.data_ptr() for t in bn], 1e-5))
-            _lib.check(self._lib.syn_pointnet_commit(self._h, net))
+                self._call_host('syn_pointnet_set_layer', net, i, w.data_ptr(), w.shape[0], w.shape[1], cb.data_ptr(),
+                                *[t.data_ptr() for t in bn], 1e-5)
+            self._call_host('syn_pointnet_commit', net)
 
     def _dev_f32(self, t: torch.Tensor) -> torch.Tensor:
         return t.to(device=self.device, dtype=torch.float32).contiguous()
@@ -383,10 +385,7 @@ class Engine:
         if tuple(lmk.shape[1:]) != (3, 68) or tuple(pool.shape) != (b, 1280) or tuple(params.shape) != (b, N_PARAMS):
             raise RuntimeError(f'mlp_for: expected (B,3,68), (B,1280), (B,62); got {tuple(lmk.shape)}, {tuple(pool.shape)}, {tuple(params.shape)}')
         res, ref = torch.empty_like(lmk), torch.empty_like(lmk)
-        with self._lock:
-            _lib.check(self._lib.syn_mlp_for(self._h, lmk.data_ptr(), pool.data_ptr(), params.data_ptr(), b, res.data_ptr(),
-                                             ref.data_ptr(), self._stream()))
-            self._done()
+        self._call('syn_mlp_for', lmk.data_ptr(), pool.data_ptr(), params.data_ptr(), b, res.data_ptr(), ref.data_ptr())
         return res, ref
 
     def mlp_rev(self, lmk: torch.Tensor) -> torch.Tensor:
@@ -394,9 +393,7 @@ class Engine:
         if lmk.dim() != 3 or tuple(lmk.shape[1:]) != (3, 68):
             raise RuntimeError(f'mlp_rev: expected (B,3,68), got {tuple(lmk.shape)}')
         out = torch.empty((lmk.shape[0], N_PARAMS), device=self.device, dtype=torch.float32)
-        with self._lock:
-            _lib.check(self._lib.syn_mlp_rev(self._h, lmk.data_ptr(), lmk.shape[0], out.data_ptr(), self._stream()))
-            self._done()
+        self._call('syn_mlp_rev', lmk.data_ptr(), lmk.shape[0], out.data_ptr())
         return out
 
     def wing_loss(self, pred: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
@@ -405,10 +402,7 @@ class Engine:
         if pred.shape != target.shape or pred.dim() != 3 or pred.shape[1] != 3:
             raise RuntimeError(f'wing_loss: expected two (B,3,N) tensors, got {tuple(pred.shape)} and {tuple(target.shape)}')
         out = torch.empty((1,), device=self.device, dtype=torch.float32)
-        with self._lock:
-            _lib.check(self._lib.syn_wing_loss(self._h, pred.data_ptr(), target.data_ptr(), pred.shape[0], pred.shape[2],
-                                               out.data_ptr(), self._stream()))
-            self._done()
+        self._call('syn_wing_loss', pred.data_ptr(), target.data_ptr(), pred.shape[0], pred.shape[2], out.data_ptr())
         return out[0]
 
     def param_loss(self, inp: torch.Tensor, target: torch.Tensor, mode: str = 'normal') -> torch.Tensor:
@@ -419,32 +413,30 @@ class Engine:
         if inp.dim() != 2 or inp.shape[1] != N_PARAMS or target.shape != inp.shape:
             raise RuntimeError('param_loss: expected two (B,62) tensors')
         out = torch.empty((inp.shape[0],), device=self.device, dtype=torch.float32)
-        with self._lock:
-            _lib.check(self._lib.syn_param_loss(self._h, inp.data_ptr(), target.data_ptr(), inp.shape[0],
-                                                0 if mode == 'normal' else 1, out.data_ptr(), self._stream()))
-            self._done()
+        self._call('syn_param_loss', inp.data_ptr(), target.data_ptr(), inp.shape[0], 0 if mode == 'normal' else 1,
+                   out.data_ptr())
         return out
 
     # ---- conv+BN backbones: ResNet and MobileNetV1, one (B,102) output ori | shape | exp | tex ---------------------
     def _load_convbn(self, family: str, arch: str, select, conv_keys, feat: int, sd: Dict[str, torch.Tensor],
                      prefix: str) -> None:
-        """``select()`` the plan of ``arch``, then hand over its conv+BN pairs in plan order and the four Linear heads
-        concatenated in the reference's output order as (102, feat) weights, and commit."""
-        set_conv, set_heads, commit = (getattr(self._lib, f'syn_{family}_{n}') for n in ('set_conv', 'set_heads', 'commit'))
-        with self._lock:
-            _lib.check(select())
+        """Select the plan of ``arch`` (``select``: the entry's name and its arguments after the handle), then hand over its
+        conv+BN pairs in plan order and the four Linear heads concatenated in the reference's output order as (102, feat)
+        weights, and commit."""
+        with self._lock:                 # held across the hand-over: another thread's layers never mix with these
+            self._call_host(*select)
             self._backbones[family] = (arch, feat)
             for i, (ck, bk) in enumerate(conv_keys):
                 w = _host_f32(sd[f'{prefix}{ck}.weight'])
                 bn = [_host_f32(sd[f'{prefix}{bk}.{k}']) for k in ('weight', 'bias', 'running_mean', 'running_var')]
-                _lib.check(set_conv(self._h, i, w.data_ptr(), w.numel(), *[t.data_ptr() for t in bn], 1e-5))
+                self._call_host(f'syn_{family}_set_conv', i, w.data_ptr(), w.numel(), *[t.data_ptr() for t in bn], 1e-5)
             order = ('fc_ori', 'fc_shape', 'fc_exp', 'fc_tex')
             w = torch.cat([_host_f32(sd[f'{prefix}{k}.weight']) for k in order]).contiguous()
             b = torch.cat([_host_f32(sd[f'{prefix}{k}.bias']) for k in order]).contiguous()
             if tuple(w.shape) != (102, feat):
                 raise RuntimeError(f'{arch} heads: expected (102, {feat}) weights, got {tuple(w.shape)}')
-            _lib.check(set_heads(self._h, w.data_ptr(), b.data_ptr()))
-            _lib.check(commit(self._h))
+            self._call_host(f'syn_{family}_set_heads', w.data_ptr(), b.data_ptr())
+            self._call_host(f'syn_{family}_commit')
 
     def _backbone(self, family: str) -> Tuple[str, int]:
         if family not in self._backbones:
@@ -462,21 +454,14 @@ class Engine:
         b = x.shape[0]
         out = torch.empty((b, 102), device=self.device, dtype=torch.float32)
         pool = torch.empty((b, self._backbone(family)[1]), device=self.device, dtype=torch.float32)
-        forward = getattr(self._lib, f'syn_{family}_forward')
-        with self._lock:
-            _lib.check(forward(self._h, x.data_ptr(), int(x.dtype == torch.uint8), b, out.data_ptr(), pool.data_ptr(),
-                               self._stream()))
-            self._done()
+        self._call(f'syn_{family}_forward', x.data_ptr(), int(x.dtype == torch.uint8), b, out.data_ptr(), pool.data_ptr())
         return out, pool
 
-    def _debug_run(self, fn, x: torch.Tensor, stage: int, rows: int, cols: int, rowmax: bool):
+    def _debug_run(self, name: str, x: torch.Tensor, stage: int, rows: int, cols: int, rowmax: bool):
         """One syn_debug_*_until run of a conv+BN backbone on fp32 crops ``x`` into (rows, cols) and, if the stage records
         them, (rows,) row maxima."""
         out, rmax = self._debug_out(rows, cols, rowmax)
-        with self._lock:
-            _lib.check(fn(self._h, x.data_ptr(), x.shape[0], stage, out.data_ptr(), rmax.data_ptr() if rowmax else None,
-                          self._stream()))
-            self._done()
+        self._call(name, x.data_ptr(), x.shape[0], stage, out.data_ptr(), rmax.data_ptr() if rowmax else None)
         return out, rmax
 
     # ResNet backbones (backbone_nets/resnet_backbone.py; BASELINE.json configs[4] is resnet50)
@@ -487,8 +472,7 @@ class Engine:
         if arch not in RESNET_ARCHS:
             raise RuntimeError(f"arch '{arch}': the ResNet backbones are {', '.join(RESNET_ARCHS)}")
         feat = 512 if RESNET_ARCHS[arch][0] < 50 else 2048
-        self._load_convbn('resnet', arch, lambda: self._lib.syn_resnet_select(self._h, *RESNET_ARCHS[arch]),
-                          resnet_conv_keys(arch), feat, sd, prefix)
+        self._load_convbn('resnet', arch, ('syn_resnet_select', *RESNET_ARCHS[arch]), resnet_conv_keys(arch), feat, sd, prefix)
 
     def load_resnet50(self, sd: Dict[str, torch.Tensor], prefix: str = '') -> None:
         """Hand a ``resnet_backbone.resnet50()`` state dict to the library (53 conv+BN pairs in execution order, the four
@@ -511,9 +495,7 @@ class Engine:
         b = x.shape[0]
         out = torch.empty((b, 102), device=self.device, dtype=torch.float32)
         pool = torch.empty((b, 2048), device=self.device, dtype=torch.float32)
-        with self._lock:
-            _lib.check(self._lib.syn_resnet50_forward(self._h, x.data_ptr(), b, out.data_ptr(), pool.data_ptr(), self._stream()))
-            self._done()
+        self._call('syn_resnet50_forward', x.data_ptr(), b, out.data_ptr(), pool.data_ptr())
         return out, pool
 
     def debug_resnet_until(self, x: torch.Tensor, stage: int):
@@ -535,7 +517,7 @@ class Engine:
             rows, cols, rm = b * d.h_out * d.h_out, d.cout, 'downsample' not in keys[stage - 1][0]
         else:
             rows, cols, rm = b, feat if stage == n + 1 else 102, stage == n + 1
-        return self._debug_run(self._lib.syn_debug_resnet_until, x, stage, rows, cols, rm)
+        return self._debug_run('syn_debug_resnet_until', x, stage, rows, cols, rm)
 
     # MobileNetV1 backbones (backbone_nets/mobilenetv1_backbone.py, the five mobilenet_* factories)
     def load_mobilenet_v1(self, sd: Dict[str, torch.Tensor], arch: str, prefix: str = '') -> None:
@@ -544,8 +526,7 @@ class Engine:
         if arch not in MBV1_WIDTHS:
             raise RuntimeError(f"arch '{arch}': MobileNetV1 widths are {', '.join(MBV1_WIDTHS)}")
         code = int(round(MBV1_WIDTHS[arch] * 100))
-        self._load_convbn('mbv1', arch, lambda: self._lib.syn_mbv1_set_widen(self._h, code), mobilenet_v1_conv_keys(),
-                          1024 * code // 100, sd, prefix)
+        self._load_convbn('mbv1', arch, ('syn_mbv1_set_widen', code), mobilenet_v1_conv_keys(), 1024 * code // 100, sd, prefix)
 
     def forward_mobilenet_v1(self, x: torch.Tensor):
         """MobileNet.forward (mobilenetv1_backbone.py:108-140): (B,3,120,120) fp32 normalised crops or raw uint8 crops ->
@@ -565,7 +546,7 @@ class Engine:
             rows, cols, rm = b * d.h_out * d.h_out, d.cout, stage == 0 or stage % 2 == 1 or stage == 26
         else:
             rows, cols, rm = b, feat if stage == 27 else 102, stage == 27
-        return self._debug_run(self._lib.syn_debug_mbv1_until, x, stage, rows, cols, rm)
+        return self._debug_run('syn_debug_mbv1_until', x, stage, rows, cols, rm)
 
     # ---- per-stage debug runs of the GEMM layers (include/synergy_b200.h syn_debug_*_until / syn_debug_gemm) ----
     RESNET_STAGES = 56
@@ -589,12 +570,8 @@ class Engine:
         out, rmax = self._debug_out(b if per_face else b * 68, cols, rm)
         pool = self._dev_f32(pool) if pool is not None else None
         params = self._dev_f32(params) if params is not None else None
-        with self._lock:
-            _lib.check(self._lib.syn_debug_pointnet_until(
-                self._h, net, lmk.data_ptr(), pool.data_ptr() if pool is not None else None,
-                params.data_ptr() if params is not None else None, b, stage, out.data_ptr(),
-                rmax.data_ptr() if rm else None, self._stream()))
-            self._done()
+        self._call('syn_debug_pointnet_until', net, lmk.data_ptr(), pool.data_ptr() if pool is not None else None,
+                   params.data_ptr() if params is not None else None, b, stage, out.data_ptr(), rmax.data_ptr() if rm else None)
         return out, rmax
 
     def debug_gemm(self, w: torch.Tensor, bias: torch.Tensor, a: torch.Tensor, rowmax_in: torch.Tensor, act: int = 0,
@@ -620,11 +597,8 @@ class Engine:
         res = self._dev_f32(residual) if residual is not None else None
         add = self._dev_f32(addend) if addend is not None else None
         ptr = lambda t: t.data_ptr() if t is not None else None
-        with self._lock:
-            _lib.check(self._lib.syn_debug_gemm(self._h, w.data_ptr(), bias.data_ptr(), n, k, act, ks, st, pad, hh, ww, cc,
-                                                a.data_ptr(), m, lda, rmi.data_ptr(), ptr(res), ptr(add), addend_group,
-                                                ptr(cm), colmax_group, out.data_ptr(), rmo.data_ptr(), self._stream()))
-            self._done()
+        self._call('syn_debug_gemm', w.data_ptr(), bias.data_ptr(), n, k, act, ks, st, pad, hh, ww, cc, a.data_ptr(), m, lda,
+                   rmi.data_ptr(), ptr(res), ptr(add), addend_group, ptr(cm), colmax_group, out.data_ptr(), rmo.data_ptr())
         return out, rmo, cm
 
     # ---- poisoned workspaces (tests only, include/synergy_b200.h syn_debug_fill_workspaces) ------------------------
@@ -632,22 +606,16 @@ class Engine:
         """Set every byte of every device workspace the handle has grown, at its allocated size, to ``byte``, ordered
         on the current stream after the previous call; returns the number of bytes filled."""
         n = C.c_size_t(0)
-        with self._lock:
-            _lib.check(self._lib.syn_debug_fill_workspaces(self._h, int(byte), C.byref(n), self._stream()))
-            self._done()
+        self._call('syn_debug_fill_workspaces', int(byte), C.byref(n))
         return int(n.value)
 
     def debug_fill_on_grow(self, byte: int) -> None:
         """Every later workspace growth sets its new buffers to ``byte`` (-1: off)."""
-        with self._lock:
-            _lib.check(self._lib.syn_debug_fill_on_grow(self._h, int(byte)))
+        self._call_host('syn_debug_fill_on_grow', int(byte))
 
     def debug_forward_until(self, x: torch.Tensor, layer: int) -> torch.Tensor:
         x = self._check_x(x)
         spec = conv_plan()[layer]
         out = torch.empty((x.shape[0], spec.h_out, spec.h_out, spec.cout), device=self.device, dtype=torch.float32)
-        with self._lock:
-            _lib.check(self._lib.syn_debug_forward_until(self._h, x.data_ptr(), x.shape[0], layer,
-                                                         out.data_ptr(), self._stream()))
-            self._done()
+        self._call('syn_debug_forward_until', x.data_ptr(), x.shape[0], layer, out.data_ptr())
         return out

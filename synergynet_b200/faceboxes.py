@@ -13,14 +13,13 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-import threading
 from typing import Dict, List, Optional
 
 import numpy as np
 import torch
 
 from . import _lib, detect
-from .engine import StreamOrder
+from .engine import Handle
 from .inference import (INTER_LINEAR, ImagePack, chunk_ranges, crop_resize_device, crop_resize_frames_device, crop_resize_images_device,
                         pack_images, stack_frames_device)
 
@@ -65,21 +64,15 @@ def state_dict_keys() -> List[str]:
     return keys
 
 
-class FaceBoxesNet:
+class FaceBoxesNet(Handle):
     """Device-side detector network: one ``syn_fb_t`` handle."""
+    _CREATE, _DESTROY = 'syn_fb_create', 'syn_fb_destroy'
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], device=None):
         self._lib = _lib.load()
         if not torch.cuda.is_available():
             raise RuntimeError('synergynet_b200.faceboxes needs a CUDA device (H100, sm_90a); there is no CPU fallback')
-        self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
-        h = C.c_void_p()
-        _lib.check(self._lib.syn_fb_create(self.device.index or 0, C.byref(h)))
-        self._h = h
-        # the handle is not re-entrant and its calls share one activation workspace: serialise the host threads and order
-        # calls that arrive on different streams, as Engine does
-        self._lock = threading.RLock()
-        self._order = StreamOrder(self.device)
+        super().__init__(torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device))
         sd = {(k[7:] if k.startswith('module.') else k): v for k, v in state_dict.items()}       # utils/functions.py:19-24
         f32 = lambda t: torch.as_tensor(t).detach().to(device='cpu', dtype=torch.float32).contiguous()
         for L in layer_plan():
@@ -94,17 +87,6 @@ class FaceBoxesNet:
                 _lib.check(self._lib.syn_fb_set_layer(self._h, L['index'], w.data_ptr(), w.numel(), b.data_ptr(), None, None, None, None, 0.0))
         _lib.check(self._lib.syn_fb_commit(self._h))
 
-    def close(self):
-        if getattr(self, '_h', None):
-            self._lib.syn_fb_destroy(self._h)
-            self._h = None
-
-    def __del__(self):  # pragma: no cover
-        try:
-            self.close()
-        except Exception:
-            pass
-
     @property
     def launch_count(self) -> int:
         return int(self._lib.syn_fb_launch_count(self._h))
@@ -118,10 +100,7 @@ class FaceBoxesNet:
         p = detect.num_priors(h, w)
         loc = torch.empty((p, 4), dtype=torch.float32, device=self.device)
         conf = torch.empty((p, 2), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device), self._lock:
-            _lib.check(self._lib.syn_fb_forward(self._h, image.data_ptr(), h, w, loc.data_ptr(), conf.data_ptr(),
-                                                self._order.begin()))
-            self._order.end()
+        self._call('syn_fb_forward', image.data_ptr(), h, w, loc.data_ptr(), conf.data_ptr())
         return loc, conf
 
     def debug_fill_workspaces(self, byte: int) -> int:
@@ -129,15 +108,12 @@ class FaceBoxesNet:
         geometry table, ordered on the current stream after the previous call; returns the number of bytes written.
         Poisoned-workspace tests only."""
         n = C.c_size_t(0)
-        with torch.cuda.device(self.device), self._lock:
-            _lib.check(self._lib.syn_fb_debug_fill_workspaces(self._h, int(byte), C.byref(n), self._order.begin()))
-            self._order.end()
+        self._call('syn_fb_debug_fill_workspaces', int(byte), C.byref(n))
         return int(n.value)
 
     def debug_fill_on_grow(self, byte: int) -> None:
         """Every later workspace growth sets its new buffers to ``byte`` (-1: off).  Poisoned-workspace tests only."""
-        with self._lock:
-            _lib.check(self._lib.syn_fb_debug_fill_on_grow(self._h, int(byte)))
+        self._call_host('syn_fb_debug_fill_on_grow', int(byte))
 
     def debug_forward_until(self, image: torch.Tensor, stage: int) -> torch.Tensor:
         """Run :meth:`forward`'s launch sequence up to launch ``stage`` (0..38, table at ``syn_fb_debug_forward_until`` in
@@ -152,11 +128,8 @@ class FaceBoxesNet:
         conf = torch.full((p * 2,), float('nan'), dtype=torch.float32, device=self.device)
         shape = debug_stage_shape(stage, h, w)
         out = torch.empty(shape, dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device), self._lock:
-            _lib.check(self._lib.syn_fb_debug_forward_until(self._h, image.data_ptr(), h, w, stage, out.data_ptr(), out.numel(),
-                                                            loc.data_ptr(), conf.data_ptr(),
-                                                            self._order.begin()))
-            self._order.end()
+        self._call('syn_fb_debug_forward_until', image.data_ptr(), h, w, stage, out.data_ptr(), out.numel(), loc.data_ptr(),
+                   conf.data_ptr())
         return out
 
     def _check_stack(self, images: torch.Tensor):
@@ -174,10 +147,7 @@ class FaceBoxesNet:
         p = detect.num_priors(h, w)
         loc = torch.empty((n, p, 4), dtype=torch.float32, device=self.device)
         conf = torch.empty((n, p, 2), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device), self._lock:
-            _lib.check(self._lib.syn_fb_forward_batch(self._h, images.data_ptr(), n, h, w, loc.data_ptr(), conf.data_ptr(),
-                                                      self._order.begin()))
-            self._order.end()
+        self._call('syn_fb_forward_batch', images.data_ptr(), n, h, w, loc.data_ptr(), conf.data_ptr())
         return loc, conf
 
     def debug_forward_batch_until(self, images: torch.Tensor, stage: int) -> torch.Tensor:
@@ -189,11 +159,8 @@ class FaceBoxesNet:
         loc = torch.full((n, p * 4), float('nan'), dtype=torch.float32, device=self.device)
         conf = torch.full((n, p * 2), float('nan'), dtype=torch.float32, device=self.device)
         out = torch.empty((n,) + tuple(debug_stage_shape(stage, h, w)), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device), self._lock:
-            _lib.check(self._lib.syn_fb_debug_forward_batch_until(self._h, images.data_ptr(), n, h, w, stage, out.data_ptr(),
-                                                                  out.numel(), loc.data_ptr(), conf.data_ptr(),
-                                                                  self._order.begin()))
-            self._order.end()
+        self._call('syn_fb_debug_forward_batch_until', images.data_ptr(), n, h, w, stage, out.data_ptr(), out.numel(),
+                   loc.data_ptr(), conf.data_ptr())
         return out
 
     def _check_images(self, images):
@@ -222,10 +189,8 @@ class FaceBoxesNet:
         loc = torch.empty((p[-1], 4), dtype=torch.float32, device=self.device)
         conf = torch.empty((p[-1], 2), dtype=torch.float32, device=self.device)
         hs, ws = pack.arrays()
-        with torch.cuda.device(self.device), self._lock:
-            _lib.check(self._lib.syn_fb_forward_images(self._h, pack.data.data_ptr(), len(pack), hs.ctypes.data, ws.ctypes.data,
-                                                       loc.data_ptr(), conf.data_ptr(), self._order.begin()))
-            self._order.end()
+        self._call('syn_fb_forward_images', pack.data.data_ptr(), len(pack), hs.ctypes.data, ws.ctypes.data, loc.data_ptr(),
+                   conf.data_ptr())
         return loc, conf, p
 
     def forward_images(self, images):
@@ -245,11 +210,8 @@ class FaceBoxesNet:
         numel = [int(np.prod(sh)) for sh in shapes]
         out = torch.empty((sum(numel),), dtype=torch.float32, device=self.device)
         hs, ws = pack.arrays()
-        with torch.cuda.device(self.device), self._lock:
-            _lib.check(self._lib.syn_fb_debug_forward_images_until(self._h, pack.data.data_ptr(), len(pack), hs.ctypes.data, ws.ctypes.data,
-                                                                   stage, out.data_ptr(), out.numel(), loc.data_ptr(), conf.data_ptr(),
-                                                                   self._order.begin()))
-            self._order.end()
+        self._call('syn_fb_debug_forward_images_until', pack.data.data_ptr(), len(pack), hs.ctypes.data, ws.ctypes.data, stage,
+                   out.data_ptr(), out.numel(), loc.data_ptr(), conf.data_ptr())
         at = np.concatenate([[0], np.cumsum(numel)]).astype(int).tolist()
         return [out[a:b].view(sh) for a, b, sh in zip(at[:-1], at[1:], shapes)]
 

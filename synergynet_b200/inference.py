@@ -84,10 +84,8 @@ def crop_resize_device(image, roi_boxes: Sequence[Sequence[float]], dsize: Tuple
     else:
         out = torch.empty((B, out_h, out_w, 3), dtype=torch.uint8, device=image.device)
         strides = (3 * out_h * out_w, 3 * out_w, 3, 1)
-    with torch.cuda.device(image.device):
-        _lib.check(_lib.load().syn_crop_resize(image.data_ptr(), image.shape[0], image.shape[1], image.shape[2], plan.data_ptr(), B,
-                                               out_h, out_w, interpolation, out.data_ptr(), *strides,
-                                               torch.cuda.current_stream(image.device).cuda_stream))
+    _lib.launch(image.device, 'syn_crop_resize', image.data_ptr(), image.shape[0], image.shape[1], image.shape[2], plan.data_ptr(), B,
+                out_h, out_w, interpolation, out.data_ptr(), *strides)
     return out
 
 
@@ -110,10 +108,8 @@ def crop_resize_frames_device(frames, frame_index: Sequence[int], roi_boxes: Seq
     else:
         out = torch.empty((B, out_h, out_w, 3), dtype=torch.uint8, device=frames.device)
         strides = (3 * out_h * out_w, 3 * out_w, 3, 1)
-    with torch.cuda.device(frames.device):
-        _lib.check(_lib.load().syn_crop_resize_batch(frames.data_ptr(), frames.shape[0], frames.shape[1], frames.shape[2],
-                                                     frames.shape[3], plan.data_ptr(), B, out_h, out_w, interpolation,
-                                                     out.data_ptr(), *strides, torch.cuda.current_stream(frames.device).cuda_stream))
+    _lib.launch(frames.device, 'syn_crop_resize_batch', frames.data_ptr(), frames.shape[0], frames.shape[1], frames.shape[2],
+                frames.shape[3], plan.data_ptr(), B, out_h, out_w, interpolation, out.data_ptr(), *strides)
     return out
 
 
@@ -201,9 +197,8 @@ def crop_resize_images_device(images: ImagePack, image_index: Sequence[int], roi
     dev = images.data.device
     plan = torch.from_numpy(plan).to(dev)
     out = torch.empty((int((3 * out_h.astype(np.int64) * out_w).sum()),), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.syn_crop_resize_images(images.data.data_ptr(), plan.data_ptr(), B, out_h.ctypes.data, out_w.ctypes.data,
-                                              interpolation, int(bool(planar)), out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+    _lib.launch(dev, 'syn_crop_resize_images', images.data.data_ptr(), plan.data_ptr(), B, out_h.ctypes.data, out_w.ctypes.data,
+                interpolation, int(bool(planar)), out.data_ptr())
     if not one:
         return out
     w, h = dsizes[0]
@@ -383,12 +378,9 @@ def draw_lines_device(images, seg_lists, thickness: int = AXIS_THICKNESS):
     buf, (a, b), n_segs, start = _segment_table(seg_lists, frames)
     if n_segs == 0:
         return images
-    dev = data.device
-    table = torch.from_numpy(buf).to(dev)
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().syn_draw_lines(data.data_ptr(), data.numel(), frames.ctypes.data, table.data_ptr(), len(sizes),
-                                              start.ctypes.data, table[a:b].data_ptr(), table[b:].data_ptr(), n_segs, int(thickness),
-                                              8, torch.cuda.current_stream(dev).cuda_stream))
+    table = torch.from_numpy(buf).to(data.device)
+    _lib.launch(data.device, 'syn_draw_lines', data.data_ptr(), data.numel(), frames.ctypes.data, table.data_ptr(), len(sizes),
+                start.ctypes.data, table[a:b].data_ptr(), table[b:].data_ptr(), n_segs, int(thickness), 8)
     return images
 
 
@@ -513,20 +505,15 @@ class ObjEncoder:
             self.launches += n
 
     def plan(self, desc, ws, offsets) -> None:
-        import torch
         from . import _lib
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().syn_obj_plan(C.byref(desc), ws.data_ptr(), ws.numel() * 8, offsets.data_ptr(),
-                                                torch.cuda.current_stream(self.device).cuda_stream))
+        _lib.launch(self.device, 'syn_obj_plan', C.byref(desc), ws.data_ptr(), ws.numel() * 8, offsets.data_ptr())
         n_lines = desc.n_keep if desc.keep_host else desc.nver
         self._launched(2 if n_lines or desc.ntri else 1)
 
     def write(self, desc, ws, offsets, out) -> None:
-        import torch
         from . import _lib
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().syn_obj_write(C.byref(desc), ws.data_ptr(), ws.numel() * 8, offsets.data_ptr(), out.data_ptr(),
-                                                 out.numel(), torch.cuda.current_stream(self.device).cuda_stream))
+        _lib.launch(self.device, 'syn_obj_write', C.byref(desc), ws.data_ptr(), ws.numel() * 8, offsets.data_ptr(), out.data_ptr(),
+                    out.numel())
         n_lines = desc.n_keep if desc.keep_host else desc.nver
         self._launched((1 if n_lines or desc.ntri else 0) + (1 if desc.batch > 1 and desc.ntri else 0))
 
