@@ -282,6 +282,14 @@ int syn_mesh_normals(const float* vertices_dev, int64_t stride_mesh, int stride_
 int syn_mesh_lighting(const float* vertices_dev, int64_t stride_mesh, int stride_vertex, int stride_coord, int batch, int nver,
                       const float* normals_dev, const syn_light_cfg_t* cfg, const float* texture_dev, uint32_t* stats_ws_dev,
                       float* colors_dev, void* stream);
+/* syn_mesh_lighting with one texture per mesh: mesh b's colours are its light times the (nver,3) float32 texture at
+ * texture_dev + b * texture_stride_mesh.  A stride of 0 shares one texture, with the bits of syn_mesh_lighting; otherwise
+ * the stride is at least 3 * nver.  The (B,nver,3) textures syn_uv_sample writes take stride 3 * nver (artistic.py and
+ * uv_texture_realFaces.py light each face with its own UV colours).  SYN_ERR_INVALID for a NULL texture or a stride
+ * outside those values, and the refusals of syn_mesh_lighting, before any launch. */
+int syn_mesh_lighting_textures(const float* vertices_dev, int64_t stride_mesh, int stride_vertex, int stride_coord, int batch,
+                               int nver, const float* normals_dev, const syn_light_cfg_t* cfg, const float* texture_dev,
+                               int64_t texture_stride_mesh, uint32_t* stats_ws_dev, float* colors_dev, void* stream);
 /* Sim3DR.rasterize (Sim3DR/Sim3DR.py:14-29 -> rasterize_kernel.cpp:217-287): draws the B meshes, in order, onto
  * image_dev (height,width,channels) uint8, each with its own depth buffer as the reference's per-face calls have
  * (utils/render.py:41-45).  colors_dev (B,nver,channels).  alpha must be 1 (the only value the reference's Python
@@ -364,6 +372,23 @@ int syn_add_weighted_u8(const uint8_t* a_dev, const uint8_t* b_dev, double alpha
 int syn_draw_lines(uint8_t* images_dev, int64_t image_bytes, const int64_t* frames_host, const int64_t* frames_dev, int n_frames,
                    const int32_t* seg_start_host, const int32_t* seg_start_dev, const int32_t* segs_dev, int n_segs, int thickness,
                    int line_type, void* stream);
+/* The UV colours of artistic.py:126-131 / uv_texture_realFaces.py:103-114 for n_faces faces, each with its own map:
+ * colors_uv = np.flip(map, 0)[coord_u, coord_v][keep], as float32 / 255 (the texture the overlay lights) and as the
+ * bytes themselves (the int64 colour rows syn_obj_write prints with colors_dot0 = 1, "233.0").
+ *   maps_dev: map_bytes uint8; map m is (h, w, 3) at byte offset off of the map table (n_maps,3) int64 (off, h, w), given
+ *     as maps_host (checked here) and maps_table_dev (its device copy, which the kernel reads): the layout of the image
+ *     tables of syn_draw_lines and syn_rasterize_images.
+ *   texels_host / texels_dev (n_maps, n_keep, 2) int32: the (row, column) of the UNFLIPPED map m that kept vertex i reads,
+ *     resolved on the host (the flip and numpy's negative-index wrap included); texels_dev 8-byte aligned.
+ *   face_map_host / face_map_dev (n_faces) int32: the map of each face.
+ *   texture_dev (n_faces, n_keep, 3) float32 and colors_dev (n_faces, n_keep, 3) int64; either may be NULL, not both.
+ * SYN_ERR_INVALID for a null pointer, a misaligned texels_dev, or counts outside 1..65535 faces, >= 1 map and kept
+ * vertex; SYN_ERR_SHAPE for a map table that is out of order, overlaps or does not fit the map bytes, a texel outside
+ * its map, or a face naming no map; all before the one launch.  No allocation and no synchronisation (graph capture is
+ * fine); host arrays are read during the call only. */
+int syn_uv_sample(const uint8_t* maps_dev, int64_t map_bytes, const int64_t* maps_host, const int64_t* maps_table_dev, int n_maps,
+                  const int32_t* texels_host, const int32_t* texels_dev, int n_keep, const int32_t* face_map_host,
+                  const int32_t* face_map_dev, int n_faces, float* texture_dev, int64_t* colors_dev, void* stream);
 
 /* ---- OBJ text of dense meshes (utils/inference.py:8-23 write_obj; artistic.py:19-31 and uv_texture_realFaces.py:21-33
  * write_obj_with_colors) -------------------------------------------------------------------------------------------

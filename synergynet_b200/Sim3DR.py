@@ -80,21 +80,30 @@ class MeshRenderer:
 
     def colors(self, vertices: torch.Tensor, normals: torch.Tensor, cfg: Optional[_lib.LightCfg] = None,
                texture: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Per-vertex light of ``RenderPipeline.__call__`` (times ``texture`` (nver,3) if given): (B,nver,3) in [0,1]."""
+        """Per-vertex light of ``RenderPipeline.__call__``, times ``texture`` if given -- (nver,3) for every mesh, or
+        (B,nver,3), one texture per mesh (``syn_mesh_lighting_textures``): (B,nver,3) in [0,1]."""
         v, view = self._view(vertices)
         b = view[4]
         cfg = cfg or _light_cfg()
         normals = normals.contiguous()
         if tuple(normals.shape) != (b, self.nver, 3) or normals.dtype != torch.float32 or normals.device != self.device:
             raise ValueError('normals must be float32 (B,nver,3) on the renderer device')
+        stats = torch.empty((b, 6), dtype=torch.int32, device=self.device)
+        out = torch.empty((b, self.nver, 3), dtype=torch.float32, device=self.device)
+        if texture is not None and texture.dim() == 3:
+            texture = texture.to(device=self.device, dtype=torch.float32).contiguous()
+            if tuple(texture.shape) != (b, self.nver, 3):
+                raise ValueError(f'texture must be (nver, 3) or (B, nver, 3) = ({b}, {self.nver}, 3), got {tuple(texture.shape)}')
+            _lib.launch(self.device, 'syn_mesh_lighting_textures', *view, normals.data_ptr(), C.byref(cfg), texture.data_ptr(),
+                        3 * self.nver, stats.data_ptr(), out.data_ptr())
+            self.launches += 2
+            return out
         tex_ptr = None
         if texture is not None:
             texture = texture.to(device=self.device, dtype=torch.float32).contiguous()
             if tuple(texture.shape) != (self.nver, 3):
                 raise ValueError('texture must be (nver, 3)')
             tex_ptr = texture.data_ptr()
-        stats = torch.empty((b, 6), dtype=torch.int32, device=self.device)
-        out = torch.empty((b, self.nver, 3), dtype=torch.float32, device=self.device)
         _lib.launch(self.device, 'syn_mesh_lighting', *view, normals.data_ptr(), C.byref(cfg), tex_ptr, stats.data_ptr(),
                     out.data_ptr())
         self.launches += 2

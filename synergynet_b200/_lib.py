@@ -112,6 +112,7 @@ SIGNATURES = {
     'syn_mesh_incidence_host': (_I, [_F, _I, _I, _F, _F]),
     'syn_mesh_normals': (_I, [_F, _L, _I, _I, _I, _I, _F, _I, _F, _F, _F, _F, _P]),
     'syn_mesh_lighting': (_I, [_F, _L, _I, _I, _I, _I, _F, C.POINTER(LightCfg), _F, _F, _F, _P]),
+    'syn_mesh_lighting_textures': (_I, [_F, _L, _I, _I, _I, _I, _F, C.POINTER(LightCfg), _F, _L, _F, _F, _P]),
     'syn_rasterize': (_I, [_F, _I, _I, _I, _F, _L, _I, _I, _I, _I, _F, _I, _F, C.c_float, _I, _F, _F, _P]),
     'syn_render_frames_plan': (_I, [_F, _L, _I, _I, _I, _I, _F, _I, _P, _I, _I, _I, _F, _F, _P]),
     'syn_rasterize_frames': (_I, [_F, _F, _I, _I, _I, _I, _F, _L, _I, _I, _I, _I, _F, _I, _F, _I, _P, _F, _F, _F, _L, _F, _L, _P]),
@@ -119,6 +120,7 @@ SIGNATURES = {
     'syn_rasterize_images': (_I, [_F, _F, _L, _P, _F, _I, _I, _F, _L, _I, _I, _I, _I, _F, _I, _F, _I, _P, _F, _F, _F, _L, _F, _L, _P]),
     'syn_add_weighted_u8': (_I, [_F, _F, C.c_double, _F, _L, _P]),
     'syn_draw_lines': (_I, [_F, _L, _P, _F, _I, _P, _F, _F, _I, _I, _I, _P]),
+    'syn_uv_sample': (_I, [_F, _L, _P, _F, _I, _P, _F, _I, _P, _F, _I, _F, _F, _P]),
     'syn_obj_workspace_size': (_L, [_I, _I, _I]),
     'syn_obj_plan': (_I, [C.POINTER(ObjDesc), _F, _L, _F, _P]),
     'syn_obj_write': (_I, [C.POINTER(ObjDesc), _F, _L, _F, _F, _L, _P]),
@@ -184,6 +186,7 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_add_weighted_u8', 'syn_fb_forward_images', 'syn_fb_debug_forward_images_until',
                                              'syn_faceboxes_decode_images', 'syn_crop_resize_images_plan_size',
                                              'syn_crop_resize_plan_images_host', 'syn_crop_resize_images', 'syn_draw_lines',
+                                             'syn_mesh_lighting_textures', 'syn_uv_sample',
                                              'syn_obj_workspace_size', 'syn_obj_plan', 'syn_obj_write',
                                              'syn_debug_fill_workspaces', 'syn_debug_fill_on_grow',
                                              'syn_fb_debug_fill_workspaces', 'syn_fb_debug_fill_on_grow')}

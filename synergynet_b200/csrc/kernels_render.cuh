@@ -110,9 +110,10 @@ __global__ void mesh_extent_kernel(MeshView m, unsigned* __restrict__ stats) {
   }
 }
 
-// light[b][i][0..2] (Sim3DR/lighting.py:37-66); with a texture (nver,3): colours = texture * light (:74)
+// light[b][i][0..2] (Sim3DR/lighting.py:37-66); with a texture: colours = texture * light (:74), mesh b's texture row i
+// at texture + b * tb + 3 i (tb = 0: one (nver,3) texture for every mesh)
 __global__ void vertex_light_kernel(MeshView m, const float* __restrict__ normals, const unsigned* __restrict__ stats,
-                                    rmath::LightCfg cfg, const float* __restrict__ texture, float* __restrict__ out) {
+                                    rmath::LightCfg cfg, const float* __restrict__ texture, long long tb, float* __restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
   if (i >= m.nver) return;
   rmath::NormStats s;
@@ -128,7 +129,7 @@ __global__ void vertex_light_kernel(MeshView m, const float* __restrict__ normal
   rmath::vertex_light(p, nn, s, cfg, l);
   float* o = out + ((size_t)b * m.nver + i) * 3;
 #pragma unroll
-  for (int k = 0; k < 3; ++k) o[k] = texture ? rmath::mul(__ldg(texture + (size_t)i * 3 + k), l[k]) : l[k];
+  for (int k = 0; k < 3; ++k) o[k] = texture ? rmath::mul(__ldg(texture + (size_t)b * tb + (size_t)i * 3 + k), l[k]) : l[k];
 }
 
 // ---- rasterisation -------------------------------------------------------------------------------------------------

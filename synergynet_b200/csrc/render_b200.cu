@@ -7,6 +7,7 @@
 #include "kernels_resize.cuh"
 #include "kernels_draw.cuh"
 #include "kernels_obj.cuh"
+#include "kernels_uv.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -134,6 +135,35 @@ int decode_launch(const float* loc, const float* conf, const FbDecodeFrames& t, 
   return SYN_OK;
 }
 
+// both lighting entries: texture_dev NULL (light only), or mesh b's (nver,3) texture at texture_dev + b * tb
+int mesh_lighting(const float* vertices_dev, int64_t stride_mesh, int stride_vertex, int stride_coord, int batch, int nver,
+                  const float* normals_dev, const syn_light_cfg_t* cfg, const float* texture_dev, int64_t tb, uint32_t* stats_ws_dev,
+                  float* colors_dev, void* stream, const char* who) {
+  MeshView m;
+  if (int rc = check_mesh(vertices_dev, stride_mesh, stride_vertex, stride_coord, batch, nver, m)) return rc;
+  if (!normals_dev || !cfg || !stats_ws_dev || !colors_dev) return fail(SYN_ERR_INVALID, "%s: null pointer", who);
+  rmath::LightCfg c;
+  c.intensity_ambient = cfg->intensity_ambient;
+  c.intensity_directional = cfg->intensity_directional;
+  c.intensity_specular = cfg->intensity_specular;
+  c.specular_exp = cfg->specular_exp;
+  for (int k = 0; k < 3; ++k) {
+    c.color_ambient[k] = cfg->color_ambient[k];
+    c.color_directional[k] = cfg->color_directional[k];
+    c.light_pos[k] = cfg->light_pos[k];
+    c.view_pos[k] = cfg->view_pos[k];
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  SYN_CUDA(cudaMemsetAsync(stats_ws_dev, 0, sizeof(uint32_t) * 6 * batch, st));
+  const int blocks = min((nver + 255) / 256, 64);
+  mesh_extent_kernel<<<dim3(blocks, batch), 256, 0, st>>>(m, stats_ws_dev);
+  SYN_LAUNCH_CHECK("mesh_extent_kernel");
+  vertex_light_kernel<<<dim3((nver + 255) / 256, batch), 256, 0, st>>>(m, normals_dev, stats_ws_dev, c, texture_dev, (long long)tb,
+                                                                        colors_dev);
+  SYN_LAUNCH_CHECK("vertex_light_kernel");
+  return SYN_OK;
+}
+
 int64_t obj_blocks(int n) { return ((int64_t)n + kObjThreads - 1) / kObjThreads; }
 
 // the shared checks of the two OBJ entries; fills the kernels' arguments
@@ -205,28 +235,19 @@ int syn_mesh_normals(const float* vertices_dev, int64_t stride_mesh, int stride_
 int syn_mesh_lighting(const float* vertices_dev, int64_t stride_mesh, int stride_vertex, int stride_coord, int batch, int nver,
                       const float* normals_dev, const syn_light_cfg_t* cfg, const float* texture_dev, uint32_t* stats_ws_dev,
                       float* colors_dev, void* stream) {
-  MeshView m;
-  if (int rc = check_mesh(vertices_dev, stride_mesh, stride_vertex, stride_coord, batch, nver, m)) return rc;
-  if (!normals_dev || !cfg || !stats_ws_dev || !colors_dev) return fail(SYN_ERR_INVALID, "syn_mesh_lighting: null pointer");
-  rmath::LightCfg c;
-  c.intensity_ambient = cfg->intensity_ambient;
-  c.intensity_directional = cfg->intensity_directional;
-  c.intensity_specular = cfg->intensity_specular;
-  c.specular_exp = cfg->specular_exp;
-  for (int k = 0; k < 3; ++k) {
-    c.color_ambient[k] = cfg->color_ambient[k];
-    c.color_directional[k] = cfg->color_directional[k];
-    c.light_pos[k] = cfg->light_pos[k];
-    c.view_pos[k] = cfg->view_pos[k];
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  SYN_CUDA(cudaMemsetAsync(stats_ws_dev, 0, sizeof(uint32_t) * 6 * batch, st));
-  const int blocks = min((nver + 255) / 256, 64);
-  mesh_extent_kernel<<<dim3(blocks, batch), 256, 0, st>>>(m, stats_ws_dev);
-  SYN_LAUNCH_CHECK("mesh_extent_kernel");
-  vertex_light_kernel<<<dim3((nver + 255) / 256, batch), 256, 0, st>>>(m, normals_dev, stats_ws_dev, c, texture_dev, colors_dev);
-  SYN_LAUNCH_CHECK("vertex_light_kernel");
-  return SYN_OK;
+  return mesh_lighting(vertices_dev, stride_mesh, stride_vertex, stride_coord, batch, nver, normals_dev, cfg, texture_dev, 0,
+                       stats_ws_dev, colors_dev, stream, "syn_mesh_lighting");
+}
+
+int syn_mesh_lighting_textures(const float* vertices_dev, int64_t stride_mesh, int stride_vertex, int stride_coord, int batch,
+                               int nver, const float* normals_dev, const syn_light_cfg_t* cfg, const float* texture_dev,
+                               int64_t texture_stride_mesh, uint32_t* stats_ws_dev, float* colors_dev, void* stream) {
+  const char* who = "syn_mesh_lighting_textures";
+  if (!texture_dev) return fail(SYN_ERR_INVALID, "%s: null texture", who);
+  if (texture_stride_mesh < 0 || (texture_stride_mesh > 0 && texture_stride_mesh < 3LL * nver))
+    return fail(SYN_ERR_INVALID, "%s: texture mesh stride %lld (0, or at least 3 * %d)", who, (long long)texture_stride_mesh, nver);
+  return mesh_lighting(vertices_dev, stride_mesh, stride_vertex, stride_coord, batch, nver, normals_dev, cfg, texture_dev,
+                       texture_stride_mesh, stats_ws_dev, colors_dev, stream, who);
 }
 
 int syn_rasterize(uint8_t* image_dev, int height, int width, int channels, const float* vertices_dev, int64_t stride_mesh,
@@ -415,6 +436,42 @@ int syn_draw_lines(uint8_t* images_dev, int64_t image_bytes, const int64_t* fram
   draw_lines_kernel<<<n_frames, kDrawThreads, 0, (cudaStream_t)stream>>>(images_dev, reinterpret_cast<const long long*>(frames_dev),
                                                                        seg_start_dev, segs_dev);
   SYN_LAUNCH_CHECK("draw_lines_kernel");
+  return SYN_OK;
+}
+
+int syn_uv_sample(const uint8_t* maps_dev, int64_t map_bytes, const int64_t* maps_host, const int64_t* maps_table_dev, int n_maps,
+                  const int32_t* texels_host, const int32_t* texels_dev, int n_keep, const int32_t* face_map_host,
+                  const int32_t* face_map_dev, int n_faces, float* texture_dev, int64_t* colors_dev, void* stream) {
+  const char* who = "syn_uv_sample";
+  if (!maps_dev || !maps_host || !maps_table_dev || !texels_host || !texels_dev || !face_map_host || !face_map_dev ||
+      (!texture_dev && !colors_dev))
+    return fail(SYN_ERR_INVALID, "%s: null pointer", who);
+  if (reinterpret_cast<uintptr_t>(texels_dev) % 8)
+    return fail(SYN_ERR_INVALID, "%s: texels_dev is not 8-byte aligned", who);
+  if (n_maps < 1 || n_keep < 1 || n_faces < 1 || n_faces > 65535 || map_bytes < 0)
+    return fail(SYN_ERR_INVALID, "%s: %d maps, %d kept vertices, %d faces (1..65535), %lld map bytes", who, n_maps, n_keep, n_faces,
+                (long long)map_bytes);
+  int64_t end = 0;                                   // the maps in memory order, disjoint, inside the map bytes
+  for (int m = 0; m < n_maps; ++m) {
+    const int64_t off = maps_host[3 * m], h = maps_host[3 * m + 1], w = maps_host[3 * m + 2];
+    if (h < 1 || w < 1 || h > INT32_MAX || w > INT32_MAX) return fail(SYN_ERR_SHAPE, "%s: map %d is %lldx%lld", who, m, (long long)h, (long long)w);
+    if (off < end || off > map_bytes || h > (map_bytes - off) / 3 / w)
+      return fail(SYN_ERR_SHAPE, "%s: map %d (%lldx%lld at byte %lld) does not fit the %lld map bytes after the map before it", who, m,
+                  (long long)h, (long long)w, (long long)off, (long long)map_bytes);
+    end = off + 3 * h * w;
+    const int32_t* t = texels_host + 2 * (int64_t)m * n_keep;
+    for (int i = 0; i < n_keep; ++i)
+      if (t[2 * i] < 0 || t[2 * i] >= h || t[2 * i + 1] < 0 || t[2 * i + 1] >= w)
+        return fail(SYN_ERR_SHAPE, "%s: texel %d of map %d is (%d, %d), outside its %lldx%lld", who, i, m, t[2 * i], t[2 * i + 1],
+                    (long long)h, (long long)w);
+  }
+  for (int f = 0; f < n_faces; ++f)
+    if (face_map_host[f] < 0 || face_map_host[f] >= n_maps)
+      return fail(SYN_ERR_SHAPE, "%s: face %d names map %d of %d", who, f, face_map_host[f], n_maps);
+  uv_sample_kernel<<<dim3((n_keep + kUvThreads - 1) / kUvThreads, n_faces), kUvThreads, 0, (cudaStream_t)stream>>>(
+      maps_dev, reinterpret_cast<const long long*>(maps_table_dev), texels_dev, n_keep, face_map_dev, texture_dev,
+      reinterpret_cast<long long*>(colors_dev));
+  SYN_LAUNCH_CHECK("uv_sample_kernel");
   return SYN_OK;
 }
 

@@ -572,8 +572,10 @@ class ObjTables:
             self._dev = (device, up(self.tri), up(self.keep), up(self.colors))
         return self._dev[1:]
 
-    def desc(self, vertices, m0: int, device):
-        """The syn_obj_desc_t of the (B,3,N) device meshes ``vertices``, meshes m0.. of the call."""
+    def desc(self, vertices, m0: int, device, colors_dev=None):
+        """The syn_obj_desc_t of the (B,3,N) device meshes ``vertices``, meshes m0.. of the call.  ``colors_dev``: the
+        meshes' own (B,n,3) int64 colour rows on the device, printed as integral floats, in place of the tables' colours."""
+        import torch
         from . import _lib
         tri, keep, col = self.upload(device)
         b, _, n = (int(s) for s in vertices.shape)
@@ -588,20 +590,28 @@ class ObjTables:
             shared = col.shape[0] == 1
             d.colors = col.data_ptr() if shared else col[m0].data_ptr()
             d.colors_stride_mesh, d.colors_dot0 = 0 if shared else 3 * self.n_lines, self.colors_dot0
+        if colors_dev is not None:
+            if colors_dev.dtype != torch.int64 or tuple(colors_dev.shape) != (b, self.n_lines, 3) or not colors_dev.is_contiguous() \
+                    or colors_dev.device != vertices.device:
+                raise ValueError(f'colors_dev must be contiguous int64 ({b}, {self.n_lines}, 3) on the meshes\' device')
+            d.colors, d.colors_stride_mesh, d.colors_dot0 = colors_dev.data_ptr(), 3 * self.n_lines, 1
         d.triangles, d.ntri, d.tri_dot0 = tri.data_ptr() if tri.numel() else None, int(self.tri.shape[0]), self.tri_dot0
-        d.tri_order = 0 if self.colors is None else 1
+        d.tri_order = 0 if self.colors is None and colors_dev is None else 1
         return d
 
-    def encode(self, vertices, m0: int = 0, chunk_bytes: int = OBJ_CHUNK_BYTES) -> list:
+    def encode(self, vertices, m0: int = 0, chunk_bytes: int = OBJ_CHUNK_BYTES, colors_dev=None) -> list:
         """The OBJ texts of the (B,3,N) CUDA meshes ``vertices`` (meshes m0.. of the call), as a list of B ``bytes``:
-        plan, one read of the offsets, write and one download per chunk of about ``chunk_bytes`` of text."""
+        plan, one read of the offsets, write and one download per chunk of about ``chunk_bytes`` of text.  ``colors_dev``
+        (B,n,3) int64 on the device: each mesh's colours, written as ``write_obj_with_colors`` writes float32 colours of
+        uint8 values ("233.0")."""
         import torch
         dev = vertices.device
         enc = obj_encoder(dev)
-        per_mesh = 40 * self.n_lines + (32 if self.colors is not None else 0) * self.n_lines + 24 * int(self.tri.shape[0]) + 1
+        coloured = self.colors is not None or colors_dev is not None
+        per_mesh = 40 * self.n_lines + (32 if coloured else 0) * self.n_lines + 24 * int(self.tri.shape[0]) + 1
         out = []
         for a, b in chunk_ranges(int(vertices.shape[0]), min(OBJ_MAX_MESHES, max(1, chunk_bytes // per_mesh))):
-            d = self.desc(vertices[a:b], m0 + a, dev)
+            d = self.desc(vertices[a:b], m0 + a, dev, None if colors_dev is None else colors_dev[a:b])
             ws = enc.workspace(b - a, self.n_lines, d.ntri)
             offsets = torch.empty(b - a + 1, dtype=torch.int64, device=dev)
             enc.plan(d, ws, offsets)
@@ -643,3 +653,135 @@ def write_obj_with_colors(obj_name, vertices, triangles, colors):
     text = obj_bytes(vertices, triangles, colors)[0]
     with open(obj_file_name(obj_name), 'wb') as f:
         f.write(text)
+
+
+# ---- UV textures (artistic.py:49-53,126-131; uv_texture_realFaces.py:47-51,103-114) ---------------------------------------
+class UVLayout:
+    """The UV layout of the textured flows: ``BFM_UV.npy`` (nver, >=2) UV coordinates, ``keptInd.npy`` the kept vertices
+    and ``deletedTri.npy`` the (3, ntri) 1-based triangles over them.  The texel coordinates are numpy's, in the array's
+    own dtype, as the scripts compute them: ``coord_u = (uv[:,1]*255.0).astype(np.int32)`` (row) and ``coord_v =
+    (uv[:,0]*255.0).astype(np.int32)`` (column).  Every refusal happens here or in :meth:`texels`, before any CUDA call."""
+
+    def __init__(self, bfm_uv, keep, deleted_tri):
+        uv = np.asarray(bfm_uv)
+        if uv.ndim != 2 or uv.shape[1] < 2 or uv.shape[0] < 1 or uv.dtype.kind != 'f':
+            raise ValueError(f'BFM_UV must be a float (nver, 2) array, got {uv.dtype} {uv.shape}')
+        with np.errstate(invalid='ignore', over='ignore'):
+            self.coord_u = (uv[:, 1] * 255.0).astype(np.int32)
+            self.coord_v = (uv[:, 0] * 255.0).astype(np.int32)
+        self.nver = int(uv.shape[0])
+        k = np.asarray(keep)
+        if k.ndim != 1 or k.dtype.kind not in 'iu' or k.size < 1:
+            raise ValueError(f'keptInd must be a non-empty 1-d integer array, got {k.dtype} {k.shape}')
+        bad = np.argwhere((k < 0) | (k >= self.nver))
+        if bad.size:
+            raise ValueError(f'keptInd[{int(bad[0, 0])}] = {int(k[bad[0, 0]])} lies outside [0, {self.nver})')
+        self.keep = np.ascontiguousarray(k, dtype=np.int64)
+        self.n_keep = int(k.size)
+        tri = np.asarray(deleted_tri)
+        if tri.ndim != 2 or tri.shape[0] != 3 or tri.shape[1] < 1 or tri.dtype.kind not in 'iu':
+            raise ValueError(f'deletedTri must be a (3, ntri) integer array, got {tri.dtype} {tri.shape}')
+        bad = np.argwhere((tri < 1) | (tri > self.n_keep))
+        if bad.size:
+            i, j = (int(x) for x in bad[0])
+            raise ValueError(f'deletedTri[{i}, {j}] - 1 = {int(tri[i, j]) - 1} lies outside [0, {self.n_keep}) kept vertices')
+        self.deleted_tri = tri                                               # written as given by write_obj_with_colors
+        self.render_tri = np.ascontiguousarray((tri.astype(np.int64) - 1).T, dtype=np.int32)   # connectivity=deletedTri-1, (ntri,3)
+        self._texels = {}
+
+    @classmethod
+    def load(cls, directory: str) -> 'UVLayout':
+        """The layout of a ``3dmm_data`` directory: ``BFM_UV.npy``, ``keptInd.npy``, ``deletedTri.npy``."""
+        import os
+        return cls(*(np.load(os.path.join(directory, f)) for f in ('BFM_UV.npy', 'keptInd.npy', 'deletedTri.npy')))
+
+    def texels(self, h: int, w: int, what: str = 'the UV map') -> np.ndarray:
+        """(n_keep, 2) int32 (row, column) of the unflipped (h, w) map that ``np.flip(map, 0)[coord_u, coord_v][keep]``
+        reads: row r in [-h, h) is row ``h-1-(r mod h)``, column c in [-w, w) is column ``c mod w``.  As the reference
+        indexes every vertex before it applies ``keep``, a coordinate outside those ranges raises ``IndexError`` for any
+        vertex, kept or not, naming it and ``what``."""
+        key = (int(h), int(w))
+        if key not in self._texels:
+            h, w = key
+            for axis, c, n in ((0, self.coord_u, h), (1, self.coord_v, w)):
+                bad = np.argwhere((c < -n) | (c >= n))
+                if bad.size:
+                    i = int(bad[0, 0])
+                    raise IndexError(f'vertex {i}: index {int(c[i])} is out of bounds for axis {axis} with size {n} of {what} '
+                                     f'({h}x{w})')
+            rows = h - 1 - np.mod(self.coord_u[self.keep].astype(np.int64), h)
+            cols = np.mod(self.coord_v[self.keep].astype(np.int64), w)
+            self._texels[key] = np.ascontiguousarray(np.stack([rows, cols], 1), dtype=np.int32)
+        return self._texels[key]
+
+
+def uv_maps_host(maps, n_images: int, overlay: bool) -> list:
+    """The UV maps of a call as a list of (h, w, 3) uint8 host arrays, one per image (``maps``: one (h, w, 3|4) map per
+    image, or one map for all of them).  A 4-channel map keeps channels 0..2, all that ``write_obj_with_colors`` prints;
+    the overlay refuses it, as the reference's ``texture *= light`` cannot broadcast it.  Grayscale and non-uint8 maps
+    raise ValueError."""
+    def host(m):
+        m = m.cpu().numpy() if hasattr(m, 'cpu') else np.asarray(m)
+        if m.dtype != np.uint8:
+            raise ValueError(f'UV maps must be uint8 (what cv2.imread(path, -1) gives for an 8-bit PNG), got {m.dtype}')
+        if m.ndim != 3 or m.shape[2] not in (3, 4) or m.shape[0] < 1 or m.shape[1] < 1:
+            raise ValueError(f'UV maps must be (h, w, 3) or (h, w, 4) colour images, got {m.shape}')
+        if m.shape[2] == 4:
+            if overlay:
+                raise ValueError('a 4-channel UV map cannot texture the overlay: the reference\'s `texture *= light` does not '
+                                 'broadcast (n, 4) against (n, 3)')
+            m = m[:, :, :3]
+        return np.ascontiguousarray(m)
+    one = (hasattr(maps, 'ndim') and maps.ndim == 3) or (hasattr(maps, 'shape') and len(maps.shape) == 3)
+    maps = [host(maps)] if one else [host(m) for m in maps]
+    if len(maps) != n_images and len(maps) != 1:
+        raise ValueError(f'{len(maps)} UV maps for {n_images} images: give one map per image, or one for all of them')
+    return maps
+
+
+class UVMaps:
+    """UV maps on one device and the texels of a :class:`UVLayout` resolved for each of their sizes, uploaded in one copy:
+    :meth:`sample` gives the textures and colours of ``syn_uv_sample`` for faces a..b-1, face f reading map
+    ``face_map[f]``."""
+
+    def __init__(self, layout: UVLayout, maps, face_map, device):
+        import torch
+        self.layout, self.device = layout, torch.device(device)
+        self.face_map = np.ascontiguousarray(face_map, dtype=np.int32).reshape(-1)
+        n = len(maps)
+        if self.face_map.size and (self.face_map.min() < 0 or self.face_map.max() >= n):
+            raise ValueError(f'face_map names maps outside [0, {n})')
+        self.texels = np.ascontiguousarray(np.stack([layout.texels(m.shape[0], m.shape[1], f'UV map {i}') for i, m in enumerate(maps)]))
+        sizes = [3 * m.shape[0] * m.shape[1] for m in maps]
+        offs = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        self.table = np.array([[offs[i], m.shape[0], m.shape[1]] for i, m in enumerate(maps)], np.int64).reshape(n, 3)
+        self.n_maps, self.map_bytes = n, int(offs[-1])
+        # one int64 buffer: table (n,3) | texels (n, n_keep, 2) int32 | face_map int32 | the map bytes
+        a = 3 * n
+        b = a + self.texels.size // 2
+        c = b + (self.face_map.size + 1) // 2
+        buf = np.zeros(c + (self.map_bytes + 7) // 8, np.int64)
+        buf[:a] = self.table.reshape(-1)
+        buf[a:b].view(np.int32)[:] = self.texels.reshape(-1)
+        buf[b:c].view(np.int32)[:self.face_map.size] = self.face_map
+        buf[c:].view(np.uint8)[:self.map_bytes] = np.concatenate([m.reshape(-1) for m in maps])
+        self.dev = torch.from_numpy(buf).to(self.device)
+        self._parts = (a, b, c)
+        self.launches = 0
+
+    def sample(self, a: int, b: int, texture: bool = True, colors: bool = False):
+        """``(texture, colors)`` of faces a..b-1: float32 (b-a, n_keep, 3) ``colors_uv[keep] / 255`` and int64 (b-a, n_keep,
+        3) ``colors_uv[keep]``, each None unless asked for."""
+        import torch
+        from . import _lib
+        pa, pb, pc = self._parts
+        k = self.layout.n_keep
+        tex = torch.empty((b - a, k, 3), dtype=torch.float32, device=self.device) if texture else None
+        col = torch.empty((b - a, k, 3), dtype=torch.int64, device=self.device) if colors else None
+        fm = np.ascontiguousarray(self.face_map[a:b])
+        fm_dev = self.dev[pb:].view(torch.int32)[a:b]
+        _lib.launch(self.device, 'syn_uv_sample', self.dev[pc:].data_ptr(), self.map_bytes, self.table.ctypes.data,
+                    self.dev.data_ptr(), self.n_maps, self.texels.ctypes.data, self.dev[pa:].data_ptr(), k, fm.ctypes.data,
+                    fm_dev.data_ptr(), b - a, None if tex is None else tex.data_ptr(), None if col is None else col.data_ptr())
+        self.launches += 1
+        return tex, col

@@ -410,16 +410,19 @@ class _SynergyBase(nn.Module):
         per_chunk = max(1, self.dense_chunk_bytes // (3 * 4 * max(eng.n_vert, 1)))
         return chunk_ranges(n_faces, per_chunk)
 
-    def _frames_front(self, frames, rects, ragged: bool = False):
+    def _frames_front(self, frames, rects, ragged: bool = False, rois=None):
         """The stages of :meth:`get_all_outputs_batch` up to the parameters, on the device: ``(engine, frame stack, faces
         per frame, frame of each face, whitened params (F,62), crop -> image maps (F,5))``; the last two are None when no
         frame has a face.  ``ragged``: ``frames`` is a list of images of any sizes (:meth:`get_all_outputs_images`) and
-        the "stack" is their :class:`~synergynet_b200.inference.ImagePack`."""
+        the "stack" is their :class:`~synergynet_b200.inference.ImagePack`.  ``rois`` (one list of boxes per frame, in
+        place of ``rects``): crop boxes used as given, without ``square_roi``."""
         dev = self._compute_device()
         eng = self._engine(dev)
         stack = pack_images(frames, dev) if ragged else stack_frames_device(frames, dev)
         n = len(stack) if ragged else int(stack.shape[0])
-        if rects is None:
+        if rois is not None:
+            rects = rois
+        elif rects is None:
             if self.face_detector is None:
                 raise RuntimeError('no face detector configured: pass rects (one list of [x0,y0,x1,y1,score] per frame) '
                                    'or set model.face_detector')
@@ -434,7 +437,7 @@ class _SynergyBase(nn.Module):
         if len(rects) != n:
             raise ValueError(f'{len(rects)} rect lists for {n} frames')
         counts = [len(r) for r in rects]
-        boxes = [square_roi(list(r)) for fr in rects for r in fr]
+        boxes = [list(r) if rois is not None else square_roi(list(r)) for fr in rects for r in fr]
         frame_index = [i for i, c in enumerate(counts) for _ in range(c)]
         if not boxes:
             return eng, stack, counts, frame_index, None, None
@@ -462,15 +465,8 @@ class _SynergyBase(nn.Module):
         The dense meshes stay on the device: they are reconstructed, lit and drawn in chunks of faces above
         ``dense_chunk_bytes`` onto the same canvases (a chunk may end inside a frame), then every frame is blended once.
         ``connectivity`` (3,ntri) 0-based replaces the model's ``triangles`` as in ``render.render``."""
-        from . import Sim3DR
-        eng, stack, counts, frame_index, params, roi5 = self._frames_front(frames, rects)
-        solid = stack.clone()
-        for r, v, col, f0, f1, chunk_counts in self._overlay_chunks(eng, stack.device, frame_index, params, roi5, tex, connectivity):
-            r.rasterize_frames(solid[f0:f1], v, col, chunk_counts, out=solid[f0:f1])
-        blended = Sim3DR.add_weighted(stack, solid, alpha)
-        if isinstance(frames, torch.Tensor) and frames.is_cuda:
-            return blended, solid
-        return blended.cpu().numpy(), solid.cpu().numpy()
+        front = self._frames_front(frames, rects)
+        return self._overlay_stack(frames, front, alpha, self._overlay_chunks(*self._chunk_args(front), tex, connectivity))
 
     def overlay_images(self, images, rects: Optional[Sequence[Sequence[Sequence[float]]]] = None, alpha: float = 0.6, tex=None,
                        connectivity=None):
@@ -484,10 +480,34 @@ class _SynergyBase(nn.Module):
         ``rects`` is None).  The dense meshes are reconstructed, lit and drawn in chunks of faces above
         ``dense_chunk_bytes`` onto the packed canvases, each chunk in place on the images it touches (a chunk may end
         inside an image); then the whole pack is blended once."""
+        front = self._frames_front(images, rects, ragged=True)
+        return self._overlay_list(images, front, alpha, self._overlay_chunks(*self._chunk_args(front), tex, connectivity))
+
+    @staticmethod
+    def _chunk_args(front):
+        eng, stack, _counts, frame_index, params, roi5 = front
+        return eng, (stack.data if isinstance(stack, ImagePack) else stack).device, frame_index, params, roi5
+
+    @staticmethod
+    def _overlay_stack(frames, front, alpha, chunks):
+        """Draw ``chunks`` (of :meth:`_overlay_chunks`) onto a copy of the frame stack of ``front`` and blend it."""
         from . import Sim3DR
-        eng, pack, counts, frame_index, params, roi5 = self._frames_front(images, rects, ragged=True)
+        stack = front[1]
+        solid = stack.clone()
+        for r, v, col, f0, f1, chunk_counts in chunks:
+            r.rasterize_frames(solid[f0:f1], v, col, chunk_counts, out=solid[f0:f1])
+        blended = Sim3DR.add_weighted(stack, solid, alpha)
+        if isinstance(frames, torch.Tensor) and frames.is_cuda:
+            return blended, solid
+        return blended.cpu().numpy(), solid.cpu().numpy()
+
+    @staticmethod
+    def _overlay_list(images, front, alpha, chunks):
+        """:meth:`_overlay_stack` for the ImagePack of ``front``: two lists of images."""
+        from . import Sim3DR
+        pack = front[1]
         solid = ImagePack(pack.data.clone(), pack.sizes)
-        for r, v, col, f0, f1, chunk_counts in self._overlay_chunks(eng, pack.data.device, frame_index, params, roi5, tex, connectivity):
+        for r, v, col, f0, f1, chunk_counts in chunks:
             part = solid.slice(f0, f1)
             r.rasterize_images(part, v, col, chunk_counts, out=part)
         blended = ImagePack(Sim3DR.add_weighted(pack.data, solid.data, alpha), pack.sizes)
@@ -497,26 +517,126 @@ class _SynergyBase(nn.Module):
         split = lambda host: [host[pack.offsets[i]:pack.offsets[i + 1]].reshape(h, w, 3) for i, (h, w) in enumerate(pack.sizes)]
         return split(hb), split(hs)
 
-    def _overlay_chunks(self, eng, device, frame_index, params, roi5, tex, connectivity):
+    def _overlay_chunks(self, eng, device, frame_index, params, roi5, tex, connectivity, uv=None):
         """The dense meshes of the overlay, chunk by chunk of ``dense_chunk_bytes``: yields ``(renderer, vertices (F,nver,3)
-        view, colours, f0, f1, meshes per frame f0..f1-1)`` for the frames f0..f1-1 the chunk draws on.  Raises the
-        engine's error flag after the last chunk."""
+        view, colours, f0, f1, meshes per frame f0..f1-1)`` for the frames f0..f1-1 the chunk draws on.  ``uv``: a
+        :class:`~synergynet_b200.inference.UVMaps` -- each mesh is then its kept vertices, drawn with the layout's
+        triangles and lit times its own UV texture (``tex`` and ``connectivity`` are not read).  Raises the engine's
+        error flag after the last chunk."""
         from . import Sim3DR
         from .inference import RENDER_CFG
         if not frame_index:
             return
-        tri = np.asarray(connectivity).T if connectivity is not None else self.triangles.T.cpu().numpy()
+        if uv is not None:
+            tri, nver = uv.layout.render_tri, uv.layout.n_keep
+            keep = torch.from_numpy(uv.layout.keep).to(device)
+        else:
+            tri = np.asarray(connectivity).T if connectivity is not None else self.triangles.T.cpu().numpy()
+            nver = eng.n_vert
         with torch.cuda.device(device):
-            r = Sim3DR._renderer_for(np.ascontiguousarray(tri, dtype=np.int32), eng.n_vert)
+            r = Sim3DR._renderer_for(np.ascontiguousarray(tri, dtype=np.int32), nver)
         cfg = Sim3DR._light_cfg(**RENDER_CFG)
-        texture = None if tex is None else torch.from_numpy(np.ascontiguousarray(tex, dtype=np.float32))
+        texture = None if tex is None or uv is not None else torch.from_numpy(np.ascontiguousarray(tex, dtype=np.float32))
         fi = np.asarray(frame_index)
         for a, b in self._dense_chunks(eng, len(frame_index)):
-            v = eng.reconstruct_image(params[a:b], roi5[a:b], dense=True).transpose(1, 2)
+            v = eng.reconstruct_image(params[a:b], roi5[a:b], dense=True)
+            if uv is not None:
+                v = v.index_select(2, keep)                                # (F,3,n_keep): m[:, keep] of every face
+                texture = uv.sample(a, b)[0]
+            v = v.transpose(1, 2)
             f0, f1 = int(fi[a]), int(fi[b - 1]) + 1                   # the frames this chunk draws on, in place
             col = r.colors(v, r.normals(v), cfg, texture)
             yield r, v, col, f0, f1, np.bincount(fi[a:b] - f0, minlength=f1 - f0)
         eng.raise_if_error()
+
+    # ---- the textured flows of artistic.py and uv_texture_realFaces.py ------------------------------------------------
+    def _uv_front(self, frames, uv_maps, uv, rects, rois, ragged: bool, overlay: bool):
+        """Every refusal of the ``uv_*`` methods, before any CUDA call; then :meth:`_frames_front` and the device maps."""
+        from .inference import UVLayout, UVMaps, uv_maps_host
+        if not isinstance(uv, UVLayout):
+            raise TypeError(f'uv must be a UVLayout, got {type(uv).__name__}')
+        if rects is not None and rois is not None:
+            raise ValueError('give rects (detector boxes, squared as get_all_outputs squares them) or rois (crop boxes used as '
+                             'given), not both')
+        if rects is None and rois is None and self.face_detector is None:
+            raise ValueError('give rects or rois, or set model.face_detector')
+        if rois is not None:
+            rois = [list(r) for r in rois]
+            if any(len(fr) and not hasattr(fr[0], '__len__') for fr in rois):    # one list of boxes for every frame
+                rois = [rois] * self._count_inputs(frames, ragged)
+            for fr in rois:
+                for r in fr:
+                    if len(r) < 4 or not (r[2] > r[0] and r[3] > r[1]):
+                        raise ValueError(f'ROI {list(r)} is empty: a crop box is [x0, y0, x1, y1(, score)] with x1 > x0, y1 > y0')
+        n = self._count_inputs(frames, ragged)
+        if uv.nver != self.u.shape[0] // 3:
+            raise ValueError(f'the UV layout has {uv.nver} vertices, the model\'s dense mesh {self.u.shape[0] // 3}')
+        maps = uv_maps_host(uv_maps, n, overlay)
+        for i, m in enumerate(maps):
+            uv.texels(m.shape[0], m.shape[1], f'UV map {i}')
+        front = self._frames_front(frames, rects, ragged=ragged, rois=rois)
+        frame_index = front[3]
+        face_map = [0] * len(frame_index) if len(maps) == 1 else frame_index
+        return front, UVMaps(uv, maps, face_map, self._chunk_args(front)[1])
+
+    @staticmethod
+    def _count_inputs(frames, ragged: bool) -> int:
+        if isinstance(frames, ImagePack):
+            return len(frames)
+        if not ragged and hasattr(frames, 'shape') and len(frames.shape) == 4:
+            return int(frames.shape[0])
+        return len(frames)
+
+    def uv_obj_batch(self, frames, uv_maps, uv, rects=None, rois=None):
+        """The textured OBJ files of artistic.py / uv_texture_realFaces.py for every face of N equally sized BGR uint8 frames:
+        one list of ``bytes`` per frame, one entry per face.  Face j of frame i is what
+        ``write_obj_with_colors(name, m[:, keep], deletedTri, np.flip(map_i, 0)[coord_u, coord_v][keep].astype(np.float32))``
+        writes, ``m`` the dense mesh ``get_all_outputs_batch`` returns for it (with ``rois``: the crop -> forward ->
+        ``predict_denseVert(param, roi)`` chain of the given box).  ``uv_maps``: one (h, w, 3|4) uint8 map per frame, or one
+        for all; ``uv``: a :class:`~synergynet_b200.inference.UVLayout`.  ``rects`` are detector boxes, squared as
+        ``get_all_outputs`` squares them; ``rois`` are crop boxes used as given (``[[0, 0, 256, 256, 1.0]]`` is
+        uv_texture_realFaces.py's), one list per frame or one list for every frame; give one or the other (or neither,
+        with ``model.face_detector`` set).  artistic.py writes only the last face of an image: entry ``[-1]``.  A frame
+        without a face gives ``[]`` (the script would write the previous image's mesh again; that is not reproduced).
+        Scripts resize with INTER_LINEAR: set ``model.resize_interpolation = 'linear'``.  The meshes and colour tables
+        never leave the device; only the text comes back."""
+        front, maps = self._uv_front(frames, uv_maps, uv, rects, rois, False, False)
+        return self._uv_obj(front, maps)
+
+    def uv_obj_images(self, images, uv_maps, uv, rects=None, rois=None):
+        """:meth:`uv_obj_batch` for N BGR uint8 images of any sizes."""
+        front, maps = self._uv_front(images, uv_maps, uv, rects, rois, True, False)
+        return self._uv_obj(front, maps)
+
+    def _uv_obj(self, front, maps):
+        from .inference import ObjTables
+        eng, _stack, counts, frame_index, params, roi5 = front
+        if not frame_index:
+            return [[] for _ in counts]
+        tables = ObjTables(maps.layout.deleted_tri, eng.n_vert, None, maps.layout.keep, len(frame_index))
+        texts = []
+        for a, b in self._dense_chunks(eng, len(frame_index)):
+            colors = maps.sample(a, b, texture=False, colors=True)[1]
+            texts += tables.encode(eng.reconstruct_image(params[a:b], roi5[a:b], dense=True), a, colors_dev=colors)
+        eng.raise_if_error()
+        return split_by_counts(texts, counts)
+
+    def uv_overlay_batch(self, frames, uv_maps, uv, rects=None, rois=None, alpha: float = 0.6):
+        """The textured overlay of uv_texture_realFaces.py for N equally sized BGR uint8 frames: ``(blended, solid)`` as
+        :meth:`overlay_batch` returns them.  Frame i's solid image is ``overlap = frame.copy()``, then for every face j in
+        rect order ``overlap = RenderPipeline(**cfg)(m_j[:, keep].T, (deletedTri - 1).T, overlap, texture=tex_j)`` with a
+        fresh ``tex_j = colors_uv[keep].astype(np.float32) / 255.0`` of map i; blended is
+        ``cv2.addWeighted(frame, 1 - alpha, overlap, alpha, 0)``.  With one face per frame that is
+        ``utils/render.render(img, [m[:, keep]], alpha, tex=tex, connectivity=deletedTri - 1)``.  Each kept mesh is lit by
+        its own extent, as the reference lights the subset it is given.  Arguments as :meth:`uv_obj_batch`; a 4-channel
+        map is refused."""
+        front, maps = self._uv_front(frames, uv_maps, uv, rects, rois, False, True)
+        return self._overlay_stack(frames, front, alpha, self._overlay_chunks(*self._chunk_args(front), None, None, maps))
+
+    def uv_overlay_images(self, images, uv_maps, uv, rects=None, rois=None, alpha: float = 0.6):
+        """:meth:`uv_overlay_batch` for N BGR uint8 images of any sizes: two lists of images, as :meth:`overlay_images`."""
+        front, maps = self._uv_front(images, uv_maps, uv, rects, rois, True, True)
+        return self._overlay_list(images, front, alpha, self._overlay_chunks(*self._chunk_args(front), None, None, maps))
 
     def pose_overlay_batch(self, frames, rects: Optional[Sequence[Sequence[Sequence[float]]]] = None):
         """The pose image of singleImage.py:112-118 for N equally sized BGR uint8 frames in one pass: every face's axes

@@ -220,3 +220,35 @@ def make_scene_u8(height: int, width: int, seed: int = 0) -> np.ndarray:
         img[inside] = img[inside] * 0.3 + rng.uniform(60, 220, 3)
     img += rng.normal(0, 5, img.shape)
     return np.clip(img, 0, 255).astype(np.uint8)
+
+
+# ---- the UV layout of the textured flows (artistic.py, uv_texture_realFaces.py) -----------------------------------------------
+def make_uv_layout(seed: int = 0, nver: int = NVER, dtype=np.float32, keep_fraction: float = 0.75):
+    """Seeded stand-ins for ``3dmm_data/BFM_UV.npy`` (nver, 2) in ``dtype``, ``keptInd.npy`` (sorted int64) and
+    ``deletedTri.npy`` ((3, ntri) int64, 1-based over the kept vertices).  The UV values include 0, 1.0 (texel 255) and the
+    neighbours of k/255 on both sides, where ``(uv * 255.0).astype(np.int32)`` changes; about one kept vertex in twenty is
+    touched by no triangle (a NaN normal in the reference, never drawn)."""
+    rng = np.random.default_rng(11000 + seed)
+    uv = rng.uniform(0.0, 1.0, (nver, 2)).astype(dtype)
+    k = rng.integers(0, 256, (nver, 2))
+    edge = (k / 255.0).astype(dtype)
+    pick = rng.integers(0, 4, (nver, 2))
+    uv = np.where(pick == 0, np.nextafter(edge, dtype(2)), np.where(pick == 1, np.nextafter(edge, dtype(-1)), uv)).astype(dtype)
+    uv = np.where(pick == 2, edge, uv).astype(dtype)
+    uv[:4] = np.array([[0, 0], [1, 1], [0, 1], [1, 0]], dtype)
+    uv = np.clip(uv, 0, 1).astype(dtype)
+    keep = np.sort(rng.choice(nver, max(1, int(nver * keep_fraction)), replace=False)).astype(np.int64)
+    n_keep = keep.size
+    used = rng.permutation(n_keep)[: max(3, n_keep - n_keep // 20)]
+    ntri = 2 * n_keep
+    tri = used[rng.integers(0, used.size, (3, ntri))].astype(np.int64) + 1
+    return uv, keep, tri
+
+
+def make_uv_map(height: int, width: int, seed: int = 0, channels: int = 3) -> np.ndarray:
+    """(h, w, channels) uint8 UV map: smooth colour ramps plus noise, so neighbouring texels differ."""
+    rng = np.random.default_rng(12000 + seed)
+    yy, xx = np.mgrid[0:height, 0:width].astype(np.float64)
+    img = np.stack([128 + 100 * np.sin(xx / (5.0 + c) + yy / (7.0 + 2 * c) + rng.uniform(0, 6)) for c in range(channels)], -1)
+    img += rng.normal(0, 12, img.shape)
+    return np.clip(img, 0, 255).astype(np.uint8)
