@@ -1,8 +1,7 @@
 // Fused inverted-residual block on tensor cores (wgmma):  1x1 expand (+BN+ReLU6) -> 3x3 depthwise (+BN+ReLU6)
 // -> 1x1 project (+BN)(+skip), reference backbone_nets/mobilenetv2_backbone.py:45-74, in ONE
-// kernel, so the 6x-expanded hidden tensor (up to 1.38 MB per face) never touches HBM.
-// The same kernel, with an im2col loader, fuses the 3x3/s2 stem conv with block 1
-// (mobilenetv2_backbone.py:127 + features[1]).
+// kernel, so the 6x-expanded hidden tensor (up to 1.38 MB per face) never touches HBM.  Blocks 2-17; the stem and
+// block 1 run in a kernel of their own (kernels_stem.cuh).
 //
 // Work item (tile) = RO output rows of one face (large maps) or FACES whole faces (8x8 / 4x4 maps).
 // Per tile the block input is converted once to fp16 hi/lo and stored in shared memory (XA); then, for
@@ -19,8 +18,8 @@
 // bulk-copy (TMA) ring (late blocks).
 //
 // Roles: warps 0..kFusedWorkerWarps-1 = workers (thread = GEMM row / pixel in the conversion, channel octets in EPI1 /
-// DW, MMA operand slabs per warpgroup), warp kFusedWorkerWarps = weight loader and stem-row stager (converged warp, bulk
-// copies under elect.sync).  smem operand tiles use the canonical K-major no-swizzle layout of tc_common.cuh (SBO 128 B,
+// DW, MMA operand slabs per warpgroup), warp kFusedWorkerWarps = weight loader (converged warp, bulk copies under
+// elect.sync).  smem operand tiles use the canonical K-major no-swizzle layout of tc_common.cuh (SBO 128 B,
 // LBO = rows/8 * 128 B).
 #pragma once
 #include "common.cuh"
@@ -36,13 +35,11 @@ static_assert(kFusedWorkerWarps % 4 == 0, "worker warps form whole warpgroups");
 __host__ __device__ constexpr int ceil_div_c(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ constexpr int round_up_c(int a, int b) { return ceil_div_c(a, b) * b; }
 
-template <int CIN_, int CHID_, int NC_, int COUT_, int W_, int STRIDE_, int RO_, int FACES_, bool RES_, bool STEM_,
-          int WSTREAM_>
+template <int CIN_, int CHID_, int NC_, int COUT_, int W_, int STRIDE_, int RO_, int FACES_, bool RES_, int WSTREAM_>
 struct FusedCfg {
-  static constexpr bool STEM = STEM_;            // GEMM1 = im2col(3x3 s2 stem conv), CIN = 27 taps
   static constexpr bool RES = RES_;
   static constexpr bool WSTREAM = WSTREAM_ > 0;  // weights streamed per chunk (ring of WSTREAM_ slots) instead of resident
-  static constexpr int CIN = CIN_;               // channels of the NHWC input (STEM: 27)
+  static constexpr int CIN = CIN_;               // channels of the NHWC input
   static constexpr int CIN_P = round_up_c(CIN_, 16);
   static constexpr int CHID = CHID_, NC = NC_, NCHUNK = CHID_ / NC_;
   static constexpr int COUT = COUT_, COUT_P = round_up_c(COUT_, 16);
@@ -79,11 +76,7 @@ struct FusedCfg {
   static constexpr int S_XA = S_WCH + WSTAGES * CHUNK_BYTES;
   static constexpr int S_A2 = S_XA + 2 * XA_PLANE;
   static constexpr int S_H = S_A2 + 2 * A2_PLANE;
-  // stem only: staged input rows [3][IN_ROWS][120] fp32, exactly as they lie in the NCHW crop (one bulk
-  // copy per channel); the left zero-pad column is a predicate in the im2col gather
-  static constexpr int IN_ROWS = 2 * ROWS_MAX + 1, IN_STRIDE = 120;
-  static constexpr int S_IN = S_H + HS_PIX * HS_STRIDE * 4;
-  static constexpr int S_TOTAL = S_IN + (STEM_ ? 3 * IN_ROWS * IN_STRIDE * 4 : 0);
+  static constexpr int S_TOTAL = S_H + HS_PIX * HS_STRIDE * 4;
   static constexpr int SMEM_BYTES = S_TOTAL + 1024;                      // + alignment slack
   static_assert(CHID_ % NC_ == 0 && NC_ % 16 == 0, "hidden chunking");
   static_assert(WO % RO_ == 0, "strips must tile the output");
@@ -94,8 +87,7 @@ struct FusedCfg {
 };
 
 struct FusedArgs {
-  const float* x;        // NHWC (B,W,W,CIN) -- or NCHW (B,3,120,120) for the stem variant
-  const uint8_t* x_u8;   // stem variant only: raw uint8 crop, normalised (v-127.5)/128 while staging; else null
+  const float* x;        // NHWC (B,W,W,CIN)
   const uint8_t* wimg;   // packed weight image (FusedCfg::W_BYTES)
   float* y;              // NHWC (B,WO,WO,COUT)
   int batch;
@@ -103,7 +95,6 @@ struct FusedArgs {
   int face_groups;       // number of face groups (tiles = face_groups * STRIPS)
   int* err;              // sticky time-out flag of the bounded mbarrier waits (mapped pinned host memory)
   int* sat;              // sticky "a block input was clamped to the fp16 range" flag (device memory)
-  int border;            // uint8 stem only: CenterCrop margin, pixels of the frame read as 0 (utils/ddfa.py:162-243); 0 = off
   int npass;             // 3 = split-fp16 x3 (hi*hi + hi*lo + lo*hi); 1 = single fp16 pass (SYN_ENGINE_TC_FUSED_1PASS)
 #ifdef SYN_FUSED_TRACE
   int trace_id;          // backbone block of this launch (1..17)
@@ -176,7 +167,7 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
   static_assert(N2 % 8 == 0 && N2 <= 256, "MMA N");
   using namespace tc;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_w, bar_wfull[4], bar_wempty[4], bar_x, bar_in;
+  __shared__ __align__(8) uint64_t bar_w, bar_wfull[4], bar_wempty[4];
 
   // keep the pointer in the shared address space (no integer round trip): a generic pointer here
   // turns every tile access into LD.E/ST.E instead of LDS/STS
@@ -209,15 +200,7 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
       mbar_init(smem_u32(&bar_wfull[i]), 1);
       mbar_init(smem_u32(&bar_wempty[i]), NWT);
     }
-    mbar_init(smem_u32(&bar_x), NWT);
-    mbar_init(smem_u32(&bar_in), 1);
     fence_mbar_init();
-  }
-  if constexpr (C::STEM) {     // staged-row buffer: the left pad column (and everything else) starts as zero;
-    float* z = reinterpret_cast<float*>(smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u) + C::S_IN);
-    for (int i = threadIdx.x; i < 3 * C::IN_ROWS * C::IN_STRIDE / 4; i += blockDim.x)   // before any bulk copy
-      reinterpret_cast<float4*>(z)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    tc::fence_proxy_async_smem();
   }
   __syncthreads();
 
@@ -226,7 +209,6 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
   uint8_t* sA2 = smem + C::S_A2;
   float* sH = reinterpret_cast<float*>(smem + C::S_H);
   const float* sB3 = reinterpret_cast<const float*>(smem + C::S_B3);
-  float* sIn = reinterpret_cast<float*>(smem + C::S_IN);   // stem variant only
 
   if (warp < NWW) {
     // =============================== workers ====================================================
@@ -234,7 +216,7 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
     for (int i = tid; i < C::HS_PIX * C::HS_STRIDE / 4; i += NWT)
       reinterpret_cast<float4*>(sH)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     mbar_wait(smem_u32(&bar_w), 0, p.err);                // b3/s3 (and, if resident, all chunks) landed
-    uint32_t g = 0, n_in = 0;                             // g = chunk counter, n_in = staged-row phases consumed
+    uint32_t g = 0;                                       // chunk counter
     asm volatile("bar.sync 5, %0;" ::"n"(NWT) : "memory");
     const uint32_t d_hi = smem_desc_hi(128);
     constexpr uint32_t LBO_W1 = (C::NC / 8) * 128, LBO_W3 = (C::COUT_P / 8) * 128;
@@ -263,7 +245,7 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
       }
     };
 
-    // Geometry of a tile + "prep": stage / convert its input into the GEMM1 A operand.  prep(next tile) runs
+    // Geometry of a tile + "prep": convert its input into the GEMM1 A operand.  prep(next tile) runs
     // BEFORE the current tile's EPI2 (XA is free once the last GEMM1 of the tile is done), so the global-load
     // latency of the conversion overlaps the output stores.
     auto prep = [&](int tile) {
@@ -279,44 +261,6 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
       const bool trace_on = blockIdx.x == 0 && tile == 2 * (int)gridDim.x && tid == 0;   // prep of the tile after the traced one
 #endif
       SYN_TRACE(0, 62, 0);
-      // ---- stem: the crop rows this strip needs, zero outside the image ------------------------------
-      if constexpr (C::STEM) {
-        const int iy_first = 2 * rf - 1, nin = 2 * (rl - rf + 1) + 1;
-        if (p.x_u8 != nullptr) {              // uint8 crops: threads load, normalise and stage
-          for (int i = tid; i < 3 * nin * 30; i += NWT) {
-            const int c4 = i % 30, r = (i / 30) % nin, ci = i / (30 * nin);
-            const int iy = iy_first + r;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (iy >= 0 && iy < kImg) {
-              uchar4 u = *reinterpret_cast<const uchar4*>(p.x_u8 + ((size_t)(f0 * 3 + ci) * kImg + iy) * kImg + c4 * 4);
-              if (p.border > 0) {                                   // zero frame of the reference loader, before normalisation
-                const int col = c4 * 4;
-                const bool row_out = iy < p.border || iy >= kImg - p.border;
-                if (row_out || col < p.border || col >= kImg - p.border) u.x = 0;
-                if (row_out || col + 1 < p.border || col + 1 >= kImg - p.border) u.y = 0;
-                if (row_out || col + 2 < p.border || col + 2 >= kImg - p.border) u.z = 0;
-                if (row_out || col + 3 < p.border || col + 3 >= kImg - p.border) u.w = 0;
-              }
-              v = make_float4(((float)u.x - 127.5f) / 128.0f, ((float)u.y - 127.5f) / 128.0f,
-                              ((float)u.z - 127.5f) / 128.0f, ((float)u.w - 127.5f) / 128.0f);
-            }
-            *reinterpret_cast<float4*>(sIn + (ci * C::IN_ROWS + r) * C::IN_STRIDE + c4 * 4) = v;
-          }
-        } else {                              // fp32 crops: rows were bulk-copied by the loader one tile ahead
-          mbar_wait(smem_u32(&bar_in), n_in & 1, p.err);
-          ++n_in;
-          for (int r = 0; r < nin; ++r) {     // rows outside the image are not copied: zero them (edge strips)
-            const int iy = iy_first + r;
-            if (iy < 0 || iy >= kImg)
-              for (int i = tid; i < 3 * 30; i += NWT)
-                *reinterpret_cast<float4*>(sIn + ((i / 30) * C::IN_ROWS + r) * C::IN_STRIDE + (i % 30) * 4) =
-                    make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-        }
-        SYN_TRACE(0, 62, 1);
-        asm volatile("bar.sync 5, %0;" ::"n"(NWT) : "memory");
-      }
-      SYN_TRACE(0, 62, 2);
       // ---- X tile -> fp16 hi/lo operand in smem ---------------------------------------------------
       // The conversion sits between the last depthwise and EPI2 of the current tile, so its global-load
       // latency is exposed once per batch of loads: all loads of a batch are issued unconditionally (from a
@@ -331,57 +275,26 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
         const int n_items = ((M1 + 63) >> 6) * KG;
         for (int e0 = xg; e0 < n_items; e0 += PB * NXG) {
           float v[PB][8];
-          if constexpr (C::STEM) {
-            // im2col of the 3x3 stride-2 pad-1 stem conv from the staged rows: k = (ci*3+ky)*3+kx.  All PB items of a
-            // thread are gathered before the first conversion (independent shared loads in flight instead of one
-            // load -> convert -> store chain per item); the kg switch makes every tap offset a compile-time constant.
+          float4 qa[PB], qb[PB];
+          bool ok[PB];
 #pragma unroll
-            for (int u = 0; u < PB; ++u) {
+          for (int u = 0; u < PB; ++u) {
+            const int e = min(e0 + u * NXG, n_items - 1);
+            const int t = e / KG, kg = e - t * KG;
+            const int m = t * 64 + r64;
+            ok[u] = (e0 + u * NXG < n_items) && (m < M1) && (kg * 8 < C::CIN);
+            const int mc = min(m, M1 - 1), kgc = min(kg, (C::CIN - 1) / 8);
+            const int f = (C::FACES > 1) ? mc / ppf : 0;
+            const int mr = mc - f * ppf;                    // pixel inside the face's valid rows
+            const float* src = p.x + ((size_t)((f0 + f) * C::W + rf) * C::W + mr) * C::CIN + kgc * 8;
+            qa[u] = __ldg(reinterpret_cast<const float4*>(src));
+            qb[u] = __ldg(reinterpret_cast<const float4*>(src + 4));
+          }
+          if (e0 == xg) SYN_TRACE(0, 62, 5);
 #pragma unroll
-              for (int j = 0; j < 8; ++j) v[u][j] = 0.f;
-              const int e = e0 + u * NXG;
-              if (e >= n_items) continue;
-              const int t = e / KG, kg = e - t * KG;
-              const int mr = t * 64 + r64;                      // FACES == 1
-              if (mr < M1) {
-                const int yl = mr / C::W, xx = mr - yl * C::W;
-                const float* base = sIn + (2 * yl) * C::IN_STRIDE + 2 * xx - 1;   // column 2xx-1+kx; -1 is the zero pad
-#pragma unroll
-                for (int kgc = 0; kgc < KG; ++kgc)
-                  if (kg == kgc) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                      const int k = kgc * 8 + j;
-                      if (k < 27) {
-                        const int ci = k / 9, ky = (k % 9) / 3, kx = k % 3;
-                        if (kx > 0 || xx > 0) v[u][j] = base[(ci * C::IN_ROWS + ky) * C::IN_STRIDE + kx];
-                      }
-                    }
-                  }
-              }
-            }
-          } else {
-            float4 qa[PB], qb[PB];
-            bool ok[PB];
-#pragma unroll
-            for (int u = 0; u < PB; ++u) {
-              const int e = min(e0 + u * NXG, n_items - 1);
-              const int t = e / KG, kg = e - t * KG;
-              const int m = t * 64 + r64;
-              ok[u] = (e0 + u * NXG < n_items) && (m < M1) && (kg * 8 < C::CIN);
-              const int mc = min(m, M1 - 1), kgc = min(kg, (C::CIN - 1) / 8);
-              const int f = (C::FACES > 1) ? mc / ppf : 0;
-              const int mr = mc - f * ppf;                    // pixel inside the face's valid rows
-              const float* src = p.x + ((size_t)((f0 + f) * C::W + rf) * C::W + mr) * C::CIN + kgc * 8;
-              qa[u] = __ldg(reinterpret_cast<const float4*>(src));
-              qb[u] = __ldg(reinterpret_cast<const float4*>(src + 4));
-            }
-            if (e0 == xg) SYN_TRACE(0, 62, 5);
-#pragma unroll
-            for (int u = 0; u < PB; ++u) {
-              v[u][0] = ok[u] ? qa[u].x : 0.f; v[u][1] = ok[u] ? qa[u].y : 0.f; v[u][2] = ok[u] ? qa[u].z : 0.f; v[u][3] = ok[u] ? qa[u].w : 0.f;
-              v[u][4] = ok[u] ? qb[u].x : 0.f; v[u][5] = ok[u] ? qb[u].y : 0.f; v[u][6] = ok[u] ? qb[u].z : 0.f; v[u][7] = ok[u] ? qb[u].w : 0.f;
-            }
+          for (int u = 0; u < PB; ++u) {
+            v[u][0] = ok[u] ? qa[u].x : 0.f; v[u][1] = ok[u] ? qa[u].y : 0.f; v[u][2] = ok[u] ? qa[u].z : 0.f; v[u][3] = ok[u] ? qa[u].w : 0.f;
+            v[u][4] = ok[u] ? qb[u].x : 0.f; v[u][5] = ok[u] ? qb[u].y : 0.f; v[u][6] = ok[u] ? qb[u].z : 0.f; v[u][7] = ok[u] ? qb[u].w : 0.f;
           }
 #pragma unroll
           for (int u = 0; u < PB; ++u) {
@@ -407,25 +320,22 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
       }
       SYN_TRACE(0, 62, 3);
       fence_proxy_async_smem();                             // XA is read by wgmma after the next worker barrier
-      mbar_arrive(smem_u32(&bar_x));                        // (stem) the staged rows are consumed
       SYN_TRACE(0, 62, 4);
 
     };
     // L2 prefetch of a tile's input (one contiguous NHWC range) a whole tile ahead of its conversion: the
     // loads in prep() then hit L2 with warm TLB entries instead of paying ~2000 cycles per batch
     auto prefetch_x = [&](int tile) {
-      if constexpr (!C::STEM) {
-        if (tile >= ntiles) return;
-        const int fg = tile / C::STRIPS, sp = tile - fg * C::STRIPS;
-        int f0, nfaces;
-        group_faces(fg, f0, nfaces);
-        const int iy0 = sp * C::RO * C::STRIDE - 1;
-        const int rf = max(iy0, 0), rl = min(iy0 + C::RWIN - 1, C::W - 1);
-        const char* base = reinterpret_cast<const char*>(p.x + ((size_t)(f0 * C::W + rf) * C::W) * C::CIN);
-        const int bytes = (C::FACES > 1 ? nfaces * C::W * C::W : (rl - rf + 1) * C::W) * C::CIN * 4;
-        for (int o = tid * 128; o < bytes; o += NWT * 128)
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(base + o));
-      }
+      if (tile >= ntiles) return;
+      const int fg = tile / C::STRIPS, sp = tile - fg * C::STRIPS;
+      int f0, nfaces;
+      group_faces(fg, f0, nfaces);
+      const int iy0 = sp * C::RO * C::STRIDE - 1;
+      const int rf = max(iy0, 0), rl = min(iy0 + C::RWIN - 1, C::W - 1);
+      const char* base = reinterpret_cast<const char*>(p.x + ((size_t)(f0 * C::W + rf) * C::W) * C::CIN);
+      const int bytes = (C::FACES > 1 ? nfaces * C::W * C::W : (rl - rf + 1) * C::W) * C::CIN * 4;
+      for (int o = tid * 128; o < bytes; o += NWT * 128)
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(base + o));
     };
     // Programmatic dependent launch: everything above (barriers, the zeroed window, the weight image) does not
     // depend on the previous kernel; its output -- this kernel's input -- is first touched below, and this kernel's
@@ -812,7 +722,7 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
       SYN_TRACE(0, 63, 4);
     }
   } else if (warp == NWW) {
-    // =============================== weight loader / stem-row stager ================================
+    // =============================== weight loader ================================================
     // The whole warp runs this control flow convergently and every batch of bulk copies sits under one elect.sync.
     const int my_tiles = (ntiles > (int)blockIdx.x) ? (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
     const uint32_t total_chunks = (uint32_t)my_tiles * C::NCHUNK;
@@ -842,35 +752,6 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
         __syncwarp();
       }
     }
-    if constexpr (C::STEM) {
-      // fp32 crops: bulk-copy (TMA) the crop rows of a tile into sIn, one tile ahead of the workers
-      auto stage_rows = [&](int tile) {
-        if (p.x_u8 != nullptr || tile >= ntiles) return;
-        if (!elect_one()) return;
-        const int fgq = tile / C::STRIPS, spq = tile - fgq * C::STRIPS;
-        const int iy0q = spq * C::RO * C::STRIDE - 1;
-        const int rfq = max(iy0q, 0), rlq = min(iy0q + C::RWIN - 1, C::W - 1);
-        const int iy_first = 2 * rfq - 1, nin = 2 * (rlq - rfq + 1) + 1;
-        const int r_lo = (iy_first < 0) ? -iy_first : 0;                     // first / last staged row inside the crop
-        const int r_hi = min(nin - 1, kImg - 1 - iy_first);
-        const uint32_t bytes = (uint32_t)(r_hi - r_lo + 1) * kImg * 4;          // contiguous in the crop and in sIn
-        mbar_expect_tx(smem_u32(&bar_in), 3 * bytes);
-        for (int ci = 0; ci < 3; ++ci)
-          bulk_g2s(smem_u32(sIn + (ci * C::IN_ROWS + r_lo) * C::IN_STRIDE),
-                   p.x + ((size_t)(fgq * 3 + ci) * kImg + iy_first + r_lo) * kImg, bytes, smem_u32(&bar_in));
-      };
-      asm volatile("griddepcontrol.wait;" ::: "memory");   // the crop rows are inputs; the rule is kept uniform
-      stage_rows(blockIdx.x);
-      __syncwarp();
-      uint32_t n_x = 0;
-      // uint8 crops are staged by the workers themselves; then nothing here waits on their bar_x phases
-      for (int tile = blockIdx.x; p.x_u8 == nullptr && tile < ntiles; tile += gridDim.x) {
-        mbar_wait(smem_u32(&bar_x), n_x & 1, p.err);        // the conversion of this tile has consumed sIn
-        ++n_x;
-        stage_rows(tile + gridDim.x);
-        __syncwarp();
-      }
-    }
   }
 }
 
@@ -891,20 +772,19 @@ inline void fused_tile_plan(int batch, int sms, int& split, int& face_groups) {
 // ---- the instantiations used by the backbone (SURVEY.md section 8(a) shape table) -------------------
 // Block 3 takes 48-channel chunks (3 per tile: fewer per-chunk barrier round trips).  The strip heights of blocks 3-6
 // are bounded by shared memory: the block input (XA) is staged there next to the hidden window.
-//                          CIN CHID NC COUT  W  S  RO FACES RES    STEM   weight ring slots (0 = resident)
-using FusedStemB1 = FusedCfg<27, 32, 32, 16, 60, 1, 6, 1, false, true, 0>;    // features[0] + features[1]
-using FusedB2 = FusedCfg<16, 96, 32, 24, 60, 2, 6, 1, false, false, 0>;       // features[2]
-using FusedB3 = FusedCfg<24, 144, 48, 24, 30, 1, 6, 1, true, false, 0>;      // features[3]
-using FusedB4 = FusedCfg<24, 144, 16, 32, 30, 2, 5, 1, false, false, 0>;      // features[4]
-using FusedB56 = FusedCfg<32, 192, 64, 32, 15, 1, 5, 1, true, false, 0>;     // features[5], [6]
-using FusedB7 = FusedCfg<32, 192, 64, 64, 15, 2, 8, 1, false, false, 0>;      // features[7]
-using FusedB8 = FusedCfg<64, 384, 64, 64, 8, 1, 8, 2, true, false, 3>;         // features[8..10]
-using FusedB11 = FusedCfg<64, 384, 64, 96, 8, 1, 8, 2, false, false, 2>;       // features[11]
-using FusedB12 = FusedCfg<96, 576, 32, 96, 8, 1, 8, 2, true, false, 3>;        // features[12], [13]
-using FusedB14 = FusedCfg<96, 576, 32, 160, 8, 2, 4, 2, false, false, 3>;      // features[14]
+//                          CIN CHID NC COUT  W  S  RO FACES RES   weight ring slots (0 = resident)
+using FusedB2 = FusedCfg<16, 96, 32, 24, 60, 2, 6, 1, false, 0>;              // features[2]
+using FusedB3 = FusedCfg<24, 144, 48, 24, 30, 1, 6, 1, true, 0>;             // features[3]
+using FusedB4 = FusedCfg<24, 144, 16, 32, 30, 2, 5, 1, false, 0>;             // features[4]
+using FusedB56 = FusedCfg<32, 192, 64, 32, 15, 1, 5, 1, true, 0>;            // features[5], [6]
+using FusedB7 = FusedCfg<32, 192, 64, 64, 15, 2, 8, 1, false, 0>;             // features[7]
+using FusedB8 = FusedCfg<64, 384, 64, 64, 8, 1, 8, 2, true, 3>;                // features[8..10]
+using FusedB11 = FusedCfg<64, 384, 64, 96, 8, 1, 8, 2, false, 2>;              // features[11]
+using FusedB12 = FusedCfg<96, 576, 32, 96, 8, 1, 8, 2, true, 3>;               // features[12], [13]
+using FusedB14 = FusedCfg<96, 576, 32, 160, 8, 2, 4, 2, false, 3>;             // features[14]
 // blocks 15-17: four faces per tile (64 GEMM rows = one MMA slab), so that the 64 x COUT fp32 D2 accumulator fits the
 // registers of the worker warpgroups
-using FusedB15 = FusedCfg<160, 960, 32, 160, 4, 1, 4, 4, true, false, 3>;      // features[15], [16]
-using FusedB17 = FusedCfg<160, 960, 32, 320, 4, 1, 4, 4, false, false, 2>;     // features[17]
+using FusedB15 = FusedCfg<160, 960, 32, 160, 4, 1, 4, 4, true, 3>;             // features[15], [16]
+using FusedB17 = FusedCfg<160, 960, 32, 320, 4, 1, 4, 4, false, 2>;            // features[17]
 
 }  // namespace syn

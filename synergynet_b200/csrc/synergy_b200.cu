@@ -12,6 +12,7 @@
 #include "kernels_simt.cuh"
 #include "kernels_tc.cuh"
 #include "kernels_fused.cuh"
+#include "kernels_stem.cuh"
 #include "kernels_tail.cuh"
 #include "kernels_dense.cuh"
 #include "kernels_gemm.cuh"
@@ -228,8 +229,8 @@ int launch_depthwise(syn_handle* h, const float* x, int layer, float* y, int bat
 }
 
 template <class C>
-int launch_fused(syn_handle* h, const float* x, int block, float* y, int batch, cudaStream_t st,
-                 const uint8_t* x_u8 = nullptr);
+int launch_fused(syn_handle* h, const float* x, int block, float* y, int batch, cudaStream_t st);
+int launch_stem(syn_handle* h, const float* x, const uint8_t* x_u8, float* y, int batch, cudaStream_t st);
 
 // Runs the backbone.  When stop_layer >= 0 the activation of that conv is copied to dbg_out and
 // the function returns early.  Otherwise params (B,62) [and pool (B,1280)] are produced.
@@ -267,14 +268,14 @@ int run_backbone(syn_handle* h, const float* x, int batch, float* params, float*
   int cur = 0;
   int li = 1;
   if (h->fused()) {
-    // stem + block 1, then blocks 2..7, each one fused launch; only block outputs exist
+    // stem + block 1, then blocks 2..17, each one fused launch; only block outputs exist
     if (stop_layer >= 0 && stop_layer <= 50 && (stop_layer < 2 || (stop_layer - 2) % 3 != 0))
       return fail(SYN_ERR_UNSUPPORTED, "conv %d lives inside a fused block and is never materialised", stop_layer);
     const float* in = x;
     for (int b = 1; b <= 17; ++b) {
       float* out = h->buf_io[cur ^ 1];
       switch (b) {
-        case 1: rc = launch_fused<FusedStemB1>(h, in, b, out, batch, st, x_u8); break;
+        case 1: rc = launch_stem(h, in, x_u8, out, batch, st); break;
         case 2: rc = launch_fused<FusedB2>(h, in, b, out, batch, st); break;
         case 3: rc = launch_fused<FusedB3>(h, in, b, out, batch, st); break;
         case 4: rc = launch_fused<FusedB4>(h, in, b, out, batch, st); break;
@@ -520,11 +521,12 @@ void pack_tc_pointwise(std::vector<uint8_t>& img, std::vector<float>& oscale, co
     }
 }
 
-// ---- weight image of one fused block (layout documented in FusedCfg) --------------------------------
-// w1: [K][CHID] folded expand (or stem) weights, dw: [9][CHID], w3: [CHID][COUT] folded project weights.
+// ---- weight image of one fused block (layout documented in FusedCfg; StemCfg uses it with one chunk) -------------
+// w1: [CIN][CHID] folded expand (or stem) weights, dw: [9][CHID], w3: [CHID][COUT] folded project weights.
 template <class C>
-void pack_fused(std::vector<uint8_t>& img, const float* w1, int K, const float* b1, const float* dw,
-                const float* bdw, const float* w3, const float* b3) {
+void pack_fused(std::vector<uint8_t>& img, const float* w1, const float* b1, const float* dw, const float* bdw,
+                const float* w3, const float* b3) {
+  constexpr int K = C::CIN;
   img.assign(C::W_BYTES, 0);
   auto put = [&](size_t byte_off, float w, size_t plane_bytes) {
     uint16_t h, l;
@@ -565,15 +567,14 @@ void pack_fused(std::vector<uint8_t>& img, const float* w1, int K, const float* 
 }
 
 template <class C>
-int launch_fused(syn_handle* h, const float* x, int block, float* y, int batch, cudaStream_t st, const uint8_t* x_u8) {
+int launch_fused(syn_handle* h, const float* x, int block, float* y, int batch, cudaStream_t st) {
   static bool attr_set[16] = {};
   if (!attr_set[h->device & 15]) {
     SYN_CUDA(cudaFuncSetAttribute(fused_mbconv_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     attr_set[h->device & 15] = true;
   }
   FusedArgs a;
-  a.x_u8 = x_u8;
-  a.x = x; a.wimg = h->d_fused + h->fused_off[block]; a.y = y; a.batch = batch; a.err = h->d_err; a.sat = h->d_sat; a.npass = h->npass(); a.border = h->center_crop;
+  a.x = x; a.wimg = h->d_fused + h->fused_off[block]; a.y = y; a.batch = batch; a.err = h->d_err; a.sat = h->d_sat; a.npass = h->npass();
 #ifdef SYN_FUSED_TRACE
   a.trace_id = block;
 #endif
@@ -593,11 +594,39 @@ int launch_fused(syn_handle* h, const float* x, int block, float* y, int batch, 
   cfg.numAttrs = 1;
   SYN_CUDA(cudaLaunchKernelEx(&cfg, fused_mbconv_kernel<C>, a));
   SYN_LAUNCH_CHECK("fused_mbconv_kernel");
-  static const char* const names[18] = {"", "fused_stem_block1", "fused_block2", "fused_block3", "fused_block4",
+  static const char* const names[18] = {"", "", "fused_block2", "fused_block3", "fused_block4",
                                         "fused_block5", "fused_block6", "fused_block7", "fused_block8", "fused_block9",
                                         "fused_block10", "fused_block11", "fused_block12", "fused_block13", "fused_block14",
                                         "fused_block15", "fused_block16", "fused_block17"};
   mark(h, st, names[block]);
+  return SYN_OK;
+}
+
+// Stem + block 1 (kernels_stem.cuh): fp32 crops x or uint8 crops x_u8 (normalised, CenterCrop border, in the kernel)
+int launch_stem(syn_handle* h, const float* x, const uint8_t* x_u8, float* y, int batch, cudaStream_t st) {
+  using C = StemCfg;
+  static bool attr_set[16] = {};
+  if (!attr_set[h->device & 15]) {
+    SYN_CUDA(cudaFuncSetAttribute(stem_block1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    attr_set[h->device & 15] = true;
+  }
+  StemArgs a;
+  a.x = x; a.x_u8 = x_u8; a.wimg = h->d_fused + h->fused_off[1]; a.y = y; a.ntiles = batch * C::STRIPS;
+  a.err = h->d_err; a.sat = h->d_sat; a.border = x_u8 != nullptr ? h->center_crop : 0; a.npass = h->npass();
+  // persistent CTAs of two strip pipelines each; programmatic dependent launch as in launch_fused
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(std::min((a.ntiles + 1) / 2, h->sm_count));
+  cfg.blockDim = dim3(kStemB1Threads);
+  cfg.dynamicSmemBytes = C::SMEM_BYTES;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  SYN_CUDA(cudaLaunchKernelEx(&cfg, stem_block1_kernel, a));
+  SYN_LAUNCH_CHECK("stem_block1_kernel");
+  mark(h, st, "fused_stem_block1");
   return SYN_OK;
 }
 
@@ -890,11 +919,11 @@ int syn_commit(syn_handle_t* h) {
       all.insert(all.end(), img.begin(), img.end());
       all.resize((all.size() + 1023) / 1024 * 1024);
     };
-    pack_fused<FusedStemB1>(img, W(0), 27, Bv(0), W(1), Bv(1), W(2), Bv(2)); add(1);
+    pack_fused<StemCfg>(img, W(0), Bv(0), W(1), Bv(1), W(2), Bv(2)); add(1);
     auto blk = [&](int b, auto tag) {      // block b >= 2: convs 3b-3 (expand), 3b-2 (dw), 3b-1 (project)
       using Cfg = decltype(tag);
       const int e = 3 * b - 3;
-      pack_fused<Cfg>(img, W(e), Cfg::CIN, Bv(e), W(e + 1), Bv(e + 1), W(e + 2), Bv(e + 2));
+      pack_fused<Cfg>(img, W(e), Bv(e), W(e + 1), Bv(e + 1), W(e + 2), Bv(e + 2));
       add(b);
     };
     blk(2, FusedB2{}); blk(3, FusedB3{}); blk(4, FusedB4{}); blk(5, FusedB56{}); blk(6, FusedB56{});
