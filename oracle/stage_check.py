@@ -34,7 +34,7 @@ TAU = {
                   'pool': 9e-7,          # 2.38e-07
                   'params': 9e-8},       # 2.27e-08
     'tc_fused': {'block': 1.4e-7,        # 3.54e-08 (block 2)
-                 'pool': 6.9e-7,         # 1.75e-07 (tail kernel)
+                 'pool': 6.9e-7,         # 1.77e-07 (tail kernel)
                  'params': 8.8e-8},      # 2.22e-08
     # The single-pass engine measures 2.06e-06 (block 15) to 3.40e-05 (block 1) and 2.46e-05 at the tail: >= 14x the bar.
 

@@ -131,6 +131,69 @@ def scale_stream_channel(sd: Dict[str, torch.Tensor], stream: int, channel: int,
     return out
 
 
+DEAD_INPUT_BOUND = 937.5         # the largest |x| the split-fp16 engines take unchanged (60000 / kActScale)
+
+
+def _bn_scale(sd: Dict[str, torch.Tensor], bn: str) -> torch.Tensor:
+    """gamma / sqrt(var + eps) of a BatchNorm in float64: what folding multiplies the conv weights by."""
+    return sd[bn + '.weight'].double() / torch.sqrt(sd[bn + '.running_var'].double() + 1e-5)
+
+
+@torch.no_grad()
+def scale_hidden_channel(sd: Dict[str, torch.Tensor], block: int, channel: int, factor: float) -> Dict[str, torch.Tensor]:
+    """Block ``block`` (1..17) with hidden channel ``channel`` dead and its folded expand weights ``factor`` times the
+    rest's: the channel a trained checkpoint gets where BN folding divides by a near-zero running variance.  For block 1
+    the hidden tensor is the stem's output, for the others the expand conv's.
+
+    The conv weights of the channel are multiplied by ``factor`` and its BN beta set so that the folded bias is below
+    -2 * sum |folded w| * 937.5: the pre-activation is negative for every input the split engines take, so the channel's
+    hidden value is 0 after the ReLU6.  The input column of the block's project conv that reads the channel (through the
+    depthwise conv) is set to 0, which changes nothing more in the function and keeps the dead channel's large error
+    scale out of the project's.  This changes the function only through that one channel, which the original network
+    had active; stream magnitudes stay as they were."""
+    out = {k: v.clone() for k, v in sd.items()}
+    pre = 'I2P.backbone.'
+    plan = conv_plan()
+    first = [s for s in plan if s.block == block and s.kind in ('expand', 'dw')][0]
+    spec = plan[0] if first.kind == 'dw' else first                 # block 1: the stem is the expand
+    proj = [s for s in plan if s.block == block and s.kind == 'project'][0]
+    w = out[pre + spec.conv_key + '.weight']
+    w[channel] *= torch.tensor(factor, dtype=torch.float32)
+    bn = pre + spec.bn_key
+    scale = _bn_scale(out, bn)[channel]
+    reach = 2.0 * float((w[channel].double() * scale).abs().sum()) * DEAD_INPUT_BOUND
+    # folded bias = beta - mean * scale
+    out[bn + '.bias'][channel] = float(out[bn + '.running_mean'][channel].double() * scale) - reach
+    out[pre + proj.conv_key + '.weight'][:, channel] = 0.0
+    return out
+
+
+@torch.no_grad()
+def scale_output_channel(sd: Dict[str, torch.Tensor], conv_index: int, channel: int, factor: float,
+                         bias: float = None) -> Dict[str, torch.Tensor]:
+    """Output channel ``channel`` of conv ``conv_index`` with gamma and beta of its BN multiplied by ``factor``: its
+    folded weights and bias scale by ``factor``, and, unlike ``scale_stream_channel``, the convs that read it are left
+    as they are, so a tiny channel needs no reader column multiplied by up to 2^149.  Exact in fp32 for a power of two
+    whose products stay normal.  ``factor`` 0 makes an all-zero channel; with ``bias`` given, beta is set so that the
+    folded bias is that value."""
+    out = {k: v.clone() for k, v in sd.items()}
+    bn = 'I2P.backbone.' + conv_plan()[conv_index].bn_key
+    out[bn + '.weight'][channel] *= torch.tensor(factor, dtype=torch.float32)
+    out[bn + '.bias'][channel] *= torch.tensor(factor, dtype=torch.float32)
+    if bias is not None:
+        assert factor == 0, 'a chosen bias is for a zero channel'
+        out[bn + '.bias'][channel] = bias              # folded bias = beta - mean * 0
+    return out
+
+
+def channel_max(sd: Dict[str, torch.Tensor], conv_index: int, channel: int) -> float:
+    """max |folded weight| of one output channel of a conv, in float64."""
+    spec = conv_plan()[conv_index]
+    pre = 'I2P.backbone.'
+    w = sd[pre + spec.conv_key + '.weight'][channel].double() * _bn_scale(sd, pre + spec.bn_key)[channel]
+    return float(w.abs().max())
+
+
 def _pow2_factors(n: int, g: torch.Generator, lo: int, hi: int) -> torch.Tensor:
     """n factors 2^k, k an integer drawn from [lo, hi], with one channel at each end of the range."""
     k = torch.randint(lo, hi + 1, (n,), generator=g)

@@ -61,7 +61,8 @@ struct FusedCfg {
   static constexpr int B3_BYTES = round_up_c(2 * COUT_P * 4, 128);       // [2][COUT_P] fp32: b3, s3
   static constexpr int W1_PLANE = NC_ * CIN_P * 2;                       // bytes, one plane of one chunk
   static constexpr int W3_PLANE = COUT_P * NC_ * 2;
-  static constexpr int DW_ROWS = 12;   // 9 taps, depthwise bias, expand bias b1, expand output scale s1
+  static constexpr int DW_ROWS = 12;   // 9 taps, depthwise bias, expand bias b1 and output scale s1 (per channel,
+                                       // rows 10-11 interleaved as {b1, b1, s1, s1} per channel pair)
   static constexpr int CH_W1 = 0, CH_W3 = 2 * W1_PLANE, CH_DW = CH_W3 + 2 * W3_PLANE;
   static constexpr int CHUNK_BYTES = round_up_c(CH_DW + DW_ROWS * DWS * 4, 128);
   static constexpr int W_BYTES = B3_BYTES + NCHUNK * CHUNK_BYTES;
@@ -372,12 +373,16 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
         return sWch + slot * C::CHUNK_BYTES;
       };
       // ---- GEMM1 + EPI1 of chunk c, one 64-row slab of D1 at a time per warpgroup: relu6(s1*D1 + b1) / 6 -> hidden
-      // window.  The first slab is in flight on entry.  The expand scale is one power of two per layer (row 11 is
-      // constant), so an element costs one FFMA.SAT.
+      // window.  The first slab is in flight on entry.  The expand scale is one power of two per hidden channel, read
+      // with the bias (rows 10-11 hold {b1, b1, s1, s1} per channel pair), so an element costs one FFMA.SAT.
       auto gemm1_epi1 = [&](int c, const uint8_t* wch) {
         const float* dwc = reinterpret_cast<const float*>(wch + C::CH_DW);
-        const float sc1 = dwc[11 * C::DWS];
-        const float* b1 = dwc + 10 * C::DWS;
+        const float* bs1 = dwc + 10 * C::DWS;
+        // a thread's columns are the same in every slab and both row halves: its NC / 8 {b1 / 6, b1 / 6, s1, s1}
+        // vectors are loaded once per chunk
+        float4 bs[C::NC / 8];
+#pragma unroll
+        for (int q = 0; q < C::NC / 8; ++q) bs[q] = *reinterpret_cast<const float4*>(bs1 + 2 * acc_col(row, 4 * q));
 #pragma unroll
         for (int j = 0; j < SPW; ++j) {
           const int s1 = wg + j * NWG;                                // warpgroup-uniform
@@ -398,9 +403,8 @@ __global__ void __launch_bounds__((kFusedWorkerWarps + 1) * 32, 1) fused_mbconv_
 #pragma unroll
               for (int q = 0; q < C::NC / 8; ++q) {
                 const int i = 4 * q + 2 * h, j0 = acc_col(row, i);
-                const float2 bq = *reinterpret_cast<const float2*>(b1 + j0);
-                *reinterpret_cast<float2*>(hrow + j0) =
-                    make_float2(__saturatef(fmaf(acc[i], sc1, bq.x)), __saturatef(fmaf(acc[i + 1], sc1, bq.y)));
+                *reinterpret_cast<float2*>(hrow + j0) = make_float2(__saturatef(fmaf(acc[i], bs[q].z, bs[q].x)),
+                                                                   __saturatef(fmaf(acc[i + 1], bs[q].w, bs[q].y)));
               }
             }
           }

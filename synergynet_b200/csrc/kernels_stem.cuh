@@ -292,8 +292,12 @@ __global__ void __launch_bounds__(kStemB1Threads, 1) stem_block1_kernel(const St
       // ---- GEMM1 + EPI1: relu6(s1*D1 + b1) / 6 -> hidden window, one 64-row slab at a time ---------------------
       issue_g1(true, acc1[0], 0);
       {
-        const float sc1 = dwc[11 * C::DWS];
-        const float* b1 = dwc + 10 * C::DWS;
+        // {b1 / 6, b1 / 6, s1, s1} per channel pair, s1 per channel: a thread's columns are the same in every slab and
+        // both row halves, so its NC / 8 vectors are loaded once per strip
+        const float* bs1 = dwc + 10 * C::DWS;
+        float4 bs[C::NC / 8];
+#pragma unroll
+        for (int q = 0; q < C::NC / 8; ++q) bs[q] = *reinterpret_cast<const float4*>(bs1 + 2 * acc_col(row, 4 * q));
 #pragma unroll
         for (int s1 = 0; s1 < C::SLABS1; ++s1) {
           if (s1 + 1 < C::SLABS1) issue_g1(s1 + 1 < slabs1, acc1[(s1 + 1) & 1], s1 + 1);
@@ -310,9 +314,8 @@ __global__ void __launch_bounds__(kStemB1Threads, 1) stem_block1_kernel(const St
 #pragma unroll
               for (int q = 0; q < C::NC / 8; ++q) {
                 const int i = 4 * q + 2 * h, j0 = acc_col(row, i);
-                const float2 bq = *reinterpret_cast<const float2*>(b1 + j0);
-                *reinterpret_cast<float2*>(hrow + j0) =
-                    make_float2(__saturatef(fmaf(acc[i], sc1, bq.x)), __saturatef(fmaf(acc[i + 1], sc1, bq.y)));
+                *reinterpret_cast<float2*>(hrow + j0) = make_float2(__saturatef(fmaf(acc[i], bs[q].z, bs[q].x)),
+                                                                   __saturatef(fmaf(acc[i + 1], bs[q].w, bs[q].y)));
               }
             }
           }

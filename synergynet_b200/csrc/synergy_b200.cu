@@ -541,8 +541,10 @@ void pack_fused(std::vector<uint8_t>& img, const float* w1, const float* b1, con
     b3p[n] = b3[n];
     b3p[C::COUT_P + n] = 1.0f / (kActScaleHost * s3[n]);
   }
-  // one power-of-two scale for the whole expand layer (the kernel keeps it in a register): max |w1| in [256,512)
-  const float s1 = channel_scale(w1, 1, K * C::CHID);
+  // one power-of-two scale per hidden channel, like the project's: max |w1| of the channel in [256,512), so that a
+  // channel far above the others (a dead one, folded with a near-zero running variance) costs the others no bits
+  std::vector<float> s1(C::CHID);
+  for (int ch = 0; ch < C::CHID; ++ch) s1[ch] = channel_scale(w1 + ch, (size_t)C::CHID, K);
   for (int c = 0; c < C::NCHUNK; ++c) {
     const size_t chunk = C::B3_BYTES + (size_t)c * C::CHUNK_BYTES;
     float* d = reinterpret_cast<float*>(img.data() + chunk + C::CH_DW);
@@ -550,13 +552,14 @@ void pack_fused(std::vector<uint8_t>& img, const float* w1, const float* b1, con
       const int ch = c * C::NC + n;
       for (int k = 0; k < K; ++k) {
         const size_t off = (size_t)(n / 8) * 128 + (size_t)(k / 8) * ((C::NC / 8) * 128) + (n % 8) * 16 + (k % 8) * 2;
-        put(chunk + C::CH_W1 + off, w1[(size_t)k * C::CHID + ch] * s1, C::W1_PLANE);
+        put(chunk + C::CH_W1 + off, w1[(size_t)k * C::CHID + ch] * s1[ch], C::W1_PLANE);
       }
       for (int t = 0; t < 9; ++t) d[t * C::DWS + n] = dw[(size_t)t * C::CHID + ch];
       // the hidden activation is kept as relu6(h)/6 in [0,1] (kernels_fused.cuh): fold the 1/6 here
       d[9 * C::DWS + n] = bdw[ch] / 6.0f;
-      d[10 * C::DWS + n] = b1[ch] / 6.0f;
-      d[11 * C::DWS + n] = 1.0f / (6.0f * kActScaleHost * s1);
+      // rows 10-11: per channel pair {b1 / 6, b1 / 6, s1, s1}, the float4 EPI1 reads for its two columns
+      d[10 * C::DWS + 2 * (n & ~1) + (n & 1)] = b1[ch] / 6.0f;
+      d[10 * C::DWS + 2 * (n & ~1) + 2 + (n & 1)] = 1.0f / (6.0f * kActScaleHost * s1[ch]);
     }
     for (int n = 0; n < C::COUT; ++n)
       for (int k = 0; k < C::NC; ++k) {
