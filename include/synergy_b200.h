@@ -201,8 +201,9 @@ int syn_param_loss(syn_handle_t* h, const float* input_dev, const float* target_
  * syn_resnet50_forward: x_dev (B,3,120,120) NCHW -> out102_dev (B,102) exactly what ResNet._forward_impl returns;
  * pool2048_dev (B,2048) = the flattened avgpool, may be NULL.  (The reference's I2P unpacks two values from this
  * backbone and fails, SURVEY.md fact 4; the Python shim adapts: params = out[:, :62], pool = the 2048-d feature.)
- * Every forward and debug run of the ResNet and MobileNetV1 backbones (syn_resnet50_forward, syn_resnet_forward,
- * syn_mbv1_forward, syn_debug_resnet_until, syn_debug_mbv1_until) takes 1 <= B <= 65535 faces per call, and returns
+ * Every forward and debug run of the ResNet, MobileNetV1 and GhostNet backbones (syn_resnet50_forward,
+ * syn_resnet_forward, syn_mbv1_forward, syn_ghost_forward, syn_debug_resnet_until, syn_debug_mbv1_until,
+ * syn_debug_ghost_until) takes 1 <= B <= 65535 faces per call, and returns
  * SYN_ERR_INVALID before any launch otherwise. */
 int syn_resnet_num_convs(void);                              /* 53 */
 int syn_resnet_conv_desc(int idx, syn_conv_desc_t* out);
@@ -254,6 +255,30 @@ int syn_mbv1_set_heads(syn_handle_t* h, const float* w102xC_host, const float* b
 int syn_mbv1_commit(syn_handle_t* h);                        /* after syn_commit */
 int syn_mbv1_forward(syn_handle_t* h, const void* x_dev, int x_is_u8, int batch, float* out102_dev, float* pool_dev,
                      void* stream);
+
+/* ---- GhostNet backbone (backbone_nets/ghostnet_backbone.py, ghostnet() at width 1.0, eval) ----------------------------
+ * 95 convolutions in state-dict order: 0 = conv_stem (3x3/s2, 3 -> 16); per GhostBottleneck ghost1.primary_conv (1x1),
+ * ghost1.cheap_operation (3x3 depthwise), conv_dw (k x k/s2 depthwise, stride-2 blocks), se.conv_reduce and
+ * se.conv_expand (1x1 with bias, SE blocks), ghost2.primary_conv, ghost2.cheap_operation (`residual` = 1: its pass adds
+ * the shortcut), shortcut.0 (k x k depthwise) and shortcut.2 (1x1) where the block has them; then blocks.9.0.conv
+ * (1x1 160 -> 960) and conv_head (1x1 960 -> 1280 with bias).  syn_ghost_conv_desc gives each one's geometry (groups =
+ * cin for a depthwise; the SE convs and conv_head have h_in = h_out = 1).  Every conv with a BatchNorm takes OIHW fp32
+ * weights + eval BatchNorm2d through syn_ghost_set_conv; the SE convs and conv_head take weights and their (cout) bias
+ * through syn_ghost_set_conv_bias; a conv given to the wrong setter, or of the wrong size, is refused.  Heads: the four
+ * Linear layers concatenated in the reference's OUTPUT order classifier_ori | classifier_shape | classifier_exp |
+ * classifier_texture -> (102, 1280) weights, (102) bias.  syn_ghost_commit comes after syn_commit; BatchNorm is folded
+ * in float64.  syn_ghost_forward: x_dev as for syn_mbv1_forward -> out102_dev (B,102) = what GhostNet.forward returns;
+ * feat1280_dev (B,1280) = the conv_head output after its ReLU (what the heads read), may be NULL.  B is bounded as for
+ * the other conv+BN backbones. */
+int syn_ghost_num_convs(void);                               /* 95 */
+int syn_ghost_conv_desc(int idx, syn_conv_desc_t* out);
+int syn_ghost_set_conv(syn_handle_t* h, int idx, const float* w_host, int64_t w_numel, const float* bn_weight_host,
+                       const float* bn_bias_host, const float* bn_mean_host, const float* bn_var_host, float eps);
+int syn_ghost_set_conv_bias(syn_handle_t* h, int idx, const float* w_host, int64_t w_numel, const float* b_host);
+int syn_ghost_set_heads(syn_handle_t* h, const float* w102x1280_host, const float* b102_host);
+int syn_ghost_commit(syn_handle_t* h);                       /* after syn_commit */
+int syn_ghost_forward(syn_handle_t* h, const void* x_dev, int x_is_u8, int batch, float* out102_dev, float* feat1280_dev,
+                      void* stream);
 
 /* ---- Sim3DR: vertex normals, lighting, z-buffer rasterisation (SURVEY.md section 8 row f2) -------------------------
  * Handle-free; every pointer is caller-owned device memory unless it says _host.  B meshes share one triangle list
@@ -656,6 +681,16 @@ int syn_debug_resnet_until(syn_handle_t* h, const float* x_dev, int batch, int s
  * of blocks 1..12), 27 avgpool (B x 1024w), 28 heads (B x 102, no row maxima).  x_dev: fp32 crops. */
 int syn_debug_mbv1_until(syn_handle_t* h, const float* x_dev, int batch, int stage, float* out_dev, unsigned* rowmax_dev,
                          void* stream);
+/* GhostNet: one stage per launch output, in launch order -- stem; per block the primary GEMM's x1, the ghost concat
+ * [x1 | cheap(x1)], conv_dw, the SE pooled vector / conv_reduce (its columns padded to a multiple of 8 with exact zeros)
+ * / conv_expand / gated map, ghost2's x1, the shortcut's depthwise / pointwise outputs, and ghost2's concat with the
+ * shortcut added; then ConvBnAct, avgpool, conv_head, heads (the last stage; 111 in all).  syn_ghost_stage_desc gives
+ * each stage's rows per face (pixels, or 1), its columns and whether it records row maxima (max |row| as fp32 bits).
+ * x_dev: fp32 crops. */
+int syn_ghost_num_stages(void);                              /* 111 */
+int syn_ghost_stage_desc(int stage, int* rows_per_face, int* cols, int* has_rowmax);
+int syn_debug_ghost_until(syn_handle_t* h, const float* x_dev, int batch, int stage, float* out_dev, unsigned* rowmax_dev,
+                          void* stream);
 /* PointNet heads (rows = B*68 point-major, or B): net 0 = MLP_for: 0..4 conv1..conv5 (64, 64, 64, 128, 1024 columns;
  * conv5 is written only by this call, without row maxima), 5 the max-pooled global features (B x 1024), 6 the face vector
  * (B x 2360), 7 conv6's face part (B x 512, no row maxima), 8 conv6's point part (512), 9 conv7 (256), 10 conv8 (128),

@@ -107,6 +107,16 @@ SIGNATURES = {
     'syn_mbv1_commit': (_I, [_P]),
     'syn_mbv1_forward': (_I, [_P, _F, _I, _I, _F, _F, _P]),
     'syn_debug_mbv1_until': (_I, [_P, _F, _I, _I, _F, _P, _P]),
+    'syn_ghost_num_convs': (_I, []),
+    'syn_ghost_conv_desc': (_I, [_I, C.POINTER(ConvDesc)]),
+    'syn_ghost_set_conv': (_I, [_P, _I, _F, _L, _F, _F, _F, _F, C.c_float]),
+    'syn_ghost_set_conv_bias': (_I, [_P, _I, _F, _L, _F]),
+    'syn_ghost_set_heads': (_I, [_P, _F, _F]),
+    'syn_ghost_commit': (_I, [_P]),
+    'syn_ghost_forward': (_I, [_P, _F, _I, _I, _F, _F, _P]),
+    'syn_ghost_num_stages': (_I, []),
+    'syn_ghost_stage_desc': (_I, [_I, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)]),
+    'syn_debug_ghost_until': (_I, [_P, _F, _I, _I, _F, _P, _P]),
     'syn_debug_pointnet_until': (_I, [_P, _I, _F, _F, _F, _I, _I, _F, _P, _P]),
     'syn_debug_gemm': (_I, [_P, _F, _F, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _I, _I, _P, _F, _F, _I, _P, _I, _F, _P, _P]),
     'syn_mesh_incidence_host': (_I, [_F, _I, _I, _F, _F]),
@@ -174,6 +184,10 @@ _CORE = {n for n in SIGNATURES if n not in ('syn_peek_error', 'syn_poll_saturati
                                              'syn_resnet_arch_num_convs', 'syn_resnet_arch_conv_desc', 'syn_resnet_select', 'syn_resnet_forward',
                                              'syn_mbv1_num_convs', 'syn_mbv1_conv_desc', 'syn_mbv1_set_widen', 'syn_mbv1_set_conv',
                                              'syn_mbv1_set_heads', 'syn_mbv1_commit', 'syn_mbv1_forward', 'syn_debug_mbv1_until',
+                                             'syn_ghost_num_convs', 'syn_ghost_conv_desc', 'syn_ghost_set_conv',
+                                             'syn_ghost_set_conv_bias', 'syn_ghost_set_heads', 'syn_ghost_commit',
+                                             'syn_ghost_forward', 'syn_ghost_num_stages', 'syn_ghost_stage_desc',
+                                             'syn_debug_ghost_until',
                                              'syn_debug_pointnet_until', 'syn_debug_gemm',
                                              'syn_mesh_incidence_host', 'syn_mesh_normals', 'syn_mesh_lighting', 'syn_rasterize', 'syn_nms',
                                              'syn_crop_resize_plan_size', 'syn_crop_resize_plan_host', 'syn_crop_resize',

@@ -5,10 +5,12 @@ here only *hold* parameters under the same ``state_dict`` keys as the reference 
 checkpoints load unchanged (SURVEY.md section 8(b); reference
 ``backbone_nets/mobilenetv2_backbone.py:33-74,104-158`` and
 ``backbone_nets/pointnet_backbone.py:7-29,67-88``).  None of them implements a torch forward:
-there is deliberately no CPU/eager fallback for the product path.
+there is deliberately no CPU/eager fallback for the product path (``GhostNetParams.forward`` and the PointNet heads'
+forward call the library).
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
 from typing import List
 
@@ -413,3 +415,173 @@ def mobilenet_05(num_classes=62, input_channel=3):
 
 def mobilenet_025(num_classes=62, input_channel=3):
     return MobileNetV1Params(0.25, num_classes, input_channel)
+
+
+# ---- GhostNet backbone (reference backbone_nets/ghostnet_backbone.py, ghostnet() at width 1.0) -----------------------------
+
+# (k, exp, c, se_ratio, s) of ghostnet() (ghostnet_backbone.py:243-266), one row per GhostBottleneck, stage by stage
+GHOSTNET_CFGS = [[[3, 16, 16, 0, 1]], [[3, 48, 24, 0, 2]], [[3, 72, 24, 0, 1]], [[5, 72, 40, 0.25, 2]],
+                 [[5, 120, 40, 0.25, 1]], [[3, 240, 80, 0, 2]],
+                 [[3, 200, 80, 0, 1], [3, 184, 80, 0, 1], [3, 184, 80, 0, 1], [3, 480, 112, 0.25, 1],
+                  [3, 672, 112, 0.25, 1]],
+                 [[5, 672, 160, 0.25, 2]],
+                 [[5, 960, 160, 0, 1], [5, 960, 160, 0.25, 1], [5, 960, 160, 0, 1], [5, 960, 160, 0.25, 1]]]
+GHOSTNET_HEADS = ('classifier_ori', 'classifier_shape', 'classifier_exp', 'classifier_texture')
+
+
+def _make_divisible(v, divisor, min_value=None):
+    """The channel rounding of ghostnet_backbone.py:18-31."""
+    min_value = divisor if min_value is None else min_value
+    new_v = max(min_value, int(v + divisor / 2) // divisor * divisor)
+    return new_v + divisor if new_v < 0.9 * v else new_v
+
+
+def _conv_bn(cin, cout, k, stride=1, groups=1):
+    return [nn.Conv2d(cin, cout, k, stride, k // 2, groups=groups, bias=False), nn.BatchNorm2d(cout)]
+
+
+class _GhostModule(nn.Module):
+    """Keys of ``GhostModule`` (primary_conv.0/.1, cheap_operation.0/.1; :78-100)."""
+
+    def __init__(self, inp, oup):
+        super().__init__()
+        init = math.ceil(oup / 2)
+        self.primary_conv = nn.Sequential(*_conv_bn(inp, init, 1))
+        self.cheap_operation = nn.Sequential(*_conv_bn(init, init, 3, 1, init))
+
+
+class _SqueezeExcite(nn.Module):
+    """Keys of ``SqueezeExcite`` (conv_reduce, conv_expand, both with bias; :41-58)."""
+
+    def __init__(self, chs):
+        super().__init__()
+        red = _make_divisible(chs * 0.25, 4)
+        self.conv_reduce = nn.Conv2d(chs, red, 1, bias=True)
+        self.conv_expand = nn.Conv2d(red, chs, 1, bias=True)
+
+
+class _GhostBottleneck(nn.Module):
+    """Keys of ``GhostBottleneck`` (ghost1, conv_dw/bn_dw, se, ghost2, shortcut; :102-166)."""
+
+    def __init__(self, cin, mid, cout, k, stride, se_ratio):
+        super().__init__()
+        self.ghost1 = _GhostModule(cin, mid)
+        if stride > 1:
+            self.conv_dw = nn.Conv2d(mid, mid, k, stride, (k - 1) // 2, groups=mid, bias=False)
+            self.bn_dw = nn.BatchNorm2d(mid)
+        self.se = _SqueezeExcite(mid) if se_ratio else None
+        self.ghost2 = _GhostModule(mid, cout)
+        if cin == cout and stride == 1:
+            self.shortcut = nn.Sequential()
+        else:
+            self.shortcut = nn.Sequential(*_conv_bn(cin, cin, k, stride, cin), *_conv_bn(cin, cout, 1))
+
+
+class _ConvBnAct(nn.Module):
+    def __init__(self, cin, cout):
+        super().__init__()
+        self.conv = nn.Conv2d(cin, cout, 1, 1, 0, bias=False)
+        self.bn1 = nn.BatchNorm2d(cout)
+
+
+class GhostNetParams(nn.Module):
+    """Key schema of ``ghostnet_backbone.GhostNet(cfgs, num_classes, width, dropout)`` (:169-233), eval mode.  Unlike the
+    other parameter containers its ``forward`` works, as the reference's standalone module does: (B,3,120,120) fp32
+    normalised crops or raw uint8 crops -> the (B,102) ori | shape | exp | tex output, computed in the sm_90a library.
+    Only width 1.0 is built (the other widths give GEMMs with K = 12, which the tensor-core GEMM cannot take)."""
+
+    def __init__(self, cfgs=None, num_classes: int = 1000, width: float = 1.0, dropout: float = 0.2):
+        super().__init__()
+        if width != 1.0:
+            raise RuntimeError(f'GhostNet width {width}: the sm_90a GhostNet is built for width 1.0 only')
+        self.cfgs = GHOSTNET_CFGS if cfgs is None else cfgs
+        if [list(map(list, c)) for c in self.cfgs] != GHOSTNET_CFGS:
+            raise RuntimeError("the sm_90a GhostNet is built for the cfgs of ghostnet_backbone.ghostnet()")
+        self.dropout = dropout
+        self.conv_stem = nn.Conv2d(3, 16, 3, 2, 1, bias=False)
+        self.bn1 = nn.BatchNorm2d(16)
+        stages, cin = [], 16
+        for cfg in self.cfgs:
+            layers = []
+            for k, exp, c, se_ratio, s in cfg:
+                cout, mid = _make_divisible(c, 4), _make_divisible(exp, 4)
+                layers.append(_GhostBottleneck(cin, mid, cout, k, s, se_ratio))
+                cin = cout
+            stages.append(nn.Sequential(*layers))
+        stages.append(nn.Sequential(_ConvBnAct(cin, 960)))
+        self.blocks = nn.Sequential(*stages)
+        self.conv_head = nn.Conv2d(960, 1280, 1, 1, 0, bias=True)
+        self.num_ori, self.num_shape, self.num_exp, self.num_texture = 12, 40, 10, 40
+        self.classifier_ori = nn.Linear(1280, 12)
+        self.classifier_shape = nn.Linear(1280, 40)
+        self.classifier_exp = nn.Linear(1280, 10)
+        self.classifier_texture = nn.Linear(1280, 40)
+        object.__setattr__(self, '_rt', None)
+
+    def _compute_device(self, t: torch.Tensor) -> torch.device:
+        """As I2P._compute_device: the input's GPU, else the GPU the parameters live on, else the current CUDA device."""
+        if t.is_cuda:
+            return t.device
+        w = self.conv_stem.weight
+        if w.is_cuda:
+            return w.device
+        if not torch.cuda.is_available():
+            raise RuntimeError('synergynet_b200: no CUDA device (H100) visible; there is no CPU fallback')
+        return torch.device('cuda', torch.cuda.current_device())
+
+    def _engine(self, device: torch.device):
+        """The engine of ``device`` with this module's weights, handed over again when the state dict changes."""
+        from .model_building import _Runtime
+        if self._rt is None:
+            object.__setattr__(self, '_rt', _Runtime())
+            self._rt._mbv2_stub = {k: v for k, v in mobilenet_v2().state_dict().items()
+                                   if not k.endswith('num_batches_tracked')}
+        rt = self._rt
+        eng = rt.get(device, lambda: rt._mbv2_stub, None)      # the shared library state comes from a MobileNetV2 commit
+        sd = {k: v for k, v in self.state_dict(keep_vars=True).items() if not k.endswith('num_batches_tracked')}
+        sig = rt._signature(list(sd.values()))
+        key = (eng.device.index, 'ghostnet')
+        with rt._lock:
+            if rt._pn_sig.get(key) != sig or getattr(eng, '_ghost_commit_of', None) is not rt._sig.get(eng.device.index):
+                eng.load_ghostnet(sd)
+                rt._pn_sig[key] = sig
+                eng._ghost_commit_of = rt._sig.get(eng.device.index)
+        return eng
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        """GhostNet.forward (:214-233) in eval mode: (B,102).  A CPU input comes back on the CPU."""
+        if self.training:
+            raise RuntimeError('GhostNetParams.forward runs the eval forward (BatchNorm statistics, no dropout); '
+                               'call .eval() first')
+        if x.dim() != 4 or tuple(x.shape[1:]) != (3, IMG, IMG):
+            raise RuntimeError(f'expected (B,3,{IMG},{IMG}) crops, got {tuple(x.shape)}')
+        dev = self._compute_device(x)
+        out, _ = self._engine(dev).forward_ghostnet(x.to(dev))
+        return out if x.is_cuda else out.to(x.device)
+
+
+def ghostnet(**kwargs):
+    """ghostnet_backbone.ghostnet(**kwargs) (:236-268)."""
+    return GhostNetParams(GHOSTNET_CFGS, **kwargs)
+
+
+def ghostnet_conv_keys():
+    """(conv key, bn key or None) of the 95 convolutions in the order of the C ABI (syn_ghost_set_conv /
+    syn_ghost_set_conv_bias): the state-dict order.  A None bn key marks a conv with a bias (the SE convs, conv_head)."""
+    out, cin = [('conv_stem', 'bn1')], 16
+    for i, cfg in enumerate(GHOSTNET_CFGS):
+        for j, (k, exp, c, se, s) in enumerate(cfg):
+            p = f'blocks.{i}.{j}.'
+            out += [(p + 'ghost1.primary_conv.0', p + 'ghost1.primary_conv.1'),
+                    (p + 'ghost1.cheap_operation.0', p + 'ghost1.cheap_operation.1')]
+            if s > 1:
+                out.append((p + 'conv_dw', p + 'bn_dw'))
+            if se:
+                out += [(p + 'se.conv_reduce', None), (p + 'se.conv_expand', None)]
+            out += [(p + 'ghost2.primary_conv.0', p + 'ghost2.primary_conv.1'),
+                    (p + 'ghost2.cheap_operation.0', p + 'ghost2.cheap_operation.1')]
+            if not (cin == c and s == 1):
+                out += [(p + 'shortcut.0', p + 'shortcut.1'), (p + 'shortcut.2', p + 'shortcut.3')]
+            cin = c
+    out += [('blocks.9.0.conv', 'blocks.9.0.bn1'), ('conv_head', None)]
+    return out

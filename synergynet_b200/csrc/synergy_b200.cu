@@ -19,6 +19,7 @@
 #include "kernels_loss.cuh"
 #include "kernels_resnet.cuh"
 #include "kernels_mbv1.cuh"
+#include "kernels_ghost.cuh"
 
 using namespace syn;
 
@@ -43,12 +44,15 @@ struct syn_resnet;      // ResNet backbones (resnet_host.inl)
 void syn_resnet_destroy(syn_resnet* s);
 struct syn_mbv1;        // MobileNetV1 backbones (mbv1_host.inl)
 void syn_mbv1_destroy(syn_mbv1* s);
+struct syn_ghost;       // GhostNet backbone (ghost_host.inl)
+void syn_ghost_destroy(syn_ghost* s);
 
 struct syn_handle {
   int device = 0;
   syn_heads* heads = nullptr;
   syn_resnet* resnet = nullptr;
   syn_mbv1* mbv1 = nullptr;
+  syn_ghost* ghost = nullptr;
   int sm_count = 0;
   int engine = SYN_ENGINE_TC_FUSED;            // default: fused tensor-core engine; 0/1 remain for cross-checks
   int center_crop = 0;                         // CenterCrop margin applied by the uint8 entry points (syn_set_center_crop)
@@ -746,6 +750,7 @@ void syn_destroy(syn_handle_t* h) {
   syn_heads_destroy(h->heads);
   syn_resnet_destroy(h->resnet);
   syn_mbv1_destroy(h->mbv1);
+  syn_ghost_destroy(h->ghost);
   cudaFree(h->d_weights); cudaFree(h->d_head_w); cudaFree(h->d_head_b); cudaFree(h->d_mean);
   cudaFree(h->d_std); cudaFree(h->d_sparse); cudaFree(h->d_dense); cudaFree(h->d_tcw); cudaFreeHost(h->d_err); cudaFree(h->d_sat); cudaFree(h->d_fused); cudaFree(h->d_tc_oscale);
   cudaFree(h->buf_io[0]); cudaFree(h->buf_io[1]); cudaFree(h->buf_hid); cudaFree(h->buf_dw);
@@ -1323,6 +1328,7 @@ int syn_debug_forward_until(syn_handle_t* h, const float* x, int batch, int laye
 #include "convbn_host.inl"
 #include "resnet_host.inl"
 #include "mbv1_host.inl"
+#include "ghost_host.inl"
 
 // ---- debug: poisoned workspaces (include/synergy_b200.h) ------------------------------------------------------------------
 extern "C" {
@@ -1348,6 +1354,7 @@ int syn_debug_fill_workspaces(syn_handle_t* h, int byte, size_t* bytes_filled, v
   SYN_CUDA(heads_fill(h->heads, byte, st, &total));
   if (h->resnet != nullptr) SYN_CUDA(h->resnet->ws.fill(byte, st, &total));
   if (h->mbv1 != nullptr) SYN_CUDA(h->mbv1->ws.fill(byte, st, &total));
+  if (h->ghost != nullptr) SYN_CUDA(h->ghost->ws.fill(byte, st, &total));
   // the host pipelines run on the handle's own streams: they start after the fill
   if (h->s_compute != nullptr && h->s_compute != st) {
     cudaEvent_t e;

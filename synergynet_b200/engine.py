@@ -14,7 +14,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .backbone import HEAD_DIMS, MBV1_WIDTHS, RESNET_ARCHS, conv_plan, mobilenet_v1_conv_keys, resnet_conv_keys
+from .backbone import (GHOSTNET_HEADS, HEAD_DIMS, MBV1_WIDTHS, RESNET_ARCHS, conv_plan, ghostnet_conv_keys,
+                       mobilenet_v1_conv_keys, resnet_conv_keys)
 
 N_PARAMS = 62
 
@@ -417,7 +418,7 @@ class Engine(Handle):
                    out.data_ptr())
         return out
 
-    # ---- conv+BN backbones: ResNet and MobileNetV1, one (B,102) output ori | shape | exp | tex ---------------------
+    # ---- conv+BN backbones: ResNet, MobileNetV1 and GhostNet, one (B,102) output ori | shape | exp | tex ---------------------
     def _load_convbn(self, family: str, arch: str, select, conv_keys, feat: int, sd: Dict[str, torch.Tensor],
                      prefix: str) -> None:
         """Select the plan of ``arch`` (``select``: the entry's name and its arguments after the handle), then hand over its
@@ -547,6 +548,48 @@ class Engine(Handle):
         else:
             rows, cols, rm = b, feat if stage == 27 else 102, stage == 27
         return self._debug_run('syn_debug_mbv1_until', x, stage, rows, cols, rm)
+
+    # GhostNet backbone (backbone_nets/ghostnet_backbone.py, ghostnet() at width 1.0)
+    def load_ghostnet(self, sd: Dict[str, torch.Tensor], prefix: str = '') -> None:
+        """Hand a ``ghostnet_backbone.ghostnet()`` state dict to the library: its 95 convs in state-dict order (conv+BN
+        pairs, and the SE convs and conv_head with their biases), the four Linear heads concatenated in the reference's
+        output order ori | shape | exp | tex (ghostnet_backbone.py:229-233), then commit."""
+        with self._lock:
+            self._backbones['ghost'] = ('ghostnet', 1280)
+            for i, (ck, bk) in enumerate(ghostnet_conv_keys()):
+                w = _host_f32(sd[f'{prefix}{ck}.weight'])
+                if bk is None:
+                    b = _host_f32(sd[f'{prefix}{ck}.bias'])
+                    self._call_host('syn_ghost_set_conv_bias', i, w.data_ptr(), w.numel(), b.data_ptr())
+                else:
+                    bn = [_host_f32(sd[f'{prefix}{bk}.{k}']) for k in ('weight', 'bias', 'running_mean', 'running_var')]
+                    self._call_host('syn_ghost_set_conv', i, w.data_ptr(), w.numel(), *[t.data_ptr() for t in bn], 1e-5)
+            w = torch.cat([_host_f32(sd[f'{prefix}{k}.weight']) for k in GHOSTNET_HEADS]).contiguous()
+            b = torch.cat([_host_f32(sd[f'{prefix}{k}.bias']) for k in GHOSTNET_HEADS]).contiguous()
+            if tuple(w.shape) != (102, 1280):
+                raise RuntimeError(f'ghostnet heads: expected (102, 1280) weights, got {tuple(w.shape)}')
+            self._call_host('syn_ghost_set_heads', w.data_ptr(), b.data_ptr())
+            self._call_host('syn_ghost_commit')
+
+    def forward_ghostnet(self, x: torch.Tensor):
+        """GhostNet.forward (ghostnet_backbone.py:214-233) in eval mode: (B,3,120,120) fp32 normalised crops or raw uint8
+        crops -> ((B,102) ori|shape|exp|tex, (B,1280) the conv_head output after its ReLU, which the heads read)."""
+        return self._forward_convbn('ghost', x)
+
+    def ghostnet_stage_desc(self, stage: int) -> Tuple[int, int, bool]:
+        """(rows per face, columns, records row maxima) of stage ``stage`` of debug_ghostnet_until."""
+        r, c, m = C.c_int(0), C.c_int(0), C.c_int(0)
+        _lib.check(self._lib.syn_ghost_stage_desc(int(stage), C.byref(r), C.byref(c), C.byref(m)))
+        return r.value, c.value, bool(m.value)
+
+    def debug_ghostnet_until(self, x: torch.Tensor, stage: int):
+        """GhostNet run up to ``stage`` (one stage per launch output, include/synergy_b200.h syn_debug_ghost_until):
+        (that stage's output as (rows, channels) -- one row per NHWC pixel, or per face --, its row maxima as int32 fp32
+        bit patterns, or None for a stage that records none)."""
+        x = self._check_x(x)
+        self._backbone('ghost')
+        rows, cols, rm = self.ghostnet_stage_desc(stage)
+        return self._debug_run('syn_debug_ghost_until', x, stage, x.shape[0] * rows, cols, rm)
 
     # ---- per-stage debug runs of the GEMM layers (include/synergy_b200.h syn_debug_*_until / syn_debug_gemm) ----
     RESNET_STAGES = 56
